@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- genes/sec of the DESeq2 Wald hot path (fitDisp MLE + fitDisp MAP + fitBeta) on B200.
+"""bench.py -- genes/sec of the DESeq2 Wald hot path (fitDisp MLE + fitDisp MAP + fitBeta) on H100.
 
 Contract (see task text): `python bench.py --gpus N --steps K --warmup W` prints ONE JSON line on rank 0.
   step      one pass of the hot path over one batch of synthetic counts: fitDisp (gene-wise MLE) ->
@@ -47,6 +47,7 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the BASELINE configs 3-5 block")
     ap.add_argument("--quick-configs", action="store_true", help="configs block at 20%% of the stated sizes")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     ap.add_argument("--r-default-probe", action="store_true", help=argparse.SUPPRESS)
     return ap.parse_args()
 
@@ -104,10 +105,39 @@ def host_bytes(n, m, p):
     return h2d, d2h
 
 
+DUMP_GENES, DUMP_MATRIX_ENTRIES = 1 << 16, 1 << 20
+
+
+def dump_outputs(outs, n, m, path):
+    """The results of the last timed step, as float64 .npy files named <call>.<result>.npy: the per-gene results (and
+    the p x n coefficient matrices) of a fixed seeded sample of at most DUMP_GENES genes, the genes x samples matrices
+    (hat diagonals, fitted means) of the first genes of that sample, at most DUMP_MATRIX_ENTRIES entries each.  The
+    sampled gene indices are genes.npy and genes_matrix.npy.  Everything stays under 64 MB."""
+    os.makedirs(path, exist_ok=True)
+    perm = np.random.default_rng(20260925).permutation(n)
+    genes = np.sort(perm[:DUMP_GENES])
+    genes_matrix = np.sort(perm[:max(1, DUMP_MATRIX_ENTRIES // m)])
+    files = {"genes": genes, "genes_matrix": genes_matrix}
+    for call, res in zip(("fit_disp_mle", "fit_disp_map", "fit_beta"), outs):
+        for k, v in res.items():
+            if v is None:
+                continue
+            a = v.detach().cpu().numpy()
+            if a.ndim == 1:
+                a = a[genes]
+            elif k in ("hat_diagonals", "mu"):                  # gene-major (n, ld): the first m columns are valid
+                a = a[genes_matrix, :m]
+            else:                                              # (p, n) coefficient matrix
+                a = a[:, genes]
+            files[f"{call}.{k}"] = a
+    for k, a in files.items():
+        np.save(os.path.join(path, k + ".npy"), np.asarray(a, dtype=np.float64))
+
+
 # ---------------------------------------------------------------- clocks
 
 class ClockSampler:
-    """SM clock / throttle-reason log for the timed region, the way /opt/skills/guides/B200_PROFILING.md does it: a
+    """SM clock / throttle-reason log for the timed region: a
     separate `nvidia-smi -lms` process started BEFORE the warm-up and stopped after the run (in-process NVML polling
     was measured to stall the launching thread by 0.3-3 ms per query; a forked nvidia-smi per sample by far more).
     Rows are attributed to the timed region by their timestamps; the GPU is kept under the same load until at least
@@ -481,7 +511,7 @@ def main():
     n, m = a.genes, a.samples
     cfg = {"workload": f"C2: {n} genes x {m} samples per GPU, ~condition (p=2) Wald: fitDisp(MLE)+fitDisp(MAP)+fitBeta",
            "genes_per_gpu": n, "samples": m, "p": 2, "parallelism": f"gene-sharded x{world}",
-           "l2": "inputs rotate over 4 device replicas (400 MB working set > 126 MB L2)"}
+           "l2": "inputs rotate over 4 device replicas (working set > 50 MB L2)"}
 
     if a.impl == "reference":
         if rank != 0:
@@ -609,12 +639,9 @@ def main():
         step(i, True)            # warm-up includes the event records the timed steps make
     torch.cuda.synchronize()
     launches0 = L.b200nb_kernel_launches()
-    # The timed region (exactly K steps between barrier + synchronize) is repeated REPEATS times and the MEDIAN
-    # repetition is reported (all repetitions are listed in config.timed_repeats_ms): the GPU boxes show an
-    # occasional ~80 ms stall that is unrelated to the workload (it hits whatever kernel happens to be running,
-    # also with garbage collection off and zero cudaMalloc/cudaFree traffic), and a single 75 ms timed region
-    # would otherwise be at its mercy.
-    REPEATS = 3
+    # The timed region is exactly K = --steps steps between barrier + synchronize.  A shared GPU host can stall a
+    # kernel now and then for reasons unrelated to the workload, so choose K large enough that one stall is noise.
+    REPEATS = 1
     no_ev = bool(os.environ.get("B200NB_NO_STEP_EVENTS"))
     rep_ms, rep_evs, rep_w0 = [], [], []
     for rep in range(REPEATS):
@@ -647,7 +674,9 @@ def main():
     total_ms = rep_ms[pick]
     evs = rep_evs[pick]
     cfg["timed_repeats_ms"] = [round(v, 3) for v in rep_ms]
-    cfg["timed_repeat_reported"] = "median of %d repetitions of the K-step timed region" % REPEATS
+    cfg["timed_repeat_reported"] = "one K-step timed region"
+    if a.dump_outputs and rank == 0:
+        dump_outputs(outs, ng, m, a.dump_outputs)
     # keep the GPU busy a little longer so the clock sampler sees load even for very short runs
     clocks = None
     if rank == 0:
@@ -773,9 +802,9 @@ def main():
     cfgs = None
     if not a.no_configs:
         try:
-            pk = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 6650.0))
+            pk = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 3350.0))
         except Exception:
-            pk = 6650.0
+            pk = 3350.0
         cfgs = configs_block(world, rank, dev, pk, quick=a.quick_configs)
 
     if rank != 0:
@@ -789,7 +818,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     dom = max(kern_ms, key=kern_ms.get)
     if dom.startswith("fit_disp"):
         alg_bytes = ng * (12 * m + 88)
@@ -803,7 +832,7 @@ def main():
         pass
     roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
                 "frac": achieved / peak, "traffic": traffic,
-                "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                "peak_source": "MEASURED_PEAKS.json (of measured)" if peaks else "H100 SXM data sheet, 3350 GB/s (not measured)",
                 "kernel_ms": kern_ms, "alg_bytes_per_launch": alg_bytes,
                 "note": "fp64 transcendental-bound path (~300 flop/B): HBM fraction is small by construction; the "
                         "binding unit is the FP64 pipe (ncu summaries under profiles/)"}

@@ -1,7 +1,7 @@
-"""deseq2_b200 -- B200-native batched negative-binomial GLM engine behind DESeq2's native boundary.
+"""deseq2_b200 -- H100-native (sm_90a) batched negative-binomial GLM engine behind DESeq2's native boundary.
 
 Scope: the ONE hot path of thelovelab/DESeq2 -- fitDisp / fitDispGrid / fitBeta
-(/root/reference/src/DESeq2.cpp:164,469,283) -- as hand-written sm_100a kernels in
+(the reference's src/DESeq2.cpp:164,469,283) -- as hand-written sm_90a kernels in
 `csrc/`, exported through the C ABI in `include/b200nb.h` (libb200nb.so), plus the host-side
 mirror of the reference's R callers needed to drive and measure it:
 

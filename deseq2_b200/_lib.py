@@ -19,7 +19,7 @@ def lib_path() -> str:
 
 
 def build(force: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a into deseq2_b200/libb200nb.so (in-tree, nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a into deseq2_b200/libb200nb.so (in-tree, nvcc cross-compiles without a GPU)."""
     args = ["make", "-C", os.path.join(_HERE, "csrc"), "-s", "-j4"]
     if force:
         args.append("-B")

@@ -136,12 +136,11 @@ std::atomic<long long> g_h2d_bytes{0}, g_d2h_bytes{0}, g_cache_hits{0}, g_cache_
     g_hashed_bytes{0};
 
 // ---------------------------------------------------------------- pinned staging ring
-// R hands over ordinary (pageable) memory; cudaMemcpy from pageable memory runs at ~9 GB/s on the GPU box.  A ring of
+// R hands over ordinary (pageable) memory; cudaMemcpy from pageable memory is slow.  A ring of
 // pinned buffers filled by the pool while the previous buffer is in flight reaches PCIe speed.
-// Size of one ring buffer and of one pool task.  One rank per host: 8 MB buffers (fewest synchronisations; 4.8 ms per C2
-// step vs 5.1 ms with 2 MB).  Several ranks per host: the four buffers of every rank should stay resident in the shared
-// last-level cache between the staging copy and the DMA that reads them -- with 8 ranks on a 2 x 60 MB-L3 host, 2 MB
-// buffers took 1.2 ms off the 9 ms step (profiles/r02_host_path.md) -- so 4 MB from two local ranks, 2 MB from four.
+// Size of one ring buffer and of one pool task.  One rank per host: 8 MB buffers (fewest synchronisations).  Several
+// ranks per host: the four buffers of every rank should stay resident in the shared last-level cache between the
+// staging copy and the DMA that reads them -- so 4 MB from two local ranks, 2 MB from four.
 // B200NB_STAGE_KB / B200NB_STAGE_BLOCK_KB override (read once, when the library loads).
 static size_t default_stage_kb() {
   const int local_ranks = hostrt::env_int("LOCAL_WORLD_SIZE", 1, 1, 64);
@@ -280,7 +279,7 @@ int h2d_rows(void* dst, const void* host, size_t n_total, size_t g0, size_t gc, 
 // ---------------------------------------------------------------- pinned result memory (b200nb_host_alloc)
 // A result matrix that the caller allocates with b200nb_host_alloc lives in page-locked memory: the device-to-host copy
 // is then ONE DMA straight into it -- no staging ring, no scatter by host threads and, above all, no first-touch page
-// faults (a freshly malloc'ed 40 MB hat-diagonal matrix costs ~3 ms of faults on the GPU box, more than the kernels).
+// faults (a freshly malloc'ed 40 MB hat-diagonal matrix costs milliseconds of faults, more than the kernels).
 // Blocks are pooled: b200nb_host_free returns them for reuse; the pool keeps at most B200NB_PINNED_POOL_MB (default
 // 1024) of idle blocks.  R can place the REALSXP itself there through allocVector3's custom allocator (r_shim/).
 struct PinBlock {
@@ -725,9 +724,8 @@ bool use_generic(int p) {
 
 // Long rows on the small-p designs too: from m = 400 samples on the segmented general-p kernels (fit_generic_seg.cuh:
 // one gene per warp, per-segment sums, 1024-entry factor table) beat the register-resident small-p kernels, whose
-// per-sample X'WX accumulation and 256-entry table are sized for short rows -- measured on the B200
-// (profiles/r02_kernel_ab.md: 25 000 x 500, p = 4: fitDisp 3.00 -> 2.38 ms, fitBeta 1.08 -> 0.99 ms; 10 000 x 1000, p = 2:
-// 1.42 -> 1.00 ms, 0.76 -> 0.59 ms; at m = 300 and below the small-p kernels win).  Only the device entry points called
+// per-sample X'WX accumulation and 256-entry table are sized for short rows (at m = 300 and below the small-p kernels
+// win).  Only the device entry points called
 // directly take this route (it fetches the design matrix: one stream sync per call); the host entry points keep the
 // small-p kernels, whose launches per row chunk overlap the uploads.  B200NB_LONG_ROWS=<m> moves the threshold, 0 = off.
 thread_local int t_in_host_call = 0;
@@ -994,7 +992,7 @@ struct PhaseClock {
 extern "C" {
 
 const char* b200nb_last_error(void) { return g_err; }
-const char* b200nb_version(void) { return "b200nb 0.2 (sm_100a)"; }
+const char* b200nb_version(void) { return "b200nb 0.2 (sm_90a)"; }
 long long b200nb_kernel_launches(void) { return g_launches.load(); }
 
 int b200nb_device_count(void) {

@@ -1,4 +1,4 @@
-// engine.h -- internal launcher interface between the C ABI (capi.cu) and the sm_100a kernels.
+// engine.h -- internal launcher interface between the C ABI (capi.cu) and the sm_90a kernels.
 // Device layout ("gene-major"): every n x m matrix is stored one gene per row with the sample axis
 // contiguous, row stride `ld` elements (ld % 4 == 0 so rows start 32-byte aligned for 128-bit loads).
 // The design matrix x stays in R's column-major m x p form (it is tiny and staged into shared memory).

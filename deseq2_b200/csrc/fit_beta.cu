@@ -1,4 +1,4 @@
-// fit_beta.cu -- per-gene ridge-penalised NB IRLS on sm_100a, one warp per gene.
+// fit_beta.cu -- per-gene ridge-penalised NB IRLS on sm_90a, one warp per gene.
 //
 // Behavioural contract (WHAT): /root/reference/src/DESeq2.cpp:283-465 (fitBeta): mu = max(nf*exp(X b), minmu),
 // w = [wt*]mu/(1+alpha*mu), z = log(mu/nf) + (y-mu)/mu, b = argmin ridge WLS, |b|>30 => iter=maxit (diverged b

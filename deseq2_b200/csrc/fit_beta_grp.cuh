@@ -1,5 +1,5 @@
-// fit_beta_grp.cuh -- several genes per warp for the IRLS kernel (the default for m <= ~330 samples; measured on B200,
-// C2 50k x 100: fitBeta 0.49 -> 0.42 ms with two genes per warp; 20k x 12: 0.24 -> 0.11 ms with four).  See fit_disp_grp.cuh for the idea;
+// fit_beta_grp.cuh -- several genes per warp for the IRLS kernel (the default for m <= ~330 samples: two genes per
+// warp at C2's 100 samples, four at 12).  See fit_disp_grp.cuh for the idea;
 // included by fit_beta.cu inside namespace nb::{anonymous}.
 //
 // A warp holds NG = 32 / GL genes, GL lanes each.  Control flow is warp-uniform: a round loads one gene per group, all

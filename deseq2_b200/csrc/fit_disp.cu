@@ -1,4 +1,4 @@
-// fit_disp.cu -- gene-wise Cox-Reid adjusted NB dispersion MLE/MAP on sm_100a, one warp per gene.
+// fit_disp.cu -- gene-wise Cox-Reid adjusted NB dispersion MLE/MAP on sm_90a, one warp per gene.
 //
 // Behavioural contract (WHAT): /root/reference/src/DESeq2.cpp:164-277 (fitDisp: Armijo back-tracking
 // ascent on log alpha, accept / reject / kappa schedule replicated decision for decision), :31-158
@@ -278,8 +278,8 @@ __device__ __forceinline__ double disp_d2(const DispRow& rv, const DispScal& sc,
 // ---------------------------------------------------------------- gene classification
 // One warp per gene: largest / smallest count and integrality decide the evaluation mode; genes are appended to
 // one list per mode so the persistent kernel can work through one mode at a time (keeps the instruction
-// working set of an SM inside the instruction cache: the first fused version stalled 70% on instruction fetch,
-// profiles/r01b_*).  lists[mode * n + i], counts[mode].
+// working set of an SM inside the instruction cache: a fused version stalls on instruction fetch).
+// lists[mode * n + i], counts[mode].
 // TAB genes ordered by the length of their count table, longest first (8 buckets of 32; used by the 8-lane kernels),
 // so that genes which share a warp in the narrow-group kernels wait for tables of similar length, and the launch ends
 // on the cheap genes.  classify_kernel records a bucket per TAB gene and counts the buckets; bucket_sort_kernel places
@@ -667,7 +667,7 @@ cudaError_t launch_disp_t(const DispArgs& a0, cudaStream_t stream) {
     int* code = lists + 3 * (size_t)a.n;
     int* sorted = lists + 4 * (size_t)a.n;
     // Table-length ordering of the TAB list only pays when four genes share a warp (8 lanes per gene: they wait for the
-    // longest table of the four; measured on B200, 20k x 12: 0.46 -> 0.36 ms) and costs 10 % at two genes per warp
+    // longest table of the four) and costs time at two genes per warp
     const bool buckets = group_lanes_disp(a.m) == 8;
     classify_kernel<<<(a.n + 7) / 8, 256, 0, stream>>>(a.y, a.y_is_f64, a.n, a.m, a.ld, lists, a.scratch + 1,
                                                        buckets ? code : nullptr, a.scratch + 8);

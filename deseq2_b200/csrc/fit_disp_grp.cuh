@@ -1,5 +1,5 @@
-// fit_disp_grp.cuh -- several genes per warp (the default for m <= ~330 samples; measured on B200, C2 50k x 100:
-// fitDisp 1.02 -> 0.92 ms with two genes per warp; 20k x 12: 0.41 -> 0.36 ms with four and table-length ordering).
+// fit_disp_grp.cuh -- several genes per warp (the default for m <= ~330 samples: two genes per warp at C2's 100
+// samples, four with table-length ordering at 12).
 //
 // Included by fit_disp.cu inside namespace nb::{anonymous}.  The product kernel gives a gene the whole warp: at
 // m = 100 the sample loop is 4 sweeps of 32 lanes (22 % of the last sweep idle) and everything that happens once per

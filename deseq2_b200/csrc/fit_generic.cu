@@ -22,10 +22,8 @@
 #include "engine.h"
 #include "nbmath.cuh"
 
-// Unroll factors of the two per-sample loops.  These kernels are instruction-cache bound, not latency bound (ncu of the
-// config-4 shape: 34 % of the stall samples no_instructions at 19k SASS instructions, 7 warps per SM): on the B200
-// unroll 1 | 2 | 4 | 8 of the dispersion loop gave 4.98 | 5.18 | 6.91 | 10.5 ms for 20 000 genes x 1000 samples, and
-// __noinline__ evaluation functions or a 128-register cap made it slower (profiles/r02_kernel_ab.md).
+// Unroll factors of the two per-sample loops.  These kernels are instruction-cache bound, not latency bound (large
+// bodies, few warps per SM at the config-4 shape), so the loops are not unrolled by default.
 #ifndef NB_EXP_GEN_UNROLL_DISP
 #define NB_EXP_GEN_UNROLL_DISP 1
 #endif
@@ -853,13 +851,11 @@ bool plan_one(int m, int p, int G, int grouped, GenShape sh, size_t extra_double
 }
 
 // Rows in shared memory whenever they fit.  Config 4 (m = 1000, two rows = 16 KB per warp) leaves 7 warps per SM; moving
-// the rows to a per-warp slice of an L2-resident global scratch buffer (rows_global) doubles the resident warps but was
-// measured 5-10 % SLOWER on the B200 (profiles/r02_kernel_ab.md: 20k x 1000, p = 10: fitDisp 6.76 -> 7.43 ms, fitBeta
-// 4.87 -> 5.02 ms): the per-pass row reads turn from shared-memory into L2 latency and the kernel is not
-// occupancy-bound.  The global path remains for rows that do not fit in shared memory at all (m > ~6000) and as the
+// the rows to a per-warp slice of an L2-resident global scratch buffer (rows_global) doubles the resident warps, but
+// the per-pass row reads turn from shared-memory into L2 latency and the kernel is not occupancy-bound.  The global path remains for rows that do not fit in shared memory at all (m > ~6000) and as the
 // A/B switch B200NB_GENERIC_ROWS=global.
 bool plan(int m, int p, int G, int grouped, GenShape sh, size_t extra_doubles, GenLaunch& out) {
-  const char* force = getenv("B200NB_GENERIC_ROWS");   // "smem" | "global": A/B switch for the measurement in profiles/
+  const char* force = getenv("B200NB_GENERIC_ROWS");   // "smem" | "global": A/B switch
   if (force && (force[0] == 's' || force[0] == 'g')) {
     sh.rows_global = force[0] == 'g';
     if (plan_one(m, p, G, grouped, sh, extra_doubles, out)) return true;

@@ -4,7 +4,7 @@
 //
 // Why a second form.  With long rows (config 4: m = 1000) the kernels of fit_generic.cu keep two fp64 rows plus
 // G x 32 lane-private accumulator slots per set in shared memory: 30 KB per warp, 7 warps per SM, 254 registers --
-// ncu shows 10 % of the warp slots occupied and every stall reason a latency (profiles/r02h_generic_*).  Here
+// few warps are resident and every stall reason is a latency.  Here
 //   * the samples are laid out sorted by design group, each lane owning a contiguous chunk of the sorted sequence
 //     (engine.h::SegLayout, prepared once per call on the host): a lane meets one or two groups per pass, keeps the
 //     per-group sums in REGISTERS and stores one value per segment (kmax x 32 slots instead of G x 32, no
@@ -17,7 +17,7 @@
 //   * the sample loops are specialised at compile time (factor table or not, second derivative or not), and the
 //     per-group work sits in ONE divergent region ahead of the warp reductions.
 // Config 4 then needs 13.6 KB (dispersion) / 9 KB (IRLS) per warp and the kernels run 16 warps per SM at <= 128
-// registers: fitDisp 5.00 -> 1.82 ms, fitBeta 3.91 -> 1.69 ms for 20 000 genes (profiles/r02_kernel_ab.md).  Weights, the
+// registers.  Weights, the
 // grid search and samplewise designs stay on the kernels of fit_generic.cu.  The device entry points also send long
 // rows (m >= 400) of designs with p <= 4 here (capi.cu::long_rows).
 
@@ -256,8 +256,6 @@ __device__ __forceinline__ void sdisp_samples(const SDispCtx& C, double alpha, d
   double aW = 0.0, aB = 0.0, aC = 0.0;
   const double* mus = S.mu;
   const unsigned short* y16 = S.y16;
-  // (a uniform full-trip loop with a guarded tail sample, and running stores instead of the segment-end test, were
-  // measured on the B200: both slower than this plain loop, profiles/r02_kernel_ab.md)
   for (int i = 1, j = lane; j < m; i++, j += 32) {
     const double mu = mus[j];
     double y;

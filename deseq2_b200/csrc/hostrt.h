@@ -196,7 +196,7 @@ inline int pci_numa_node(const char* pci_bus_id) {   // "0000:1b:00.0" (any case
 
 // CPUs the container may burn per scheduling period (cgroup v2 cpu.max, v1 cpu.cfs_quota_us / cfs_period_us), rounded
 // up; 0 = no quota.  A process whose runnable (spinning!) threads exceed it is throttled as a whole for the rest of the
-// 100 ms period -- measured on the 1-GPU lease (affinity 128 CPUs, quota 16): holes of 40-90 ms in the host timeline.
+// 100 ms period, which leaves holes of tens of ms in the host timeline.
 inline int cgroup_cpu_quota() {
   long long q = -1, per = 100000;
   if (FILE* f = fopen("/sys/fs/cgroup/cpu.max", "r")) {

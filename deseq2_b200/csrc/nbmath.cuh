@@ -1,12 +1,11 @@
-// nbmath.cuh -- fp64 device math for the NB-GLM kernels (sm_100a).
+// nbmath.cuh -- fp64 device math for the NB-GLM kernels (sm_90a).
 //
 // Own implementations of the special functions the reference pulls from R's nmath
 // (Rf_lgammafn / Rf_digamma / Rf_trigamma, call sites /root/reference/src/DESeq2.cpp:50-58,90-96,139-145)
 // and of log() for strictly positive normal arguments.  Written for the GPU's FP64 pipe:
 //   * one log + one reciprocal per fused lgamma/digamma pair, the rest FMAs;
 //   * every polynomial coefficient lives in a __constant__ table so it reaches the DFMA as a uniform-register
-//     operand filled by LDCU.128 (two coefficients per instruction) -- the first profile
-//     (profiles/r01a_fit_disp_sass_hist.txt) showed 30% of issue slots spent on UMOV/IMAD.MOV pairs
+//     operand (two coefficients per instruction) instead of issue slots spent on UMOV/IMAD.MOV pairs
 //     materialising 64-bit immediates;
 //   * no special-case branches (callers guarantee positive, finite, normal inputs).
 #pragma once
@@ -63,8 +62,7 @@ __device__ const double4 g_logtab[129] = {
 };
 // The grid point c is rebuilt from k with two integer instructions instead of being loaded, and the table is split into
 // {1/c, hi(log c)} (one LDS.128) and lo(log c) (one LDS.64): 24 instead of 32 bytes of shared-memory traffic per call.
-// The random-index fetch is the kernels' top short-scoreboard stall and bank-conflict source; measured on B200 (C2):
-// fitDisp 0.92 -> 0.87 ms against the single double4 table.
+// The random-index fetch is the kernels' top short-scoreboard stall and bank-conflict source.
 __shared__ double2 s_logA[129];
 __shared__ double s_logL[129];
 

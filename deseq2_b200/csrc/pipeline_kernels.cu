@@ -96,7 +96,7 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
 
 // The same pre-steps for a design with G <= 32 distinct rows (factor designs: config 4 has m = 1000, p = 10, G = 10).
 // prep_kernel streams the p x m projection and the m x p design through every gene (2 p m loads and FMAs per gene,
-// L2 latency bound at 8 warps per SM: 5 ms for 50 000 x 1000); here a sample only adds its value and its log to its
+// L2 latency bound at 8 warps per SM); here a sample only adds its value and its log to its
 // group's lane-private slot, the projection is applied to the G group sums and the fitted value is read per group.
 __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int mpad, int ps) {
   extern __shared__ __align__(16) double smem[];

@@ -74,8 +74,7 @@ def _projection(x):
     """(X'X)^-1 X' (p x m) WITHOUT a BLAS / LAPACK call.  numpy hands `x.T @ x` and linalg.solve to OpenBLAS, whose
     worker threads (one per CPU the process may run on: 64-128 on the GPU hosts) then busy-wait for ~100 ms; under a
     container CPU quota (the 1-GPU lease: cpu.max = 16 CPUs) that spin exhausts the quota and the kernel throttles the
-    WHOLE process for the rest of the period -- measured: DESeq_device on the config-4 shape took 100-170 ms instead of
-    54 ms, with random 40-90 ms holes in the host timeline (profiles/r02_pipeline_host_stalls.md).  The matrices
+    WHOLE process for the rest of the period, leaving random holes of tens of ms in the host timeline.  The matrices
     are p x p with p <= 32: einsum's own loops and a Gauss-Jordan sweep with partial pivoting are plenty."""
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape

@@ -1,5 +1,5 @@
 /*
- * b200nb.h -- C ABI of the B200-native batched negative-binomial GLM engine (libb200nb.so, sm_100a).
+ * b200nb.h -- C ABI of the H100-native batched negative-binomial GLM engine (libb200nb.so, sm_90a).
  *
  * This is the drop-in boundary for the ONE hot path of thelovelab/DESeq2: the three native routines the R
  * package reaches through .Call (registration table /root/reference/src/RcppExports.cpp:84-94):

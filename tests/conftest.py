@@ -12,7 +12,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def _gpu_usable():
@@ -31,7 +31,7 @@ def pytest_collection_modifyitems(config, items):
     on a CUDA box whose engine library is missing -- that has to fail loudly)."""
     if _gpu_usable():
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (run on an H100: pytest -m gpu)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -61,3 +61,64 @@ def rel_err(a, b, floor=1e-12):
     a = np.asarray(a, dtype=np.float64)
     b = np.asarray(b, dtype=np.float64)
     return np.abs(a - b) / np.maximum(np.abs(b), floor)
+
+
+REFERENCE_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference", "outputs.npz")
+REF_ROWS, REF_COLS = 48, 8
+
+
+class StoredReference:
+    """Outputs of the reference's own src/DESeq2.cpp (compiled unchanged into oracle/_ref, see oracle/ref.py) on the
+    tests' inputs, stored in tests/golden/reference/outputs.npz so that the comparisons run without the reference.
+
+    Every call names its case.  The file keeps, per case, the outputs at a fixed seeded sample of REF_ROWS genes
+    (`rows`; every gene for fitDispGrid) and, for the genes x samples hat diagonals, of REF_COLS samples (`cols`);
+    `at(result, stored)` picks the same entries out of a full result.  tests/golden/reference/make.py rewrites the file: with
+    DESEQ2_RECORD_REFERENCE=1 every call runs the reference library and records what it returned."""
+
+    def __init__(self):
+        self.record = os.environ.get("DESEQ2_RECORD_REFERENCE") == "1"
+        self.stored = dict(np.load(REFERENCE_GOLDEN)) if os.path.exists(REFERENCE_GOLDEN) else {}
+        if self.record:
+            from oracle import ref as R
+            R.build()
+            self.R = R
+
+    def _call(self, fn, case, kw):
+        if self.record:
+            out = getattr(self.R, fn)(**kw)
+            n = len(out["log_alpha"] if "log_alpha" in out else out["beta_mat"])
+            rng = np.random.default_rng(int.from_bytes(case.encode(), "little") % 2 ** 63)
+            keep = n if fn == "fitDispGrid" else min(n, REF_ROWS)     # one small vector: kept whole
+            rows = np.sort(rng.choice(n, keep, replace=False))
+            m = np.asarray(kw["ySEXP"]).shape[1]
+            cols = np.sort(rng.choice(m, min(m, REF_COLS), replace=False))
+            for k, v in at(out, {"rows": rows, "cols": cols}).items():
+                self.stored[f"{case}/{k}"] = v
+            self.stored[f"{case}/rows"], self.stored[f"{case}/cols"] = rows.astype(np.int32), cols.astype(np.int32)
+            np.savez_compressed(REFERENCE_GOLDEN, **self.stored)
+        pre = case + "/"
+        got = {k[len(pre):]: v for k, v in self.stored.items() if k.startswith(pre)}
+        assert got, f"no stored reference outputs for case {case!r} (tests/golden/reference/make.py)"
+        return got
+
+    def fitDisp(self, case, **kw):
+        return self._call("fitDisp", case, kw)
+
+    def fitDispGrid(self, case, **kw):
+        return self._call("fitDispGrid", case, kw)
+
+    def fitBeta(self, case, **kw):
+        return self._call("fitBeta", case, kw)
+
+
+def at(res, stored):
+    """The entries of a full fitDisp / fitBeta / fitDispGrid result that a StoredReference case holds."""
+    rows, cols = stored["rows"], stored["cols"]
+    out = {}
+    for k, v in res.items():
+        if k in ("rows", "cols"):
+            continue
+        v = np.asarray(v)
+        out[k] = v[rows][:, cols] if k == "hat_diagonals" else v[rows]
+    return out

@@ -1,6 +1,6 @@
 """The product's CUDA kernels, executed on the CPU by the SIMT emulator (tests/simt_emu/), against the oracle.
 
-tests/simt_emu/build_emu.py compiles deseq2_b200/csrc/*.cu -- the very sources nvcc compiles for sm_100a, with three
+tests/simt_emu/build_emu.py compiles deseq2_b200/csrc/*.cu -- the very sources nvcc compiles for sm_90a, with three
 mechanical rewrites (launch syntax, `extern __shared__`, one PTX statement) -- into libb200nb_emu.so, which exports
 the same C ABI (include/b200nb.h).  This module points the ctypes loader at that library and runs the parity cases of
 tests/test_parity_gpu.py / tests/test_golden.py (the -m gpu tests) at reduced gene counts, with the same acceptance
@@ -45,11 +45,8 @@ import test_parity_gpu as TP
 import test_parity_reference_gpu as TPR      # noqa: E402
 
 def _ref():
-    from oracle import ref as R
-    if not R.available():
-        pytest.skip("oracle/_ref not available")
-    R.build()
-    return R
+    from helpers import StoredReference
+    return StoredReference()
 
 
 CASES = [

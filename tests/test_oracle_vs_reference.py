@@ -1,26 +1,26 @@
-"""The reference pin (VERDICT r01 #2): the CPU oracle (oracle/nbglm_oracle.c, a restatement) against the REFERENCE'S OWN
-translation unit, /root/reference/src/DESeq2.cpp, compiled unchanged into oracle/_ref/libdeseq2_ref.so against stand-in
-Rcpp / Armadillo / Rmath headers (oracle/ref_standin/, oracle/Makefile `ref`).  All three entry points, weights (incl.
+"""The reference pin: the CPU oracle (oracle/nbglm_oracle.c, a restatement) against the REFERENCE'S OWN translation
+unit, src/DESeq2.cpp, compiled unchanged into oracle/_ref/libdeseq2_ref.so against stand-in Rcpp / Armadillo / Rmath
+headers (oracle/ref_standin/, oracle/Makefile `ref`).  The reference's outputs on these inputs are stored at a seeded
+sample of genes in tests/golden/reference/outputs.npz (helpers.StoredReference).  All three entry points, weights (incl.
 Cox-Reid row / column removal), both useQR branches, ridge, normalisation-factor matrices, maxit = 0, INTSXP and REALSXP
-counts, the divergence sentinel of test_optim.R, chunked == whole.
+counts, the divergence sentinel of test_optim.R.
 
 Tolerances: fitBeta / fitDispGrid / the posterior and its derivatives are the same formulas evaluated by two
 implementations of the same fp64 arithmetic (only the p x p linear algebra and the nmath restatement differ), so they
 must agree to 1e-9; fitDisp's control flow (iter, iter_accept) must be IDENTICAL for every gene whose decisions are not
 knife-edge (oracle margin > 64 rounding bounds, see oracle_fit_disp)."""
+import os
+import subprocess
+
 import numpy as np
 import pytest
 
-from helpers import DISP_KEYS, beta_args, disp_args, make_case, rel_err
+from helpers import DISP_KEYS, StoredReference, at, beta_args, disp_args, make_case, rel_err
 
 
 @pytest.fixture(scope="module")
 def ref():
-    from oracle import ref as R
-    if not R.available():
-        pytest.skip("oracle/_ref not built and /root/reference absent")
-    R.build()
-    return R
+    return StoredReference()
 
 
 TIGHT = 1e-9
@@ -70,7 +70,8 @@ def _cmp_beta(o, r, name):
 def test_fit_disp_mle(oracle, ref, n, m, seed):
     c = make_case(n, m, seed=seed)
     a = disp_args(c, c["mu"], np.log(c["alpha0"]))
-    _cmp_disp(oracle.fitDisp(**a, with_margin=True), ref.fitDisp(**a), m=a["ySEXP"].shape[1], name=f"mle {n}x{m}", min_same=0.9)
+    r = ref.fitDisp(f"fit_disp_mle_{n}x{m}_{seed}", **a)
+    _cmp_disp(at(oracle.fitDisp(**a, with_margin=True), r), r, m=a["ySEXP"].shape[1], name=f"mle {n}x{m}", min_same=0.9)
 
 
 def test_fit_disp_map_prior_and_real_counts(oracle, ref):
@@ -79,9 +80,11 @@ def test_fit_disp_map_prior_and_real_counts(oracle, ref):
     fit = 0.1 + 4.0 / c["baseMean"]
     a = disp_args(c, c["mu"], mle["log_alpha"], prior_mean=np.log(fit), sigmasq=0.6, usePrior=True,
                   y=c["counts"].astype(np.float64))           # REALSXP counts (the INTSXP coercion is the default path)
-    _cmp_disp(oracle.fitDisp(**a, with_margin=True), ref.fitDisp(**a), m=a["ySEXP"].shape[1], name="map")
+    r = ref.fitDisp("fit_disp_map_real_counts", **a)
+    _cmp_disp(at(oracle.fitDisp(**a, with_margin=True), r), r, m=a["ySEXP"].shape[1], name="map")
     a = disp_args(c, c["mu"], np.log(c["alpha0"]), useCR=False)
-    _cmp_disp(oracle.fitDisp(**a, with_margin=True), ref.fitDisp(**a), m=a["ySEXP"].shape[1], name="noCR", min_same=0.9)
+    r = ref.fitDisp("fit_disp_no_cr", **a)
+    _cmp_disp(at(oracle.fitDisp(**a, with_margin=True), r), r, m=a["ySEXP"].shape[1], name="noCR", min_same=0.9)
 
 
 def _weights_for(shape, seed, p_small=0.08):
@@ -100,11 +103,13 @@ def test_fit_disp_weights_and_designs(oracle, ref, design, seed):
     c = make_case(300, m, x=x, seed=seed)
     alpha = np.clip(0.1 + 4 / c["baseMean"], 1e-8, m)
     mu = c["mu"] if c["mu"] is not None else np.maximum(
-        c["nf"] * np.exp(ref.fitBeta(**beta_args(c, alpha))["beta_mat"] @ x.T), 0.5)
+        c["nf"] * np.exp(oracle.fitBeta(**beta_args(c, alpha))["beta_mat"] @ x.T), 0.5)
     w = _weights_for(c["counts"].shape, seed)
     a = disp_args(c, mu, np.log(c["alpha0"]), prior_mean=np.log(alpha), sigmasq=0.8, usePrior=True, weights=w,
                   useWeights=True)
-    _cmp_disp(oracle.fitDisp(**a, with_margin=True), ref.fitDisp(**a), m=a["ySEXP"].shape[1], name=f"weights/{design}", min_same=0.9)
+    r = ref.fitDisp(f"fit_disp_weights_{design}", **a)
+    _cmp_disp(at(oracle.fitDisp(**a, with_margin=True), r), r, m=a["ySEXP"].shape[1], name=f"weights/{design}",
+              min_same=0.9)
 
 
 def test_fit_disp_weights_drop_a_design_column(oracle, ref):
@@ -115,7 +120,9 @@ def test_fit_disp_weights_drop_a_design_column(oracle, ref):
     w = np.ones(c["counts"].shape)
     w[:, m // 2:] = 5e-3
     a = disp_args(c, c["mu"], np.log(c["alpha0"]), weights=w, useWeights=True)
-    _cmp_disp(oracle.fitDisp(**a, with_margin=True), ref.fitDisp(**a), m=a["ySEXP"].shape[1], name="dropped column", min_same=0.85)
+    r = ref.fitDisp("fit_disp_weights_dropped_column", **a)
+    _cmp_disp(at(oracle.fitDisp(**a, with_margin=True), r), r, m=a["ySEXP"].shape[1], name="dropped column",
+              min_same=0.85)
 
 
 @pytest.mark.parametrize("usePrior,useWeights", [(True, False), (False, False), (True, True)])
@@ -126,7 +133,8 @@ def test_fit_disp_grid(oracle, ref, usePrior, useWeights):
     kw = dict(ySEXP=c["counts"], xSEXP=c["x"], mu_hatSEXP=c["mu"], disp_gridSEXP=grid,
               log_alpha_prior_meanSEXP=np.log(0.1 + 4 / c["baseMean"]), log_alpha_prior_sigmasqSEXP=0.5,
               usePriorSEXP=usePrior, weightsSEXP=w, useWeightsSEXP=useWeights, weightThresholdSEXP=1e-2, useCRSEXP=True)
-    o, r = oracle.fitDispGrid(**kw)["log_alpha"], ref.fitDispGrid(**kw)["log_alpha"]
+    r = ref.fitDispGrid(f"fit_disp_grid_{usePrior}_{useWeights}", **kw)
+    o, r = at(oracle.fitDispGrid(**kw), r)["log_alpha"], r["log_alpha"]
     assert np.mean(o == r) > 0.99                              # same grid point unless two values tie to rounding
     assert np.max(np.abs(o - r)) < 2.0 * (grid[1] - grid[0]) / 9.5
 
@@ -137,7 +145,8 @@ def test_fit_beta(oracle, ref, n, m, seed, useQR):
     c = make_case(n, m, seed=seed)
     alpha = np.clip(0.1 + 4.0 / c["baseMean"], 1e-8, 10)
     a = beta_args(c, alpha, useQR=useQR)
-    _cmp_beta(oracle.fitBeta(**a), ref.fitBeta(**a), f"beta {n}x{m} qr={useQR}")
+    r = ref.fitBeta(f"fit_beta_{n}x{m}_{seed}_{useQR}", **a)
+    _cmp_beta(at(oracle.fitBeta(**a), r), r, f"beta {n}x{m} qr={useQR}")
 
 
 @pytest.mark.parametrize("design,seed,useQR", [("batch", 61, True), ("factor4", 62, False), ("intercept", 63, True),
@@ -162,15 +171,17 @@ def test_fit_beta_designs_weights_nf_matrix_ridge(oracle, ref, design, seed, use
         lam[-1] = 0.3
     a = beta_args(c, alpha, nf=nf, weights=w, useWeights=True, useQR=useQR, lam=lam, x=x,
                   contrast=np.r_[np.zeros(p - 1), 1.0])
-    _cmp_beta(oracle.fitBeta(**a), ref.fitBeta(**a), f"beta/{design}")
+    r = ref.fitBeta(f"fit_beta_{design}", **a)
+    _cmp_beta(at(oracle.fitBeta(**a), r), r, f"beta/{design}")
 
 
 def test_fit_beta_maxit0_and_divergence_sentinel(oracle, ref):
     c = make_case(200, 24, seed=34)
     alpha = np.clip(0.1 + 4.0 / c["baseMean"], 1e-8, 10)
-    fit = ref.fitBeta(**beta_args(c, alpha))
+    fit = oracle.fitBeta(**beta_args(c, alpha))
     a = beta_args(c, alpha, beta0=fit["beta_mat"], maxit=0, useQR=False, contrast=np.array([0.0, 1.0]))
-    o, r = oracle.fitBeta(**a), ref.fitBeta(**a)
+    r = ref.fitBeta("fit_beta_maxit0", **a)
+    o = at(oracle.fitBeta(**a), r)
     assert np.all(r["iter"] == 0)
     _cmp_beta(o, r, "maxit0")
     # test_optim.R:29-39: the 0/1000 row must report iter == maxit in the reference and in the oracle
@@ -178,30 +189,22 @@ def test_fit_beta_maxit0_and_divergence_sentinel(oracle, ref):
     x = np.c_[np.ones(10), np.r_[np.zeros(5), np.ones(5)]]
     args = (y, x, np.ones((2, 10)), [0.1, 0.1], [1, 0], np.ones((2, 2)), np.full(2, 1e-6) / np.log(2) ** 2, None,
             False, 1e-8, 100, True, 0.5)
-    o, r = oracle.fitBeta(*args), ref.fitBeta(*args)
+    names = ("ySEXP", "xSEXP", "nfSEXP", "alpha_hatSEXP", "contrastSEXP", "beta_matSEXP", "lambdaSEXP", "weightsSEXP",
+             "useWeightsSEXP", "tolSEXP", "maxitSEXP", "useQRSEXP", "minmuSEXP")
+    o, r = oracle.fitBeta(*args), ref.fitBeta("fit_beta_divergence_sentinel", **dict(zip(names, args)))
     assert r["iter"][0] == 100 and r["iter"][1] < 100 and np.array_equal(o["iter"], r["iter"])
 
 
-def test_reference_chunked_equals_whole(ref):
-    """test_parallel.R:12-37 on the reference build itself: BiocParallel-style gene chunks == one call."""
-    c = make_case(300, 12, seed=9)
-    a = disp_args(c, c["mu"], np.log(c["alpha0"]))
-    w, s = ref.fitDisp(**a), ref.fitDisp(**a, nthreads=3)
-    for k in DISP_KEYS + ("iter", "iter_accept"):
-        assert np.array_equal(w[k], s[k], equal_nan=True), k
-    alpha = np.clip(0.1 + 4.0 / c["baseMean"], 1e-8, 10)
-    b = beta_args(c, alpha)
-    w, s = ref.fitBeta(**b), ref.fitBeta(**b, nthreads=4)
-    for k in w:
-        assert np.array_equal(w[k], s[k], equal_nan=True), k
-
-
-def test_standin_nmath_against_mpmath(oracle, ref):
+def test_standin_nmath_against_mpmath(oracle, tmp_path):
     """The nmath stand-in behind the reference build (oracle/ref_standin/rmath_standin.c) at 40 digits."""
     import ctypes as C
 
     import mpmath as mp
-    L = ref.lib()
+    src = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "ref_standin",
+                       "rmath_standin.c")
+    so = str(tmp_path / "librmath_standin.so")
+    subprocess.check_call(["gcc", "-O2", "-fPIC", "-ffp-contract=off", "-shared", "-o", so, src, "-lm"])
+    L = C.CDLL(so)
     for f in ("Rf_lgammafn", "Rf_digamma", "Rf_trigamma"):
         getattr(L, f).restype = C.c_double
         getattr(L, f).argtypes = [C.c_double]
