@@ -238,4 +238,10 @@ cudaError_t launch_special_test(const double* x, int n, double* lg, double* dg, 
 
 int device_sm_count();
 
+// Grid of a persistent-queue kernel: one resident wave (SMs x the CTAs per SM the occupancy calculator allows for
+// `threads` and `smem` bytes of dynamic shared memory), and no more CTAs than ceil(n / genes_per_cta) can keep busy;
+// at least 1.  Raises the kernel's dynamic shared-memory limit to `smem` first.  The occupancy answer is cached per
+// (kernel address, threads, smem).
+cudaError_t persistent_grid(const void* kernel, int threads, size_t smem, int genes_per_cta, int n, unsigned* grid);
+
 }  // namespace nb

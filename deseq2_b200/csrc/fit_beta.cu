@@ -3,7 +3,8 @@
 // Behavioural contract (WHAT): /root/reference/src/DESeq2.cpp:283-465 (fitBeta): mu = max(nf*exp(X b), minmu),
 // w = [wt*]mu/(1+alpha*mu), z = log(mu/nf) + (y-mu)/mu, b = argmin ridge WLS, |b|>30 => iter=maxit (diverged b
 // kept), deviance = -2 sum [wt*] log NB(y; mu, 1/alpha), stop when t>0 and |dev-dev_old|/(|dev|+0.1) < tol, NaN =>
-// iter=maxit; post-loop hat diagonal, sandwich covariance, contrast numerator/denominator (:429-455).
+// iter=maxit (the stop and divergence rules are deseq_rules.cuh's); post-loop hat diagonal, sandwich covariance,
+// contrast numerator/denominator (:429-455).
 // HOW is new:
 //   * one fused pass per iteration updates mu, the deviance, AND accumulates X'WX / X'Wz for the next solve,
 //     so a gene costs (iterations + 1) passes over its row (held in shared memory) and one warp all-reduce
@@ -16,6 +17,7 @@
 //     y (log mu + log alpha) - (y + r) log1p(mu alpha), r = 1/alpha: one exp and one log1p per sample per
 //     iteration, accurate for every alpha in [1e-8, m];
 //   * log(mu/nf) is never formed: mu = exp(eta + log nf) so log(mu/nf) = eta unless the minmu clamp bites.
+#include "deseq_rules.cuh"
 #include "engine.h"
 #include "smallp.cuh"
 
@@ -119,17 +121,142 @@ __device__ __forceinline__ void beta_pass(const BetaRow& rv, const double (&beta
   } else if constexpr (NA <= GL) {
     group_allreduce_sum_rs<NA, GL>(acc, lane);
   } else {
-#pragma unroll
-    for (int o = GL / 2; o > 0; o >>= 1) {
-#pragma unroll
-      for (int i = 0; i < NA; i++) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], o);
-    }
+    group_allreduce_sum_n<NA, GL>(acc);
   }
   dev_var = acc[0];
 #pragma unroll
   for (int i = 0; i < NS; i++) XtWX.v[i] = acc[1 + i];
 #pragma unroll
   for (int a = 0; a < P; a++) XtWz[a] = acc[1 + NS + a];
+}
+
+// stage the row of gene g (128-bit loads) into the group's shared-memory rows: y, log nf (nf matrix only), w (USE_W);
+// lg = lane inside the group of GL lanes.  `valid` false: the group has no gene this round and nothing is loaded.
+template <bool USE_W, int GL>
+__device__ __forceinline__ void stage_beta_row(const BetaArgs& A, size_t off, bool valid, int mpad, int lg, double* ys,
+                                               double* lnfs, double* wsm) {
+  if (valid) {
+    for (int j4 = lg * 4; j4 < mpad; j4 += 4 * GL) {
+      double yv[4];
+      if (A.y_is_f64) {
+        const double2* p2 = reinterpret_cast<const double2*>(static_cast<const double*>(A.y) + off + j4);
+        const double2 a0 = __ldg(p2), a1 = __ldg(p2 + 1);
+        yv[0] = a0.x; yv[1] = a0.y; yv[2] = a1.x; yv[3] = a1.y;
+      } else {
+        const int4 v = __ldg(reinterpret_cast<const int4*>(static_cast<const int32_t*>(A.y) + off + j4));
+        yv[0] = v.x; yv[1] = v.y; yv[2] = v.z; yv[3] = v.w;
+      }
+#pragma unroll
+      for (int q = 0; q < 4; q++) ys[j4 + q] = yv[q];
+      if (!A.nf_is_vector) {
+        const double2* n2 = reinterpret_cast<const double2*>(A.nf + off + j4);
+        const double2 n0 = __ldg(n2), n1 = __ldg(n2 + 1);
+        lnfs[j4 + 0] = log(n0.x); lnfs[j4 + 1] = log(n0.y); lnfs[j4 + 2] = log(n1.x); lnfs[j4 + 3] = log(n1.y);
+      }
+      if (USE_W) {
+        const double2* w2 = reinterpret_cast<const double2*>(A.w + off + j4);
+        const double2 w0 = __ldg(w2), w1 = __ldg(w2 + 1);
+        wsm[j4 + 0] = w0.x; wsm[j4 + 1] = w0.y; wsm[j4 + 2] = w1.x; wsm[j4 + 3] = w1.y;
+      }
+    }
+  }
+  __syncwarp();
+}
+
+// mu-independent part of the deviance: sum_j [w_j] (lgamma(y_j + r) - lgamma(r) - lgamma(y_j + 1)), 0 when maxit = 0
+template <bool USE_W, int GL>
+__device__ __forceinline__ double deviance_const(const BetaArgs& A, const BetaRow& rv, double r, int lg) {
+  if (A.maxit <= 0) return 0.0;
+  const double lg_r = lgamma_pos(r);
+  double c = 0.0;
+  for (int j = lg; j < A.m; j += GL) {
+    const double y = rv.y[j];
+    double t = lgamma_diff(y, r, lg_r) - log_factorial(y);
+    if (USE_W) t *= rv.w[j];
+    c += t;
+  }
+  return group_allreduce_sum<GL>(c);
+}
+
+// post-loop block (src/DESeq2.cpp:429-455): hat diagonal, sandwich variance, contrast and the stores of gene g.  XtWX
+// belongs to the mu currently in shared memory.  Every lane of the group computes; `valid` false stores nothing.
+template <int P, bool USE_W, int GL>
+__device__ __forceinline__ void beta_finish(const BetaArgs& A, unsigned int g, bool valid, int lg, const BetaRow& rv,
+                                            const SymP<P>& XtWX, const double (&lam)[P], const double (&contrast)[P],
+                                            const double (&beta)[P], double alpha, const IrlsProgress& ir) {
+  const size_t off = (size_t)g * A.ld;
+  SymP<P> M = XtWX, Ainv;
+  double s[P];
+#pragma unroll
+  for (int k = 0; k < P; k++) M.at(k, k) += lam[k];
+#pragma unroll
+  for (int k = 0; k < P; k++) s[k] = rsqrt(M.get(k, k));
+#pragma unroll
+  for (int a = 0; a < P; a++)
+#pragma unroll
+    for (int b = 0; b <= a; b++) M.at(a, b) *= s[a] * s[b];
+  chol_factor<P>(M);
+  chol_inverse<P>(M, Ainv);
+#pragma unroll
+  for (int a = 0; a < P; a++)
+#pragma unroll
+    for (int b = 0; b <= a; b++) Ainv.at(a, b) *= s[a] * s[b];
+
+  __syncwarp();
+  if (valid && (A.hat_diag != nullptr || A.mu_out != nullptr)) {
+    for (int j = lg; j < A.m; j += GL) {
+      const double mu = rv.mu[j];
+      if (A.mu_out != nullptr) A.mu_out[off + j] = mu;
+      if (A.hat_diag != nullptr) {
+        double w = mu * rcp_fast(fma(alpha, mu, 1.0));
+        if (USE_W) w *= rv.w[j];
+        double xv[P];
+#pragma unroll
+        for (int k = 0; k < P; k++) xv[k] = rv.x[k * rv.mpad + j];
+        double q = 0.0;
+#pragma unroll
+        for (int a = 0; a < P; a++) {
+          q = fma(xv[a] * xv[a], Ainv.get(a, a), q);
+#pragma unroll
+          for (int b = 0; b < a; b++) q = fma(2.0 * xv[a] * xv[b], Ainv.get(a, b), q);
+        }
+        A.hat_diag[off + j] = w * q;
+      }
+    }
+  }
+  // sigma = Ainv * XtWX * Ainv
+  double T[P][P];
+  sym_mul_full<P>(Ainv, XtWX, T);
+  double cn = 0.0, cd = 0.0;
+  double var[P];
+  double sc_[P];   // sigma * contrast
+#pragma unroll
+  for (int a = 0; a < P; a++) sc_[a] = 0.0;
+#pragma unroll
+  for (int a = 0; a < P; a++) {
+#pragma unroll
+    for (int b = 0; b < P; b++) {
+      double sab = 0.0;
+#pragma unroll
+      for (int k = 0; k < P; k++) sab = fma(T[a][k], Ainv.get(k, b), sab);
+      if (a == b) var[a] = sab;
+      sc_[a] = fma(sab, contrast[b], sc_[a]);
+    }
+    cn = fma(contrast[a], beta[a], cn);
+  }
+#pragma unroll
+  for (int a = 0; a < P; a++) cd = fma(contrast[a], sc_[a], cd);
+  if (valid && lg == 0) {
+#pragma unroll
+    for (int k = 0; k < P; k++) {
+      A.beta_out[(size_t)g + (size_t)A.n * k] = beta[k];
+      A.beta_var[(size_t)g + (size_t)A.n * k] = var[k];
+    }
+    A.iter[g] = ir.it;
+    A.contrast_num[g] = cn;
+    A.contrast_denom[g] = sqrt(cd);
+    A.deviance[g] = ir.dev;
+  }
 }
 
 #ifndef NB_LB_THREADS
@@ -169,40 +296,13 @@ __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_beta_kernel(con
     contrast[k] = A.contrast[k];
   }
   const double minmu = A.minmu, log_minmu = log(A.minmu);
-  const double large = 30.0;
 
   for (;;) {
     unsigned int g = 0;
     if (lane == 0) g = atomicAdd(A.counter, 1u);
     g = __shfl_sync(0xffffffffu, g, 0);
     if (g >= (unsigned int)A.n) break;
-    const size_t off = (size_t)g * A.ld;
-
-    // ---- stage the row (128-bit loads)
-    for (int j4 = lane * 4; j4 < mpad; j4 += 128) {
-      double yv[4];
-      if (A.y_is_f64) {
-        const double2* p2 = reinterpret_cast<const double2*>(static_cast<const double*>(A.y) + off + j4);
-        const double2 a0 = __ldg(p2), a1 = __ldg(p2 + 1);
-        yv[0] = a0.x; yv[1] = a0.y; yv[2] = a1.x; yv[3] = a1.y;
-      } else {
-        const int4 v = __ldg(reinterpret_cast<const int4*>(static_cast<const int32_t*>(A.y) + off + j4));
-        yv[0] = v.x; yv[1] = v.y; yv[2] = v.z; yv[3] = v.w;
-      }
-#pragma unroll
-      for (int q = 0; q < 4; q++) ys[j4 + q] = yv[q];
-      if (!A.nf_is_vector) {
-        const double2* n2 = reinterpret_cast<const double2*>(A.nf + off + j4);
-        const double2 n0 = __ldg(n2), n1 = __ldg(n2 + 1);
-        lnfs[j4 + 0] = log(n0.x); lnfs[j4 + 1] = log(n0.y); lnfs[j4 + 2] = log(n1.x); lnfs[j4 + 3] = log(n1.y);
-      }
-      if (USE_W) {
-        const double2* w2 = reinterpret_cast<const double2*>(A.w + off + j4);
-        const double2 w0 = __ldg(w2), w1 = __ldg(w2 + 1);
-        wsm[j4 + 0] = w0.x; wsm[j4 + 1] = w0.y; wsm[j4 + 2] = w1.x; wsm[j4 + 3] = w1.y;
-      }
-    }
-    __syncwarp();
+    stage_beta_row<USE_W, 32>(A, (size_t)g * A.ld, true, mpad, lane, ys, lnfs, wsm);
 
     double beta[P];
 #pragma unroll
@@ -210,30 +310,16 @@ __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_beta_kernel(con
     const double alpha = A.alpha_hat[g];
     const double r = 1.0 / alpha;
     const double log_alpha = log(alpha);
-
-    // mu-independent part of the deviance
-    double devc = 0.0;
-    if (A.maxit > 0) {
-      const double lg_r = lgamma_pos(r);
-      double c = 0.0;
-      for (int j = lane; j < A.m; j += 32) {
-        const double y = ys[j];
-        double t = lgamma_diff(y, r, lg_r) - log_factorial(y);
-        if (USE_W) t *= wsm[j];
-        c += t;
-      }
-      devc = warp_allreduce_sum(c);
-    }
+    const double devc = deviance_const<USE_W, 32>(A, rv, r, lane);
 
     SymP<P> XtWX;
     double XtWz[P];
     double dv;
-    double dev = 0.0, dev_old = 0.0;
-    double it = 0.0;
+    IrlsProgress ir;
     // t = -1: the pass at the starting values (mu, weights for the first solve); t >= 0: IRLS iterations
     for (int t = -1; t < A.maxit; t++) {
       if (t >= 0) {
-        it += 1.0;
+        ir.start_iteration();
         SymP<P> M = XtWX;
 #pragma unroll
         for (int k = 0; k < P; k++) {
@@ -243,91 +329,13 @@ __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_beta_kernel(con
         spd_solve_equilibrated<P>(M, beta);
         bool big = false;
 #pragma unroll
-        for (int k = 0; k < P; k++) big = big || (fabs(beta[k]) > large);
-        if (big) { it = (double)A.maxit; break; }
+        for (int k = 0; k < P; k++) big = big || (fabs(beta[k]) > kBetaLarge);
+        if (big) { ir.diverged(A.maxit); break; }
       }
       beta_pass<P, USE_W>(rv, beta, alpha, r, log_alpha, minmu, log_minmu, lane, dv, XtWX, XtWz);
-      if (t < 0) continue;
-      dev = -2.0 * (dv + devc);
-      const double conv_test = fabs(dev - dev_old) / (fabs(dev) + 0.1);
-      if (isnan(conv_test)) { it = (double)A.maxit; break; }
-      if ((t > 0) && (conv_test < A.tol)) break;
-      dev_old = dev;
+      if (t >= 0 && ir.stop_after_pass(dv, devc, A)) break;
     }
-
-    // ---- post-loop block (src/DESeq2.cpp:429-455); XtWX belongs to the mu currently in shared memory
-    SymP<P> M = XtWX, Ainv;
-    double s[P];
-#pragma unroll
-    for (int k = 0; k < P; k++) M.at(k, k) += lam[k];
-#pragma unroll
-    for (int k = 0; k < P; k++) s[k] = rsqrt(M.get(k, k));
-#pragma unroll
-    for (int a = 0; a < P; a++)
-#pragma unroll
-      for (int b = 0; b <= a; b++) M.at(a, b) *= s[a] * s[b];
-    chol_factor<P>(M);
-    chol_inverse<P>(M, Ainv);
-#pragma unroll
-    for (int a = 0; a < P; a++)
-#pragma unroll
-      for (int b = 0; b <= a; b++) Ainv.at(a, b) *= s[a] * s[b];
-
-    __syncwarp();
-    if (A.hat_diag != nullptr || A.mu_out != nullptr) {
-      for (int j = lane; j < A.m; j += 32) {
-        const double mu = mus[j];
-        if (A.mu_out != nullptr) A.mu_out[off + j] = mu;
-        if (A.hat_diag != nullptr) {
-          double w = mu * rcp_fast(fma(alpha, mu, 1.0));
-          if (USE_W) w *= wsm[j];
-          double xv[P];
-#pragma unroll
-          for (int k = 0; k < P; k++) xv[k] = xs[k * mpad + j];
-          double q = 0.0;
-#pragma unroll
-          for (int a = 0; a < P; a++) {
-            q = fma(xv[a] * xv[a], Ainv.get(a, a), q);
-#pragma unroll
-            for (int b = 0; b < a; b++) q = fma(2.0 * xv[a] * xv[b], Ainv.get(a, b), q);
-          }
-          A.hat_diag[off + j] = w * q;
-        }
-      }
-    }
-    // sigma = Ainv * XtWX * Ainv
-    double T[P][P];
-    sym_mul_full<P>(Ainv, XtWX, T);
-    double cn = 0.0, cd = 0.0;
-    double var[P];
-    double sc_[P];   // sigma * contrast
-#pragma unroll
-    for (int a = 0; a < P; a++) sc_[a] = 0.0;
-#pragma unroll
-    for (int a = 0; a < P; a++) {
-#pragma unroll
-      for (int b = 0; b < P; b++) {
-        double sab = 0.0;
-#pragma unroll
-        for (int k = 0; k < P; k++) sab = fma(T[a][k], Ainv.get(k, b), sab);
-        if (a == b) var[a] = sab;
-        sc_[a] = fma(sab, contrast[b], sc_[a]);
-      }
-      cn = fma(contrast[a], beta[a], cn);
-    }
-#pragma unroll
-    for (int a = 0; a < P; a++) cd = fma(contrast[a], sc_[a], cd);
-    if (lane == 0) {
-#pragma unroll
-      for (int k = 0; k < P; k++) {
-        A.beta_out[(size_t)g + (size_t)A.n * k] = beta[k];
-        A.beta_var[(size_t)g + (size_t)A.n * k] = var[k];
-      }
-      A.iter[g] = it;
-      A.contrast_num[g] = cn;
-      A.contrast_denom[g] = sqrt(cd);
-      A.deviance[g] = dev;
-    }
+    beta_finish<P, USE_W, 32>(A, g, true, lane, rv, XtWX, lam, contrast, beta, alpha, ir);
     __syncwarp();
   }
 }
@@ -335,28 +343,17 @@ __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_beta_kernel(con
 #include "fit_beta_grp.cuh"
 
 template <int P, bool USE_W, int GL>
-cudaError_t launch_beta_grp(const BetaArgs& a, int mpad, size_t fixed, size_t rowbytes, int sms, cudaStream_t stream,
+cudaError_t launch_beta_grp(const BetaArgs& a, int mpad, size_t fixed, size_t rowbytes, cudaStream_t stream,
                             bool& launched) {
   constexpr int NG = 32 / GL, GW = GrpShape<GL>::threads / 32;
   const size_t gsmem = fixed + (size_t)GW * NG * rowbytes;
   launched = false;
   if (gsmem > (size_t)227 * 1024 / GrpShape<GL>::ctas) return cudaSuccess;
   auto kg = fit_beta_grp_kernel<P, USE_W, GL>;
-  static size_t g_smem = 0;
-  static int g_ctas = 0;
-  cudaError_t e = cudaSuccess;
-  if (g_smem != gsmem || g_ctas < 1) {
-    e = cudaFuncSetAttribute(kg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsmem);
-    if (e != cudaSuccess) return e;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&g_ctas, kg, GrpShape<GL>::threads, gsmem);
-    if (e != cudaSuccess) return e;
-    if (g_ctas < 1) return cudaErrorLaunchOutOfResources;
-    g_smem = gsmem;
-  }
-  long long gg = (long long)sms * g_ctas;
-  const long long gwant = ((long long)a.n + GW * NG - 1) / (GW * NG);
-  if (gg > gwant) gg = gwant;
-  kg<<<(unsigned)(gg < 1 ? 1 : gg), GrpShape<GL>::threads, gsmem, stream>>>(a, mpad);
+  unsigned grid = 0;
+  const cudaError_t e = persistent_grid(reinterpret_cast<const void*>(kg), GrpShape<GL>::threads, gsmem, GW * NG, a.n, &grid);
+  if (e != cudaSuccess) return e;
+  kg<<<grid, GrpShape<GL>::threads, gsmem, stream>>>(a, mpad);
   launched = true;
   return cudaGetLastError();
 }
@@ -373,37 +370,19 @@ cudaError_t launch_beta_t(const BetaArgs& a, cudaStream_t stream) {
   if (fixed + warps * rowbytes > smem_cap) return cudaErrorInvalidValue;
   const size_t smem = fixed + warps * rowbytes;
   auto kern = fit_beta_kernel<P, USE_W>;
-  // the attribute / occupancy queries are made once per (kernel, shared-memory size) and cached
-  static size_t cached_smem[2] = {0, 0};
-  static int cached_ctas[2] = {0, 0};
-  const int slot = 0;
-  cudaError_t e = cudaSuccess;
-  if (cached_smem[slot] != smem || cached_ctas[slot] < 1) {
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    int c = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kern, warps * 32, smem);
-    if (e != cudaSuccess) return e;
-    if (c < 1) return cudaErrorLaunchOutOfResources;
-    cached_smem[slot] = smem;
-    cached_ctas[slot] = c;
-  }
-  const int ctas_per_sm = cached_ctas[slot];
-  const int sms = device_sm_count();
-  long long want = ((long long)a.n + warps - 1) / warps;
-  long long grid = (long long)sms * ctas_per_sm;
-  if (grid > want) grid = want;
-  if (grid < 1) grid = 1;
-  e = cudaMemsetAsync(a.counter, 0, sizeof(unsigned int), stream);
+  cudaError_t e = cudaMemsetAsync(a.counter, 0, sizeof(unsigned int), stream);
   if (e != cudaSuccess) return e;
   {
     const int gl = group_lanes_beta(a.m);
     bool launched = false;
-    if (gl == 8) e = launch_beta_grp<P, USE_W, 8>(a, mpad, fixed, rowbytes, sms, stream, launched);
-    else if (gl == 16) e = launch_beta_grp<P, USE_W, 16>(a, mpad, fixed, rowbytes, sms, stream, launched);
+    if (gl == 8) e = launch_beta_grp<P, USE_W, 8>(a, mpad, fixed, rowbytes, stream, launched);
+    else if (gl == 16) e = launch_beta_grp<P, USE_W, 16>(a, mpad, fixed, rowbytes, stream, launched);
     if (e != cudaSuccess || launched) return e;
   }
-  kern<<<(unsigned)grid, warps * 32, smem, stream>>>(a, warps, mpad);
+  unsigned grid = 0;
+  e = persistent_grid(reinterpret_cast<const void*>(kern), warps * 32, smem, warps, a.n, &grid);
+  if (e != cudaSuccess) return e;
+  kern<<<grid, warps * 32, smem, stream>>>(a, warps, mpad);
   return cudaGetLastError();
 }
 

@@ -6,7 +6,7 @@
 // groups run IRLS passes together, a group whose gene has converged / diverged (or that got no gene) keeps executing the
 // pass at the coefficients of its last valid pass -- an idempotent recomputation, shared memory and X'WX end up with
 // the same values -- until the slowest group of the warp is done.  Arithmetic per gene: the product kernel's
-// (beta_pass with GL lanes); decisions: the reference's (src/DESeq2.cpp:334-383 / :388-425, post-loop :429-455).
+// (stage_beta_row, beta_pass, beta_finish with GL lanes); decisions: deseq_rules.cuh::IrlsProgress.
 #pragma once
 
 // CTA shape per group width: 16 lanes (2 genes per warp): 256 threads, 2 CTAs per SM; 8 lanes (4 genes per warp): 128
@@ -84,7 +84,6 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
     contrast[k] = A.contrast[k];
   }
   const double minmu = A.minmu, log_minmu = log(A.minmu);
-  const double large = 30.0;
 
   for (;;) {
     unsigned int g = 0;
@@ -93,35 +92,7 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
     const bool valid = g < (unsigned int)A.n;
     if (!__any_sync(0xffffffffu, valid)) break;
     if (!valid) g = 0;
-    const size_t off = (size_t)g * A.ld;
-
-    // ---- stage the row (128-bit loads), GL lanes
-    if (valid) {
-      for (int j4 = lg * 4; j4 < mpad; j4 += 4 * GL) {
-        double yv[4];
-        if (A.y_is_f64) {
-          const double2* p2 = reinterpret_cast<const double2*>(static_cast<const double*>(A.y) + off + j4);
-          const double2 a0 = __ldg(p2), a1 = __ldg(p2 + 1);
-          yv[0] = a0.x; yv[1] = a0.y; yv[2] = a1.x; yv[3] = a1.y;
-        } else {
-          const int4 v = __ldg(reinterpret_cast<const int4*>(static_cast<const int32_t*>(A.y) + off + j4));
-          yv[0] = v.x; yv[1] = v.y; yv[2] = v.z; yv[3] = v.w;
-        }
-#pragma unroll
-        for (int q = 0; q < 4; q++) ys[j4 + q] = yv[q];
-        if (!A.nf_is_vector) {
-          const double2* n2 = reinterpret_cast<const double2*>(A.nf + off + j4);
-          const double2 n0 = __ldg(n2), n1 = __ldg(n2 + 1);
-          lnfs[j4 + 0] = log(n0.x); lnfs[j4 + 1] = log(n0.y); lnfs[j4 + 2] = log(n1.x); lnfs[j4 + 3] = log(n1.y);
-        }
-        if (USE_W) {
-          const double2* w2 = reinterpret_cast<const double2*>(A.w + off + j4);
-          const double2 w0 = __ldg(w2), w1 = __ldg(w2 + 1);
-          wsm[j4 + 0] = w0.x; wsm[j4 + 1] = w0.y; wsm[j4 + 2] = w1.x; wsm[j4 + 3] = w1.y;
-        }
-      }
-    }
-    __syncwarp();
+    stage_beta_row<USE_W, GL>(A, (size_t)g * A.ld, valid, mpad, lg, ys, lnfs, wsm);
 
     double beta[P], beta_eval[P];
 #pragma unroll
@@ -130,21 +101,7 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
     const double r = 1.0 / alpha;
     const double log_alpha = log(alpha);
 
-    // mu-independent part of the deviance
-    double devc = 0.0;
-    if (A.maxit > 0) {
-      const double lg_r = lgamma_pos(r);
-      double c = 0.0;
-      for (int j = lg; j < A.m; j += GL) {
-        const double y = ys[j];
-        double t = lgamma_diff(y, r, lg_r) - log_factorial(y);
-        if (USE_W) t *= wsm[j];
-        c += t;
-      }
-#pragma unroll
-      for (int o = GL / 2; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-      devc = c;
-    }
+    const double devc = deviance_const<USE_W, GL>(A, rv, r, lg);
 
     SymP<P> XtWX;
     double XtWz[P];
@@ -152,13 +109,12 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
     for (int i = 0; i < SymP<P>::N; i++) XtWX.v[i] = 0.0;
 #pragma unroll
     for (int k = 0; k < P; k++) XtWz[k] = 0.0;
-    double dev = 0.0, dev_old = 0.0;
-    double it = 0.0;
+    IrlsProgress ir;
     bool first = true;       // the pass at the starting values is still to come
     bool active = valid;
     while (__any_sync(0xffffffffu, active)) {
       if (active && !first) {
-        it += 1.0;
+        ir.start_iteration();
         SymP<P> M = XtWX;
 #pragma unroll
         for (int k = 0; k < P; k++) {
@@ -168,9 +124,9 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
         spd_solve_equilibrated<P>(M, beta);
         bool big = false;
 #pragma unroll
-        for (int k = 0; k < P; k++) big = big || (fabs(beta[k]) > large);
-        if (big) {             // diverged: keep the diverged beta, do not re-evaluate (src/DESeq2.cpp:357-360)
-          it = (double)A.maxit;
+        for (int k = 0; k < P; k++) big = big || (fabs(beta[k]) > kBetaLarge);
+        if (big) {             // diverged: keep the diverged beta, do not re-evaluate
+          ir.diverged(A.maxit);
           active = false;
         }
       }
@@ -189,97 +145,13 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
           XtWz[k] = XtWz_new[k];
           beta_eval[k] = beta[k];
         }
-        if (first) {
-          first = false;
-        } else {
-          dev = -2.0 * (dv + devc);
-          const double conv_test = fabs(dev - dev_old) / (fabs(dev) + 0.1);
-          if (isnan(conv_test)) {
-            it = (double)A.maxit;
-            active = false;
-          } else if ((it > 1.0) && (conv_test < A.tol)) {
-            active = false;
-          } else {
-            dev_old = dev;
-          }
-        }
-        if (it >= (double)A.maxit) active = false;
+        if (first) first = false;
+        else if (ir.stop_after_pass(dv, devc, A)) active = false;
+        if (ir.it >= (double)A.maxit) active = false;   // the reference's `for (t = 0; t < maxit; t++)`
       }
     }
 
-    // ---- post-loop block (src/DESeq2.cpp:429-455); XtWX belongs to the mu currently in shared memory
-    SymP<P> M = XtWX, Ainv;
-    double s[P];
-#pragma unroll
-    for (int k = 0; k < P; k++) M.at(k, k) += lam[k];
-#pragma unroll
-    for (int k = 0; k < P; k++) s[k] = rsqrt(M.get(k, k));
-#pragma unroll
-    for (int a = 0; a < P; a++)
-#pragma unroll
-      for (int b = 0; b <= a; b++) M.at(a, b) *= s[a] * s[b];
-    chol_factor<P>(M);
-    chol_inverse<P>(M, Ainv);
-#pragma unroll
-    for (int a = 0; a < P; a++)
-#pragma unroll
-      for (int b = 0; b <= a; b++) Ainv.at(a, b) *= s[a] * s[b];
-
-    __syncwarp();
-    if (valid && (A.hat_diag != nullptr || A.mu_out != nullptr)) {
-      for (int j = lg; j < A.m; j += GL) {
-        const double mu = mus[j];
-        if (A.mu_out != nullptr) A.mu_out[off + j] = mu;
-        if (A.hat_diag != nullptr) {
-          double w = mu * rcp_fast(fma(alpha, mu, 1.0));
-          if (USE_W) w *= wsm[j];
-          double xv[P];
-#pragma unroll
-          for (int k = 0; k < P; k++) xv[k] = xs[k * mpad + j];
-          double q = 0.0;
-#pragma unroll
-          for (int a = 0; a < P; a++) {
-            q = fma(xv[a] * xv[a], Ainv.get(a, a), q);
-#pragma unroll
-            for (int b = 0; b < a; b++) q = fma(2.0 * xv[a] * xv[b], Ainv.get(a, b), q);
-          }
-          A.hat_diag[off + j] = w * q;
-        }
-      }
-    }
-    // sigma = Ainv * XtWX * Ainv
-    double T[P][P];
-    sym_mul_full<P>(Ainv, XtWX, T);
-    double cn = 0.0, cd = 0.0;
-    double var[P];
-    double sc_[P];   // sigma * contrast
-#pragma unroll
-    for (int a = 0; a < P; a++) sc_[a] = 0.0;
-#pragma unroll
-    for (int a = 0; a < P; a++) {
-#pragma unroll
-      for (int b = 0; b < P; b++) {
-        double sab = 0.0;
-#pragma unroll
-        for (int k = 0; k < P; k++) sab = fma(T[a][k], Ainv.get(k, b), sab);
-        if (a == b) var[a] = sab;
-        sc_[a] = fma(sab, contrast[b], sc_[a]);
-      }
-      cn = fma(contrast[a], beta[a], cn);
-    }
-#pragma unroll
-    for (int a = 0; a < P; a++) cd = fma(contrast[a], sc_[a], cd);
-    if (valid && lg == 0) {
-#pragma unroll
-      for (int k = 0; k < P; k++) {
-        A.beta_out[(size_t)g + (size_t)A.n * k] = beta[k];
-        A.beta_var[(size_t)g + (size_t)A.n * k] = var[k];
-      }
-      A.iter[g] = it;
-      A.contrast_num[g] = cn;
-      A.contrast_denom[g] = sqrt(cd);
-      A.deviance[g] = dev;
-    }
+    beta_finish<P, USE_W, GL>(A, g, valid, lg, rv, XtWX, lam, contrast, beta, alpha, ir);
     __syncwarp();
   }
 }

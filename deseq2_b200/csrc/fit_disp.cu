@@ -3,7 +3,7 @@
 // Behavioural contract (WHAT): /root/reference/src/DESeq2.cpp:164-277 (fitDisp: Armijo back-tracking
 // ascent on log alpha, accept / reject / kappa schedule replicated decision for decision), :31-158
 // (log posterior and its first two derivatives, Cox-Reid term with weight-threshold row/column
-// subsetting) and :469-513 (fitDispGrid).  HOW is new:
+// subsetting) and :469-513 (fitDispGrid).  The line-search and grid decisions are deseq_rules.cuh's.  HOW is new:
 //   * the gene's row (counts, mu, weights) is staged once into shared memory with 128-bit loads;
 //     every lane owns samples lane, lane+32, ...; all per-gene scalars are warp-uniform;
 //   * one fused pass per proposal evaluates the log posterior AND its derivative (they share
@@ -24,6 +24,7 @@
 //   * X'WX, X'dWX are accumulated per lane and combined with xor-butterfly shuffles (bitwise identical in
 //     every lane, so control flow stays warp-uniform); the p x p Cholesky runs in registers;
 //   * genes are pulled from an atomic work queue by persistent warps (trip counts vary 1..maxit).
+#include "deseq_rules.cuh"
 #include "engine.h"
 #include "smallp.cuh"
 
@@ -53,15 +54,6 @@ constexpr int pow2_ceil(int n) { int p = 1; while (p < n) p <<= 1; return p; }
 // One fused pass: lp (and dlp when WANT_D) at log-alpha `a`.
 // GL = lanes per gene: 32 (one warp per gene) or 16 / 8 (two / four genes per warp, fit_disp_grp.cuh) with
 // `lane` the lane index inside the group; reductions then stay inside the group.
-template <int N, int GL>
-__device__ __forceinline__ void group_allreduce_sum_n(double (&v)[N]) {
-#pragma unroll
-  for (int o = GL / 2; o > 0; o >>= 1) {
-#pragma unroll
-    for (int i = 0; i < N; i++) v[i] += __shfl_xor_sync(0xffffffffu, v[i], o);
-  }
-}
-
 template <int P, bool USE_W, bool WANT_D, int MODE, int GL = 32>
 __device__ __forceinline__ void disp_eval_mode(const DispRow& rv, const DispScal& sc, double a, double pm,
                                                double sum_wy, int lane, double& lp, double& dlp) {
@@ -238,8 +230,7 @@ __device__ __forceinline__ double disp_d2(const DispRow& rv, const DispScal& sc,
         }
     }
   }
-  if (GL == 32) warp_allreduce_sum_n(acc);
-  else group_allreduce_sum_n<2 + 3 * NS, GL>(acc);
+  group_allreduce_sum_n<2 + 3 * NS, GL>(acc);
   double cr2 = 0.0, dcr = 0.0;
   if (sc.use_cr) {
     SymP<P> B, dB, d2B, Bi;
@@ -345,144 +336,108 @@ struct DispWarpSmem {
   double *ys, *mus, *wsm, *tab;
 };
 
-// stage one gene row into the warp's shared-memory slice (128-bit loads); returns sum_j w_j y_j and max y
-template <bool USE_W>
-__device__ __forceinline__ void stage_row(const DispArgs& A, unsigned int g, int mpad, int lane, const DispWarpSmem& S,
-                                          double& sum_wy, double& ymax) {
+// stage the row of gene g into the group's shared-memory slice (128-bit loads); lg = lane inside the group of GL lanes.
+// Returns sum_j w_j y_j and max y.  `valid` false: the group has no gene this round -- nothing is loaded (the slice
+// keeps the previous gene, which is fine to evaluate).
+template <bool USE_W, int GL>
+__device__ __forceinline__ void stage_row(const DispArgs& A, unsigned int g, bool valid, int mpad, int lg,
+                                          const DispWarpSmem& S, double& sum_wy, double& ymax) {
   double sum_wy_l = 0.0, ymax_l = 0.0;
   const size_t off = (size_t)g * A.ld;
-  for (int j4 = lane * 4; j4 < mpad; j4 += 128) {
-    double yv[4];
-    if (A.y_is_f64) {
-      const double2* p2 = reinterpret_cast<const double2*>(static_cast<const double*>(A.y) + off + j4);
-      const double2 a0 = __ldg(p2), a1 = __ldg(p2 + 1);
-      yv[0] = a0.x; yv[1] = a0.y; yv[2] = a1.x; yv[3] = a1.y;
-    } else {
-      const int4 v = __ldg(reinterpret_cast<const int4*>(static_cast<const int32_t*>(A.y) + off + j4));
-      yv[0] = v.x; yv[1] = v.y; yv[2] = v.z; yv[3] = v.w;
-    }
-    const double2* m2 = reinterpret_cast<const double2*>(A.mu + off + j4);
-    const double2 m0 = __ldg(m2), m1 = __ldg(m2 + 1);
-    const double mv[4] = {m0.x, m0.y, m1.x, m1.y};
-    double wv[4] = {1.0, 1.0, 1.0, 1.0};
-    if (USE_W) {
-      const double2* w2 = reinterpret_cast<const double2*>(A.w + off + j4);
-      const double2 w0 = __ldg(w2), w1 = __ldg(w2 + 1);
-      wv[0] = w0.x; wv[1] = w0.y; wv[2] = w1.x; wv[3] = w1.y;
-    }
+  if (valid) {
+    for (int j4 = lg * 4; j4 < mpad; j4 += 4 * GL) {
+      double yv[4];
+      if (A.y_is_f64) {
+        const double2* p2 = reinterpret_cast<const double2*>(static_cast<const double*>(A.y) + off + j4);
+        const double2 a0 = __ldg(p2), a1 = __ldg(p2 + 1);
+        yv[0] = a0.x; yv[1] = a0.y; yv[2] = a1.x; yv[3] = a1.y;
+      } else {
+        const int4 v = __ldg(reinterpret_cast<const int4*>(static_cast<const int32_t*>(A.y) + off + j4));
+        yv[0] = v.x; yv[1] = v.y; yv[2] = v.z; yv[3] = v.w;
+      }
+      const double2* m2 = reinterpret_cast<const double2*>(A.mu + off + j4);
+      const double2 m0 = __ldg(m2), m1 = __ldg(m2 + 1);
+      const double mv[4] = {m0.x, m0.y, m1.x, m1.y};
+      double wv[4] = {1.0, 1.0, 1.0, 1.0};
+      if (USE_W) {
+        const double2* w2 = reinterpret_cast<const double2*>(A.w + off + j4);
+        const double2 w0 = __ldg(w2), w1 = __ldg(w2 + 1);
+        wv[0] = w0.x; wv[1] = w0.y; wv[2] = w1.x; wv[3] = w1.y;
+      }
 #pragma unroll
-    for (int q = 0; q < 4; q++) {
-      const int j = j4 + q;
-      S.ys[j] = yv[q];
-      S.mus[j] = mv[q];
-      if (USE_W) S.wsm[j] = wv[q];
-      if (j < A.m) {
-        sum_wy_l += wv[q] * yv[q];
-        ymax_l = fmax(ymax_l, yv[q]);
+      for (int q = 0; q < 4; q++) {
+        const int j = j4 + q;
+        S.ys[j] = yv[q];
+        S.mus[j] = mv[q];
+        if (USE_W) S.wsm[j] = wv[q];
+        if (j < A.m) {
+          sum_wy_l += wv[q] * yv[q];
+          ymax_l = fmax(ymax_l, yv[q]);
+        }
       }
     }
   }
-  sum_wy = warp_allreduce_sum(sum_wy_l);
-  ymax = warp_allreduce_max(ymax_l);
+  sum_wy = group_allreduce_sum<GL>(sum_wy_l);
+  ymax = group_allreduce_max<GL>(ymax_l);
   __syncwarp();
 }
 
-// c_k = sum_j w_j [y_j > k], k = 0 .. ymax-1: shared-memory histogram + suffix scan (TAB mode)
-template <bool USE_W>
-__device__ __forceinline__ void build_table(const DispWarpSmem& S, int m, int lane) {
-  for (int k = lane; k < kTabMax; k += 32) S.tab[k] = 0.0;
+// c_k = sum_j w_j [y_j > k], k = 0 .. ymax-1, for the group's gene: shared-memory histogram + suffix scan over the GL
+// lanes (TAB mode)
+template <bool USE_W, int GL>
+__device__ __forceinline__ void build_table(const DispWarpSmem& S, int m, int lg) {
+  for (int k = lg; k < kTabMax; k += GL) S.tab[k] = 0.0;
   __syncwarp();
   if (USE_W) {
-    // weighted histogram in a FIXED order (bin k belongs to lane k % 32, which adds its samples in index order):
+    // weighted histogram in a FIXED order (bin k belongs to lane k % GL, which adds its samples in index order):
     // floating-point atomics would make c_k -- and with it `iter` on knife-edge genes -- vary from run to run
     for (int j = 0; j < m; j++) {
       const int v = (int)S.ys[j];
-      if (v >= 1 && ((v - 1) & 31) == lane) S.tab[v - 1] += S.wsm[j];
+      if (v >= 1 && v <= kTabMax && ((v - 1) % GL) == lg) S.tab[v - 1] += S.wsm[j];
     }
   } else {
-    for (int j = lane; j < m; j += 32) {
+    for (int j = lg; j < m; j += GL) {
       const int v = (int)S.ys[j];
-      if (v >= 1) atomicAdd(&S.tab[v - 1], 1.0);   // integer-valued sums: exact in any order
+      if (v >= 1 && v <= kTabMax) atomicAdd(&S.tab[v - 1], 1.0);   // integer-valued sums: exact in any order
     }
   }
   __syncwarp();
-  constexpr int PER = kTabMax / 32;
+  constexpr int PER = kTabMax / GL;
   double loc[PER];
   double run = 0.0;
 #pragma unroll
   for (int q = PER - 1; q >= 0; q--) {
-    run += S.tab[lane * PER + q];
+    run += S.tab[lg * PER + q];
     loc[q] = run;
   }
-  double above = run;  // inclusive suffix scan over lanes
+  double above = run;  // inclusive suffix scan over the lanes of the group
 #pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const double t = __shfl_down_sync(0xffffffffu, above, o);
-    if (lane + o < 32) above += t;
+  for (int o = 1; o < GL; o <<= 1) {
+    const double t = __shfl_down_sync(0xffffffffu, above, o, GL);
+    if (lg + o < GL) above += t;
   }
   above -= run;
   __syncwarp();
 #pragma unroll
-  for (int q = 0; q < PER; q++) S.tab[lane * PER + q] = loc[q] + above;
+  for (int q = 0; q < PER; q++) S.tab[lg * PER + q] = loc[q] + above;
   __syncwarp();
 }
 
-// the line search of one gene (src/DESeq2.cpp:201-265) with a single evaluation site
+// the line search of one gene (deseq_rules.cuh::DispLineSearch) with a single evaluation site; t = -1 is the
+// evaluation at the starting point, t >= 0 are the proposals
 template <int P, bool USE_W, int MODE>
 __device__ __forceinline__ void line_search_gene(const DispArgs& A, const DispRow& rv, const DispScal& sc,
                                                  unsigned int g, double sum_wy, int lane) {
-  const double epsilon = 1.0e-4;
   const double pm = A.prior_mean[g];
-  double a = A.log_alpha_in[g];
-  double lp = 0.0, dlp = 0.0, initial_lp = 0.0, initial_dlp = 0.0;
-  double kappa = A.kappa_0;
-  double change = -1.0;
-  int it = 0, acc_n = 0;
-  // t = -1 is the evaluation at the starting point (:205-206); t >= 0 are the proposals (:212-259)
+  DispLineSearch ls(A.log_alpha_in[g], A.kappa_0);
   for (int t = -1; t < A.maxit; t++) {
-    double a_new = a;
-    if (t >= 0) {
-      it++;
-      const double a_propose = a + kappa * dlp;
-      if (a_propose < -30.0) kappa = (-30.0 - a) / dlp;
-      if (a_propose > 10.0) kappa = (10.0 - a) / dlp;
-      a_new = a + kappa * dlp;
-    }
+    const double a_new = ls.propose();
     double lp_new, dlp_new;
     disp_eval_mode<P, USE_W, true, MODE>(rv, sc, a_new, pm, sum_wy, lane, lp_new, dlp_new);
-    if (t < 0) {
-      lp = initial_lp = lp_new;
-      dlp = initial_dlp = dlp_new;
-      continue;
-    }
-    const double theta_kappa = -1.0 * lp_new;
-    const double theta_hat_kappa = -1.0 * lp - kappa * epsilon * dlp * dlp;
-    if (theta_kappa <= theta_hat_kappa) {
-      acc_n++;
-      a = a_new;
-      change = lp_new - lp;
-      if (change < A.tol) { lp = lp_new; break; }
-      if (a < A.min_log_alpha) break;
-      lp = lp_new;
-      dlp = dlp_new;
-      kappa = fmin(kappa * 1.1, A.kappa_0);
-      if (acc_n % 5 == 0) kappa = kappa / 2.0;
-    } else {
-      kappa = kappa / 2.0;
-    }
+    if (ls.take(lp_new, dlp_new, A)) break;
   }
-  const double d2 = disp_d2<P, USE_W>(rv, sc, MODE, a, lane);
-  if (lane == 0) {
-    A.log_alpha[g] = a;
-    A.iter[g] = it;
-    A.iter_accept[g] = acc_n;
-    A.last_change[g] = change;
-    A.initial_lp[g] = initial_lp;
-    A.initial_dlp[g] = initial_dlp;
-    A.last_lp[g] = lp;
-    A.last_dlp[g] = dlp;
-    A.last_d2lp[g] = d2;
-  }
+  const double d2 = disp_d2<P, USE_W>(rv, sc, MODE, ls.a, lane);
+  if (lane == 0) ls.store(A, g, d2);
 }
 
 #ifndef NB_LB_THREADS
@@ -524,9 +479,9 @@ __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_disp_kernel(con
     else { mode = MODE_GEN; g = A.mode_lists[2 * (size_t)A.n + (q - n0 - n1)]; }
 
     double sum_wy, ymax;
-    stage_row<USE_W>(A, g, mpad, lane, S, sum_wy, ymax);
+    stage_row<USE_W, 32>(A, g, true, mpad, lane, S, sum_wy, ymax);
     if (mode == MODE_TAB) {
-      build_table<USE_W>(S, A.m, lane);
+      build_table<USE_W, 32>(S, A.m, lane);
       rv.ntab = (int)ymax;
       line_search_gene<P, USE_W, MODE_TAB>(A, rv, sc, g, sum_wy, lane);
     } else if (mode == MODE_BIG) {
@@ -539,10 +494,6 @@ __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_disp_kernel(con
 }
 
 #include "fit_disp_grp.cuh"
-#ifdef NB_EXP_TMA_ROWS
-#include "tma_rows_exp.cuinc"
-#endif
-
 
 // fitDispGrid (src/DESeq2.cpp:492-510): rare path (non-converged genes only); generic evaluation mode
 template <int P, bool USE_W>
@@ -568,55 +519,33 @@ __global__ void __launch_bounds__(256, 2) fit_disp_grid_kernel(const DispArgs A,
     g = __shfl_sync(0xffffffffu, g, 0);
     if (g >= (unsigned int)A.n) break;
     double sum_wy, ymax;
-    stage_row<USE_W>(A, g, mpad, lane, S, sum_wy, ymax);
+    stage_row<USE_W, 32>(A, g, true, mpad, lane, S, sum_wy, ymax);
     const double pm = A.prior_mean[g];
-    const int gn = A.grid_n;
-    const double delta = A.grid[1] - A.grid[0];
-    double best = 0.0, a_hat = 0.0, a_best = 0.0, start = 0.0, end = 0.0, step = 0.0;
-    for (int t = 0; t < 2 * gn; t++) {
-      const int tt = (t < gn) ? t : t - gn;
-      if (t == gn) {
-        start = a_hat - delta;
-        end = a_hat + delta;
-        step = (end - start) / (double)(gn - 1);
-      }
-      const double a = (t < gn) ? A.grid[tt] : ((tt == gn - 1) ? end : start + tt * step);
+    DispGridSearch gs(A);
+    for (int t = 0; t < gs.evaluations(); t++) {
+      const double a = gs.point(t);
       double lp, dummy;
       disp_eval_mode<P, USE_W, false, MODE_GEN>(rv, sc, a, pm, sum_wy, lane, lp, dummy);
-      if (tt == 0 || lp > best) {
-        best = lp;
-        if (t < gn) a_hat = a; else a_best = a;
-      }
+      gs.take(t, a, lp);
     }
-    if (lane == 0) A.log_alpha[g] = a_best;
+    if (lane == 0) A.log_alpha[g] = gs.a_best;
     __syncwarp();
   }
 }
 
 // launch the GL-lanes-per-gene experiment kernel if its shared-memory slices fit; `launched` tells
 template <int P, bool USE_W, int GL>
-cudaError_t launch_disp_grp(const DispArgs& a, int mpad, size_t xbytes, size_t rowbytes, int sms, cudaStream_t stream,
+cudaError_t launch_disp_grp(const DispArgs& a, int mpad, size_t xbytes, size_t rowbytes, cudaStream_t stream,
                             bool& launched) {
   constexpr int NG = 32 / GL, GW = GrpShape<GL>::threads / 32;
   const size_t gsmem = xbytes + (size_t)GW * NG * rowbytes;
   launched = false;
   if (gsmem > (size_t)227 * 1024 / GrpShape<GL>::ctas) return cudaSuccess;
   auto kg = fit_disp_grp_kernel<P, USE_W, GL>;
-  static size_t g_smem = 0;
-  static int g_ctas = 0;
-  cudaError_t e = cudaSuccess;
-  if (g_smem != gsmem || g_ctas < 1) {
-    e = cudaFuncSetAttribute(kg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsmem);
-    if (e != cudaSuccess) return e;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&g_ctas, kg, GrpShape<GL>::threads, gsmem);
-    if (e != cudaSuccess) return e;
-    if (g_ctas < 1) return cudaErrorLaunchOutOfResources;
-    g_smem = gsmem;
-  }
-  long long gg = (long long)sms * g_ctas;
-  const long long gwant = ((long long)a.n + GW * NG - 1) / (GW * NG);
-  if (gg > gwant) gg = gwant;
-  kg<<<(unsigned)(gg < 1 ? 1 : gg), GrpShape<GL>::threads, gsmem, stream>>>(a, mpad);
+  unsigned grid = 0;
+  const cudaError_t e = persistent_grid(reinterpret_cast<const void*>(kg), GrpShape<GL>::threads, gsmem, GW * NG, a.n, &grid);
+  if (e != cudaSuccess) return e;
+  kg<<<grid, GrpShape<GL>::threads, gsmem, stream>>>(a, mpad);
   launched = true;
   return cudaGetLastError();
 }
@@ -633,84 +562,47 @@ cudaError_t launch_disp_t(const DispArgs& a0, cudaStream_t stream) {
   while (warps > 1 && xbytes + warps * rowbytes > smem_cap / 2) warps >>= 1;   // aim for >= 2 CTAs/SM
   if (xbytes + warps * rowbytes > smem_cap) return cudaErrorInvalidValue;
   const size_t smem = xbytes + warps * rowbytes;
-  const bool grid_mode = a.grid != nullptr;
-  auto kern = grid_mode ? fit_disp_grid_kernel<P, USE_W> : fit_disp_kernel<P, USE_W>;
-  // the attribute / occupancy queries are made once per (kernel, shared-memory size) and cached
-  static size_t cached_smem[2] = {0, 0};
-  static int cached_ctas[2] = {0, 0};
-  const int slot = (grid_mode ? 1 : 0);
-  cudaError_t e = cudaSuccess;
-  if (cached_smem[slot] != smem || cached_ctas[slot] < 1) {
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    int c = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kern, warps * 32, smem);
-    if (e != cudaSuccess) return e;
-    if (c < 1) return cudaErrorLaunchOutOfResources;
-    cached_smem[slot] = smem;
-    cached_ctas[slot] = c;
-  }
-  const int ctas_per_sm = cached_ctas[slot];
-  const int sms = device_sm_count();
-  long long want = ((long long)a.n + warps - 1) / warps;
-  long long grid = (long long)sms * ctas_per_sm;   // persistent: one resident wave, genes come from the queue
-  if (grid > want) grid = want;
-  if (grid < 1) grid = 1;
   // scratch: [queue counter | 3 mode counters | 3 n gene lists]
-  e = cudaMemsetAsync(a.scratch, 0, kDispScratchHead * sizeof(unsigned int), stream);
+  cudaError_t e = cudaMemsetAsync(a.scratch, 0, kDispScratchHead * sizeof(unsigned int), stream);
   if (e != cudaSuccess) return e;
   a.counter = a.scratch;
   a.mode_counts = a.scratch + 1;
   a.mode_lists = reinterpret_cast<int*>(a.scratch + kDispScratchHead);
-  if (!grid_mode) {
-    int* lists = reinterpret_cast<int*>(a.scratch + kDispScratchHead);
-    int* code = lists + 3 * (size_t)a.n;
-    int* sorted = lists + 4 * (size_t)a.n;
-    // Table-length ordering of the TAB list only pays when four genes share a warp (8 lanes per gene: they wait for the
-    // longest table of the four) and costs time at two genes per warp
-    const bool buckets = group_lanes_disp(a.m) == 8;
-    classify_kernel<<<(a.n + 7) / 8, 256, 0, stream>>>(a.y, a.y_is_f64, a.n, a.m, a.ld, lists, a.scratch + 1,
-                                                       buckets ? code : nullptr, a.scratch + 8);
+  unsigned grid = 0;
+  if (a.grid != nullptr) {   // fitDispGrid: one queue, no evaluation-mode classification, one gene per warp
+    auto kg = fit_disp_grid_kernel<P, USE_W>;
+    e = persistent_grid(reinterpret_cast<const void*>(kg), warps * 32, smem, warps, a.n, &grid);
+    if (e != cudaSuccess) return e;
+    kg<<<grid, warps * 32, smem, stream>>>(a, warps, mpad);
+    return cudaGetLastError();
+  }
+  int* lists = reinterpret_cast<int*>(a.scratch + kDispScratchHead);
+  int* code = lists + 3 * (size_t)a.n;
+  int* sorted = lists + 4 * (size_t)a.n;
+  // Table-length ordering of the TAB list only pays when four genes share a warp (8 lanes per gene: they wait for the
+  // longest table of the four) and costs time at two genes per warp
+  const int gl = group_lanes_disp(a.m);
+  const bool buckets = gl == 8;
+  classify_kernel<<<(a.n + 7) / 8, 256, 0, stream>>>(a.y, a.y_is_f64, a.n, a.m, a.ld, lists, a.scratch + 1,
+                                                     buckets ? code : nullptr, a.scratch + 8);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  if (buckets) {
+    bucket_sort_kernel<<<(a.n + 255) / 256 > 1184 ? 1184 : (a.n + 255) / 256, 256, 0, stream>>>(lists, code, a.scratch + 1 + MODE_TAB, a.scratch + 8, a.scratch + 16, sorted);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    if (buckets) {
-      bucket_sort_kernel<<<(a.n + 255) / 256 > 1184 ? 1184 : (a.n + 255) / 256, 256, 0, stream>>>(lists, code, a.scratch + 1 + MODE_TAB, a.scratch + 8, a.scratch + 16, sorted);
-      e = cudaGetLastError();
-      if (e != cudaSuccess) return e;
-      // entries beyond the TAB count are never read by the kernels, so copying the whole n-entry region is harmless
-      e = cudaMemcpyAsync(lists, sorted, sizeof(int) * (size_t)a.n, cudaMemcpyDeviceToDevice, stream);
-      if (e != cudaSuccess) return e;
-    }
+    // entries beyond the TAB count are never read by the kernels, so copying the whole n-entry region is harmless
+    e = cudaMemcpyAsync(lists, sorted, sizeof(int) * (size_t)a.n, cudaMemcpyDeviceToDevice, stream);
+    if (e != cudaSuccess) return e;
   }
-  if (!grid_mode) {
-    const int gl = group_lanes_disp(a.m);
-    bool launched = false;
-    if (gl == 8) e = launch_disp_grp<P, USE_W, 8>(a, mpad, xbytes, rowbytes, sms, stream, launched);
-    else if (gl == 16) e = launch_disp_grp<P, USE_W, 16>(a, mpad, xbytes, rowbytes, sms, stream, launched);
-    if (e != cudaSuccess || launched) return e;
-  }
-#ifdef NB_EXP_TMA_ROWS
-  if (!grid_mode) {   // experiment: one gene per warp with the mean row prefetched by TMA bulk copies (tma_rows_exp.cuinc)
-    const size_t trow = ((size_t)(NROW + 1) * mpad + kTabMax + 2) * sizeof(double);
-    int tw = NB_LB_THREADS / 32;
-    while (tw > 1 && xbytes + tw * trow > smem_cap / 2) tw >>= 1;
-    if (xbytes + tw * trow <= smem_cap) {
-      auto kt = fit_disp_tma_kernel<P, USE_W>;
-      const size_t tsm = xbytes + tw * trow;
-      e = cudaFuncSetAttribute(kt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsm);
-      if (e != cudaSuccess) return e;
-      int c = 0;
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kt, tw * 32, tsm);
-      if (e != cudaSuccess || c < 1) return e != cudaSuccess ? e : cudaErrorLaunchOutOfResources;
-      long long tg = (long long)sms * c;
-      const long long twant = ((long long)a.n + tw - 1) / tw;
-      if (tg > twant) tg = twant;
-      kt<<<(unsigned)(tg < 1 ? 1 : tg), tw * 32, tsm, stream>>>(a, tw, mpad);
-      return cudaGetLastError();
-    }
-  }
-#endif
-  kern<<<(unsigned)grid, warps * 32, smem, stream>>>(a, warps, mpad);
+  bool launched = false;
+  if (gl == 8) e = launch_disp_grp<P, USE_W, 8>(a, mpad, xbytes, rowbytes, stream, launched);
+  else if (gl == 16) e = launch_disp_grp<P, USE_W, 16>(a, mpad, xbytes, rowbytes, stream, launched);
+  if (e != cudaSuccess || launched) return e;
+  auto kern = fit_disp_kernel<P, USE_W>;
+  e = persistent_grid(reinterpret_cast<const void*>(kern), warps * 32, smem, warps, a.n, &grid);
+  if (e != cudaSuccess) return e;
+  kern<<<grid, warps * 32, smem, stream>>>(a, warps, mpad);
   return cudaGetLastError();
 }
 

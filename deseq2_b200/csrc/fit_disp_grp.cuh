@@ -47,169 +47,23 @@ inline int group_lanes_disp(int m) {
   return m <= 40 ? 8 : 16;
 }
 
-template <int GL>
-__device__ __forceinline__ double group_allreduce_sum(double v) {
-#pragma unroll
-  for (int o = GL / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-template <int GL>
-__device__ __forceinline__ double group_allreduce_max(double v) {
-#pragma unroll
-  for (int o = GL / 2; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-// stage the row of gene g into the group's shared-memory slice; lg = lane inside the group.  `valid` false: the
-// group has no gene this round -- nothing is loaded (the slice keeps the previous gene, which is fine to evaluate).
-template <bool USE_W, int GL>
-__device__ __forceinline__ void stage_row_g(const DispArgs& A, unsigned int g, bool valid, int mpad, int lg,
-                                            const DispWarpSmem& S, double& sum_wy, double& ymax) {
-  double sum_wy_l = 0.0, ymax_l = 0.0;
-  const size_t off = (size_t)g * A.ld;
-  if (valid) {
-    for (int j4 = lg * 4; j4 < mpad; j4 += 4 * GL) {
-      double yv[4];
-      if (A.y_is_f64) {
-        const double2* p2 = reinterpret_cast<const double2*>(static_cast<const double*>(A.y) + off + j4);
-        const double2 a0 = __ldg(p2), a1 = __ldg(p2 + 1);
-        yv[0] = a0.x; yv[1] = a0.y; yv[2] = a1.x; yv[3] = a1.y;
-      } else {
-        const int4 v = __ldg(reinterpret_cast<const int4*>(static_cast<const int32_t*>(A.y) + off + j4));
-        yv[0] = v.x; yv[1] = v.y; yv[2] = v.z; yv[3] = v.w;
-      }
-      const double2* m2 = reinterpret_cast<const double2*>(A.mu + off + j4);
-      const double2 m0 = __ldg(m2), m1 = __ldg(m2 + 1);
-      const double mv[4] = {m0.x, m0.y, m1.x, m1.y};
-      double wv[4] = {1.0, 1.0, 1.0, 1.0};
-      if (USE_W) {
-        const double2* w2 = reinterpret_cast<const double2*>(A.w + off + j4);
-        const double2 w0 = __ldg(w2), w1 = __ldg(w2 + 1);
-        wv[0] = w0.x; wv[1] = w0.y; wv[2] = w1.x; wv[3] = w1.y;
-      }
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        const int j = j4 + q;
-        S.ys[j] = yv[q];
-        S.mus[j] = mv[q];
-        if (USE_W) S.wsm[j] = wv[q];
-        if (j < A.m) {
-          sum_wy_l += wv[q] * yv[q];
-          ymax_l = fmax(ymax_l, yv[q]);
-        }
-      }
-    }
-  }
-  sum_wy = group_allreduce_sum<GL>(sum_wy_l);
-  ymax = group_allreduce_max<GL>(ymax_l);
-  __syncwarp();
-}
-
-// c_k = sum_j w_j [y_j > k] for the group's gene: shared-memory histogram + suffix scan over GL lanes
-template <bool USE_W, int GL>
-__device__ __forceinline__ void build_table_g(const DispWarpSmem& S, int m, int lg) {
-  for (int k = lg; k < kTabMax; k += GL) S.tab[k] = 0.0;
-  __syncwarp();
-  if (USE_W) {
-    // weighted histogram in a fixed order (bin k belongs to lane k % GL of the group): see build_table
-    for (int j = 0; j < m; j++) {
-      const int v = (int)S.ys[j];
-      if (v >= 1 && v <= kTabMax && ((v - 1) % GL) == lg) S.tab[v - 1] += S.wsm[j];
-    }
-  } else {
-    for (int j = lg; j < m; j += GL) {
-      const int v = (int)S.ys[j];
-      if (v >= 1 && v <= kTabMax) atomicAdd(&S.tab[v - 1], 1.0);
-    }
-  }
-  __syncwarp();
-  constexpr int PER = kTabMax / GL;
-  double loc[PER];
-  double run = 0.0;
-#pragma unroll
-  for (int q = PER - 1; q >= 0; q--) {
-    run += S.tab[lg * PER + q];
-    loc[q] = run;
-  }
-  double above = run;  // inclusive suffix scan over the lanes of the group
-#pragma unroll
-  for (int o = 1; o < GL; o <<= 1) {
-    const double t = __shfl_down_sync(0xffffffffu, above, o, GL);
-    if (lg + o < GL) above += t;
-  }
-  above -= run;
-  __syncwarp();
-#pragma unroll
-  for (int q = 0; q < PER; q++) S.tab[lg * PER + q] = loc[q] + above;
-  __syncwarp();
-}
-
-// One round of the line search for the NG genes a warp holds (src/DESeq2.cpp:201-265), warp-uniform control flow.
+// One round of the line search for the NG genes a warp holds (deseq_rules.cuh::DispLineSearch), warp-uniform control
+// flow: a group whose gene has stopped, or that got no gene, evaluates at its frozen a until every group is done.
 template <int P, bool USE_W, int MODE, int GL>
 __device__ __forceinline__ void line_search_round(const DispArgs& A, const DispRow& rv, const DispScal& sc,
                                                   unsigned int g, bool valid, double sum_wy, int lg) {
-  const double epsilon = 1.0e-4;
   const double pm = valid ? A.prior_mean[g] : 0.0;
-  double a = valid ? A.log_alpha_in[g] : 0.0;
-  double lp = 0.0, dlp = 0.0, initial_lp = 0.0, initial_dlp = 0.0;
-  double kappa = A.kappa_0;
-  double change = -1.0;
-  int it = 0, acc_n = 0;
-  bool first = true;                 // the evaluation at the starting point (:205-206) is still to come
+  DispLineSearch ls(valid ? A.log_alpha_in[g] : 0.0, A.kappa_0);
   bool active = valid;               // false once this group's gene has stopped
   while (__any_sync(0xffffffffu, active)) {
-    double a_new = a;
-    if (active && !first) {
-      it++;
-      const double a_propose = a + kappa * dlp;
-      if (a_propose < -30.0) kappa = (-30.0 - a) / dlp;
-      if (a_propose > 10.0) kappa = (10.0 - a) / dlp;
-      a_new = a + kappa * dlp;
-    }
+    const double a_new = active ? ls.propose() : ls.a;
     double lp_new, dlp_new;
     disp_eval_mode<P, USE_W, true, MODE, GL>(rv, sc, a_new, pm, sum_wy, lg, lp_new, dlp_new);
-    if (active) {
-      if (first) {
-        lp = initial_lp = lp_new;
-        dlp = initial_dlp = dlp_new;
-        first = false;
-      } else {
-        const double theta_kappa = -1.0 * lp_new;
-        const double theta_hat_kappa = -1.0 * lp - kappa * epsilon * dlp * dlp;
-        if (theta_kappa <= theta_hat_kappa) {
-          acc_n++;
-          a = a_new;
-          change = lp_new - lp;
-          if (change < A.tol) {
-            lp = lp_new;
-            active = false;
-          } else if (a < A.min_log_alpha) {
-            active = false;
-          } else {
-            lp = lp_new;
-            dlp = dlp_new;
-            kappa = fmin(kappa * 1.1, A.kappa_0);
-            if (acc_n % 5 == 0) kappa = kappa / 2.0;
-          }
-        } else {
-          kappa = kappa / 2.0;
-        }
-      }
-      if (it >= A.maxit) active = false;   // the reference's `for (t = 0; t < maxit; t++)`
-    }
+    // the reference's `for (t = 0; t < maxit; t++)` bounds the proposals
+    if (active) active = !ls.take(lp_new, dlp_new, A) && ls.it < A.maxit;
   }
-  const double d2 = disp_d2<P, USE_W, GL>(rv, sc, MODE, a, lg);
-  if (valid && lg == 0) {
-    A.log_alpha[g] = a;
-    A.iter[g] = it;
-    A.iter_accept[g] = acc_n;
-    A.last_change[g] = change;
-    A.initial_lp[g] = initial_lp;
-    A.initial_dlp[g] = initial_dlp;
-    A.last_lp[g] = lp;
-    A.last_dlp[g] = dlp;
-    A.last_d2lp[g] = d2;
-  }
+  const double d2 = disp_d2<P, USE_W, GL>(rv, sc, MODE, ls.a, lg);
+  if (valid && lg == 0) ls.store(A, g, d2);
 }
 
 // One kernel for the three evaluation-mode families, one family after the other, each with its own queue counter
@@ -254,9 +108,9 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
       if (!__any_sync(0xffffffffu, valid)) break;
       const unsigned int g = valid ? (unsigned int)list[q] : 0u;
       double sum_wy, ymax;
-      stage_row_g<USE_W, GL>(A, g, valid, mpad, lg, S, sum_wy, ymax);
+      stage_row<USE_W, GL>(A, g, valid, mpad, lg, S, sum_wy, ymax);
       if (mode == MODE_TAB) {
-        build_table_g<USE_W, GL>(S, A.m, lg);
+        build_table<USE_W, GL>(S, A.m, lg);
         rv.ntab = valid ? (int)ymax : 0;
         line_search_round<P, USE_W, MODE_TAB, GL>(A, rv, sc, g, valid, sum_wy, lg);
       } else if (mode == MODE_BIG) {

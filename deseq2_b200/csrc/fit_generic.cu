@@ -19,6 +19,7 @@
 
 #include <mutex>
 
+#include "deseq_rules.cuh"
 #include "engine.h"
 #include "nbmath.cuh"
 
@@ -466,7 +467,6 @@ __global__ void __launch_bounds__(256, 1) fit_disp_generic_kernel(const DispArgs
   C.use_w = A.use_weights;
   C.saturated = A.saturated && A.grouped && A.G == A.p && !A.use_weights;
   C.sat_logdet = A.sat_logdet;
-  const double epsilon = 1.0e-4;
 
   for (;;) {
     unsigned int g = 0;
@@ -486,76 +486,25 @@ __global__ void __launch_bounds__(256, 1) fit_disp_generic_kernel(const DispArgs
     double lp_new, dlp_new, d2;
 
     if (A.grid != nullptr) {
-      const int gn = A.grid_n;
-      const double delta = A.grid[1] - A.grid[0];
-      double best = 0.0, a_hat = 0.0, a_best = 0.0, start = 0.0, end = 0.0, step = 0.0;
-      for (int t = 0; t < 2 * gn; t++) {
-        const int tt = (t < gn) ? t : t - gn;
-        if (t == gn) {
-          start = a_hat - delta;
-          end = a_hat + delta;
-          step = (end - start) / (double)(gn - 1);
-        }
-        const double a = (t < gn) ? A.grid[tt] : ((tt == gn - 1) ? end : start + tt * step);
+      DispGridSearch gs(A);
+      for (int t = 0; t < gs.evaluations(); t++) {
+        const double a = gs.point(t);
         gdisp_eval(C, a, pm, lane, false, false, lp_new, dlp_new, d2);
-        if (tt == 0 || lp_new > best) {
-          best = lp_new;
-          if (t < gn) a_hat = a; else a_best = a;
-        }
+        gs.take(t, a, lp_new);
       }
-      if (lane == 0) A.log_alpha[g] = a_best;
+      if (lane == 0) A.log_alpha[g] = gs.a_best;
       __syncwarp();
       continue;
     }
 
-    double a = A.log_alpha_in[g];
-    double lp = 0.0, dlp = 0.0, initial_lp = 0.0, initial_dlp = 0.0;
-    double kappa = A.kappa_0;
-    double change = -1.0;
-    int it = 0, acc_n = 0;
-    for (int t = -1; t < A.maxit; t++) {
-      double a_new = a;
-      if (t >= 0) {
-        it++;
-        const double a_propose = a + kappa * dlp;
-        if (a_propose < -30.0) kappa = (-30.0 - a) / dlp;
-        if (a_propose > 10.0) kappa = (10.0 - a) / dlp;
-        a_new = a + kappa * dlp;
-      }
+    DispLineSearch ls(A.log_alpha_in[g], A.kappa_0);
+    for (int t = -1; t < A.maxit; t++) {   // t = -1: the evaluation at the starting point
+      const double a_new = ls.propose();
       gdisp_eval(C, a_new, pm, lane, true, false, lp_new, dlp_new, d2);
-      if (t < 0) {
-        lp = initial_lp = lp_new;
-        dlp = initial_dlp = dlp_new;
-        continue;
-      }
-      const double theta_kappa = -1.0 * lp_new;
-      const double theta_hat_kappa = -1.0 * lp - kappa * epsilon * dlp * dlp;
-      if (theta_kappa <= theta_hat_kappa) {
-        acc_n++;
-        a = a_new;
-        change = lp_new - lp;
-        if (change < A.tol) { lp = lp_new; break; }
-        if (a < A.min_log_alpha) break;
-        lp = lp_new;
-        dlp = dlp_new;
-        kappa = fmin(kappa * 1.1, A.kappa_0);
-        if (acc_n % 5 == 0) kappa = kappa / 2.0;
-      } else {
-        kappa = kappa / 2.0;
-      }
+      if (ls.take(lp_new, dlp_new, A)) break;
     }
-    gdisp_eval(C, a, pm, lane, true, true, lp_new, dlp_new, d2);
-    if (lane == 0) {
-      A.log_alpha[g] = a;
-      A.iter[g] = it;
-      A.iter_accept[g] = acc_n;
-      A.last_change[g] = change;
-      A.initial_lp[g] = initial_lp;
-      A.initial_dlp[g] = initial_dlp;
-      A.last_lp[g] = lp;
-      A.last_dlp[g] = dlp;
-      A.last_d2lp[g] = d2;
-    }
+    gdisp_eval(C, ls.a, pm, lane, true, true, lp_new, dlp_new, d2);
+    if (lane == 0) ls.store(A, g, d2);
     __syncwarp();
   }
 }
@@ -681,7 +630,6 @@ __global__ void __launch_bounds__(256, 1) fit_beta_generic_kernel(const BetaArgs
   double* rhs = S.v1;
   double* sc = S.v2;     // equilibration scales
   double* tmp = S.v3;
-  const double large = 30.0;
 
   for (;;) {
     unsigned int g = 0;
@@ -715,10 +663,9 @@ __global__ void __launch_bounds__(256, 1) fit_beta_generic_kernel(const BetaArgs
       devc = warp_allreduce_sum(c);
     }
     gbeta_pass(C, beta, alpha, r, log_alpha, false, lane);
-    double dev = 0.0, dev_old = 0.0;
-    double it = 0.0;
+    IrlsProgress ir;
     for (int t = 0; t < A.maxit; t++) {
-      it += 1.0;
+      ir.start_iteration();
       // normal equations (X'WX + Lambda) b = X'Wz, Jacobi-equilibrated Cholesky
       build_xtwx(C.D, S.WA, B, lane);
       if (lane < p) {
@@ -753,16 +700,12 @@ __global__ void __launch_bounds__(256, 1) fit_beta_generic_kernel(const BetaArgs
       bool big = false;
       if (lane < p) {
         beta[lane] = rhs[lane] * sc[lane];
-        big = fabs(beta[lane]) > large;
+        big = fabs(beta[lane]) > kBetaLarge;
       }
       __syncwarp();
-      if (__any_sync(0xffffffffu, big)) { it = (double)A.maxit; break; }
+      if (__any_sync(0xffffffffu, big)) { ir.diverged(A.maxit); break; }
       const double dv = gbeta_pass(C, beta, alpha, r, log_alpha, true, lane);
-      dev = -2.0 * (dv + devc);
-      const double conv_test = fabs(dev - dev_old) / (fabs(dev) + 0.1);
-      if (isnan(conv_test)) { it = (double)A.maxit; break; }
-      if ((t > 0) && (conv_test < A.tol)) break;
-      dev_old = dev;
+      if (ir.stop_after_pass(dv, devc, A)) break;
     }
     // ---- post-loop block (src/DESeq2.cpp:429-455): W sums belong to the mu now in shared memory
     build_xtwx(C.D, S.WA, B, lane);
@@ -815,10 +758,10 @@ __global__ void __launch_bounds__(256, 1) fit_beta_generic_kernel(const BetaArgs
     cd = warp_allreduce_sum(cd);
     cn = warp_allreduce_sum(cn);
     if (lane == 0) {
-      A.iter[g] = it;
+      A.iter[g] = ir.it;
       A.contrast_num[g] = cn;
       A.contrast_denom[g] = sqrt(cd);
-      A.deviance[g] = dev;
+      A.deviance[g] = ir.dev;
     }
     __syncwarp();
   }
@@ -915,34 +858,22 @@ bool plan_seg(size_t fixed, size_t warp_bytes, int max_warps, SegPlan& out) {
   out.smem = fixed + (size_t)warps * warp_bytes;
   return true;
 }
-template <typename K>
-cudaError_t seg_grid(K kernel, const SegPlan& P, int n, long long* grid) {
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P.smem);
-  if (e != cudaSuccess) return e;
-  int ctas_per_sm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kernel, P.warps * 32, P.smem);
-  if (e != cudaSuccess) return e;
-  if (ctas_per_sm < 1) return cudaErrorLaunchOutOfResources;
-  const long long want = ((long long)n + P.warps - 1) / P.warps;
-  long long g = (long long)device_sm_count() * ctas_per_sm;
-  if (g > want) g = want;
-  *grid = g < 1 ? 1 : g;
-  return cudaSuccess;
-}
 template <int MAXT>
 cudaError_t launch_disp_seg_t(const DispArgs& a, const SegPlan& P, cudaStream_t stream) {
-  long long grid = 1;
-  cudaError_t e = seg_grid(fit_disp_seg_kernel<MAXT>, P, a.n, &grid);
+  unsigned grid = 0;
+  cudaError_t e = persistent_grid(reinterpret_cast<const void*>(fit_disp_seg_kernel<MAXT>), P.warps * 32, P.smem, P.warps,
+                                  a.n, &grid);
   if (e != cudaSuccess) return e;
-  fit_disp_seg_kernel<MAXT><<<(unsigned)grid, P.warps * 32, P.smem, stream>>>(a, P.mpad, P.ps, P.warp_bytes);
+  fit_disp_seg_kernel<MAXT><<<grid, P.warps * 32, P.smem, stream>>>(a, P.mpad, P.ps, P.warp_bytes);
   return cudaGetLastError();
 }
 template <int MAXT>
 cudaError_t launch_beta_seg_t(const BetaArgs& a, const SegPlan& P, cudaStream_t stream) {
-  long long grid = 1;
-  cudaError_t e = seg_grid(fit_beta_seg_kernel<MAXT>, P, a.n, &grid);
+  unsigned grid = 0;
+  cudaError_t e = persistent_grid(reinterpret_cast<const void*>(fit_beta_seg_kernel<MAXT>), P.warps * 32, P.smem, P.warps,
+                                  a.n, &grid);
   if (e != cudaSuccess) return e;
-  fit_beta_seg_kernel<MAXT><<<(unsigned)grid, P.warps * 32, P.smem, stream>>>(a, P.mpad, P.ps, P.warp_bytes);
+  fit_beta_seg_kernel<MAXT><<<grid, P.warps * 32, P.smem, stream>>>(a, P.mpad, P.ps, P.warp_bytes);
   return cudaGetLastError();
 }
 
@@ -969,16 +900,9 @@ cudaError_t launch_fit_disp_generic(const DispArgs& a0, cudaStream_t stream) {
   GenLaunch L;
   const GenShape sh{1, 0, a.use_weights != 0, 1, 3, 0};
   if (!plan(a.m, a.p, a.G, a.grouped, sh, 0, L)) return cudaErrorInvalidValue;
-  cudaError_t e = cudaFuncSetAttribute(fit_disp_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem);
+  unsigned grid = 0;
+  cudaError_t e = persistent_grid(reinterpret_cast<const void*>(fit_disp_generic_kernel), L.warps * 32, L.smem, L.warps, a.n, &grid);
   if (e != cudaSuccess) return e;
-  int ctas_per_sm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, fit_disp_generic_kernel, L.warps * 32, L.smem);
-  if (e != cudaSuccess) return e;
-  if (ctas_per_sm < 1) return cudaErrorLaunchOutOfResources;
-  long long want = ((long long)a.n + L.warps - 1) / L.warps;
-  long long grid = (long long)device_sm_count() * ctas_per_sm;
-  if (grid > want) grid = want;
-  if (grid < 1) grid = 1;
   a.row_scratch = nullptr;
   if (L.rows_global) {
     e = row_scratch((size_t)grid * L.warps * gen_rows(sh) * L.mpad * sizeof(double), &a.row_scratch);
@@ -987,7 +911,7 @@ cudaError_t launch_fit_disp_generic(const DispArgs& a0, cudaStream_t stream) {
   e = cudaMemsetAsync(a.scratch, 0, 4 * sizeof(unsigned int), stream);
   if (e != cudaSuccess) return e;
   a.counter = a.scratch;
-  fit_disp_generic_kernel<<<(unsigned)grid, L.warps * 32, L.smem, stream>>>(a, L.mpad, L.ps, L.warp_doubles);
+  fit_disp_generic_kernel<<<grid, L.warps * 32, L.smem, stream>>>(a, L.mpad, L.ps, L.warp_doubles);
   return cudaGetLastError();
 }
 
@@ -1012,16 +936,9 @@ cudaError_t launch_fit_beta_generic(const BetaArgs& a0, cudaStream_t stream) {
   const int mpad = (a.m + 3) & ~3;
   const GenShape sh{a.nf_is_vector ? 0 : 1, 1, a.use_weights != 0, 0, 2, 0};
   if (!plan(a.m, a.p, a.G, a.grouped, sh, (size_t)mpad + 64, L)) return cudaErrorInvalidValue;
-  cudaError_t e = cudaFuncSetAttribute(fit_beta_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem);
+  unsigned grid = 0;
+  cudaError_t e = persistent_grid(reinterpret_cast<const void*>(fit_beta_generic_kernel), L.warps * 32, L.smem, L.warps, a.n, &grid);
   if (e != cudaSuccess) return e;
-  int ctas_per_sm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, fit_beta_generic_kernel, L.warps * 32, L.smem);
-  if (e != cudaSuccess) return e;
-  if (ctas_per_sm < 1) return cudaErrorLaunchOutOfResources;
-  long long want = ((long long)a.n + L.warps - 1) / L.warps;
-  long long grid = (long long)device_sm_count() * ctas_per_sm;
-  if (grid > want) grid = want;
-  if (grid < 1) grid = 1;
   a.row_scratch = nullptr;
   if (L.rows_global) {
     e = row_scratch((size_t)grid * L.warps * gen_rows(sh) * L.mpad * sizeof(double), &a.row_scratch);
@@ -1029,7 +946,7 @@ cudaError_t launch_fit_beta_generic(const BetaArgs& a0, cudaStream_t stream) {
   }
   e = cudaMemsetAsync(a.counter, 0, sizeof(unsigned int), stream);
   if (e != cudaSuccess) return e;
-  fit_beta_generic_kernel<<<(unsigned)grid, L.warps * 32, L.smem, stream>>>(a, L.mpad, L.ps, L.warp_doubles);
+  fit_beta_generic_kernel<<<grid, L.warps * 32, L.smem, stream>>>(a, L.mpad, L.ps, L.warp_doubles);
   return cudaGetLastError();
 }
 

@@ -435,7 +435,6 @@ __global__ void __launch_bounds__(MAXT, 1) fit_disp_seg_kernel(const DispArgs A,
   C.use_cr = A.use_cr;
   C.sat_logdet = A.sat_logdet;
   const SDispWarp& S = C.S;
-  const double epsilon = 1.0e-4;
   const int tab_limit = seg_tab_limit(A.m);
 
   for (;;) {
@@ -480,54 +479,14 @@ __global__ void __launch_bounds__(MAXT, 1) fit_disp_seg_kernel(const DispArgs A,
     }
     const double pm = A.prior_mean[g];
     double lp_new, dlp_new, d2 = 0.0;
-    double a = A.log_alpha_in[g];
-    double lp = 0.0, dlp = 0.0, initial_lp = 0.0, initial_dlp = 0.0;
-    double kappa = A.kappa_0;
-    double change = -1.0;
-    int it = 0, acc_n = 0;
-    for (int t = -1; t < A.maxit; t++) {   // src/DESeq2.cpp:205-259, decision for decision
-      double a_new = a;
-      if (t >= 0) {
-        it++;
-        const double a_propose = a + kappa * dlp;
-        if (a_propose < -30.0) kappa = (-30.0 - a) / dlp;
-        if (a_propose > 10.0) kappa = (10.0 - a) / dlp;
-        a_new = a + kappa * dlp;
-      }
+    DispLineSearch ls(A.log_alpha_in[g], A.kappa_0);
+    for (int t = -1; t < A.maxit; t++) {   // t = -1: the evaluation at the starting point
+      const double a_new = ls.propose();
       sdisp_eval<false>(C, a_new, pm, lane, lp_new, dlp_new, d2);
-      if (t < 0) {
-        lp = initial_lp = lp_new;
-        dlp = initial_dlp = dlp_new;
-        continue;
-      }
-      const double theta_kappa = -1.0 * lp_new;
-      const double theta_hat_kappa = -1.0 * lp - kappa * epsilon * dlp * dlp;
-      if (theta_kappa <= theta_hat_kappa) {
-        acc_n++;
-        a = a_new;
-        change = lp_new - lp;
-        if (change < A.tol) { lp = lp_new; break; }
-        if (a < A.min_log_alpha) break;
-        lp = lp_new;
-        dlp = dlp_new;
-        kappa = fmin(kappa * 1.1, A.kappa_0);
-        if (acc_n % 5 == 0) kappa = kappa / 2.0;
-      } else {
-        kappa = kappa / 2.0;
-      }
+      if (ls.take(lp_new, dlp_new, A)) break;
     }
-    sdisp_eval<true>(C, a, pm, lane, lp_new, dlp_new, d2);
-    if (lane == 0) {
-      A.log_alpha[g] = a;
-      A.iter[g] = it;
-      A.iter_accept[g] = acc_n;
-      A.last_change[g] = change;
-      A.initial_lp[g] = initial_lp;
-      A.initial_dlp[g] = initial_dlp;
-      A.last_lp[g] = lp;
-      A.last_dlp[g] = dlp;
-      A.last_d2lp[g] = d2;
-    }
+    sdisp_eval<true>(C, ls.a, pm, lane, lp_new, dlp_new, d2);
+    if (lane == 0) ls.store(A, g, d2);
     __syncwarp();
   }
 }
@@ -704,7 +663,6 @@ __global__ void __launch_bounds__(MAXT, 1) fit_beta_seg_kernel(const BetaArgs A,
   double* rhs = S.v1;
   double* sc = S.v2;     // equilibration scales
   double* tmp = S.v3;
-  const double large = 30.0;
 
   for (;;) {
     unsigned int g = 0;
@@ -744,10 +702,9 @@ __global__ void __launch_bounds__(MAXT, 1) fit_beta_seg_kernel(const BetaArgs A,
       devc = warp_allreduce_sum(c);
     }
     sbeta_pass<false>(C, beta, alpha, r, log_alpha, lane);
-    double dev = 0.0, dev_old = 0.0;
-    double it = 0.0;
+    IrlsProgress ir;
     for (int t = 0; t < A.maxit; t++) {
-      it += 1.0;
+      ir.start_iteration();
       // normal equations (X'WX + Lambda) b = X'Wz, Jacobi-equilibrated Cholesky
       build_xtwx_pairs(C.D, C.P, S.WA, B, lane);
       if (lane < p) {
@@ -781,16 +738,12 @@ __global__ void __launch_bounds__(MAXT, 1) fit_beta_seg_kernel(const BetaArgs A,
       bool big = false;
       if (lane < p) {
         beta[lane] = rhs[lane] * sc[lane];
-        big = fabs(beta[lane]) > large;
+        big = fabs(beta[lane]) > kBetaLarge;
       }
       __syncwarp();
-      if (__any_sync(0xffffffffu, big)) { it = (double)A.maxit; break; }   // mu / eta stay those of the previous beta (:357-360)
+      if (__any_sync(0xffffffffu, big)) { ir.diverged(A.maxit); break; }   // mu / eta stay those of the previous beta
       const double dv = sbeta_pass<true>(C, beta, alpha, r, log_alpha, lane);
-      dev = -2.0 * (dv + devc);
-      const double conv_test = fabs(dev - dev_old) / (fabs(dev) + 0.1);
-      if (isnan(conv_test)) { it = (double)A.maxit; break; }
-      if ((t > 0) && (conv_test < A.tol)) break;
-      dev_old = dev;
+      if (ir.stop_after_pass(dv, devc, A)) break;
     }
     // ---- post-loop block (src/DESeq2.cpp:429-455): the W sums and eta belong to the last pass
     build_xtwx_pairs(C.D, C.P, S.WA, B, lane);
@@ -840,10 +793,10 @@ __global__ void __launch_bounds__(MAXT, 1) fit_beta_seg_kernel(const BetaArgs A,
     cd = warp_allreduce_sum(cd);
     cn = warp_allreduce_sum(cn);
     if (lane == 0) {
-      A.iter[g] = it;
+      A.iter[g] = ir.it;
       A.contrast_num[g] = cn;
       A.contrast_denom[g] = sqrt(cd);
-      A.deviance[g] = dev;
+      A.deviance[g] = ir.dev;
     }
     __syncwarp();
   }

@@ -1,7 +1,13 @@
 // layout.cu -- layout conversion between R's column-major n x m matrices (genes fastest; what
 // .Call hands over, /root/reference/src/DESeq2.cpp:165-169,285-287) and the engine's gene-major
 // rows (sample axis contiguous, row stride ld) that the warp-per-gene kernels read with 128-bit loads.
-// Plain tiled shared-memory transposes: both global sides are fully coalesced.
+// Plain tiled shared-memory transposes: both global sides are fully coalesced.  Also the device queries the launchers
+// share (SM count, persistent-grid size).
+#include <algorithm>
+#include <mutex>
+#include <utility>
+#include <vector>
+
 #include "engine.h"
 #include "nbmath.cuh"
 
@@ -132,6 +138,42 @@ int device_sm_count() {
     if (sms <= 0) sms = 132;   // H100 SXM
   }
   return sms;
+}
+
+cudaError_t persistent_grid(const void* kernel, int threads, size_t smem, int genes_per_cta, int n, unsigned* grid) {
+  struct Occupancy {
+    const void* kernel;
+    int threads;
+    size_t smem;
+    int ctas_per_sm;
+  };
+  static std::mutex mu;
+  static std::vector<Occupancy> cache;
+  static std::vector<std::pair<const void*, size_t>> smem_limit;   // the limit last set per kernel
+  std::lock_guard<std::mutex> lk(mu);
+  auto lim = std::find_if(smem_limit.begin(), smem_limit.end(), [&](const auto& l) { return l.first == kernel; });
+  if (lim == smem_limit.end() || lim->second != smem) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    if (lim == smem_limit.end()) smem_limit.emplace_back(kernel, smem);
+    else lim->second = smem;
+  }
+  auto hit = std::find_if(cache.begin(), cache.end(), [&](const Occupancy& o) {
+    return o.kernel == kernel && o.threads == threads && o.smem == smem;
+  });
+  if (hit == cache.end()) {
+    int c = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kernel, threads, smem);
+    if (e != cudaSuccess) return e;
+    if (c < 1) return cudaErrorLaunchOutOfResources;
+    cache.push_back({kernel, threads, smem, c});
+    hit = cache.end() - 1;
+  }
+  const long long want = ((long long)n + genes_per_cta - 1) / genes_per_cta;
+  long long g = (long long)device_sm_count() * hit->ctas_per_sm;
+  if (g > want) g = want;
+  *grid = (unsigned)(g < 1 ? 1 : g);
+  return cudaSuccess;
 }
 
 }  // namespace nb

@@ -260,26 +260,35 @@ __device__ __forceinline__ double trigamma_pos(double x) {
 }
 
 // ---------------------------------------------------------------- warp helpers
-__device__ __forceinline__ double warp_allreduce_sum(double v) {
+// xor-butterfly all-reduces inside aligned groups of GL lanes (GL = 32: the whole warp); every lane of a group ends
+// with the same bits
+template <int GL>
+__device__ __forceinline__ double group_allreduce_sum(double v) {
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  for (int o = GL / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
 
-__device__ __forceinline__ double warp_allreduce_max(double v) {
+template <int GL>
+__device__ __forceinline__ double group_allreduce_max(double v) {
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+  for (int o = GL / 2; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
 
-template <int N>
-__device__ __forceinline__ void warp_allreduce_sum_n(double (&v)[N]) {
+template <int N, int GL>
+__device__ __forceinline__ void group_allreduce_sum_n(double (&v)[N]) {
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
+  for (int o = GL / 2; o > 0; o >>= 1) {
 #pragma unroll
     for (int i = 0; i < N; i++) v[i] += __shfl_xor_sync(0xffffffffu, v[i], o);
   }
 }
+
+__device__ __forceinline__ double warp_allreduce_sum(double v) { return group_allreduce_sum<32>(v); }
+__device__ __forceinline__ double warp_allreduce_max(double v) { return group_allreduce_max<32>(v); }
+template <int N>
+__device__ __forceinline__ void warp_allreduce_sum_n(double (&v)[N]) { group_allreduce_sum_n<N, 32>(v); }
 
 // All-reduce of N per-lane partial sums, N a power of two <= 32, as a butterfly reduce-scatter followed by
 // an all-gather: log2(N) halving exchange rounds (N/2 + N/4 + ... + 1 values shuffled), plain butterflies for
