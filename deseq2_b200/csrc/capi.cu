@@ -1302,6 +1302,29 @@ int b200nb_cooks_dev(const void* y, int y_type, const double* mu, const double* 
   return 0;
 }
 
+int b200nb_beta_prior_quantile_dev(const double* beta_log2, int n, int p, const double* base_mean,
+                                   const double* disp_fit, const int32_t* col_a, const int32_t* col_b, int k,
+                                   double prob, double* out_q, void* stream) {
+  if (n < 1 || p < 1 || k < 0) return fail("bad dimensions n=%d p=%d k=%d", n, p, k);
+  if (!(prob > 0.0 && prob < 1.0)) return fail("prob=%g must lie in (0, 1)", prob);
+  if (k == 0) return 0;
+  // the column list is tiny (k <= a few hundred): fetch it once to check every index (one stream sync)
+  std::vector<int32_t> ca((size_t)k), cb((size_t)k);
+  CU(cudaMemcpyAsync(ca.data(), col_a, k * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  CU(cudaMemcpyAsync(cb.data(), col_b, k * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  CU(cudaStreamSynchronize((cudaStream_t)stream));
+  for (int c = 0; c < k; c++) {
+    if (ca[c] < 0 || ca[c] >= p) return fail("column %d: a=%d must lie in [0, %d)", c, ca[c], p);
+    if (cb[c] < -1 || cb[c] >= p) return fail("column %d: b=%d must lie in [-1, %d)", c, cb[c], p);
+  }
+  nb::BetaPriorQArgs a{};
+  a.beta = beta_log2; a.n = n; a.base_mean = base_mean; a.disp_fit = disp_fit; a.col_a = col_a; a.col_b = col_b;
+  a.k = k; a.prob = prob; a.out_q = out_q;
+  CU(nb::launch_beta_prior_quantile(a, (cudaStream_t)stream));
+  g_launches++;
+  return 0;
+}
+
 int b200nb_size_factors_dev(const void* y, int y_type, int poscounts, int n, int m, long long ld,
                             double* loggeomeans, double* scratch_gm, double* scratch_cm, double* size_factors,
                             int32_t* n_finite, void* stream) {

@@ -197,6 +197,20 @@ struct SizeFactorArgs {
 };
 cudaError_t launch_size_factors(const SizeFactorArgs& a, cudaStream_t stream);
 
+// estimateBetaPriorVar's weighted upper quantile (beta_prior.cuh, launched from size_factors.cu)
+struct BetaPriorQArgs {
+  const double* beta;          // n x p column-major, log2 scale
+  int n;
+  const double* base_mean;     // n
+  const double* disp_fit;      // n
+  const int32_t* col_a;        // k: column c = beta[:, a] - (b < 0 ? 0 : beta[:, b])
+  const int32_t* col_b;        // k
+  int k;
+  double prob;
+  double* out_q;               // k (out)
+};
+cudaError_t launch_beta_prior_quantile(const BetaPriorQArgs& a, cudaStream_t stream);
+
 // Cook's distances (pipeline_kernels.cu)
 struct CooksArgs {
   const void* y;

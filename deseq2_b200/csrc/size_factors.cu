@@ -11,7 +11,10 @@
 //   sf_median_kernel  one CTA per sample: exact median by a most-significant-byte-first radix select on the
 //                     order-preserving 64-bit image of the doubles (8 histogram passes + one pass for the upper
 //                     middle element when the count is even) -- no sort, no scratch beyond 256 shared counters.
+// The same one-CTA-per-column radix refinement computes estimateBetaPriorVar's weighted upper quantiles
+// (beta_prior_quantile_kernel, beta_prior.cuh); both kernels start through launch_per_column.
 #include "engine.h"
+#include "beta_prior.cuh"
 #include "nbmath.cuh"
 
 #include <math.h>
@@ -128,6 +131,13 @@ __global__ void __launch_bounds__(512) sf_median_kernel(const double* __restrict
   if (tid == 0) size_factors[blockIdx.x] = exp(med);
 }
 
+// One CTA per column with static shared memory only: the launch site of the column-select kernels of this file.
+template <class... P, class... A>
+cudaError_t launch_per_column(void (*kern)(P...), int columns, int threads, cudaStream_t stream, A... args) {
+  kern<<<columns, threads, 0, stream>>>(args...);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 cudaError_t launch_size_factors(const SizeFactorArgs& a, cudaStream_t stream) {
@@ -139,8 +149,12 @@ cudaError_t launch_size_factors(const SizeFactorArgs& a, cudaStream_t stream) {
   if (e != cudaSuccess) return e;
   e = launch_to_col_major(a.ratios, a.ratios_colmajor, a.n, a.m, a.ld, stream);
   if (e != cudaSuccess) return e;
-  sf_median_kernel<<<a.m, 512, 0, stream>>>(a.ratios_colmajor, a.n, a.size_factors);
-  return cudaGetLastError();
+  return launch_per_column(sf_median_kernel, a.m, 512, stream, a.ratios_colmajor, a.n, a.size_factors);
+}
+
+cudaError_t launch_beta_prior_quantile(const BetaPriorQArgs& a, cudaStream_t stream) {
+  if (a.k == 0) return cudaSuccess;
+  return launch_per_column(beta_prior_quantile_kernel, a.k, kBpThreads, stream, a);
 }
 
 }  // namespace nb

@@ -2,7 +2,7 @@
 device, only a handful of scalars ever reach the host.
 
 Same sequence as deseq2_b200/pipeline.py (the numpy restatement of R/core.R:280-432 with test="Wald",
-fitType="parametric", betaPrior=FALSE, no weights, no outlier replacement), but
+fitType="parametric", no weights, no outlier replacement; betaPrior=FALSE by default), but
   * the pre-steps (base mean/variance, rough + moments dispersion, linear-model mu, IRLS start values) are one
     CUDA kernel (b200nb_prep_dev, csrc/pipeline_kernels.cu),
   * the parametric dispersion-trend fit is one single-CTA kernel (b200nb_trend_fit_dev),
@@ -10,6 +10,10 @@ fitType="parametric", betaPrior=FALSE, no weights, no outlier replacement), but
   * the elementwise rules between them (noIncrease, convergence flags, clamps, outlier rule, MAD, Wald statistic
     and p-value) are a few torch tensor ops -- plumbing, not the product.
 This is SURVEY.md section 8(f) rows 2-3 (pre-steps and Wald statistics on device) layered on rows (a)-(e).
+DESeq_device(betaPrior=True, factors=...) runs the reference's betaPrior=TRUE Wald path for additive factor designs
+(fitGLMsWithPrior, R/fitNbinomGLMs.R:242-337): the MLE fit above, the prior variance of estimateBetaPriorVar
+("weighted": one launch of b200nb_beta_prior_quantile_dev, csrc/beta_prior.cuh, for all columns and level contrasts,
+then averagePriorsOverLevels in torch), and the MAP fit on the expanded model matrix.
 """
 from __future__ import annotations
 
@@ -146,6 +150,73 @@ def cooks(y, mu, hat, x, sizeFactors, want_matrix=True):
                             len(sizes), n, m, p, ld, _p(out["cooks"]), _p(out["maxCooks"]), _p(out["robustDisp"]),
                             _stream())
     _lib.check(rc, "cooks_dev")
+    return out
+
+
+def beta_prior_quantile(beta, baseMean, dispFit, col_a, col_b, prob):
+    """b200nb_beta_prior_quantile_dev: Hmisc.wtd.quantile(|x_c|, 1/(1/baseMean + dispFit), prob, normwt=TRUE) over the
+    entries with |x_c| < 10, for every column x_c = beta[a] - (b < 0 ? 0 : beta[b]).  beta: (p, n) contiguous device
+    tensor (log2 scale); col_a / col_b: integer sequences of equal length k.  Returns (k,) with NaN where no entry
+    is kept."""
+    L = _lib.lib()
+    dev = beta.device
+    p, n = beta.shape
+    ca = torch.as_tensor(np.asarray(col_a, dtype=np.int32), device=dev)
+    cb = torch.as_tensor(np.asarray(col_b, dtype=np.int32), device=dev)
+    out = torch.empty(ca.numel(), dtype=F64, device=dev)
+    _lib.check(L.b200nb_beta_prior_quantile_dev(_p(beta), n, p, _p(baseMean), _p(dispFit), _p(ca), _p(cb), ca.numel(),
+                                                float(prob), _p(out), _stream()), "beta_prior_quantile_dev")
+    return out
+
+
+def beta_prior_columns(fidx):
+    """The columns estimateBetaPriorVar takes quantiles of, for a standard factor design whose column c belongs to
+    factor fidx[c] (-1 = intercept): every non-intercept column, then addAllContrasts' differences of each factor's
+    level columns in R's is/js order (R/expanded.R:76-98).  Returns (col_a, col_b, factor of each column)."""
+    fidx = np.asarray(fidx)
+    a = [c for c in range(len(fidx)) if fidx[c] >= 0]
+    b = [-1] * len(a)
+    owner = [int(fidx[c]) for c in a]
+    for f in sorted({int(v) for v in fidx if v >= 0}):
+        cols = np.flatnonzero(fidx == f)
+        for j in range(len(cols) - 1):
+            for i in range(j + 1, len(cols)):
+                a.append(int(cols[i]))
+                b.append(int(cols[j]))
+                owner.append(f)
+    return np.asarray(a, np.int32), np.asarray(b, np.int32), np.asarray(owner)
+
+
+def estimate_beta_prior_var(betaMatrix, factors, baseMean, dispFit, upperQuantile=0.05):
+    """estimateBetaPriorVar (R/core.R:1601-1689, betaPriorMethod "weighted", expanded model matrix) on the device.
+    betaMatrix: (n, p) MLE log2 fold changes on the standard matrix factorDesign(factors)[0] (DESeq_device's
+    "betaMatrix"); baseMean / dispFit: (n,) device tensors.  The quantiles of all columns and contrasts are one kernel
+    launch; averagePriorsOverLevels (R/expanded.R:20-73) is a few torch ops.  Returns the prior variances of the
+    EXPANDED matrix's columns as a device tensor (1e6 for the intercept).  Raises ValueError like R when one of
+    them is NA or not positive (one host read)."""
+    from scipy import stats as _st
+    from .pipeline import factorDesign
+    _, _, fidx, _ = factorDesign(factors, expanded=False)
+    _, enames, efidx, _ = factorDesign(factors, expanded=True)
+    bt = betaMatrix.T.contiguous()                                      # (p, n): a view's base when it is one
+    dev = bt.device
+    col_a, col_b, owner = beta_prior_columns(fidx)
+    if bt.shape[1] > 1:
+        q = beta_prior_quantile(bt, baseMean, dispFit, col_a, col_b, 1.0 - upperQuantile)
+        z = float(_st.norm.ppf(1.0 - upperQuantile / 2.0))
+        pv = torch.where(torch.isnan(q), torch.full_like(q, 1e6), (q / z) ** 2)   # no kept entry: wide prior
+    else:                                                               # one gene: betaMatrix^2, no quantile
+        a = torch.as_tensor(col_a.astype(np.int64), device=dev)
+        b = torch.as_tensor(col_b.astype(np.int64), device=dev)
+        x = bt[a, 0] - torch.where(b >= 0, bt[b.clamp(min=0), 0], torch.zeros_like(bt[a, 0]))
+        pv = x ** 2
+    out = torch.full((len(efidx),), 1e6, dtype=F64, device=dev)
+    owner_d = torch.as_tensor(owner, device=dev)
+    for f in sorted({int(v) for v in efidx if v >= 0}):
+        out[torch.as_tensor(efidx == f, device=dev)] = pv[owner_d == f].mean()
+    bad = (torch.isnan(out) | (out <= 0)).cpu().numpy()
+    if bad.any():
+        raise ValueError("beta prior for " + ",".join(np.asarray(enames)[bad]) + " is NA or not greater than 0")
     return out
 
 
@@ -313,7 +384,8 @@ def _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp,
 
 
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
-                 outlierSD=2.0, minReplicatesForReplace=np.inf, allgather=None, useOptim=True):
+                 outlierSD=2.0, minReplicatesForReplace=np.inf, allgather=None, useOptim=True, betaPrior=False,
+                 factors=None):
     """y: gene-major (N, ld) device tensor of counts (int32 or float64).  Returns a dict of device tensors over the
     rows with a non-zero sum (`idx` maps them back to the N input rows) plus the trend / prior scalars.
     sizeFactors=None estimates them on the device first (median of ratios, R/core.R:535-578; returned under
@@ -324,10 +396,26 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     allgather: for the gene-sharded multi-GPU run (deseq2_b200/sharded.py::sharded_DESeq_device): a callable that
     concatenates each of a LIST of per-gene 1-D device tensors over the ranks, in rank order (one collective).  It is used at the one point where the
     reference needs every gene (R/parallel.R:25-28): the dispersion trend and the prior variance are then fitted,
-    identically on every rank, to all genes' baseMean / dispGeneEst instead of the shard's."""
+    identically on every rank, to all genes' baseMean / dispGeneEst instead of the shard's.  With betaPrior it is
+    called once more, for the MLE coefficients the prior variance is estimated from (R/parallel.R:39-40).
+    betaPrior=True: nbinomWaldTest with a zero-centred normal prior on the coefficients (fitGLMsWithPrior,
+    R/fitNbinomGLMs.R:242-337) for an additive factor design: `factors` are the level-code vectors of
+    pipeline.factorDesign and x must be factorDesign(factors)[0].  The dispersions and the MLE fit (whose mu / H give
+    Cook's distances) are on x; the prior variance comes from the MLE log2 fold changes (estimate_beta_prior_var) and
+    the reported coefficients, standard errors, Wald statistics and deviance from the MAP fit on the expanded matrix
+    factorDesign(factors, expanded=True)[0] with lambda = 1 / betaPriorVar.  Adds "mleBetaMatrix", "betaPriorVar" and
+    "modelMatrix" (the expanded matrix)."""
     dev = y.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
+    if betaPrior:
+        from .pipeline import factorDesign
+        if factors is None:
+            raise ValueError("betaPrior=True needs the design factors (factors=...)")
+        if not np.array_equal(x, factorDesign(factors)[0]):
+            raise ValueError("betaPrior=True: x must be the standard model matrix of the factors, factorDesign(factors)[0]")
+        if np.isfinite(minReplicatesForReplace):
+            raise ValueError("outlier replacement (finite minReplicatesForReplace) is not supported with betaPrior=True")
     estimated = sizeFactors is None
     if estimated:
         sizeFactors = size_factors(y, m)["sizeFactors"].cpu().numpy()
@@ -441,8 +529,13 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     betaConv, n_optim = _optim_fallback(ynz, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, minmu, ll,
                                         useOptim=useOptim)
     mark("loglik+optim")
-    betaMatrix = fb["beta_mat"] / LN2                      # (p, n)
-    betaSE = torch.sqrt(torch.clamp(fb["beta_var_mat"], min=0.0)) / LN2
+    fit, fit_ll, prior = fb, ll, {}
+    if betaPrior:
+        fit, fit_ll, betaConv, prior = _fit_with_prior(ynz, factors, sfd, dispersion, fb, bm, bm_all, tr, allgather,
+                                                       betaTol, maxit, minmu, useOptim)
+        mark("beta_prior_var+fit_beta_map")
+    betaMatrix = fit["beta_mat"] / LN2                     # (p, n)
+    betaSE = torch.sqrt(torch.clamp(fit["beta_var_mat"], min=0.0)) / LN2
     stat = betaMatrix / betaSE
     pval = 2.0 * torch.special.ndtr(-stat.abs())
     from .pipeline import nOrMoreInCell
@@ -453,15 +546,49 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     res = {"stage_ms": stage_ms, "maxCooks": ck["maxCooks"], "idx": idx, "baseMean": bm, "dispGeneEst": dge, "dispFit": dispFit, "dispMAP": dispMAP,
             "dispersion": dispersion, "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": rm["iter"],
             "betaMatrix": betaMatrix.T, "betaSE": betaSE.T, "WaldStatistic": stat.T, "WaldPvalue": pval.T,
-            "betaIter": fb["iter"], "betaConv": betaConv, "n_optim": n_optim, "deviance": -2.0 * ll["logLike"], "mu": mu_cooks,
+            "betaIter": fit["iter"], "betaConv": betaConv, "n_optim": n_optim, "deviance": -2.0 * fit_ll["logLike"], "mu": mu_cooks,
             "H": fb["hat_diagonals"], "trendCoefs": tr[:2], "varLogDispEsts": varLogDispEsts,
             "dispPriorVar": dispPriorVar, "n_refit_geneest": n_refit_geneest, "n_refit_map": int(gi2.numel()),
             "n_input_rows": y.shape[0], "sizeFactors": np.asarray(sizeFactors, dtype=np.float64)}
+    res.update(prior)
     if do_replace and m > p:
         _replace_and_refit(res, ynz, ck["cooks"], x, sizeFactors, sfd, tr, varLogDispEsts, dispPriorVar,
                            minReplicatesForReplace, minDisp, kappa_0, dispTol, maxit, betaTol, minmu, outlierSD,
                            useOptim=useOptim)
     return res
+
+
+def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, tr, allgather, betaTol, maxit, minmu, useOptim):
+    """The betaPrior half of fitGLMsWithPrior (R/fitNbinomGLMs.R:242-337) after the MLE fit `mle`: prior variance
+    over all genes, then the MAP fit on the expanded matrix, its log-likelihood and the optim fallback with the same
+    lambda.  Returns (fit, loglik, betaConv, extra result entries)."""
+    from .pipeline import factorDesign
+    dev = ynz.device
+    p = mle["beta_mat"].shape[0]
+    mleBeta = mle["beta_mat"] / LN2                                     # (p, n), log2 scale
+    if allgather is not None:
+        # ONE packed collective: the p - 1 non-intercept MLE columns of every gene; the intercept's prior is fixed
+        g = allgather([mleBeta[k] for k in range(1, p)])
+        beta_all = torch.stack([torch.zeros_like(g[0])] + list(g))
+    else:
+        beta_all = mleBeta
+    pv = estimate_beta_prior_var(beta_all.T, factors, bm_all, tr[0] + tr[1] / bm_all)
+    x_exp = factorDesign(factors, expanded=True)[0]
+    pe = x_exp.shape[1]
+    xe = D.x_to_device(x_exp, dev)
+    lam = 1.0 / (LN2 ** 2 * pv)
+    contrast = torch.zeros(pe, dtype=F64, device=dev)
+    contrast[0] = 1.0
+    # the expanded matrix is rank deficient: start at (log baseMean, 0, ..., 0) (R/fitNbinomGLMs.R:146-151)
+    beta0 = torch.zeros((pe, ynz.shape[0]), dtype=F64, device=dev)
+    beta0[0] = torch.log(bm)
+    fit = D.fit_beta(ynz, xe, sfd, dispersion, contrast, beta0, lam, betaTol, maxit, minmu=minmu, want_hat=False,
+                     want_mu=False)
+    ll = D.nb_loglik(ynz, xe, sfd, dispersion, fit["beta_mat"], want_mu=False)
+    betaConv, n_optim = _optim_fallback(ynz, xe, sfd, dispersion, fit, beta0, lam, contrast, maxit, minmu, ll,
+                                        useOptim=useOptim)
+    return fit, ll, betaConv, {"mleBetaMatrix": mleBeta.T, "betaPriorVar": pv.cpu().numpy(), "modelMatrix": x_exp,
+                               "n_optim_map": n_optim}
 
 
 def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, varLogDispEsts, dispPriorVar, minReplicates, minDisp,

@@ -20,7 +20,7 @@ numpy, one function per R function, same names, so the engine can be driven and 
   robustMethodOfMomentsDisp / trimmedCellVariance / calculateCooksDistance / recordMaxCooks   R/core.R:2277-2359
   fitGLMsWithPrior / estimateBetaPriorVar / Hmisc.wtd.quantile / addAllContrasts / averagePriorsOverLevels /
   makeExpandedModelMatrix (additive factor designs)   R/fitNbinomGLMs.R:242-337, R/core.R:1601-1689, 2762-2803, R/expanded.R
-  DESeq                          R/core.R:280-432    (test="Wald", fitType="parametric", betaPrior=FALSE)
+  DESeq                          R/core.R:280-432    (test="Wald", fitType="parametric", betaPrior=FALSE or TRUE)
 
 `engine` is any object with fitDisp / fitDispGrid / fitBeta taking the reference's argument names
 (deseq2_b200.wrappers is the product engine and the default; tests and the bench's CPU baseline pass the
@@ -658,6 +658,8 @@ def estimateBetaPriorVar(betaMatrix, names, fidx, baseMean, dispFit, expandedTyp
                     colsets.append((f"f{f}Cntrst", M[:, i] - M[:, j], f))
 
     def one(x):
+        if len(x) == 1:                             # a single gene: betaMatrix^2, no quantile (R/core.R:1648-1666)
+            return float(x[0] ** 2)
         fin = np.abs(x) < 10
         if fin.sum() == 0:
             return 1e6
@@ -674,35 +676,47 @@ def estimateBetaPriorVar(betaMatrix, names, fidx, baseMean, dispFit, expandedTyp
 
 
 def fitGLMsWithPrior(counts, nf, factors, dispersion, baseMean, dispFit, engine=None, betaTol=1e-8, maxit=100,
-                     useQR=True, minmu=0.5):
+                     useQR=True, minmu=0.5, useOptim=True):
     """R/fitNbinomGLMs.R:242-337 for an additive factor design with the expanded model matrix (the default when
     betaPrior=TRUE): MLE fit on the standard matrix -> estimateBetaPriorVar -> MAP fit on the expanded matrix with
-    lambda = 1 / betaPriorVar."""
+    lambda = 1 / betaPriorVar.  useOptim goes to both fits (fitNbinomGLMs)."""
     x_std, names, fidx, _ = factorDesign(factors, expanded=False)
     mle = fitNbinomGLMs(counts, nf, x_std, dispersion, engine=engine, betaTol=betaTol, maxit=maxit, useQR=useQR,
-                        minmu=minmu)
+                        minmu=minmu, useOptim=useOptim)
     _, mean_by_factor = estimateBetaPriorVar(mle["betaMatrix"], names, fidx, baseMean, dispFit, expandedType=True)
     x_exp, enames, efidx, _ = factorDesign(factors, expanded=True)
     betaPriorVar = np.array([1e6 if f < 0 else mean_by_factor[int(f)] for f in efidx])
     if np.any(betaPriorVar == 0):
         raise ValueError("beta prior variances are equal to zero for some variables")
     fit = fitNbinomGLMs(counts, nf, x_exp, dispersion, lambda_=1.0 / betaPriorVar, engine=engine, betaTol=betaTol,
-                        maxit=maxit, useQR=useQR, minmu=minmu)
+                        maxit=maxit, useQR=useQR, minmu=minmu, useOptim=useOptim)
     return {"fit": fit, "H": mle["hat_diagonals"], "mu": mle["mu"], "betaPriorVar": betaPriorVar,
             "modelMatrix": x_exp, "mleBetaMatrix": mle["betaMatrix"], "names": enames, "mle": mle}
 
 
-def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.inf, useOptim=True):
-    """R/core.R:280-432 with test='Wald', fitType='parametric', betaPrior=FALSE.
+def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.inf, useOptim=True, betaPrior=False,
+          factors=None):
+    """R/core.R:280-432 with test='Wald', fitType='parametric', betaPrior=FALSE by default.
     minReplicatesForReplace: the reference's default is 7 (outlier replacement + refit whenever a design cell has >= 7
     samples, R/core.R:419-426, refitWithoutOutliers :2484-2565); the default here is Inf = off, which is what the
     engine parity tests and bench.py's `full_pipeline` exercise.  With a finite value the result also carries
     `replace` (genes refitted), `replaceable` (samples) and `replaceCounts`.
+    betaPrior=True (additive factor designs only; x must be factorDesign(factors)[0], no outlier replacement): the
+    Wald test goes through fitGLMsWithPrior -- coefficients, SEs, statistics and deviance of the MAP fit on the
+    expanded matrix, Cook's distances from the MLE fit -- and the result also carries `mleBetaMatrix`,
+    `betaPriorVar` and `modelMatrix` (the expanded matrix).
     Returns per-gene vectors over ALL rows; all-zero rows carry NaN (buildDataFrameWithNARows, R/core.R:2232)."""
     engine = engine or _default_engine
     counts = np.asarray(counts)
     N, m = counts.shape
     p = x.shape[1]
+    if betaPrior:
+        if factors is None:
+            raise ValueError("betaPrior=True needs the design factors (factors=...)")
+        if not np.array_equal(np.asarray(x, dtype=np.float64), factorDesign(factors)[0]):
+            raise ValueError("betaPrior=True: x must be the standard model matrix of the factors, factorDesign(factors)[0]")
+        if np.isfinite(minReplicatesForReplace):
+            raise ValueError("outlier replacement (finite minReplicatesForReplace) is not supported with betaPrior=True")
     if sizeFactors is None:
         sizeFactors = estimateSizeFactorsForMatrix(counts)
     mvAll = getBaseMeansAndVariances(counts, sizeFactors)
@@ -715,15 +729,28 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     mp = estimateDispersionsMAP(cnz, x, ge["mu"], ge["dispGeneEst"], tf["dispFit"], dispPriorVar,
                                 tf["varLogDispEsts"], engine=engine)
     nf = np.broadcast_to(sizeFactors[None, :], cnz.shape)
-    wt = nbinomWaldTest(cnz, nf, x, mp["dispersion"], engine=engine, useOptim=useOptim)
-    cooks = calculateCooksDistance(cnz, wt["mu"], wt["hat_diagonals"], sizeFactors, x)      # R/core.R:1457-1460
+    prior = {}
+    if betaPrior:
+        gp = fitGLMsWithPrior(cnz, nf, factors, mp["dispersion"], mv["baseMean"], tf["dispFit"], engine=engine,
+                              useOptim=useOptim)
+        wt = dict(gp["fit"])
+        with np.errstate(divide="ignore", invalid="ignore"):
+            wt["WaldStatistic"] = wt["betaMatrix"] / wt["betaSE"]
+        wt.update(WaldPvalue=2.0 * _sp.ndtr(-np.abs(wt["WaldStatistic"])), deviance=-2.0 * wt["logLike"])
+        cooks = calculateCooksDistance(cnz, gp["mu"], gp["H"], sizeFactors, x)             # MLE mu / H (R/core.R:1416-1460)
+        prior = {"betaPriorVar": gp["betaPriorVar"], "modelMatrix": gp["modelMatrix"]}
+    else:
+        wt = nbinomWaldTest(cnz, nf, x, mp["dispersion"], engine=engine, useOptim=useOptim)
+        cooks = calculateCooksDistance(cnz, wt["mu"], wt["hat_diagonals"], sizeFactors, x)  # R/core.R:1457-1460
     per_gene = {"baseMean": mv["baseMean"], "dispGeneEst": ge["dispGeneEst"], "dispFit": tf["dispFit"],
                 "dispMAP": mp["dispMAP"], "dispersion": mp["dispersion"], "dispOutlier": mp["dispOutlier"].astype(float),
                 "betaMatrix": wt["betaMatrix"], "betaSE": wt["betaSE"], "WaldStatistic": wt["WaldStatistic"],
                 "WaldPvalue": wt["WaldPvalue"], "betaConv": wt["betaConv"].astype(float), "betaIter": wt["betaIter"],
                 "deviance": wt["deviance"], "dispGeneIter": ge["dispGeneIter"].astype(float),
                 "dispIter": mp["dispIter"].astype(float), "maxCooks": recordMaxCooks(x, cooks)}
-    extra = {}
+    if betaPrior:
+        per_gene["mleBetaMatrix"] = gp["mleBetaMatrix"]
+    extra = dict(prior)
     if np.isfinite(minReplicatesForReplace) and nOrMoreInCell(x, minReplicatesForReplace).any():
         # ---- refitWithoutOutliers (R/core.R:2484-2565) on the rows that had a count replaced
         newc, replace, replaceable = replaceOutliers(cnz, cooks, sizeFactors, x, minReplicates=minReplicatesForReplace)

@@ -134,7 +134,10 @@ def sharded_DESeq_device(y_local, x, sizeFactors, **kw):
     issues TWO per-gene collectives: one packed all-gather of (baseMean, dispGeneEst) for the global step and ONE packed
     all-gather of the results (dispersion, betaMatrix, betaSE, WaldPvalue: 1 + 3p doubles per gene), plus an 8-byte
     all-reduce that agrees on the buffer size; the n x m matrices never leave their shard.  Returns the shard's result
-    dict (device tensors) plus "gathered": the results of ALL genes on every rank, in rank order, and "collectives"."""
+    dict (device tensors) plus "gathered": the results of ALL genes on every rank, in rank order, and "collectives".
+    betaPrior=True, factors=... (passed on to DESeq_device): the prior variance is estimated over all genes
+    (R/parallel.R:39-40) through ONE more packed all-gather of the p - 1 non-intercept MLE columns; the gathered
+    results then carry the expanded matrix's columns."""
     from . import device_pipeline as DP
     pg = PackedGather(y_local.shape[0], y_local.device)
     res = DP.DESeq_device(y_local, x, sizeFactors, allgather=pg, **kw)

@@ -154,6 +154,17 @@ int b200nb_size_factors_dev(const void* y, int y_type, int poscounts, int n, int
                             double* loggeomeans, double* scratch_gm, double* scratch_cm, double* size_factors,
                             int32_t* n_finite, void* stream);
 
+/* b200nb_beta_prior_quantile_dev: the weighted upper quantile of estimateBetaPriorVar (betaPriorMethod "weighted",
+ * R/core.R:1601-1689, 2416-2419; Hmisc.wtd.quantile with normwt = TRUE, :2762-2900).  For each of the k columns
+ * x_c = beta[:, a] - (b < 0 ? 0 : beta[:, b]) (col_a / col_b are device ints; b >= 0 gives addAllContrasts'
+ * differences, R/expanded.R:76-98) out_q[c] = wtd.quantile(|x_c|, w, prob) over the entries with |x_c| < 10 and a
+ * weight w = 1/(1/base_mean + disp_fit) that is neither NaN nor 0; NaN when no entry is kept.  beta_log2 is n x p
+ * column-major (log2 scale).  Deterministic: two calls on the same input give the same bits.  Needs n >= 1, p >= 1,
+ * k >= 0, 0 <= a < p, -1 <= b < p, 0 < prob < 1 (the indices are fetched to the host once to check them). */
+int b200nb_beta_prior_quantile_dev(const double* beta_log2, int n, int p, const double* base_mean,
+                                   const double* disp_fit, const int32_t* col_a, const int32_t* col_b, int k,
+                                   double prob, double* out_q, void* stream);
+
 /* ---- housekeeping */
 const char* b200nb_last_error(void);
 int b200nb_device_count(void);            /* number of visible CUDA devices (0 if none / no driver) */
