@@ -47,6 +47,8 @@ SIGNATURES = {
     "b200nb_to_gene_major_dev": [vp, vp, _I, _I, _LL, _I, vp],
     "b200nb_to_col_major_dev": [vp, vp, _I, _I, _LL, vp],
     "b200nb_prep_dev": [vp, _I, vp, vp, vp, _D, _D, _D, _D, _I, _I, _I, _LL, vp, vp, vp, vp, vp, vp, vp],
+    "b200nb_prep_weighted_dev": [vp, _I, vp, vp, vp, _D, _D, _D, _D, _I, _I, _I, _LL, vp, vp, vp, vp, vp, vp, vp, _D,
+                                 vp, vp, vp, vp],
     "b200nb_trend_fit_dev": [vp, vp, _I, _D, vp, vp],
     "b200nb_cooks_dev": [vp, _I, vp, vp, vp, vp, vp, _I, _I, _I, _I, _LL, vp, vp, vp, vp],
     "b200nb_size_factors_dev": [vp, _I, _I, _I, _I, _LL, vp, vp, vp, vp, vp, vp],

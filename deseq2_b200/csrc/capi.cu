@@ -1245,29 +1245,65 @@ int b200nb_to_col_major_dev(const double* src, double* dst, int n, int m, long l
   return 0;
 }
 
-int b200nb_prep_dev(const void* y, int y_type, const double* x, const double* proj, const double* size_factors,
-                    double xim, double min_disp, double max_disp, double minmu, int n, int m, int p, long long ld,
-                    double* base_mean, double* base_var, int32_t* all_zero, double* alpha0, double* mu_lin,
-                    double* beta0, void* stream) {
+static int prep_args(nb::PrepArgs& a, const void* y, int y_type, const double* x, const double* proj,
+                     const double* size_factors, double xim, double min_disp, double max_disp, double minmu, int n,
+                     int m, int p, long long ld, double* base_mean, double* base_var, int32_t* all_zero,
+                     double* alpha0, double* mu_lin, double* beta0) {
   if (check_dims(n, m, p)) return 1;
   if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
   if (m <= p) return fail("prep needs m > p (m=%d, p=%d)", m, p);
-  nb::PrepArgs a{};
+  a = nb::PrepArgs{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.x = x; a.proj = proj; a.size_factors = size_factors; a.xim = xim;
   a.min_disp = min_disp; a.max_disp = max_disp; a.minmu = minmu; a.n = n; a.m = m; a.p = p; a.ld = ld;
   a.base_mean = base_mean; a.base_var = base_var; a.all_zero = all_zero; a.alpha0 = alpha0; a.mu_lin = mu_lin;
   a.beta0 = beta0;
   a.gid = nullptr; a.xg = nullptr; a.G = 0;
+  return 0;
+}
+
+static int prep_launch(nb::PrepArgs& a, void* stream) {
   const char* pg = getenv("B200NB_PREP_GROUPED");   // "0": always the streaming kernel (A/B switch, read per call)
-  if (n > 0 && (long long)m * p >= 1024 && !(pg && pg[0] == '0')) {
+  if (a.n > 0 && (long long)a.m * a.p >= 1024 && !(pg && pg[0] == '0')) {
     // long rows: a design with few distinct rows is handled per group (this fetches the m x p design: one stream sync)
     DesignDev dd;
-    if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
+    if (prepare_design_from_device(a.x, a.m, a.p, (cudaStream_t)stream, &dd)) return 1;
     if (dd.grouped) { a.gid = dd.gid; a.xg = dd.xg; a.G = dd.G; }
   }
   CU(nb::launch_prep(a, (cudaStream_t)stream));
-  if (n > 0) g_launches++;
+  if (a.n > 0) g_launches++;
   return 0;
+}
+
+int b200nb_prep_dev(const void* y, int y_type, const double* x, const double* proj, const double* size_factors,
+                    double xim, double min_disp, double max_disp, double minmu, int n, int m, int p, long long ld,
+                    double* base_mean, double* base_var, int32_t* all_zero, double* alpha0, double* mu_lin,
+                    double* beta0, void* stream) {
+  nb::PrepArgs a;
+  if (prep_args(a, y, y_type, x, proj, size_factors, xim, min_disp, max_disp, minmu, n, m, p, ld, base_mean, base_var,
+                all_zero, alpha0, mu_lin, beta0))
+    return 1;
+  return prep_launch(a, stream);
+}
+
+int b200nb_prep_weighted_dev(const void* y, int y_type, const double* x, const double* proj,
+                             const double* size_factors, double xim, double min_disp, double max_disp, double minmu,
+                             int n, int m, int p, long long ld, double* base_mean, double* base_var,
+                             int32_t* all_zero, double* alpha0, double* mu_lin, double* beta0, const double* weights,
+                             double weight_threshold, double* out_weights_norm, int32_t* out_weights_fail,
+                             int32_t* out_status, void* stream) {
+  nb::PrepArgs a;
+  if (prep_args(a, y, y_type, x, proj, size_factors, xim, min_disp, max_disp, minmu, n, m, p, ld, base_mean, base_var,
+                all_zero, alpha0, mu_lin, beta0))
+    return 1;
+  if (p > 32) return fail("weighted prep supports p <= 32 (p=%d)", p);
+  if (n > 0 && (weights == nullptr || out_weights_norm == nullptr || out_weights_fail == nullptr ||
+                out_status == nullptr))
+    return fail("weighted prep needs weights, out_weights_norm, out_weights_fail and out_status");
+  if (!(weight_threshold >= 0.0)) return fail("weight_threshold must be >= 0");
+  a.weights = weights; a.weight_threshold = weight_threshold; a.weights_norm = out_weights_norm;
+  a.weights_fail = out_weights_fail; a.status = out_status;
+  if (n > 0) CU(cudaMemsetAsync(out_status, 0, sizeof(int32_t), (cudaStream_t)stream));
+  return prep_launch(a, stream);
 }
 
 int b200nb_trend_fit_dev(const double* means, const double* disps, int n, double min_disp, double* out4,

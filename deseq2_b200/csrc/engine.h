@@ -179,6 +179,14 @@ struct PrepArgs {
   const int* gid;              // m: design group of sample j
   const double* xg;            // G x (p|1): the distinct design rows
   int G;
+  // observation weights (b200nb_prep_weighted_dev; the unweighted kernels never read these).  base_mean / base_var
+  // are then of w * K/s with the RAW weights; rough dispersion, mu_lin and beta0 stay unweighted.
+  const double* weights;       // gene-major n x ld, raw assay weights
+  double weight_threshold;     // rank test 2 keeps the samples with normalised weight > this
+  double* weights_norm;        // gene-major n x ld: weights / row maximum (padding columns written as 0)
+  int32_t* weights_fail;       // n: 1 = a rank test of getAndCheckWeights fails
+  int32_t* status;             // 1 int, incremented once per row with a negative / NaN / infinite weight or no
+                               // positive weight (the reference stops on each of these)
 };
 cudaError_t launch_prep(const PrepArgs& a, cudaStream_t stream);
 

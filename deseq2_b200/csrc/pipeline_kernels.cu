@@ -10,6 +10,14 @@
 //   parametricDispersionFit   R/core.R:2166-2189      Gamma GLM (identity link) disp ~ a0 + a1/mean, iterated trimming
 // prep_kernel: one warp per gene; the projection P = (X'X)^-1 X' (p x m) is computed once on the host.
 // trend_fit_kernel: ONE CTA runs the whole iteratively re-trimmed IRLS on the device (no host round trips).
+// With observation weights (template flag W, b200nb_prep_weighted_dev) the same read of the count row also reads the
+// raw weight row and adds, from getAndCheckWeights (R/core.R:2697-2752) and the weighted getBaseMeansAndVariances:
+//   baseMean / baseVar of w * K/s with the RAW weights (R/core.R:2140-2145); moments dispersion from this pair,
+//   rough dispersion and the start values unweighted as in the reference;
+//   weights / rowmax(weights) written to an n x ld matrix; rows with a negative / NaN / infinite weight or no positive
+//   weight counted into a status word (the reference stops on them: stopifnot, then qr() on NaN);
+//   weightsFail = !(rank(w * X) == p && rank(X[w > threshold, nonzero columns]) == ncol), R's qr() rank (LINPACK
+//   dqrdc2, tol 1e-7) decided from the two p x p Gram matrices (gram_full_rank).
 #include <mutex>
 
 #include "engine.h"
@@ -18,36 +26,98 @@
 namespace nb {
 namespace {
 
+// Whether R's qr(Z)$rank equals the number of active columns of Z, decided from the Gram matrix A = Z'Z alone (p x p
+// row-major in this warp's shared memory, p <= 32; overwritten).  `active`: bit k = column k of Z takes part (the
+// rest are left out, as R drops all-zero columns before its second test); nrows: the number of rows of Z.
+// dqrdc2 walks the columns in order and moves a column to the end when its norm after the Householder steps so far is
+// below tol = 1e-7 times its original norm (1 for a zero column); the rank is then (columns - moved), at most nrows.
+// So the rank is full exactly when nrows >= columns and no column is moved.  The squared norm of column c left after
+// the steps for the columns before it is the Schur-complement diagonal of A, so an unpivoted elimination that compares
+// each diagonal with tol^2 times the original one makes the same decision in exact arithmetic.  In floating point it
+// can differ from dqrdc2 only at knife edges: a squared norm ratio within a few dozen ulps of tol^2 (dqrdc2 also
+// downdates its column norms instead of recomputing them).
+__device__ bool gram_full_rank(double* A, int p, int nrows, unsigned active, int lane) {
+  if (nrows < __popc(active)) return false;
+  const double tol = 1e-7;
+  const double orig = (lane < p) ? A[lane * p + lane] : 0.0;
+  for (int c = 0; c < p; c++) {
+    if (!((active >> c) & 1u)) continue;
+    const double d = A[c * p + c];
+    const double oc = __shfl_sync(0xffffffffu, orig, c);
+    if (!(d >= tol * tol * (oc == 0.0 ? 1.0 : oc))) return false;   // moved to the end: rank < columns (NaN too)
+    if (lane > c && lane < p && ((active >> lane) & 1u)) {
+      const double f = A[lane * p + c] / d;
+      for (int k = c + 1; k < p; k++)
+        if ((active >> k) & 1u) A[lane * p + k] = fma(-f, A[c * p + k], A[lane * p + k]);
+    }
+    __syncwarp();
+  }
+  return true;
+}
+
+// the columns of a Gram matrix with a non-zero diagonal (R: mm.sub[, colSums(abs(mm.sub)) > 0])
+__device__ __forceinline__ unsigned gram_nonzero_columns(const double* A, int p, int lane) {
+  return __ballot_sync(0xffffffffu, lane < p && A[lane * p + lane] > 0.0);
+}
+
+// per-warp shared-memory doubles the weighted kernels add after the unweighted layout (0 for W = false)
+template <bool W>
+__host__ __device__ __forceinline__ size_t prep_weighted_extra(int mpad, int p, bool grouped) {
+  if constexpr (W) return grouped ? (size_t)p * p + 64 : (size_t)mpad + 2 * (size_t)p * p;
+  else return 0;
+}
+
+// the per-gene outputs of the weighted variant (lane 0)
+__device__ __forceinline__ void store_weight_flags(const PrepArgs& A, int g, bool invalid, bool ok) {
+  A.weights_fail[g] = ok ? 0 : 1;
+  if (invalid) atomicAdd(A.status, 1);
+}
+
+template <bool W>
 __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
   extern __shared__ __align__(16) double smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int mpad = (A.m + 3) & ~3;
   double* sf = smem;                                   // mpad
-  double* wrow = smem + mpad + (size_t)warp * (2 * mpad + 64);
+  double* wrow = smem + mpad + (size_t)warp * (2 * mpad + 64 + prep_weighted_extra<W>(mpad, A.p, false));
   double* vn = wrow;                                   // normalised counts
   double* vl = wrow + mpad;                            // log(norm + 0.1)
   double* coef = wrow + 2 * mpad;                      // 32: P * norm
   double* coefl = coef + 32;                           // 32: P * log(norm + .1)
+  double* wn = coefl + 32;                             // W: mpad, the weights (raw, then normalised)
+  double* gram = wn + mpad;                            // W: 2 p x p Gram matrices
   for (int j = threadIdx.x; j < A.m; j += blockDim.x) sf[j] = A.size_factors[j];
   __syncthreads();
   const int g = blockIdx.x * (blockDim.x >> 5) + warp;
   if (g >= A.n) return;
   const size_t off = (size_t)g * A.ld;
   double s = 0.0, s2 = 0.0, raw = 0.0;
+  double wmax = 0.0;
+  bool bad = false;
   for (int j = lane; j < A.m; j += 32) {
     const double y = A.y_is_f64 ? static_cast<const double*>(A.y)[off + j] : (double)static_cast<const int32_t*>(A.y)[off + j];
     const double v = y / sf[j];
     vn[j] = v;
     vl[j] = log(v + 0.1);
-    s += v;
+    if constexpr (W) {
+      const double w = A.weights[off + j];
+      wn[j] = w;
+      s += w * v;
+      wmax = fmax(wmax, w);
+      bad = bad || !(w >= 0.0);
+    } else {
+      s += v;
+    }
     raw += y;
   }
   s = warp_allreduce_sum(s);
   raw = warp_allreduce_sum(raw);
   const double bm = s / (double)A.m;
   for (int j = lane; j < A.m; j += 32) {
-    const double d = vn[j] - bm;
+    double d;
+    if constexpr (W) d = wn[j] * vn[j] - bm;
+    else d = vn[j] - bm;
     s2 = fma(d, d, s2);
   }
   s2 = warp_allreduce_sum(s2);
@@ -82,6 +152,46 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
     if (A.mu_lin != nullptr) A.mu_lin[off + j] = fmax(f * sf[j], A.minmu);
   }
   rs = warp_allreduce_sum(rs);
+  bool invalid = false, ok = true;
+  if constexpr (W) {
+    // normalise by the row maximum, then the Gram matrices of w * X and of X on the samples with w > threshold
+    wmax = warp_allreduce_max(wmax);
+    invalid = __any_sync(0xffffffffu, bad) || !(wmax > 0.0) || !(wmax < INFINITY);
+    double kept = 0.0;
+    for (int j = lane; j < A.m; j += 32) {
+      const double w = wn[j] / wmax;
+      wn[j] = w;
+      A.weights_norm[off + j] = w;
+      kept += (w > A.weight_threshold) ? 1.0 : 0.0;
+    }
+    for (int j = A.m + lane; j < A.ld; j += 32) A.weights_norm[off + j] = 0.0;
+    kept = warp_allreduce_sum(kept);
+    __syncwarp();
+    const int p = A.p;
+    double* g1 = gram;
+    double* g2 = gram + p * p;
+    for (int a = 0; a < p; a++) {
+      for (int b = a; b < p; b++) {
+        double t1 = 0.0, t2 = 0.0;
+        for (int j = lane; j < A.m; j += 32) {
+          const double xx = __ldg(A.x + (size_t)a * A.m + j) * __ldg(A.x + (size_t)b * A.m + j);
+          const double w = wn[j];
+          t1 = fma(w * w, xx, t1);
+          if (w > A.weight_threshold) t2 += xx;
+        }
+        t1 = warp_allreduce_sum(t1);
+        t2 = warp_allreduce_sum(t2);
+        if (lane == 0) {
+          g1[a * p + b] = g1[b * p + a] = t1;
+          g2[a * p + b] = g2[b * p + a] = t2;
+        }
+      }
+    }
+    __syncwarp();
+    const unsigned act2 = gram_nonzero_columns(g2, p, lane);
+    ok = gram_full_rank(g1, p, A.m, (p == 32) ? 0xffffffffu : ((1u << p) - 1u), lane);
+    ok = gram_full_rank(g2, p, (int)kept, act2, lane) && ok;
+  }
   if (lane == 0) {
     const double rough = fmax(rs / (double)(A.m - A.p), 0.0);
     const double moments = (bv - A.xim * bm) / (bm * bm);
@@ -91,6 +201,7 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
     A.base_var[g] = bv;
     A.alpha0[g] = a0;
     A.all_zero[g] = (raw == 0.0) ? 1 : 0;
+    if constexpr (W) store_weight_flags(A, g, invalid, ok);
   }
 }
 
@@ -98,6 +209,7 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
 // prep_kernel streams the p x m projection and the m x p design through every gene (2 p m loads and FMAs per gene,
 // L2 latency bound at 8 warps per SM); here a sample only adds its value and its log to its
 // group's lane-private slot, the projection is applied to the G group sums and the fitted value is read per group.
+template <bool W>
 __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int mpad, int ps) {
   extern __shared__ __align__(16) double smem[];
   const int lane = threadIdx.x & 31;
@@ -108,7 +220,8 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
   double* xg = Pg + (size_t)p * G;                     // G x ps
   int* rep = reinterpret_cast<int*>(xg + (size_t)G * ps);          // 32: one sample of each group
   unsigned char* gidb = reinterpret_cast<unsigned char*>(rep + 32);   // mpad
-  double* wrow = reinterpret_cast<double*>(gidb + mpad) + (size_t)warp * (mpad + 2 * (size_t)G * 32 + 3 * 32 + 2 * 32);
+  double* wrow = reinterpret_cast<double*>(gidb + mpad) +
+                 (size_t)warp * (mpad + 2 * (size_t)G * 32 + 3 * 32 + 2 * 32 + prep_weighted_extra<W>(mpad, p, true));
   double* vn = wrow;                                   // normalised counts
   double* accN = wrow + mpad;                          // G x 32 lane-private sums of the normalised counts
   double* accL = accN + (size_t)G * 32;                // G x 32: of log(norm + 0.1)
@@ -117,6 +230,9 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
   double* fit = gsL + 32;                              // 32: fitted value of each group
   double* coef = fit + 32;                             // 32: P * norm
   double* coefl = coef + 32;                           // 32: P * log(norm + .1)
+  double* gsW = coefl + 32;                            // W, 32: group sums of the squared normalised weights
+  double* gsC = gsW + 32;                              // W, 32: group counts of normalised weights > threshold
+  double* gram = gsC + 32;                             // W: p x p Gram matrix
   for (int j = threadIdx.x; j < A.m; j += blockDim.x) {
     sf[j] = A.size_factors[j];
     const int g = A.gid[j];
@@ -135,6 +251,8 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
     accL[t * 32 + lane] = 0.0;
   }
   double s = 0.0, s2 = 0.0, raw = 0.0;
+  double wmax = 0.0;
+  bool bad = false;
   for (int j = lane; j < A.m; j += 32) {
     const double y = A.y_is_f64 ? static_cast<const double*>(A.y)[off + j] : (double)static_cast<const int32_t*>(A.y)[off + j];
     const double v = y / sf[j];
@@ -142,14 +260,23 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
     const int slot = gidb[j] * 32 + lane;
     accN[slot] += v;
     accL[slot] += log(v + 0.1);
-    s += v;
+    if constexpr (W) {
+      const double w = A.weights[off + j];
+      s += w * v;
+      wmax = fmax(wmax, w);
+      bad = bad || !(w >= 0.0);
+    } else {
+      s += v;
+    }
     raw += y;
   }
   s = warp_allreduce_sum(s);
   raw = warp_allreduce_sum(raw);
   const double bm = s / (double)A.m;
   for (int j = lane; j < A.m; j += 32) {
-    const double d = vn[j] - bm;
+    double d;
+    if constexpr (W) d = A.weights[off + j] * vn[j] - bm;     // the row is in L1 from the pass above
+    else d = vn[j] - bm;
     s2 = fma(d, d, s2);
   }
   s2 = warp_allreduce_sum(s2);
@@ -191,6 +318,53 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
     if (A.mu_lin != nullptr) A.mu_lin[off + j] = fmax(f * sf[j], A.minmu);
   }
   rs = warp_allreduce_sum(rs);
+  bool invalid = false, ok = true;
+  if constexpr (W) {
+    // normalise by the row maximum; the Gram matrices need only each group's sum of w^2 and count of w > threshold
+    // (the lane-private slots are free again: their group sums were taken above)
+    wmax = warp_allreduce_max(wmax);
+    invalid = __any_sync(0xffffffffu, bad) || !(wmax > 0.0) || !(wmax < INFINITY);
+    for (int t = 0; t < G; t++) {
+      accN[t * 32 + lane] = 0.0;
+      accL[t * 32 + lane] = 0.0;
+    }
+    for (int j = lane; j < A.m; j += 32) {
+      const double w = A.weights[off + j] / wmax;
+      A.weights_norm[off + j] = w;
+      const int slot = gidb[j] * 32 + lane;
+      accN[slot] = fma(w, w, accN[slot]);
+      accL[slot] += (w > A.weight_threshold) ? 1.0 : 0.0;
+    }
+    for (int j = A.m + lane; j < A.ld; j += 32) A.weights_norm[off + j] = 0.0;
+    __syncwarp();
+    if (lane < G) {
+      double a = 0.0, b = 0.0;
+      for (int l = 0; l < 32; l++) {
+        a += accN[lane * 32 + ((l + lane) & 31)];
+        b += accL[lane * 32 + ((l + lane) & 31)];
+      }
+      gsW[lane] = a;
+      gsC[lane] = b;
+    }
+    __syncwarp();
+    double kept = 0.0;
+    for (int t = 0; t < G; t++) kept += gsC[t];
+    // lane b builds column b of sum_t c_t x_t x_t' (x_t: the distinct design rows), first c = w^2, then c = count
+    for (int pass = 0; pass < 2; pass++) {
+      const double* c = pass == 0 ? gsW : gsC;
+      if (lane < p)
+        for (int a = 0; a < p; a++) {
+          double t1 = 0.0;
+          for (int t = 0; t < G; t++) t1 = fma(c[t] * xg[t * ps + a], xg[t * ps + lane], t1);
+          gram[a * p + lane] = t1;
+        }
+      __syncwarp();
+      const bool full = pass == 0 ? gram_full_rank(gram, p, A.m, (p == 32) ? 0xffffffffu : ((1u << p) - 1u), lane)
+                                  : gram_full_rank(gram, p, (int)kept, gram_nonzero_columns(gram, p, lane), lane);
+      ok = ok && full;
+      __syncwarp();
+    }
+  }
   if (lane == 0) {
     const double rough = fmax(rs / (double)(A.m - A.p), 0.0);
     const double moments = (bv - A.xim * bm) / (bm * bm);
@@ -200,6 +374,7 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
     A.base_var[g] = bv;
     A.alpha0[g] = a0;
     A.all_zero[g] = (raw == 0.0) ? 1 : 0;
+    if constexpr (W) store_weight_flags(A, g, invalid, ok);
   }
 }
 
@@ -343,30 +518,41 @@ __global__ void __launch_bounds__(512) trend_fit_kernel(const double* __restrict
 
 }  // namespace
 
+// a.weights != nullptr selects the weighted instantiations; their larger per-warp scratch may run fewer warps per CTA
 cudaError_t launch_prep(const PrepArgs& a, cudaStream_t stream) {
   if (a.n == 0) return cudaSuccess;
+  const bool weighted = a.weights != nullptr;
   if (a.G > 0 && a.G <= 32) {
-    const int mpad = (a.m + 7) & ~7, ps = a.p | 1, warps = 8;
+    const int mpad = (a.m + 7) & ~7, ps = a.p | 1;
+    int warps = 8;
     const size_t fixed = ((size_t)mpad + (size_t)a.p * a.G + (size_t)a.G * ps) * sizeof(double) + 32 * sizeof(int) + mpad;
-    const size_t per_warp = ((size_t)mpad + 2 * (size_t)a.G * 32 + 5 * 32) * sizeof(double);
-    const size_t smem = fixed + warps * per_warp;
+    const size_t per_warp = ((size_t)mpad + 2 * (size_t)a.G * 32 + 5 * 32 +
+                             (weighted ? prep_weighted_extra<true>(mpad, a.p, true) : 0)) * sizeof(double);
+    size_t smem = fixed + warps * per_warp;
+    while (weighted && warps > 1 && smem > 200 * 1024) {
+      warps >>= 1;
+      smem = fixed + warps * per_warp;
+    }
     if (smem <= 200 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(prep_grouped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      const auto kern = weighted ? prep_grouped_kernel<true> : prep_grouped_kernel<false>;
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
-      prep_grouped_kernel<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a, mpad, ps);
+      kern<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a, mpad, ps);
       return cudaGetLastError();
     }
   }
   const int mpad = (a.m + 3) & ~3;
+  const size_t per_warp = 2 * (size_t)mpad + 64 + (weighted ? prep_weighted_extra<true>(mpad, a.p, false) : 0);
   int warps = 8;
-  size_t smem = ((size_t)mpad + (size_t)warps * (2 * mpad + 64)) * sizeof(double);
+  size_t smem = ((size_t)mpad + (size_t)warps * per_warp) * sizeof(double);
   while (warps > 1 && smem > 200 * 1024) {
     warps >>= 1;
-    smem = ((size_t)mpad + (size_t)warps * (2 * mpad + 64)) * sizeof(double);
+    smem = ((size_t)mpad + (size_t)warps * per_warp) * sizeof(double);
   }
-  cudaError_t e = cudaFuncSetAttribute(prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  const auto kern = weighted ? prep_kernel<true> : prep_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  prep_kernel<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a);
+  kern<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a);
   return cudaGetLastError();
 }
 

@@ -2,7 +2,7 @@
 device, only a handful of scalars ever reach the host.
 
 Same sequence as deseq2_b200/pipeline.py (the numpy restatement of R/core.R:280-432 with test="Wald",
-fitType="parametric", no weights, no outlier replacement; betaPrior=FALSE by default), but
+fitType="parametric", no outlier replacement by default; betaPrior=FALSE by default), but
   * the pre-steps (base mean/variance, rough + moments dispersion, linear-model mu, IRLS start values) are one
     CUDA kernel (b200nb_prep_dev, csrc/pipeline_kernels.cu),
   * the parametric dispersion-trend fit is one single-CTA kernel (b200nb_trend_fit_dev),
@@ -14,6 +14,10 @@ DESeq_device(betaPrior=True, factors=...) runs the reference's betaPrior=TRUE Wa
 (fitGLMsWithPrior, R/fitNbinomGLMs.R:242-337): the MLE fit above, the prior variance of estimateBetaPriorVar
 ("weighted": one launch of b200nb_beta_prior_quantile_dev, csrc/beta_prior.cuh, for all columns and level contrasts,
 then averagePriorsOverLevels in torch), and the MAP fit on the expanded model matrix.
+DESeq_device(weights=...), nbinomLRT_device(weights=...) and getContrast_device(weights=...) take observation
+weights (the "weights" assay): the weight checks and the weighted pre-steps are the weighted instantiation of the prep
+kernel (b200nb_prep_weighted_dev), and every fit passes the normalised weights to the engine's weighted fitDisp /
+fitDispGrid / fitBeta / log-likelihood / optim entry points.
 """
 from __future__ import annotations
 
@@ -97,8 +101,12 @@ def _projection(x):
     return np.ascontiguousarray(aug[:, p:])
 
 
-def prep(y, x, sizeFactors, minDisp=1e-8, minmu=0.5, want_mu=True, want_beta0=True):
-    """b200nb_prep_dev.  y: gene-major (n, ld) int32/float64 device tensor; x: (m, p) numpy; sizeFactors: (m,) numpy."""
+def prep(y, x, sizeFactors, minDisp=1e-8, minmu=0.5, want_mu=True, want_beta0=True, weights=None,
+         weightThreshold=1e-2):
+    """b200nb_prep_dev.  y: gene-major (n, ld) int32/float64 device tensor; x: (m, p) numpy; sizeFactors: (m,) numpy.
+    weights: gene-major (n, ld) float64 device tensor of raw observation weights -> b200nb_prep_weighted_dev, which
+    adds "weightsNorm" (n, ld: weights / row maximum), "weightsFail" (n,) int32 and "status" (1,) int32, the number
+    of rows whose weights the reference rejects (the caller raises when it is not 0).  mu_lin is not computed then."""
     L = _lib.lib()
     dev = y.device
     n, ld = y.shape
@@ -112,12 +120,46 @@ def prep(y, x, sizeFactors, minDisp=1e-8, minmu=0.5, want_mu=True, want_beta0=Tr
            "allZero": torch.empty(n, dtype=torch.int32, device=dev), "alpha0": torch.empty(n, dtype=F64, device=dev),
            "mu_lin": _ws("mu_lin", (n, ld), F64, dev) if want_mu else None,
            "beta0": torch.empty((p, n), dtype=F64, device=dev) if want_beta0 else None}
-    rc = L.b200nb_prep_dev(_p(y), 0 if y.dtype == torch.int32 else 1, _p(xd), _p(projd), _p(sfd),
-                           float(np.mean(1.0 / np.asarray(sizeFactors))), float(minDisp), float(max(10, m)),
-                           float(minmu), n, m, p, ld, _p(out["baseMean"]), _p(out["baseVar"]), _p(out["allZero"]),
-                           _p(out["alpha0"]), _p(out["mu_lin"]), _p(out["beta0"]), _stream())
-    _lib.check(rc, "prep_dev")
+    args = (_p(y), 0 if y.dtype == torch.int32 else 1, _p(xd), _p(projd), _p(sfd),
+            float(np.mean(1.0 / np.asarray(sizeFactors))), float(minDisp), float(max(10, m)), float(minmu), n, m, p, ld,
+            _p(out["baseMean"]), _p(out["baseVar"]), _p(out["allZero"]), _p(out["alpha0"]))
+    if weights is None:
+        rc = L.b200nb_prep_dev(*args, _p(out["mu_lin"]), _p(out["beta0"]), _stream())
+        _lib.check(rc, "prep_dev")
+    else:
+        _check_weights_tensor(weights, y)
+        out["mu_lin"] = None
+        out["weightsNorm"] = torch.empty((n, ld), dtype=F64, device=dev)
+        out["weightsFail"] = torch.empty(n, dtype=torch.int32, device=dev)
+        out["status"] = torch.zeros(1, dtype=torch.int32, device=dev)
+        rc = L.b200nb_prep_weighted_dev(*args, None, _p(out["beta0"]), _p(weights), float(weightThreshold),
+                                        _p(out["weightsNorm"]), _p(out["weightsFail"]), _p(out["status"]), _stream())
+        _lib.check(rc, "prep_weighted_dev")
     out["xd"], out["sfd"] = xd, sfd
+    return out
+
+
+def _check_weights_tensor(weights, y):
+    if not isinstance(weights, torch.Tensor) or weights.dtype != F64 or weights.device != y.device:
+        raise ValueError("weights must be a float64 tensor on the counts' device")
+    if tuple(weights.shape) != tuple(y.shape) or not weights.is_contiguous():
+        raise ValueError(f"weights must be a contiguous gene-major tensor of the counts' shape {tuple(y.shape)}, "
+                         f"got {tuple(weights.shape)}")
+
+
+def normalize_weights(weights, y, m):
+    """weights / row maximum over the first m columns (the normalisation of getContrast and fitNbinomGLMs,
+    R/results.R:794, R/core.R:2700-2702), padding columns 0.  Idempotent: normalised rows come back bit for bit.
+    Raises ValueError, with one host read, on a negative or NaN weight or a row without a positive, finite maximum."""
+    _check_weights_tensor(weights, y)
+    w = weights[:, :m]
+    wmax = w.max(dim=1).values if w.shape[0] else torch.zeros(0, dtype=F64, device=w.device)
+    bad = (~(w >= 0)).any(dim=1) | ~(wmax > 0) | ~torch.isfinite(wmax)
+    if bool(bad.any()):
+        raise ValueError(f"{int(bad.sum())} row(s) of weights have a negative or NaN weight or no positive, finite "
+                         "maximum")
+    out = torch.zeros_like(weights)
+    out[:, :m] = w / wmax[:, None]
     return out
 
 
@@ -227,21 +269,26 @@ def _median(v):
     return s[k // 2] if k % 2 else 0.5 * (s[k // 2 - 1] + s[k // 2])
 
 
-def _grid_refit(y, xd, mu, sel, m, prior_mean, prior_sigmasq, usePrior):
+def _grid_refit(y, xd, mu, sel, m, prior_mean, prior_sigmasq, usePrior, weights=None, weightThreshold=1e-2):
     """fitDispGridWrapper (R/wrappers.R:63-83) on the genes flagged in boolean `sel`; returns (idx, alpha)."""
     idx = torch.nonzero(sel).squeeze(1)
     if idx.numel() == 0:
         return idx, None
     grid = np.linspace(np.log(1e-8), np.log(max(10, m)), 20)
     pm = prior_mean[idx] if prior_mean is not None else torch.zeros(idx.numel(), dtype=F64, device=y.device)
-    la = D.fit_disp_grid(y[idx].contiguous(), xd, mu[idx].contiguous(), grid, pm, prior_sigmasq, usePrior)["log_alpha"]
+    w = None if weights is None else weights[idx].contiguous()
+    la = D.fit_disp_grid(y[idx].contiguous(), xd, mu[idx].contiguous(), grid, pm, prior_sigmasq, usePrior, weights=w,
+                         weightThreshold=weightThreshold)["log_alpha"]
     return idx, torch.exp(la)
 
 
-def getContrast_device(ynz, x, sizeFactors, dispersion, betaMatrix, contrast, betaPriorVar=None, minmu=0.5):
+def getContrast_device(ynz, x, sizeFactors, dispersion, betaMatrix, contrast, betaPriorVar=None, minmu=0.5,
+                       weights=None):
     """getContrast (R/results.R:760-827) on device tensors: fitBeta's maxit = 0 mode (covariance at the given betas).
     ynz: gene-major counts the model was fitted to; betaMatrix: (n, p) log2-scale coefficients (DESeq_device's
-    "betaMatrix").  Returns log2FoldChange, lfcSE, stat, pvalue as device tensors."""
+    "betaMatrix").  weights: gene-major (n, ld) float64 observation weights of the same rows (raw, or DESeq_device's
+    normalised "weights"), normalised by the row maximum and passed to fitBeta without the rank tests, as in the
+    reference.  Returns log2FoldChange, lfcSE, stat, pvalue as device tensors."""
     dev = ynz.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
@@ -252,19 +299,22 @@ def getContrast_device(ynz, x, sizeFactors, dispersion, betaMatrix, contrast, be
     lam = torch.as_tensor(1.0 / (LN2 ** 2 * pv), device=dev)
     sfd = torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=dev)
     beta_nat = (betaMatrix.T * LN2).contiguous()                       # (p, n) = column-major n x p, natural log scale
+    wn = None if weights is None else normalize_weights(weights, ynz, m)
     r = D.fit_beta(ynz, D.x_to_device(x, dev), sfd, dispersion, torch.as_tensor(contrast, device=dev), beta_nat, lam,
-                   1e-8, 0, useQR=False, minmu=minmu, want_hat=False, want_mu=False)
+                   1e-8, 0, useQR=False, minmu=minmu, weights=wn, want_hat=False, want_mu=False)
     est, se = r["contrast_num"] / LN2, r["contrast_denom"] / LN2
     stat = est / se
     return {"log2FoldChange": est, "lfcSE": se, "stat": stat, "pvalue": 2.0 * torch.special.ndtr(-stat.abs())}
 
 
-def _optim_fallback(ysrc, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, minmu, ll, useOptim=True):
+def _optim_fallback(ysrc, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, minmu, ll, useOptim=True,
+                    weights=None):
     """R/fitNbinomGLMs.R:186-227 on device results: rows with NA coefficients or non-positive variances -- and, with
     useOptim (the reference's default), rows whose IRLS did not converge -- are refitted by b200nb_beta_optim_dev
     (fitNbinomGLMsOptim, :340-407); their coefficients, standard errors (sandwich at the clamped mean, :386-396),
     fitted means and log-likelihoods are overwritten in `fb` / `ll` in place.  The hat diagonals keep the IRLS values,
-    as in the reference (:234).  Returns betaConv (n,) bool.  Costs one host sync (the number of such rows)."""
+    as in the reference (:234).  With weights the objective, the sandwich and the log-likelihood are weighted
+    (:343-400).  Returns betaConv (n,) bool.  Costs one host sync (the number of such rows)."""
     beta = fb["beta_mat"]                                             # (p, n), natural-log scale
     betaConv = fb["iter"] < maxit
     rowStable = ~torch.isnan(beta).any(dim=0)
@@ -280,10 +330,12 @@ def _optim_fallback(ysrc, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, 
     start = torch.nan_to_num(start, nan=0.0)
     ysub = ysrc[rows].contiguous()
     asub = dispersion[rows].contiguous()
-    o = D.beta_optim(ysub, xd, sfd, asub, lam, start)
-    cov = D.fit_beta(ysub, xd, sfd, asub, contrast, o["beta_mat"], lam, 1e-8, 0, minmu=minmu, want_hat=False,
-                     want_mu=False)
-    l2 = D.nb_loglik(ysub, xd, sfd, asub, o["beta_mat"], want_mu=ll.get("mu") is not None, minmu=minmu)
+    wsub = None if weights is None else weights[rows].contiguous()
+    o = D.beta_optim(ysub, xd, sfd, asub, lam, start, weights=wsub)
+    cov = D.fit_beta(ysub, xd, sfd, asub, contrast, o["beta_mat"], lam, 1e-8, 0, minmu=minmu, weights=wsub,
+                     want_hat=False, want_mu=False)
+    l2 = D.nb_loglik(ysub, xd, sfd, asub, o["beta_mat"], weights=wsub, want_mu=ll.get("mu") is not None,
+                     minmu=minmu)
     fb["beta_mat"][:, rows] = o["beta_mat"]
     fb["beta_var_mat"][:, rows] = cov["beta_var_mat"]
     fb["contrast_num"][rows] = cov["contrast_num"]
@@ -297,26 +349,33 @@ def _optim_fallback(ysrc, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, 
 
 
 def nbinomLRT_device(ynz, x_full, x_reduced, sizeFactors, dispersion, betaTol=1e-8, maxit=100, minmu=0.5,
-                     useOptim=True):
+                     useOptim=True, weights=None):
     """nbinomLRT (R/core.R:1787-2012) on device tensors: two IRLS fits, LRT statistic 2 (logLike_full - logLike_reduced)
     (R/core.R:1877) and its chi-square p-value.  The log-likelihoods are evaluated at the UNCLAMPED fitted means
     nf * exp(x beta) as the reference does (R/fitNbinomGLMs.R:180-182) by b200nb_nb_loglik_dev -- NOT taken from the IRLS
-    kernel's deviance, which is at the minmu-clamped mean and differs by several units when a design cell is all zeros."""
+    kernel's deviance, which is at the minmu-clamped mean and differs by several units when a design cell is all zeros.
+    weights: gene-major (n, ld) float64 observation weights of the rows (raw or normalised): both fits, their
+    log-likelihoods and the optim fallback are weighted, and an intercept-only reduced model takes the reference's
+    weighted closed form (R/fitNbinomGLMs.R:99-137) instead of an IRLS fit."""
     dev = ynz.device
     sfd = torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=dev)
+    wn = None if weights is None else normalize_weights(weights, ynz, np.asarray(x_full).shape[0])
     res = {}
     for name, x in (("full", x_full), ("reduced", x_reduced)):
         x = np.asarray(x, dtype=np.float64)
         m, p = x.shape
+        if wn is not None and name == "reduced" and p == 1 and np.all(x == 1):
+            res[name] = _intercept_only_weighted(ynz, sfd, dispersion, wn, m)
+            continue
         pr = prep(ynz, x, sizeFactors, minmu=minmu, want_mu=False)
         contrast = torch.zeros(p, dtype=F64, device=dev)
         contrast[0] = 1.0
         lam = torch.full((p,), 1e-6 / LN2 ** 2, dtype=F64, device=dev)
         res[name] = D.fit_beta(ynz, pr["xd"], sfd, dispersion, contrast, pr["beta0"], lam, betaTol, maxit, minmu=minmu,
-                               want_hat=(name == "full"), want_mu=False)
-        ll = D.nb_loglik(ynz, pr["xd"], sfd, dispersion, res[name]["beta_mat"], want_mu=(name == "full"))
+                               weights=wn, want_hat=(name == "full"), want_mu=False)
+        ll = D.nb_loglik(ynz, pr["xd"], sfd, dispersion, res[name]["beta_mat"], weights=wn, want_mu=(name == "full"))
         res[name]["conv"], _ = _optim_fallback(ynz, pr["xd"], sfd, dispersion, res[name], pr["beta0"], lam, contrast,
-                                               maxit, minmu, ll, useOptim=useOptim)
+                                               maxit, minmu, ll, useOptim=useOptim, weights=wn)
         res[name]["logLike"], res[name]["mu"] = ll["logLike"], ll["mu"]
     df = x_full.shape[1] - x_reduced.shape[1]
     stat = 2.0 * (res["full"]["logLike"] - res["reduced"]["logLike"])
@@ -326,6 +385,19 @@ def nbinomLRT_device(ynz, x_full, x_reduced, sizeFactors, dispersion, betaTol=1e
             "betaSE": (torch.sqrt(torch.clamp(res["full"]["beta_var_mat"], min=0.0)) / LN2).T,
             "fullBetaConv": res["full"]["conv"], "reducedBetaConv": res["reduced"]["conv"],
             "mu": res["full"]["mu"], "H": res["full"]["hat_diagonals"]}
+
+
+def _intercept_only_weighted(ynz, sfd, dispersion, wn, m):
+    """R/fitNbinomGLMs.R:99-137 with weights: beta = log2(sum(w K/s) / sum(w)), log-likelihood sum(w log dnbinom) at
+    mu = s 2^beta (b200nb_nb_loglik_dev with the weights); no IRLS."""
+    dev = ynz.device
+    norm = ynz[:, :m].to(F64) / sfd[None, :]
+    w = wn[:, :m]
+    beta = torch.log((w * norm).sum(dim=1) / w.sum(dim=1))[None, :].contiguous()    # (1, n), natural-log scale
+    ones = torch.ones((1, m), dtype=F64, device=dev)
+    ll = D.nb_loglik(ynz, ones, sfd, dispersion, beta, weights=wn, want_mu=False)
+    return {"beta_mat": beta, "logLike": ll["logLike"], "mu": None,
+            "conv": torch.ones(ynz.shape[0], dtype=torch.bool, device=dev)}
 
 
 def _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp, kappa_0, dispTol, maxit, betaTol,
@@ -385,7 +457,7 @@ def _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp,
 
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
                  outlierSD=2.0, minReplicatesForReplace=np.inf, allgather=None, useOptim=True, betaPrior=False,
-                 factors=None):
+                 factors=None, weights=None, weightThreshold=1e-2):
     """y: gene-major (N, ld) device tensor of counts (int32 or float64).  Returns a dict of device tensors over the
     rows with a non-zero sum (`idx` maps them back to the N input rows) plus the trend / prior scalars.
     sizeFactors=None estimates them on the device first (median of ratios, R/core.R:535-578; returned under
@@ -404,10 +476,24 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     Cook's distances) are on x; the prior variance comes from the MLE log2 fold changes (estimate_beta_prior_var) and
     the reported coefficients, standard errors, Wald statistics and deviance from the MAP fit on the expanded matrix
     factorDesign(factors, expanded=True)[0] with lambda = 1 / betaPriorVar.  Adds "mleBetaMatrix", "betaPriorVar" and
-    "modelMatrix" (the expanded matrix)."""
+    "modelMatrix" (the expanded matrix).
+    weights: observation weights (the "weights" assay) as a gene-major (N, ld) float64 device tensor aligned with y.
+    getAndCheckWeights (R/core.R:2697-2752) runs in the weighted prep kernel: rows with a negative, NaN or infinite
+    weight or no positive weight raise ValueError, and rows whose weights leave the design rank deficient
+    ("weightsFail", over the N input rows; a warning as in R) are dropped with the all-zero rows.  baseMean / baseVar
+    use the raw weights; mu comes from a weighted GLM fit (no linear mu); the gene-wise fitDisp / fitDispGrid get
+    max(w, 1e-6), every other fit the normalised weights, returned under "weights" for the rows in idx.  Weights are
+    not supported with betaPrior=True or outlier replacement (ValueError)."""
     dev = y.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
+    if weights is not None:
+        _check_weights_tensor(weights, y)
+        if betaPrior:
+            raise ValueError("observation weights are not supported with betaPrior=True")
+        if np.isfinite(minReplicatesForReplace):
+            raise ValueError("observation weights are not supported with outlier replacement "
+                             "(finite minReplicatesForReplace)")
     if betaPrior:
         from .pipeline import factorDesign
         if factors is None:
@@ -433,15 +519,40 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             _t[0] = now
 
     maxDisp = float(max(10, m))
-    linearMu = modelMatrixGroups(x) == p
-    # rows with a zero sum are dropped before anything else (R/core.R:706), so every later array is aligned
-    idx = torch.nonzero(y[:, :m].sum(dim=1) != 0).squeeze(1)
-    ynz = y if idx.numel() == y.shape[0] else y[idx].contiguous()
-    pr = prep(ynz, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu)
+    linearMu = modelMatrixGroups(x) == p and weights is None
+    wn = wdisp = weightsFail = None
+    if weights is None:
+        # rows with a zero sum are dropped before anything else (R/core.R:706), so every later array is aligned
+        idx = torch.nonzero(y[:, :m].sum(dim=1) != 0).squeeze(1)
+        ynz = y if idx.numel() == y.shape[0] else y[idx].contiguous()
+        pr = prep(ynz, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu)
+        bm = pr["baseMean"]
+        alpha0 = pr["alpha0"]
+        beta0 = pr["beta0"]
+    else:
+        # the weighted prep runs on all rows: getAndCheckWeights checks every row and its weightsFail rows join the
+        # all-zero rows (R/core.R:2733-2736) before the same drop
+        pr = prep(y, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=False, weights=weights,
+                  weightThreshold=weightThreshold)
+        weightsFail = pr["weightsFail"] != 0
+        keep = (pr["allZero"] == 0) & ~weightsFail
+        n_bad, n_fail = (int(v) for v in torch.stack([pr["status"][0].to(torch.int64),
+                                                       weightsFail.sum()]).cpu().tolist())
+        if n_bad:
+            raise ValueError(f"{n_bad} row(s) of weights have a negative, NaN or infinite weight or no positive weight")
+        if n_fail:
+            import warnings
+            warnings.warn(f"for {n_fail} row(s), the weights as supplied won't allow parameter estimation, producing "
+                          "a degenerate design matrix. These rows have been flagged in weightsFail and treated as if "
+                          "the row contained all zeros.")
+        idx = torch.nonzero(keep).squeeze(1)
+        if idx.numel() == y.shape[0]:
+            ynz, bm, alpha0, beta0, wn = y, pr["baseMean"], pr["alpha0"], pr["beta0"], pr["weightsNorm"]
+        else:
+            ynz, bm, alpha0 = y[idx].contiguous(), pr["baseMean"][idx], pr["alpha0"][idx]
+            beta0, wn = pr["beta0"][:, idx].contiguous(), pr["weightsNorm"][idx].contiguous()
+        wdisp = torch.clamp(wn, min=1e-6)                   # pmax(weights, 1e-6) for the gene-wise estimate (:702)
     xd, sfd = pr["xd"], pr["sfd"]
-    bm = pr["baseMean"]
-    alpha0 = pr["alpha0"]
-    beta0 = pr["beta0"]
     n = idx.numel()
     contrast = torch.zeros(p, dtype=F64, device=dev)
     contrast[0] = 1.0
@@ -451,6 +562,16 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     # ---- estimateDispersionsGeneEst (R/core.R:657-860)
     if linearMu:
         mu = pr["mu_lin"]
+    elif weights is not None:
+        # fitNbinomGLMs with the normalised weights, its defaults minmu = 0.5 and useOptim = TRUE (R/core.R:752-755
+        # passes neither), its unclamped mean nf exp(x beta) (R/fitNbinomGLMs.R:180; the optim rows' own, :383)
+        # bounded at minmu (:764)
+        fb0 = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=0.5, weights=wn,
+                         want_hat=False, want_mu=False)
+        ll0 = D.nb_loglik(ynz, xd, sfd, alpha0, fb0["beta_mat"], weights=wn,
+                          out_mu=_ws("mu_glm", tuple(ynz.shape), F64, dev))
+        _optim_fallback(ynz, xd, sfd, alpha0, fb0, beta0, lam, contrast, maxit, 0.5, ll0, useOptim=True, weights=wn)
+        mu = ll0["mu"].clamp_(min=minmu)
     else:
         nn0 = ynz.shape[0]
         vec = lambda: torch.empty(nn0, dtype=F64, device=dev)
@@ -461,13 +582,14 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
         mu = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=minmu, out=out0)["mu"]
     la0 = torch.log(alpha0)
     mark("mu")
-    r = D.fit_disp(ynz, xd, mu, la0, la0, 1.0, min_log_alpha, kappa_0, dispTol, maxit, False)
+    r = D.fit_disp(ynz, xd, mu, la0, la0, 1.0, min_log_alpha, kappa_0, dispTol, maxit, False, weights=wdisp,
+                   weightThreshold=weightThreshold)
     mark("fit_disp_mle")
     dge = torch.clamp(torch.exp(r["log_alpha"]), max=maxDisp)
     noIncrease = r["last_lp"] < r["initial_lp"] + r["initial_lp"].abs() / 1e6
     dge = torch.where(noIncrease, alpha0, dge)
     conv = (r["iter"] < maxit) & (r["iter"] != 1)
-    gi, ga = _grid_refit(ynz, xd, mu, (~conv) & (dge > minDisp * 10), m, None, 1.0, False)
+    gi, ga = _grid_refit(ynz, xd, mu, (~conv) & (dge > minDisp * 10), m, None, 1.0, False, wdisp, weightThreshold)
     if ga is not None:
         dge[gi] = ga
     dge = torch.clamp(dge, minDisp, maxDisp)
@@ -502,10 +624,11 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     # ---- estimateDispersionsMAP (R/core.R:943-1131)
     dispInit = torch.where(dge > 0.1 * dispFit, dge, dispFit)
     logFit = torch.log(dispFit)
-    rm = D.fit_disp(ynz, xd, mu, torch.log(dispInit), logFit, dispPriorVar, min_log_alpha, kappa_0, dispTol, maxit, True)
+    rm = D.fit_disp(ynz, xd, mu, torch.log(dispInit), logFit, dispPriorVar, min_log_alpha, kappa_0, dispTol, maxit, True,
+                    weights=wn, weightThreshold=weightThreshold)
     mark("fit_disp_map")
     dispMAP = torch.exp(rm["log_alpha"])
-    gi2, ga2 = _grid_refit(ynz, xd, mu, rm["iter"] >= maxit, m, logFit, dispPriorVar, True)
+    gi2, ga2 = _grid_refit(ynz, xd, mu, rm["iter"] >= maxit, m, logFit, dispPriorVar, True, wn, weightThreshold)
     if ga2 is not None:
         dispMAP[gi2] = ga2
     dispMAP = torch.clamp(dispMAP, minDisp, maxDisp)
@@ -519,15 +642,15 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             "iter": torch.empty(nn, dtype=F64, device=dev), "contrast_num": torch.empty(nn, dtype=F64, device=dev),
             "contrast_denom": torch.empty(nn, dtype=F64, device=dev), "deviance": torch.empty(nn, dtype=F64, device=dev),
             "hat_diagonals": _ws("H", (nn, ldd), F64, dev), "mu": None}
-    fb = D.fit_beta(ynz, xd, sfd, dispersion, contrast, beta0, lam, betaTol, maxit, minmu=minmu, out=outb)
+    fb = D.fit_beta(ynz, xd, sfd, dispersion, contrast, beta0, lam, betaTol, maxit, minmu=minmu, weights=wn, out=outb)
     mark("fit_beta")
     # Cook's distances and the reported deviance use the UNCLAMPED fitted mean nf * exp(x beta) and the log-likelihood
     # at it, which the reference recomputes in R right after the native call (R/fitNbinomGLMs.R:180-182): one small
     # kernel (b200nb_nb_loglik_dev); the IRLS kernel's fused mean / deviance are at the minmu clamp.
-    ll = D.nb_loglik(ynz, xd, sfd, dispersion, fb["beta_mat"], out_mu=_ws("mu_cooks", (nn, ldd), F64, dev))
+    ll = D.nb_loglik(ynz, xd, sfd, dispersion, fb["beta_mat"], weights=wn, out_mu=_ws("mu_cooks", (nn, ldd), F64, dev))
     # rows the IRLS could not fit go to the box-constrained maximiser (R/fitNbinomGLMs.R:203-227, useOptim = TRUE)
     betaConv, n_optim = _optim_fallback(ynz, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, minmu, ll,
-                                        useOptim=useOptim)
+                                        useOptim=useOptim, weights=wn)
     mark("loglik+optim")
     fit, fit_ll, prior = fb, ll, {}
     if betaPrior:
@@ -551,6 +674,8 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             "dispPriorVar": dispPriorVar, "n_refit_geneest": n_refit_geneest, "n_refit_map": int(gi2.numel()),
             "n_input_rows": y.shape[0], "sizeFactors": np.asarray(sizeFactors, dtype=np.float64)}
     res.update(prior)
+    if weights is not None:
+        res["weightsFail"], res["weights"] = weightsFail, wn
     if do_replace and m > p:
         _replace_and_refit(res, ynz, ck["cooks"], x, sizeFactors, sfd, tr, varLogDispEsts, dispPriorVar,
                            minReplicatesForReplace, minDisp, kappa_0, dispTol, maxit, betaTol, minmu, outlierSD,

@@ -21,11 +21,15 @@ numpy, one function per R function, same names, so the engine can be driven and 
   fitGLMsWithPrior / estimateBetaPriorVar / Hmisc.wtd.quantile / addAllContrasts / averagePriorsOverLevels /
   makeExpandedModelMatrix (additive factor designs)   R/fitNbinomGLMs.R:242-337, R/core.R:1601-1689, 2762-2803, R/expanded.R
   DESeq                          R/core.R:280-432    (test="Wald", fitType="parametric", betaPrior=FALSE or TRUE)
+  getAndCheckWeights             R/core.R:2697-2752  (observation weights: row-max normalisation, two rank tests per
+                                 gene with a restatement of LINPACK dqrdc2, the rank routine of R's qr())
+
+Observation weights (a "weights" assay) go through every step above that takes them in the reference, except
+betaPrior=TRUE and outlier replacement, which raise with weights.
 
 `engine` is any object with fitDisp / fitDispGrid / fitBeta taking the reference's argument names
 (deseq2_b200.wrappers is the product engine and the default; tests and the bench's CPU baseline pass the
-oracle).  Not restated (out of scope, SURVEY.md section 8f): local / mean trend fits,
-observation weights in the glue, results()/lfcShrink().
+oracle).  Not restated (out of scope, SURVEY.md section 8f): local / mean trend fits, results()/lfcShrink().
 """
 from __future__ import annotations
 
@@ -54,11 +58,85 @@ def estimateSizeFactorsForMatrix(counts):
     return sf
 
 
-def getBaseMeansAndVariances(counts, sizeFactors):
-    """R/core.R:2138-2157 (no weights)."""
+def getBaseMeansAndVariances(counts, sizeFactors, weights=None):
+    """R/core.R:2138-2157.  With weights: mean and variance of the RAW weights times the normalised counts; allZero
+    stays the unweighted row sum."""
     norm = np.asarray(counts, dtype=np.float64) / sizeFactors[None, :]
+    if weights is not None:
+        norm = np.asarray(weights, dtype=np.float64) * norm
     return {"baseMean": norm.mean(axis=1), "baseVar": norm.var(axis=1, ddof=1),
             "allZero": np.asarray(counts).sum(axis=1) == 0}
+
+
+def dqrdc2_rank(z, tol=1e-7):
+    """The rank R's qr(z) reports: LINPACK dqrdc2 (R's src/appl/dqrdc2.f), Householder with limited column pivoting.
+    Columns are taken in order; one whose norm after the transformations so far falls below tol times its original norm
+    (1 for a zero column) is moved to the end and no longer counted.  The norms are downdated as dqrdc2 does, and
+    recomputed when the downdate loses precision."""
+    x = np.array(z, dtype=np.float64)
+    n, p = x.shape
+    if n == 0 or p == 0:
+        return 0
+    qraux = np.sqrt((x * x).sum(axis=0))
+    work1 = qraux.copy()
+    work2 = np.where(qraux == 0.0, 1.0, qraux)
+    k = p + 1                                     # 1-based, as in the Fortran
+    for l in range(min(n, p)):                    # 0-based column / row l
+        while l + 1 < k and qraux[l] < work2[l] * tol:
+            x[:, l:] = np.roll(x[:, l:], -1, axis=1)
+            qraux[l:] = np.roll(qraux[l:], -1)
+            work1[l:] = np.roll(work1[l:], -1)
+            work2[l:] = np.roll(work2[l:], -1)
+            k -= 1
+        if l == n - 1:
+            continue
+        nrmxl = np.sqrt(np.sum(x[l:, l] ** 2))
+        if nrmxl == 0.0:
+            continue
+        if x[l, l] != 0.0:
+            nrmxl = np.copysign(nrmxl, x[l, l])
+        x[l:, l] /= nrmxl
+        x[l, l] += 1.0
+        for j in range(l + 1, p):
+            t = -np.dot(x[l:, l], x[l:, j]) / x[l, l]
+            x[l:, j] += t * x[l:, l]
+            if qraux[j] == 0.0:
+                continue
+            tt = max(1.0 - (abs(x[l, j]) / qraux[j]) ** 2, 0.0)
+            if abs(tt) < 1e-6:
+                qraux[j] = np.sqrt(np.sum(x[l + 1:, j] ** 2))
+                work1[j] = qraux[j]
+            else:
+                qraux[j] = qraux[j] * np.sqrt(tt)
+        qraux[l] = x[l, l]
+        x[l, l] = -nrmxl
+    return min(k - 1, n)
+
+
+def getAndCheckWeights(weights, x, weightThreshold=1e-2):
+    """R/core.R:2697-2752 for a full-rank model matrix.  Returns (weights / row maximum, weightsFail).  Raises
+    ValueError where the reference stops: a negative or NaN weight (stopifnot), a row without a positive weight or an
+    infinite weight (NaN after the normalisation, which qr() rejects).  A gene fails unless qr(w * X) has rank p and
+    X on the samples with w > weightThreshold, all-zero columns dropped, has full column rank."""
+    w = np.asarray(weights, dtype=np.float64)
+    x = np.asarray(x, dtype=np.float64)
+    if w.ndim != 2 or w.shape[1] != x.shape[0]:
+        raise ValueError(f"weights must have one column per sample: shape {w.shape}, {x.shape[0]} samples")
+    if not np.all(w >= 0):
+        raise ValueError("weights must be non-negative and not NaN")
+    wmax = w.max(axis=1) if w.shape[0] else np.zeros(0)
+    if np.any(~(wmax > 0)) or np.any(~np.isfinite(wmax)):
+        raise ValueError("every row of weights needs a positive, finite maximum")
+    wn = w / wmax[:, None]
+    p = x.shape[1]
+    fail = np.zeros(len(wn), bool)
+    for i in range(len(wn)):
+        test1 = dqrdc2_rank(wn[i][:, None] * x) == p
+        sub = x[wn[i] > weightThreshold]
+        sub = sub[:, np.abs(sub).sum(axis=0) > 0]
+        test2 = dqrdc2_rank(sub) == sub.shape[1]
+        fail[i] = not (test1 and test2)
+    return wn, fail
 
 
 def linearModelMu(y, x):
@@ -105,8 +183,8 @@ def _lgamma_diff(y, r):
     return out
 
 
-def nbinomLogLike(counts, mu, disp):
-    """R/core.R:2208-2217 without weights: rowSums(dnbinom(counts, mu = mu, size = 1/disp, log = TRUE)).  Evaluated in
+def nbinomLogLike(counts, mu, disp, weights=None):
+    """R/core.R:2208-2217: rowSums(weights * dnbinom(counts, mu = mu, size = 1/disp, log = TRUE)).  Evaluated in
     the cancellation-free direct form (the same as the device kernels), with dnbinom_mu's point mass at mu = 0."""
     y = np.asarray(counts, dtype=np.float64)
     mu = np.asarray(mu, dtype=np.float64)
@@ -115,28 +193,34 @@ def nbinomLogLike(counts, mu, disp):
         t = (_lgamma_diff(y, 1.0 / alpha) - _sp.gammaln(y + 1) + _sp.xlogy(y, mu * alpha)
              - (y + 1.0 / alpha) * np.log1p(mu * alpha))
     t = np.where(mu == 0, np.where(y == 0, 0.0, -np.inf), t)
+    if weights is not None:
+        t = np.asarray(weights, dtype=np.float64) * t
     return t.sum(axis=1)
 
 
 def estimateDispersionsGeneEst(counts, sizeFactors, x, engine=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6,
-                               maxit=100, useCR=True, weightThreshold=1e-2, minmu=0.5, mv=None):
-    """R/core.R:657-860 for niter=1, no weights.  `counts` holds only the non-all-zero rows."""
+                               maxit=100, useCR=True, weightThreshold=1e-2, minmu=0.5, mv=None, weights=None):
+    """R/core.R:657-860 for niter=1.  `counts` holds only the non-all-zero rows; `weights` (optional) are the
+    normalised weights of those rows (getAndCheckWeights).  With weights there is no linear mu (:738-741), mu comes
+    from the weighted GLM fit, and fitDisp / fitDispGrid get pmax(weights, 1e-6) (:702)."""
     engine = engine or _default_engine
     counts = np.asarray(counts)
     n, m = counts.shape
     p = x.shape[1]
     if mv is None:
-        mv = getBaseMeansAndVariances(counts, sizeFactors)
+        mv = getBaseMeansAndVariances(counts, sizeFactors)      # with weights the caller passes the weighted pair
     norm = counts / sizeFactors[None, :]
+    useWeights = weights is not None
+    wdisp = np.maximum(weights, 1e-6) if useWeights else None
     roughDisp = roughDispEstimate(norm, x)
     momentsDisp = momentsDispEstimate(mv["baseMean"], mv["baseVar"], sizeFactors)
     alpha_hat = np.minimum(roughDisp, momentsDisp)
     maxDisp = max(10, m)
     alpha_hat = alpha_init = np.minimum(np.maximum(minDisp, alpha_hat), maxDisp)
-    linearMu = modelMatrixGroups(x) == p
+    linearMu = modelMatrixGroups(x) == p and not useWeights
     nf = np.broadcast_to(sizeFactors[None, :], (n, m))
     if not linearMu:
-        fit = fitNbinomGLMs(counts, nf, x, alpha_hat, engine=engine)
+        fit = fitNbinomGLMs(counts, nf, x, alpha_hat, engine=engine, weights=weights)
         fitMu = fit["mu"]
     else:
         fitMu = linearModelMu(norm, x) * nf
@@ -144,7 +228,7 @@ def estimateDispersionsGeneEst(counts, sizeFactors, x, engine=None, minDisp=1e-8
     dispRes = fitDispWrapper(ySEXP=counts, xSEXP=x, mu_hatSEXP=fitMu, log_alphaSEXP=np.log(alpha_hat),
                              log_alpha_prior_meanSEXP=np.log(alpha_hat), log_alpha_prior_sigmasqSEXP=1.0,
                              min_log_alphaSEXP=np.log(minDisp / 10), kappa_0SEXP=kappa_0, tolSEXP=dispTol,
-                             maxitSEXP=maxit, usePriorSEXP=False, weightsSEXP=None, useWeightsSEXP=False,
+                             maxitSEXP=maxit, usePriorSEXP=False, weightsSEXP=wdisp, useWeightsSEXP=useWeights,
                              weightThresholdSEXP=weightThreshold, useCRSEXP=useCR, engine=engine)
     dispIter = dispRes["iter"]
     dispGeneEst = np.minimum(np.exp(dispRes["log_alpha"]), maxDisp)
@@ -155,7 +239,8 @@ def estimateDispersionsGeneEst(counts, sizeFactors, x, engine=None, minDisp=1e-8
     if refitDisp.sum() > 0:
         dispGrid = fitDispGridWrapper(y=counts[refitDisp], x=x, mu=fitMu[refitDisp],
                                       logAlphaPriorMean=np.zeros(int(refitDisp.sum())), logAlphaPriorSigmaSq=1.0,
-                                      usePrior=False, weightsSEXP=None, useWeightsSEXP=False,
+                                      usePrior=False, weightsSEXP=wdisp[refitDisp] if useWeights else None,
+                                      useWeightsSEXP=useWeights,
                                       weightThresholdSEXP=weightThreshold, useCRSEXP=useCR, engine=engine)
         dispGeneEst[refitDisp] = dispGrid
     dispGeneEst = np.minimum(np.maximum(dispGeneEst, minDisp), maxDisp)
@@ -287,16 +372,17 @@ def estimateDispersionsPriorVar(varLogDispEsts, m, p, dispGeneEst=None, dispFit=
 
 def estimateDispersionsMAP(counts, x, mu, dispGeneEst, dispFit, dispPriorVar, varLogDispEsts, engine=None,
                            outlierSD=2.0, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, useCR=True,
-                           weightThreshold=1e-2):
-    """R/core.R:943-1131, type='DESeq2', no weights."""
+                           weightThreshold=1e-2, weights=None):
+    """R/core.R:943-1131, type='DESeq2'.  `weights`: the normalised weights, unclamped (:1001-1007, 1036, 1057)."""
     engine = engine or _default_engine
     n, m = np.asarray(counts).shape
     dispInit = np.where(dispGeneEst > 0.1 * dispFit, dispGeneEst, dispFit)
     dispResMAP = fitDispWrapper(ySEXP=counts, xSEXP=x, mu_hatSEXP=mu, log_alphaSEXP=np.log(dispInit),
                                 log_alpha_prior_meanSEXP=np.log(dispFit), log_alpha_prior_sigmasqSEXP=dispPriorVar,
                                 min_log_alphaSEXP=np.log(minDisp / 10), kappa_0SEXP=kappa_0, tolSEXP=dispTol,
-                                maxitSEXP=maxit, usePriorSEXP=True, weightsSEXP=None, useWeightsSEXP=False,
-                                weightThresholdSEXP=weightThreshold, useCRSEXP=useCR, engine=engine)
+                                maxitSEXP=maxit, usePriorSEXP=True, weightsSEXP=weights,
+                                useWeightsSEXP=weights is not None, weightThresholdSEXP=weightThreshold,
+                                useCRSEXP=useCR, engine=engine)
     dispMAP = np.exp(dispResMAP["log_alpha"])
     dispIter = dispResMAP["iter"]
     dispConv = dispIter < maxit
@@ -304,8 +390,9 @@ def estimateDispersionsMAP(counts, x, mu, dispGeneEst, dispFit, dispPriorVar, va
     if refitDisp.sum() > 0:
         dispGrid = fitDispGridWrapper(y=np.asarray(counts)[refitDisp], x=x, mu=mu[refitDisp],
                                       logAlphaPriorMean=np.log(dispFit)[refitDisp], logAlphaPriorSigmaSq=dispPriorVar,
-                                      usePrior=True, weightsSEXP=None, useWeightsSEXP=False,
-                                      weightThresholdSEXP=weightThreshold, useCRSEXP=True, engine=engine)
+                                      usePrior=True, weightsSEXP=None if weights is None else weights[refitDisp],
+                                      useWeightsSEXP=weights is not None, weightThresholdSEXP=weightThreshold,
+                                      useCRSEXP=True, engine=engine)
         dispMAP[refitDisp] = dispGrid
     maxDisp = max(10, m)
     dispMAP = np.minimum(np.maximum(dispMAP, minDisp), maxDisp)
@@ -317,9 +404,10 @@ def estimateDispersionsMAP(counts, x, mu, dispGeneEst, dispFit, dispPriorVar, va
 
 
 def fitNbinomGLMsOptim(counts, nf, x, lambda_, rowsForOptim, rowStable, alpha_hat, betaMatrix, betaSE, betaConv,
-                       beta_mat, mu, logLike, minmu=0.5):
+                       beta_mat, mu, logLike, minmu=0.5, weights=None):
     """R/fitNbinomGLMs.R:340-407: L-BFGS-B on the penalised NB log-likelihood (log2 scale, box [-30, 30]) for the rows
-    the IRLS left unconverged / unstable; standard errors from the sandwich at the optimum.  No weights."""
+    the IRLS left unconverged / unstable; standard errors from the sandwich at the optimum.  With weights the
+    log-likelihood and the sandwich's working weights are multiplied by them."""
     from scipy import optimize as _so
     counts = np.asarray(counts, dtype=np.float64)
     lam = np.asarray(lambda_, dtype=np.float64)
@@ -330,10 +418,11 @@ def fitNbinomGLMsOptim(counts, nf, x, lambda_, rowsForOptim, rowStable, alpha_ha
     for row in rowsForOptim:
         betaRow = betaMatrix[row] if (rowStable[row] and np.all(np.abs(betaMatrix[row]) < large)) else beta_mat[row]
         nfr, k, alpha = nf[row], counts[row], alpha_hat[row]
+        wr = None if weights is None else weights[row][None, :]
 
         def objective(p_):
             mu_row = nfr * 2.0 ** (x @ p_)
-            ll = nbinomLogLike(k[None, :], mu_row[None, :], np.array([alpha]))[0]
+            ll = nbinomLogLike(k[None, :], mu_row[None, :], np.array([alpha]), wr)[0]
             logPrior = np.sum(-0.5 * np.log(2 * np.pi / lam) - 0.5 * lam * p_ ** 2)   # dnorm(p, 0, sqrt(1/lambda), log=TRUE)
             v = -(ll + logPrior)
             return v if np.isfinite(v) else 1e300
@@ -347,17 +436,21 @@ def fitNbinomGLMsOptim(counts, nf, x, lambda_, rowsForOptim, rowStable, alpha_ha
         mu[row] = mu_row
         mu_row = np.maximum(mu_row, minmu)
         w = 1.0 / (1.0 / mu_row + alpha)
+        if wr is not None:
+            w = wr[0] * w
         xtwx = (x.T * w) @ x
         inv = np.linalg.inv(xtwx + np.diag(lamNat))
         sigma = inv @ xtwx @ inv
         betaSE[row] = np.sqrt(np.maximum(np.diag(sigma), 0.0)) / LN2
-        logLike[row] = nbinomLogLike(k[None, :], mu_row[None, :], np.array([alpha]))[0]
+        logLike[row] = nbinomLogLike(k[None, :], mu_row[None, :], np.array([alpha]), wr)[0]
     return {"betaMatrix": betaMatrix, "betaSE": betaSE, "betaConv": betaConv, "mu": mu, "logLike": logLike}
 
 
 def fitNbinomGLMs(counts, nf, x, alpha_hat, lambda_=None, engine=None, betaTol=1e-8, maxit=100, useQR=True,
-                  minmu=0.5, useOptim=True, forceOptim=False):
-    """R/fitNbinomGLMs.R:29-236 without weights.  As in the reference (:203-227) rows with NA coefficients or
+                  minmu=0.5, useOptim=True, forceOptim=False, weights=None):
+    """R/fitNbinomGLMs.R:29-236; `weights`: normalised observation weights (getAndCheckWeights), or None.  An
+    intercept-only model with the default wide prior takes the closed form (_fit_intercept_only, :99-137).  As in the
+    reference (:203-227) rows with NA coefficients or
     non-positive variances ALWAYS go to the L-BFGS-B fallback, and with useOptim=TRUE (the reference's default, :30)
     so do the rows whose IRLS did not converge (iter == maxit, which includes the |beta| > 30 sentinel).  Parity tests
     that need the engine's raw output pass useOptim=False."""
@@ -367,6 +460,8 @@ def fitNbinomGLMs(counts, nf, x, alpha_hat, lambda_=None, engine=None, betaTol=1
     p = x.shape[1]
     if lambda_ is None:
         lambda_ = np.full(p, 1e-6)
+    if weights is not None and p == 1 and np.all(x == 1) and np.all(np.asarray(lambda_) <= 1e-6):
+        return _fit_intercept_only(counts, nf, alpha_hat, weights)
     norm = counts / nf
     if np.linalg.matrix_rank(x) == p:
         Q, R = np.linalg.qr(x)
@@ -377,10 +472,10 @@ def fitNbinomGLMs(counts, nf, x, alpha_hat, lambda_=None, engine=None, betaTol=1
         beta_mat[:, 0] = np.log(norm.mean(axis=1))
     lambdaNatLogScale = np.asarray(lambda_, dtype=np.float64) / LN2 ** 2
     betaRes = fitBetaWrapper(ySEXP=counts, xSEXP=x, nfSEXP=nf, alpha_hatSEXP=alpha_hat, beta_matSEXP=beta_mat,
-                             lambdaSEXP=lambdaNatLogScale, weightsSEXP=None, useWeightsSEXP=False, tolSEXP=betaTol,
-                             maxitSEXP=maxit, useQRSEXP=useQR, minmuSEXP=minmu, engine=engine)
+                             lambdaSEXP=lambdaNatLogScale, weightsSEXP=weights, useWeightsSEXP=weights is not None,
+                             tolSEXP=betaTol, maxitSEXP=maxit, useQRSEXP=useQR, minmuSEXP=minmu, engine=engine)
     mu = nf * np.exp(betaRes["beta_mat"] @ x.T)
-    logLike = nbinomLogLike(counts, mu, alpha_hat)
+    logLike = nbinomLogLike(counts, mu, alpha_hat, weights)
     betaConv = betaRes["iter"] < maxit
     betaMatrix = betaRes["beta_mat"] / LN2
     betaSE = np.sqrt(np.maximum(betaRes["beta_var_mat"], 0.0)) / LN2
@@ -392,7 +487,8 @@ def fitNbinomGLMs(counts, nf, x, alpha_hat, lambda_=None, engine=None, betaTol=1
     if True:
         if rows.size:
             o = fitNbinomGLMsOptim(counts, np.broadcast_to(nf, counts.shape), x, lambda_, rows, rowStable, alpha_hat,
-                                   betaMatrix, betaSE, betaConv, beta_mat / LN2, mu, logLike, minmu=minmu)
+                                   betaMatrix, betaSE, betaConv, beta_mat / LN2, mu, logLike, minmu=minmu,
+                                   weights=weights)
             betaMatrix, betaSE, betaConv, mu, logLike = (o["betaMatrix"], o["betaSE"], o["betaConv"], o["mu"],
                                                          o["logLike"])
     return {"logLike": logLike, "betaConv": betaConv, "betaMatrix": betaMatrix, "betaSE": betaSE, "mu": mu,
@@ -400,10 +496,10 @@ def fitNbinomGLMs(counts, nf, x, alpha_hat, lambda_=None, engine=None, betaTol=1
 
 
 def nbinomWaldTest(counts, nf, x, dispersion, engine=None, betaTol=1e-8, maxit=100, useQR=True, minmu=0.5,
-                   useOptim=True):
+                   useOptim=True, weights=None):
     """R/core.R:1332-1565, betaPrior=FALSE, useT=FALSE; Cook's distances are not restated."""
     fit = fitNbinomGLMs(counts, nf, x, dispersion, engine=engine, betaTol=betaTol, maxit=maxit, useQR=useQR,
-                        minmu=minmu, useOptim=useOptim)
+                        minmu=minmu, useOptim=useOptim, weights=weights)
     with np.errstate(divide="ignore", invalid="ignore"):
         WaldStatistic = fit["betaMatrix"] / fit["betaSE"]
     WaldPvalue = 2.0 * _sp.ndtr(-np.abs(WaldStatistic))
@@ -526,11 +622,14 @@ def replaceOutliers(counts, cooks, sizeFactors, x, trim=0.2, cooksCutoff=None, m
     return out, replace, whichSamples
 
 
-def getContrast(counts, nf, x, dispersion, betaMatrix, contrast, betaPriorVar=None, engine=None, minmu=0.5):
+def getContrast(counts, nf, x, dispersion, betaMatrix, contrast, betaPriorVar=None, engine=None, minmu=0.5,
+                weights=None):
     """R/results.R:760-827: a numeric contrast c of the fitted coefficients, batched over genes through fitBeta's
     maxit = 0 mode (no IRLS iteration: covariance at the given betas, c'beta and sqrt(c' Sigma c)).  `counts` are the
     counts the model was fitted to (replaceCounts after an outlier refit), `betaMatrix` is on the log2 scale; rows are
-    the non-all-zero genes.  Returns log2FoldChange, lfcSE, stat, pvalue (useT = FALSE)."""
+    the non-all-zero genes.  `weights` (optional, the same rows) are normalised by their row maximum and passed to
+    fitBeta, without the rank tests (R/results.R:786-807).  Returns log2FoldChange, lfcSE, stat, pvalue (useT =
+    FALSE)."""
     engine = engine or _default_engine
     counts = np.asarray(counts)
     n, m = counts.shape
@@ -541,9 +640,17 @@ def getContrast(counts, nf, x, dispersion, betaMatrix, contrast, betaPriorVar=No
     if betaPriorVar is None:
         betaPriorVar = np.full(p, 1e6)                                    # betaPrior = FALSE (R/core.R:1421)
     lam = 1.0 / (LN2 ** 2 * np.asarray(betaPriorVar, dtype=np.float64))
+    if weights is not None:
+        w = np.asarray(weights, dtype=np.float64)
+        if w.shape != counts.shape:
+            raise ValueError(f"weights have shape {w.shape}, expected {counts.shape}")
+        if not np.all(w >= 0):
+            raise ValueError("weights must be non-negative and not NaN")
+        weights = w / w.max(axis=1)[:, None]
     r = engine.fitBeta(ySEXP=counts, xSEXP=x, nfSEXP=np.broadcast_to(nf, counts.shape), alpha_hatSEXP=dispersion,
                        contrastSEXP=contrast, beta_matSEXP=LN2 * np.asarray(betaMatrix, dtype=np.float64),
-                       lambdaSEXP=lam, weightsSEXP=None, useWeightsSEXP=False, tolSEXP=1e-8, maxitSEXP=0,
+                       lambdaSEXP=lam, weightsSEXP=weights, useWeightsSEXP=weights is not None, tolSEXP=1e-8,
+                       maxitSEXP=0,
                        useQRSEXP=False, minmuSEXP=minmu)
     est = np.asarray(r["contrast_num"]).reshape(n) / LN2
     se = np.asarray(r["contrast_denom"]).reshape(n) / LN2
@@ -552,13 +659,19 @@ def getContrast(counts, nf, x, dispersion, betaMatrix, contrast, betaPriorVar=No
     return {"log2FoldChange": est, "lfcSE": se, "stat": stat, "pvalue": 2.0 * _sp.ndtr(-np.abs(stat))}
 
 
-def _fit_intercept_only(counts, nf, alpha_hat):
-    """R/fitNbinomGLMs.R:99-137: reduced model ~1 with the default wide prior needs no IRLS (no native call)."""
+def _fit_intercept_only(counts, nf, alpha_hat, weights=None):
+    """R/fitNbinomGLMs.R:99-137: reduced model ~1 with the default wide prior needs no IRLS (no native call).  With
+    weights: beta = log2(sum(w K/s) / sum(w)), and the log-likelihood and the working weights are multiplied by w."""
     norm = counts / nf
-    betaMatrix = np.log2(norm.mean(axis=1))[:, None]
+    if weights is None:
+        betaMatrix = np.log2(norm.mean(axis=1))[:, None]
+    else:
+        betaMatrix = np.log2((weights * norm).sum(axis=1) / weights.sum(axis=1))[:, None]
     mu = nf * (2.0 ** betaMatrix)
-    logLike = nbinomLogLike(counts, mu, alpha_hat)
+    logLike = nbinomLogLike(counts, mu, alpha_hat, weights)
     w = 1.0 / (1.0 / mu + alpha_hat[:, None])
+    if weights is not None:
+        w = weights * w
     xtwx = w.sum(axis=1)
     return {"logLike": logLike, "betaConv": np.ones(len(counts), bool), "betaMatrix": betaMatrix,
             "betaSE": (np.sqrt(1.0 / xtwx) / LN2)[:, None], "mu": mu, "betaIter": np.ones(len(counts)),
@@ -566,20 +679,20 @@ def _fit_intercept_only(counts, nf, alpha_hat):
 
 
 def nbinomLRT(counts, nf, full, reduced, dispersion, engine=None, betaTol=1e-8, maxit=100, useQR=True, minmu=0.5,
-              useOptim=True):
+              useOptim=True, weights=None):
     """R/core.R:1787-2012 with user-supplied model matrices, betaPrior=FALSE; Cook's distances are not restated.
-    `full` / `reduced` are m x p model matrices (reduced nested in full)."""
+    `full` / `reduced` are m x p model matrices (reduced nested in full); `weights`: normalised weights or None."""
     from scipy import stats as _st
     counts = np.asarray(counts)
     if reduced.shape[1] >= full.shape[1]:
         raise ValueError("less than one degree of freedom, perhaps full and reduced models are not in the correct order")
     fullModel = fitNbinomGLMs(counts, nf, full, dispersion, engine=engine, betaTol=betaTol, maxit=maxit, useQR=useQR,
-                              minmu=minmu, useOptim=useOptim)
+                              minmu=minmu, useOptim=useOptim, weights=weights)
     if reduced.shape[1] == 1 and np.all(reduced == 1):
-        reducedModel = _fit_intercept_only(counts, nf, dispersion)
+        reducedModel = _fit_intercept_only(counts, nf, dispersion, weights)
     else:
         reducedModel = fitNbinomGLMs(counts, nf, reduced, dispersion, engine=engine, betaTol=betaTol, maxit=maxit,
-                                     useQR=useQR, minmu=minmu, useOptim=useOptim)
+                                     useQR=useQR, minmu=minmu, useOptim=useOptim, weights=weights)
     df = full.shape[1] - reduced.shape[1]
     LRTStatistic = 2.0 * (fullModel["logLike"] - reducedModel["logLike"])
     LRTPvalue = _st.chi2.sf(LRTStatistic, df)
@@ -695,7 +808,7 @@ def fitGLMsWithPrior(counts, nf, factors, dispersion, baseMean, dispFit, engine=
 
 
 def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.inf, useOptim=True, betaPrior=False,
-          factors=None):
+          factors=None, weights=None, weightThreshold=1e-2, minmu=0.5):
     """R/core.R:280-432 with test='Wald', fitType='parametric', betaPrior=FALSE by default.
     minReplicatesForReplace: the reference's default is 7 (outlier replacement + refit whenever a design cell has >= 7
     samples, R/core.R:419-426, refitWithoutOutliers :2484-2565); the default here is Inf = off, which is what the
@@ -705,6 +818,11 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     Wald test goes through fitGLMsWithPrior -- coefficients, SEs, statistics and deviance of the MAP fit on the
     expanded matrix, Cook's distances from the MLE fit -- and the result also carries `mleBetaMatrix`,
     `betaPriorVar` and `modelMatrix` (the expanded matrix).
+    weights: an (N, m) matrix of observation weights (the "weights" assay).  getAndCheckWeights normalises each row by
+    its maximum and flags the rows whose weights leave the design rank deficient; those rows are treated as all-zero
+    rows (NaN results) and reported in `weightsFail`.  baseMean / baseVar use the raw weights, every fit the
+    normalised ones.  Not supported with betaPrior=True or outlier replacement (ValueError).
+    minmu: the lower bound on the fitted mean (R's minmu; 1e-6 is the usual single-cell setting).
     Returns per-gene vectors over ALL rows; all-zero rows carry NaN (buildDataFrameWithNARows, R/core.R:2232)."""
     engine = engine or _default_engine
     counts = np.asarray(counts)
@@ -717,17 +835,36 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
             raise ValueError("betaPrior=True: x must be the standard model matrix of the factors, factorDesign(factors)[0]")
         if np.isfinite(minReplicatesForReplace):
             raise ValueError("outlier replacement (finite minReplicatesForReplace) is not supported with betaPrior=True")
+    if weights is not None:
+        if np.shape(weights) != counts.shape:
+            raise ValueError(f"weights have shape {np.shape(weights)}, expected {counts.shape}")
+        if betaPrior:
+            raise ValueError("observation weights are not supported with betaPrior=True")
+        if np.isfinite(minReplicatesForReplace):
+            raise ValueError("observation weights are not supported with outlier replacement "
+                             "(finite minReplicatesForReplace)")
+        wnAll, weightsFail = getAndCheckWeights(weights, x, weightThreshold)
     if sizeFactors is None:
         sizeFactors = estimateSizeFactorsForMatrix(counts)
-    mvAll = getBaseMeansAndVariances(counts, sizeFactors)
+    mvAll = getBaseMeansAndVariances(counts, sizeFactors, weights)
     nz = ~mvAll["allZero"]
+    wnz = None
+    if weights is not None:
+        nz = nz & ~weightsFail
+        wnz = wnAll[nz]
+        if weightsFail.any():
+            import warnings
+            warnings.warn(f"for {int(weightsFail.sum())} row(s), the weights as supplied won't allow parameter "
+                          "estimation, producing a degenerate design matrix. These rows have been flagged in "
+                          "weightsFail and treated as if the row contained all zeros.")
     cnz = counts[nz]
     mv = {k: v[nz] for k, v in mvAll.items()}
-    ge = estimateDispersionsGeneEst(cnz, sizeFactors, x, engine=engine, mv=mv)
+    ge = estimateDispersionsGeneEst(cnz, sizeFactors, x, engine=engine, mv=mv, weights=wnz,
+                                    weightThreshold=weightThreshold, minmu=minmu)
     tf = estimateDispersionsFit(ge["dispGeneEst"], ge["baseMean"])
     dispPriorVar = estimateDispersionsPriorVar(tf["varLogDispEsts"], m, p, ge["dispGeneEst"], tf["dispFit"])
     mp = estimateDispersionsMAP(cnz, x, ge["mu"], ge["dispGeneEst"], tf["dispFit"], dispPriorVar,
-                                tf["varLogDispEsts"], engine=engine)
+                                tf["varLogDispEsts"], engine=engine, weights=wnz, weightThreshold=weightThreshold)
     nf = np.broadcast_to(sizeFactors[None, :], cnz.shape)
     prior = {}
     if betaPrior:
@@ -740,7 +877,8 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
         cooks = calculateCooksDistance(cnz, gp["mu"], gp["H"], sizeFactors, x)             # MLE mu / H (R/core.R:1416-1460)
         prior = {"betaPriorVar": gp["betaPriorVar"], "modelMatrix": gp["modelMatrix"]}
     else:
-        wt = nbinomWaldTest(cnz, nf, x, mp["dispersion"], engine=engine, useOptim=useOptim)
+        wt = nbinomWaldTest(cnz, nf, x, mp["dispersion"], engine=engine, useOptim=useOptim, minmu=minmu,
+                            weights=wnz)
         cooks = calculateCooksDistance(cnz, wt["mu"], wt["hat_diagonals"], sizeFactors, x)  # R/core.R:1457-1460
     per_gene = {"baseMean": mv["baseMean"], "dispGeneEst": ge["dispGeneEst"], "dispFit": tf["dispFit"],
                 "dispMAP": mp["dispMAP"], "dispersion": mp["dispersion"], "dispOutlier": mp["dispOutlier"].astype(float),
@@ -801,5 +939,10 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
                 "trendCoefs": tf["coefs"], "varLogDispEsts": tf["varLogDispEsts"], "n_refit_geneest": ge["n_refit"],
                 "n_refit_map": mp["n_refit"]})
     res["baseMean"] = np.where(nz, res["baseMean"], 0.0)
+    if weights is not None:
+        res["baseMean"] = np.where(mvAll["allZero"], 0.0, mvAll["baseMean"])    # weightsFail rows keep theirs
+        res["weightsFail"] = weightsFail
+        res["weights"] = wnz
+        res["idx"] = np.flatnonzero(nz)
     res.update(extra)
     return res

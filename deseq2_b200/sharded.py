@@ -137,7 +137,9 @@ def sharded_DESeq_device(y_local, x, sizeFactors, **kw):
     dict (device tensors) plus "gathered": the results of ALL genes on every rank, in rank order, and "collectives".
     betaPrior=True, factors=... (passed on to DESeq_device): the prior variance is estimated over all genes
     (R/parallel.R:39-40) through ONE more packed all-gather of the p - 1 non-intercept MLE columns; the gathered
-    results then carry the expanded matrix's columns."""
+    results then carry the expanded matrix's columns.
+    weights=w_local (passed on to DESeq_device): this shard's rows of the observation weights, gene-major like
+    y_local; no collective is added (the global step's gather carries the weighted baseMean)."""
     from . import device_pipeline as DP
     pg = PackedGather(y_local.shape[0], y_local.device)
     res = DP.DESeq_device(y_local, x, sizeFactors, allgather=pg, **kw)

@@ -136,6 +136,21 @@ int b200nb_prep_dev(const void* y, int y_type, const double* x, const double* pr
                     double* beta0, void* stream);
 int b200nb_trend_fit_dev(const double* means, const double* disps, int n, double min_disp, double* out4,
                          void* stream);
+/* b200nb_prep_weighted_dev: b200nb_prep_dev with observation weights (gene-major n x ld, raw assay weights), p <= 32:
+ *   base_mean, base_var of w * K/s with the raw weights (R/core.R:2140-2145); alpha0 from the weighted moments and
+ *   the unweighted rough dispersion; mu_lin and beta0 unweighted (pass mu_lin = NULL: with weights the reference
+ *   fits mu by IRLS);
+ *   out_weights_norm (gene-major n x ld) = weights / row maximum, padding columns 0       R/core.R:2700-2702
+ *   out_weights_fail[n] = 1 where rank(w * X) < p or X on the samples with normalised w > weight_threshold (all-zero
+ *     columns dropped) is rank deficient, R's qr() rank with tol 1e-7                     R/core.R:2706-2722
+ *   out_status (one device int, zeroed by the call) = number of rows with a negative, NaN or infinite weight or no
+ *     positive weight; the reference stops on them, so the caller must raise when it is not 0. */
+int b200nb_prep_weighted_dev(const void* y, int y_type, const double* x, const double* proj,
+                             const double* size_factors, double xim, double min_disp, double max_disp, double minmu,
+                             int n, int m, int p, long long ld, double* base_mean, double* base_var,
+                             int32_t* all_zero, double* alpha0, double* mu_lin, double* beta0, const double* weights,
+                             double weight_threshold, double* out_weights_norm, int32_t* out_weights_fail,
+                             int32_t* out_status, void* stream);
 
 /* b200nb_cooks_dev: calculateCooksDistance + recordMaxCooks + robustMethodOfMomentsDisp (R/core.R:2277-2359).
  * cells = distinct design rows: cell_ptr (ncell+1) / cell_samples (m, sample indices grouped by cell), device ints.
