@@ -49,9 +49,12 @@ SIGNATURES = {
     "b200nb_prep_dev": [vp, _I, vp, vp, vp, _D, _D, _D, _D, _I, _I, _I, _LL, vp, vp, vp, vp, vp, vp, vp],
     "b200nb_prep_weighted_dev": [vp, _I, vp, vp, vp, _D, _D, _D, _D, _I, _I, _I, _LL, vp, vp, vp, vp, vp, vp, vp, _D,
                                  vp, vp, vp, vp],
+    "b200nb_prep_nf_dev": [vp, _I, vp, vp, vp, _D, _D, _D, _D, _I, _I, _I, _LL, vp, vp, vp, vp, vp, vp, vp],
     "b200nb_trend_fit_dev": [vp, vp, _I, _D, vp, vp],
     "b200nb_cooks_dev": [vp, _I, vp, vp, vp, vp, vp, _I, _I, _I, _I, _LL, vp, vp, vp, vp],
+    "b200nb_cooks_nf_dev": [vp, _I, vp, vp, vp, vp, vp, _I, _I, _I, _I, _LL, vp, vp, vp, vp],
     "b200nb_size_factors_dev": [vp, _I, _I, _I, _I, _LL, vp, vp, vp, vp, vp, vp],
+    "b200nb_size_factors_norm_dev": [vp, _I, vp, _I, _I, _I, _LL, vp, vp, vp, vp, vp, vp],
     "b200nb_beta_prior_quantile_dev": [vp, _I, _I, vp, vp, vp, vp, _I, _D, vp, vp],
     "b200nb_last_error": [],
     "b200nb_device_count": [],

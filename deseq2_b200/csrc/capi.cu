@@ -1306,6 +1306,19 @@ int b200nb_prep_weighted_dev(const void* y, int y_type, const double* x, const d
   return prep_launch(a, stream);
 }
 
+int b200nb_prep_nf_dev(const void* y, int y_type, const double* x, const double* proj, const double* nf, double xim,
+                       double min_disp, double max_disp, double minmu, int n, int m, int p, long long ld,
+                       double* base_mean, double* base_var, int32_t* all_zero, double* alpha0, double* mu_lin,
+                       double* beta0, void* stream) {
+  nb::PrepArgs a;
+  if (prep_args(a, y, y_type, x, proj, nullptr, xim, min_disp, max_disp, minmu, n, m, p, ld, base_mean, base_var,
+                all_zero, alpha0, mu_lin, beta0))
+    return 1;
+  if (n > 0 && nf == nullptr) return fail("prep_nf needs the normalization factor matrix");
+  a.nf = nf;
+  return prep_launch(a, stream);
+}
+
 int b200nb_trend_fit_dev(const double* means, const double* disps, int n, double min_disp, double* out4,
                          void* stream) {
   if (n < 1) return fail("trend fit needs at least one gene");
@@ -1314,16 +1327,37 @@ int b200nb_trend_fit_dev(const double* means, const double* disps, int n, double
   return 0;
 }
 
+static int cooks_common(const void* y, int y_type, const double* mu, const double* hat, const double* size_factors,
+                        const double* nf, const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n,
+                        int m, int p, long long ld, double* cooks, double* max_cooks, double* robust_disp,
+                        void* stream);
+
 int b200nb_cooks_dev(const void* y, int y_type, const double* mu, const double* hat, const double* size_factors,
                      const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n, int m, int p,
                      long long ld, double* cooks, double* max_cooks, double* robust_disp, void* stream) {
+  return cooks_common(y, y_type, mu, hat, size_factors, nullptr, cell_ptr, cell_samples, ncell, n, m, p, ld, cooks,
+                      max_cooks, robust_disp, stream);
+}
+
+int b200nb_cooks_nf_dev(const void* y, int y_type, const double* mu, const double* hat, const double* nf,
+                        const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n, int m, int p,
+                        long long ld, double* cooks, double* max_cooks, double* robust_disp, void* stream) {
+  if (n > 0 && nf == nullptr) return fail("cooks_nf needs the normalization factor matrix");
+  return cooks_common(y, y_type, mu, hat, nullptr, nf, cell_ptr, cell_samples, ncell, n, m, p, ld, cooks, max_cooks,
+                      robust_disp, stream);
+}
+
+static int cooks_common(const void* y, int y_type, const double* mu, const double* hat, const double* size_factors,
+                        const double* nf, const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n,
+                        int m, int p, long long ld, double* cooks, double* max_cooks, double* robust_disp,
+                        void* stream) {
   if (check_dims(n, m, p)) return 1;
   if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
   if (ncell < 1 || ncell > m) return fail("bad number of design cells %d", ncell);
   nb::CooksArgs a{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.mu = mu; a.hat = hat; a.size_factors = size_factors;
   a.cell_ptr = cell_ptr; a.cell_samples = cell_samples; a.ncell = ncell; a.n = n; a.m = m; a.p = p; a.ld = ld;
-  a.cooks = cooks; a.max_cooks = max_cooks; a.robust_disp = robust_disp;
+  a.cooks = cooks; a.max_cooks = max_cooks; a.robust_disp = robust_disp; a.nf = nf;
   a.max_cell = 0;
   if (n > 0 && m > 256) {
     // long rows: the size of the largest cell decides how much per-warp scratch the trimmed means need (one small
@@ -1361,19 +1395,34 @@ int b200nb_beta_prior_quantile_dev(const double* beta_log2, int n, int p, const 
   return 0;
 }
 
-int b200nb_size_factors_dev(const void* y, int y_type, int poscounts, int n, int m, long long ld,
-                            double* loggeomeans, double* scratch_gm, double* scratch_cm, double* size_factors,
-                            int32_t* n_finite, void* stream) {
+static int size_factors_common(const void* y, int y_type, const double* divisor, int poscounts, int n, int m,
+                               long long ld, double* loggeomeans, double* scratch_gm, double* scratch_cm,
+                               double* size_factors, int32_t* n_finite, void* stream) {
   if (check_dims(n, m, 1)) return 1;
   if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
   if (n < 1) return fail("size factors need at least one gene");
   nb::SizeFactorArgs a{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.poscounts = poscounts ? 1 : 0; a.n = n; a.m = m; a.ld = ld;
   a.loggeomeans = loggeomeans; a.ratios = scratch_gm; a.ratios_colmajor = scratch_cm; a.size_factors = size_factors;
-  a.n_finite = n_finite;
+  a.n_finite = n_finite; a.divisor = divisor;
   CU(nb::launch_size_factors(a, (cudaStream_t)stream));
   g_launches += 3;
   return 0;
+}
+
+int b200nb_size_factors_dev(const void* y, int y_type, int poscounts, int n, int m, long long ld,
+                            double* loggeomeans, double* scratch_gm, double* scratch_cm, double* size_factors,
+                            int32_t* n_finite, void* stream) {
+  return size_factors_common(y, y_type, nullptr, poscounts, n, m, ld, loggeomeans, scratch_gm, scratch_cm,
+                             size_factors, n_finite, stream);
+}
+
+int b200nb_size_factors_norm_dev(const void* y, int y_type, const double* divisor, int poscounts, int n, int m,
+                                 long long ld, double* loggeomeans, double* scratch_gm, double* scratch_cm,
+                                 double* size_factors, int32_t* n_finite, void* stream) {
+  if (divisor == nullptr) return fail("size_factors_norm needs the divisor matrix");
+  return size_factors_common(y, y_type, divisor, poscounts, n, m, ld, loggeomeans, scratch_gm, scratch_cm,
+                             size_factors, n_finite, stream);
 }
 
 /* ------------------------------------------------------------------ host entry points */

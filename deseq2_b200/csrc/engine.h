@@ -187,6 +187,9 @@ struct PrepArgs {
   int32_t* weights_fail;       // n: 1 = a rank test of getAndCheckWeights fails
   int32_t* status;             // 1 int, incremented once per row with a negative / NaN / infinite weight or no
                                // positive weight (the reference stops on each of these)
+  // gene-specific normalization factors (b200nb_prep_nf_dev; nullptr: size_factors): gene-major n x ld, read in place
+  // of size_factors; xim is then mean(1 / colMeans(nf)) over the non-all-zero rows
+  const double* nf;
 };
 cudaError_t launch_prep(const PrepArgs& a, cudaStream_t stream);
 
@@ -202,6 +205,7 @@ struct SizeFactorArgs {
   double* ratios_colmajor;     // n x m column-major scratch
   double* size_factors;        // m (out)
   int* n_finite;               // out: genes with a finite log geometric mean
+  const double* divisor;       // gene-major n x ld or nullptr: the size factors of K / divisor (estimateNormFactors)
 };
 cudaError_t launch_size_factors(const SizeFactorArgs& a, cudaStream_t stream);
 
@@ -234,6 +238,7 @@ struct CooksArgs {
   double* cooks;               // gene-major n x ld or nullptr
   double* max_cooks;           // n
   double* robust_disp;         // n
+  const double* nf;            // gene-major n x ld normalization factors, read in place of size_factors; or nullptr
 };
 cudaError_t launch_cooks(const CooksArgs& a, cudaStream_t stream);
 cudaError_t launch_trend_fit(const double* means, const double* disps, int n, double min_disp, double* out4,

@@ -67,14 +67,22 @@ __host__ __device__ __forceinline__ size_t prep_weighted_extra(int mpad, int p, 
   else return 0;
 }
 
+// the divisor of sample j of the gene at row offset off: its normalization factor (NF) or its size factor
+template <bool NF>
+__device__ __forceinline__ double norm_factor(const double* __restrict__ nf, const double* sf, size_t off, int j) {
+  if constexpr (NF) return __ldg(nf + off + j);
+  else return sf[j];
+}
+
 // the per-gene outputs of the weighted variant (lane 0)
 __device__ __forceinline__ void store_weight_flags(const PrepArgs& A, int g, bool invalid, bool ok) {
   A.weights_fail[g] = ok ? 0 : 1;
   if (invalid) atomicAdd(A.status, 1);
 }
 
-template <bool W>
+template <bool W, bool NF>
 __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
+  static_assert(!(W && NF), "observation weights together with normalization factors are not supported");
   extern __shared__ __align__(16) double smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -87,7 +95,8 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
   double* coefl = coef + 32;                           // 32: P * log(norm + .1)
   double* wn = coefl + 32;                             // W: mpad, the weights (raw, then normalised)
   double* gram = wn + mpad;                            // W: 2 p x p Gram matrices
-  for (int j = threadIdx.x; j < A.m; j += blockDim.x) sf[j] = A.size_factors[j];
+  if constexpr (!NF)
+    for (int j = threadIdx.x; j < A.m; j += blockDim.x) sf[j] = A.size_factors[j];
   __syncthreads();
   const int g = blockIdx.x * (blockDim.x >> 5) + warp;
   if (g >= A.n) return;
@@ -97,7 +106,7 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
   bool bad = false;
   for (int j = lane; j < A.m; j += 32) {
     const double y = A.y_is_f64 ? static_cast<const double*>(A.y)[off + j] : (double)static_cast<const int32_t*>(A.y)[off + j];
-    const double v = y / sf[j];
+    const double v = y / norm_factor<NF>(A.nf, sf, off, j);   // NF: the gene's row, read again for mu_lin
     vn[j] = v;
     vl[j] = log(v + 0.1);
     if constexpr (W) {
@@ -149,7 +158,7 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
     const double mu1 = fmax(1.0, f);
     const double d = vn[j] - mu1;
     rs += (d * d - mu1) / (mu1 * mu1);
-    if (A.mu_lin != nullptr) A.mu_lin[off + j] = fmax(f * sf[j], A.minmu);
+    if (A.mu_lin != nullptr) A.mu_lin[off + j] = fmax(f * norm_factor<NF>(A.nf, sf, off, j), A.minmu);
   }
   rs = warp_allreduce_sum(rs);
   bool invalid = false, ok = true;
@@ -209,8 +218,9 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
 // prep_kernel streams the p x m projection and the m x p design through every gene (2 p m loads and FMAs per gene,
 // L2 latency bound at 8 warps per SM); here a sample only adds its value and its log to its
 // group's lane-private slot, the projection is applied to the G group sums and the fitted value is read per group.
-template <bool W>
+template <bool W, bool NF>
 __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int mpad, int ps) {
+  static_assert(!(W && NF), "observation weights together with normalization factors are not supported");
   extern __shared__ __align__(16) double smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -221,7 +231,8 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
   int* rep = reinterpret_cast<int*>(xg + (size_t)G * ps);          // 32: one sample of each group
   unsigned char* gidb = reinterpret_cast<unsigned char*>(rep + 32);   // mpad
   double* wrow = reinterpret_cast<double*>(gidb + mpad) +
-                 (size_t)warp * (mpad + 2 * (size_t)G * 32 + 3 * 32 + 2 * 32 + prep_weighted_extra<W>(mpad, p, true));
+                 (size_t)warp * (mpad + 2 * (size_t)G * 32 + 3 * 32 + 2 * 32 + prep_weighted_extra<W>(mpad, p, true) +
+                                 (NF ? mpad : 0));
   double* vn = wrow;                                   // normalised counts
   double* accN = wrow + mpad;                          // G x 32 lane-private sums of the normalised counts
   double* accL = accN + (size_t)G * 32;                // G x 32: of log(norm + 0.1)
@@ -233,8 +244,9 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
   double* gsW = coefl + 32;                            // W, 32: group sums of the squared normalised weights
   double* gsC = gsW + 32;                              // W, 32: group counts of normalised weights > threshold
   double* gram = gsC + 32;                             // W: p x p Gram matrix
+  double* nfw = coefl + 32;                            // NF: mpad, the gene's normalization factors
   for (int j = threadIdx.x; j < A.m; j += blockDim.x) {
-    sf[j] = A.size_factors[j];
+    if constexpr (!NF) sf[j] = A.size_factors[j];
     const int g = A.gid[j];
     gidb[j] = (unsigned char)g;
     rep[g] = j;                                        // any sample of the group (racing writers, all valid)
@@ -253,9 +265,14 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
   double s = 0.0, s2 = 0.0, raw = 0.0;
   double wmax = 0.0;
   bool bad = false;
+  // NF: the gene's factors go to a per-warp shared row first (each lane its own entries), so that the loops below
+  // keep no more live state than with size factors (a second read of the global row spilled)
+  if constexpr (NF)
+    for (int j = lane; j < A.m; j += 32) nfw[j] = A.nf[off + j];
+  const double* nfr = NF ? nfw : sf;
   for (int j = lane; j < A.m; j += 32) {
     const double y = A.y_is_f64 ? static_cast<const double*>(A.y)[off + j] : (double)static_cast<const int32_t*>(A.y)[off + j];
-    const double v = y / sf[j];
+    const double v = y / nfr[j];                       // NF: group sums of K/nf, fits scaled by nf_ij
     vn[j] = v;
     const int slot = gidb[j] * 32 + lane;
     accN[slot] += v;
@@ -315,7 +332,7 @@ __global__ void __launch_bounds__(256) prep_grouped_kernel(const PrepArgs A, int
     const double mu1 = fmax(1.0, f);
     const double d = vn[j] - mu1;
     rs += (d * d - mu1) / (mu1 * mu1);
-    if (A.mu_lin != nullptr) A.mu_lin[off + j] = fmax(f * sf[j], A.minmu);
+    if (A.mu_lin != nullptr) A.mu_lin[off + j] = fmax(f * nfr[j], A.minmu);
   }
   rs = warp_allreduce_sum(rs);
   bool invalid = false, ok = true;
@@ -518,23 +535,28 @@ __global__ void __launch_bounds__(512) trend_fit_kernel(const double* __restrict
 
 }  // namespace
 
-// a.weights != nullptr selects the weighted instantiations; their larger per-warp scratch may run fewer warps per CTA
+// a.weights != nullptr selects the weighted instantiations (their larger per-warp scratch may run fewer warps per
+// CTA), a.nf != nullptr the normalization-factor ones (the grouped one adds an mpad row per warp; the shared
+// size-factor row goes unused)
 cudaError_t launch_prep(const PrepArgs& a, cudaStream_t stream) {
   if (a.n == 0) return cudaSuccess;
   const bool weighted = a.weights != nullptr;
+  const bool nf = a.nf != nullptr;
   if (a.G > 0 && a.G <= 32) {
     const int mpad = (a.m + 7) & ~7, ps = a.p | 1;
     int warps = 8;
     const size_t fixed = ((size_t)mpad + (size_t)a.p * a.G + (size_t)a.G * ps) * sizeof(double) + 32 * sizeof(int) + mpad;
     const size_t per_warp = ((size_t)mpad + 2 * (size_t)a.G * 32 + 5 * 32 +
-                             (weighted ? prep_weighted_extra<true>(mpad, a.p, true) : 0)) * sizeof(double);
+                             (weighted ? prep_weighted_extra<true>(mpad, a.p, true) : 0) + (nf ? mpad : 0)) *
+                            sizeof(double);
     size_t smem = fixed + warps * per_warp;
-    while (weighted && warps > 1 && smem > 200 * 1024) {
+    while ((weighted || nf) && warps > 1 && smem > 200 * 1024) {
       warps >>= 1;
       smem = fixed + warps * per_warp;
     }
     if (smem <= 200 * 1024) {
-      const auto kern = weighted ? prep_grouped_kernel<true> : prep_grouped_kernel<false>;
+      const auto kern = weighted ? prep_grouped_kernel<true, false>
+                                 : (nf ? prep_grouped_kernel<false, true> : prep_grouped_kernel<false, false>);
       cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
       kern<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a, mpad, ps);
@@ -549,7 +571,7 @@ cudaError_t launch_prep(const PrepArgs& a, cudaStream_t stream) {
     warps >>= 1;
     smem = ((size_t)mpad + (size_t)warps * per_warp) * sizeof(double);
   }
-  const auto kern = weighted ? prep_kernel<true> : prep_kernel<false>;
+  const auto kern = weighted ? prep_kernel<true, false> : (nf ? prep_kernel<false, true> : prep_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   kern<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a);
@@ -701,6 +723,8 @@ __host__ __device__ inline size_t cooks_warp_doubles(int m, int mpad, int max_ce
   return (size_t)mpad + sqlen + (sqlen == mpad ? (mpad + 7) / 8 : 0);
 }
 
+// NF: the robust dispersion and the trimmed means are of K/nf (gene-major nf); otherwise of K/s (shared s)
+template <bool NF>
 __global__ void __launch_bounds__(256) cooks_kernel(const CooksArgs A) {
   extern __shared__ __align__(16) double smem[];
   const int lane = threadIdx.x & 31;
@@ -717,7 +741,7 @@ __global__ void __launch_bounds__(256) cooks_kernel(const CooksArgs A) {
   for (int i = threadIdx.x; i <= A.ncell; i += blockDim.x) cell_ptr[i] = A.cell_ptr[i];
   for (int i = threadIdx.x; i < A.m; i += blockDim.x) {
     cell_samples[i] = A.cell_samples[i];
-    sf[i] = A.size_factors[i];
+    if constexpr (!NF) sf[i] = A.size_factors[i];
   }
   __syncthreads();
   const double trimratio[3] = {1.0 / 3.0, 1.0 / 4.0, 1.0 / 8.0};
@@ -726,9 +750,11 @@ __global__ void __launch_bounds__(256) cooks_kernel(const CooksArgs A) {
   if (g >= A.n) return;
   const size_t off = (size_t)g * A.ld;
   double s = 0.0;
+  if constexpr (NF)                                             // staged in vn and divided in place (as in prep)
+    for (int j = lane; j < A.m; j += 32) vn[j] = A.nf[off + j];
   for (int j = lane; j < A.m; j += 32) {
     const double y = A.y_is_f64 ? static_cast<const double*>(A.y)[off + j] : (double)static_cast<const int32_t*>(A.y)[off + j];
-    const double v = y / sf[j];
+    const double v = y / (NF ? vn[j] : sf[j]);
     vn[j] = v;
     s += v;
   }
@@ -815,9 +841,10 @@ cudaError_t launch_cooks(const CooksArgs& a, cudaStream_t stream) {
   int warps = (2 * bytes(8) <= 220 * 1024) ? 8 : 4;
   while (warps > 1 && bytes(warps) > 200 * 1024) warps >>= 1;
   const size_t smem = bytes(warps);
-  cudaError_t e = cudaFuncSetAttribute(cooks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  const auto kern = a.nf != nullptr ? cooks_kernel<true> : cooks_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  cooks_kernel<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a);
+  kern<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a);
   return cudaGetLastError();
 }
 

@@ -31,6 +31,10 @@ __device__ __forceinline__ double value_of(unsigned long long k) {
   return __longlong_as_double((long long)b);
 }
 
+// DIV: the ratios of K / divisor (estimateNormFactors, R/core.R:2160): log(K/d) - loggeomean, where loggeomean is the
+// mean of log(K/d) for "ratio" and log(geoMeanNZ(K)) = log(exp(sum log K[K > 0] / m)) of the raw counts for
+// "poscounts" (the geoMeans estimateSizeFactors passes, R/methods.R:377-390)
+template <bool DIV>
 __global__ void __launch_bounds__(256) sf_ratio_kernel(const SizeFactorArgs A) {
   init_log_table();
   const int lane = threadIdx.x & 31;
@@ -44,9 +48,15 @@ __global__ void __launch_bounds__(256) sf_ratio_kernel(const SizeFactorArgs A) {
     const double y = A.y_is_f64 ? static_cast<const double*>(A.y)[off + j]
                                 : (double)static_cast<const int32_t*>(A.y)[off + j];
     if (y > 0.0) {
-      const double l = log_pos(y);
-      A.ratios[off + j] = l;                                 // log K_ij for now; the mean is subtracted below
-      s += l;
+      if constexpr (DIV) {
+        const double l = log(y / A.divisor[off + j]);
+        A.ratios[off + j] = l;
+        s += A.poscounts ? log_pos(y) : l;
+      } else {
+        const double l = log_pos(y);
+        A.ratios[off + j] = l;                               // log K_ij for now; the mean is subtracted below
+        s += l;
+      }
       pos++;
     } else {
       zeros++;
@@ -56,7 +66,9 @@ __global__ void __launch_bounds__(256) sf_ratio_kernel(const SizeFactorArgs A) {
   zeros = (int)warp_allreduce_sum((double)zeros);
   pos = (int)warp_allreduce_sum((double)pos);
   const bool finite = A.poscounts ? (pos > 0) : (zeros == 0);
-  const double lg = finite ? s / (double)A.m : -inf;
+  double lg = finite ? s / (double)A.m : -inf;
+  if constexpr (DIV)
+    if (finite && A.poscounts) lg = log(exp(lg));
   __syncwarp();
   for (int j = lane; j < A.m; j += 32) {
     const double y = A.y_is_f64 ? static_cast<const double*>(A.y)[off + j]
@@ -144,7 +156,8 @@ cudaError_t launch_size_factors(const SizeFactorArgs& a, cudaStream_t stream) {
   if (a.n == 0 || a.m == 0) return cudaSuccess;
   cudaError_t e = cudaMemsetAsync(a.n_finite, 0, sizeof(int), stream);
   if (e != cudaSuccess) return e;
-  sf_ratio_kernel<<<(a.n + 7) / 8, 256, 0, stream>>>(a);
+  const auto ratio = a.divisor != nullptr ? sf_ratio_kernel<true> : sf_ratio_kernel<false>;
+  ratio<<<(a.n + 7) / 8, 256, 0, stream>>>(a);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   e = launch_to_col_major(a.ratios, a.ratios_colmajor, a.n, a.m, a.ld, stream);

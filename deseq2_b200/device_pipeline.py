@@ -18,6 +18,11 @@ DESeq_device(weights=...), nbinomLRT_device(weights=...) and getContrast_device(
 weights (the "weights" assay): the weight checks and the weighted pre-steps are the weighted instantiation of the prep
 kernel (b200nb_prep_weighted_dev), and every fit passes the normalised weights to the engine's weighted fitDisp /
 fitDispGrid / fitBeta / log-likelihood / optim entry points.
+DESeq_device(normalizationFactors=...) (or avgTxLength=..., estimated by normalization_factors), nbinomLRT_device and
+getContrast_device take gene-specific normalization factors (the "normalizationFactors" assay): the pre-steps and
+Cook's distances are the nf instantiations of their kernels (b200nb_prep_nf_dev, b200nb_cooks_nf_dev), and every fit
+gets the nf rows of its genes, which the engine's fitBeta / log-likelihood / optim entry points take in place of the
+size-factor vector.
 """
 from __future__ import annotations
 
@@ -78,6 +83,76 @@ def size_factors(y, m, type="ratio"):
     return out
 
 
+def _check_positive_matrix(t, y, m, name):
+    """A gene-major float64 tensor of the counts' shape on their device whose first m columns are finite and > 0
+    (normalizationFactors<-, R/methods.R:345-350).  One host read."""
+    if not isinstance(t, torch.Tensor) or t.dtype != F64 or t.device != y.device:
+        raise ValueError(f"{name} must be a float64 tensor on the counts' device")
+    if tuple(t.shape) != tuple(y.shape) or not t.is_contiguous():
+        raise ValueError(f"{name} must be a contiguous gene-major tensor of the counts' shape {tuple(y.shape)}, "
+                         f"got {tuple(t.shape)}")
+    v = t[:, :m]
+    if bool((~(torch.isfinite(v) & (v > 0))).any()):
+        raise ValueError(f"{name} must be finite and positive")
+
+
+def normalization_factors(y, m, normMatrix=None, avgTxLength=None, type="ratio"):
+    """estimateSizeFactors with a normMatrix or an avgTxLength assay (R/methods.R:363-406) on the device: exactly one of
+    the two, a gene-major (n, ld) float64 tensor aligned with y.  avgTxLength is first divided by its row geometric
+    mean.  estimateNormFactors (R/core.R:2159-2163): the median-of-ratios size factors of K / normMatrix
+    (b200nb_size_factors_norm_dev; for "poscounts" the log geometric means come from the raw counts and the factors are
+    rescaled to geometric mean 1, R/core.R:573-576), then nf = normMatrix * sf divided by its row geometric mean.
+    Returns {"normalizationFactors": (n, ld) device tensor (padding columns 1), "sizeFactors": (m,)}.
+    Raises ValueError for a non-positive / non-finite matrix and when every gene contains a zero."""
+    if type not in ("ratio", "poscounts"):
+        raise ValueError("type must be 'ratio' or 'poscounts'")
+    if (normMatrix is None) == (avgTxLength is None):
+        raise ValueError("give exactly one of normMatrix and avgTxLength")
+    name = "normMatrix" if normMatrix is not None else "avgTxLength"
+    src = normMatrix if normMatrix is not None else avgTxLength
+    _check_positive_matrix(src, y, m, name)
+    L = _lib.lib()
+    dev = y.device
+    n, ld = y.shape
+    nm = src[:, :m]
+    if avgTxLength is not None:
+        nm = nm / torch.exp(torch.log(nm).mean(dim=1, keepdim=True))
+    d = torch.ones((n, ld), dtype=F64, device=dev)
+    d[:, :m] = nm
+    sf = torch.empty(m, dtype=F64, device=dev)
+    lg = torch.empty(n, dtype=F64, device=dev)
+    nfin = torch.zeros(1, dtype=torch.int32, device=dev)
+    gm = _ws("sf_ratios", (n, ld), F64, dev)
+    cm = _ws("sf_ratios_cm", (n * m,), F64, dev)
+    _lib.check(L.b200nb_size_factors_norm_dev(_p(y), 1 if y.dtype == F64 else 0, _p(d), int(type == "poscounts"), n,
+                                              m, ld, _p(lg), _p(gm), _p(cm), _p(sf), _p(nfin), _stream()),
+               "size_factors_norm")
+    if int(nfin.item()) == 0:
+        raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
+    if type == "poscounts":
+        sf = sf / torch.exp(torch.log(sf).mean())
+    nf = nm * sf[None, :]
+    nf = nf / torch.exp(torch.log(nf).mean(dim=1, keepdim=True))
+    d[:, :m] = nf
+    return {"normalizationFactors": d, "sizeFactors": sf}
+
+
+def nf_column_sums(nf, m):
+    """The two numbers per sample that momentsDispEstimate's xim needs from a set of rows: their nf column sums (m,)
+    and their count.  Summed over the ranks in rank order by the sharded driver."""
+    return nf[:, :m].sum(dim=0), nf.shape[0]
+
+
+def nf_xim(colsum, count):
+    """xim = mean(1 / colMeans(nf)) (R/core.R:2440-2441) from nf_column_sums."""
+    return float((1.0 / (colsum / count)).mean().item())
+
+
+def _rows(nfd, rows):
+    """The normalization factors of `rows` (a gene-major matrix), or the size-factor vector unchanged."""
+    return nfd[rows].contiguous() if nfd.dim() == 2 else nfd
+
+
 def _projection(x):
     """(X'X)^-1 X' (p x m) WITHOUT a BLAS / LAPACK call.  numpy hands `x.T @ x` and linalg.solve to OpenBLAS, whose
     worker threads (one per CPU the process may run on: 64-128 on the GPU hosts) then busy-wait for ~100 ms; under a
@@ -102,11 +177,13 @@ def _projection(x):
 
 
 def prep(y, x, sizeFactors, minDisp=1e-8, minmu=0.5, want_mu=True, want_beta0=True, weights=None,
-         weightThreshold=1e-2):
+         weightThreshold=1e-2, normalizationFactors=None, xim=None):
     """b200nb_prep_dev.  y: gene-major (n, ld) int32/float64 device tensor; x: (m, p) numpy; sizeFactors: (m,) numpy.
     weights: gene-major (n, ld) float64 device tensor of raw observation weights -> b200nb_prep_weighted_dev, which
     adds "weightsNorm" (n, ld: weights / row maximum), "weightsFail" (n,) int32 and "status" (1,) int32, the number
-    of rows whose weights the reference rejects (the caller raises when it is not 0).  mu_lin is not computed then."""
+    of rows whose weights the reference rejects (the caller raises when it is not 0).  mu_lin is not computed then.
+    normalizationFactors: gene-major (n, ld) float64 device tensor of the same rows -> b200nb_prep_nf_dev
+    (sizeFactors is ignored); xim defaults to mean(1 / colMeans(nf)) over these rows.  "sfd" is then this matrix."""
     L = _lib.lib()
     dev = y.device
     n, ld = y.shape
@@ -115,15 +192,26 @@ def prep(y, x, sizeFactors, minDisp=1e-8, minmu=0.5, want_mu=True, want_beta0=Tr
     proj = _projection(x)                                      # (X'X)^-1 X', p x m
     xd = D.x_to_device(x, dev)
     projd = torch.as_tensor(np.ascontiguousarray(proj), device=dev)
-    sfd = torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=dev)
+    nf = normalizationFactors
+    if nf is None:
+        sfd = torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=dev)
+        xim = float(np.mean(1.0 / np.asarray(sizeFactors)))
+    else:
+        if weights is not None:
+            raise ValueError("observation weights together with normalization factors are not supported")
+        sfd = nf
+        if xim is None:
+            xim = nf_xim(*nf_column_sums(nf, m))
     out = {"baseMean": torch.empty(n, dtype=F64, device=dev), "baseVar": torch.empty(n, dtype=F64, device=dev),
            "allZero": torch.empty(n, dtype=torch.int32, device=dev), "alpha0": torch.empty(n, dtype=F64, device=dev),
            "mu_lin": _ws("mu_lin", (n, ld), F64, dev) if want_mu else None,
            "beta0": torch.empty((p, n), dtype=F64, device=dev) if want_beta0 else None}
-    args = (_p(y), 0 if y.dtype == torch.int32 else 1, _p(xd), _p(projd), _p(sfd),
-            float(np.mean(1.0 / np.asarray(sizeFactors))), float(minDisp), float(max(10, m)), float(minmu), n, m, p, ld,
-            _p(out["baseMean"]), _p(out["baseVar"]), _p(out["allZero"]), _p(out["alpha0"]))
-    if weights is None:
+    args = (_p(y), 0 if y.dtype == torch.int32 else 1, _p(xd), _p(projd), _p(sfd), float(xim), float(minDisp),
+            float(max(10, m)), float(minmu), n, m, p, ld, _p(out["baseMean"]), _p(out["baseVar"]), _p(out["allZero"]),
+            _p(out["alpha0"]))
+    if nf is not None:
+        _lib.check(L.b200nb_prep_nf_dev(*args, _p(out["mu_lin"]), _p(out["beta0"]), _stream()), "prep_nf_dev")
+    elif weights is None:
         rc = L.b200nb_prep_dev(*args, _p(out["mu_lin"]), _p(out["beta0"]), _stream())
         _lib.check(rc, "prep_dev")
     else:
@@ -172,8 +260,9 @@ def trend_fit(means, disps, minDisp=1e-8):
     return out
 
 
-def cooks(y, mu, hat, x, sizeFactors, want_matrix=True):
-    """b200nb_cooks_dev: Cook's distances, their per-gene maximum and the robust moments dispersion."""
+def cooks(y, mu, hat, x, sizeFactors, want_matrix=True, normalizationFactors=None):
+    """b200nb_cooks_dev: Cook's distances, their per-gene maximum and the robust moments dispersion.
+    normalizationFactors: gene-major (n, ld) of the same rows -> b200nb_cooks_nf_dev (sizeFactors is ignored)."""
     from .pipeline import designCells
     L = _lib.lib()
     dev = y.device
@@ -185,12 +274,13 @@ def cooks(y, mu, hat, x, sizeFactors, want_matrix=True):
     ptr = np.r_[0, np.cumsum(sizes)].astype(np.int32)
     ptrd = torch.as_tensor(ptr, device=dev)
     ordd = torch.as_tensor(order, device=dev)
-    sfd = torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=dev)
+    nf = normalizationFactors
+    sfd = nf if nf is not None else torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=dev)
     out = {"cooks": torch.empty((n, ld), dtype=F64, device=dev) if want_matrix else None,
            "maxCooks": torch.empty(n, dtype=F64, device=dev), "robustDisp": torch.empty(n, dtype=F64, device=dev)}
-    rc = L.b200nb_cooks_dev(_p(y), 0 if y.dtype == torch.int32 else 1, _p(mu), _p(hat), _p(sfd), _p(ptrd), _p(ordd),
-                            len(sizes), n, m, p, ld, _p(out["cooks"]), _p(out["maxCooks"]), _p(out["robustDisp"]),
-                            _stream())
+    entry = L.b200nb_cooks_nf_dev if nf is not None else L.b200nb_cooks_dev
+    rc = entry(_p(y), 0 if y.dtype == torch.int32 else 1, _p(mu), _p(hat), _p(sfd), _p(ptrd), _p(ordd),
+               len(sizes), n, m, p, ld, _p(out["cooks"]), _p(out["maxCooks"]), _p(out["robustDisp"]), _stream())
     _lib.check(rc, "cooks_dev")
     return out
 
@@ -283,21 +373,22 @@ def _grid_refit(y, xd, mu, sel, m, prior_mean, prior_sigmasq, usePrior, weights=
 
 
 def getContrast_device(ynz, x, sizeFactors, dispersion, betaMatrix, contrast, betaPriorVar=None, minmu=0.5,
-                       weights=None):
+                       weights=None, normalizationFactors=None):
     """getContrast (R/results.R:760-827) on device tensors: fitBeta's maxit = 0 mode (covariance at the given betas).
     ynz: gene-major counts the model was fitted to; betaMatrix: (n, p) log2-scale coefficients (DESeq_device's
     "betaMatrix").  weights: gene-major (n, ld) float64 observation weights of the same rows (raw, or DESeq_device's
     normalised "weights"), normalised by the row maximum and passed to fitBeta without the rank tests, as in the
-    reference.  Returns log2FoldChange, lfcSE, stat, pvalue as device tensors."""
+    reference.  normalizationFactors: gene-major (n, ld) float64 factors of the same rows, in place of sizeFactors
+    (None then).  Returns log2FoldChange, lfcSE, stat, pvalue as device tensors."""
     dev = ynz.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
+    sfd = _size_or_norm_factors(ynz, m, sizeFactors, normalizationFactors, weights)
     contrast = np.asarray(contrast, dtype=np.float64)
     if contrast.shape != (p,):
         raise ValueError("numeric contrast vector should have one element for every element of 'resultsNames(object)'")
     pv = np.full(p, 1e6) if betaPriorVar is None else np.asarray(betaPriorVar, dtype=np.float64)
     lam = torch.as_tensor(1.0 / (LN2 ** 2 * pv), device=dev)
-    sfd = torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=dev)
     beta_nat = (betaMatrix.T * LN2).contiguous()                       # (p, n) = column-major n x p, natural log scale
     wn = None if weights is None else normalize_weights(weights, ynz, m)
     r = D.fit_beta(ynz, D.x_to_device(x, dev), sfd, dispersion, torch.as_tensor(contrast, device=dev), beta_nat, lam,
@@ -305,6 +396,21 @@ def getContrast_device(ynz, x, sizeFactors, dispersion, betaMatrix, contrast, be
     est, se = r["contrast_num"] / LN2, r["contrast_denom"] / LN2
     stat = est / se
     return {"log2FoldChange": est, "lfcSE": se, "stat": stat, "pvalue": 2.0 * torch.special.ndtr(-stat.abs())}
+
+
+def _size_or_norm_factors(y, m, sizeFactors, normalizationFactors, weights):
+    """getSizeOrNormFactors (R/core.R:2221-2228) for the fits: the checked nf matrix, or the size factors as a device
+    vector.  Raises ValueError when both or neither are given, or nf together with weights."""
+    if normalizationFactors is None:
+        if sizeFactors is None:
+            raise ValueError("give sizeFactors or normalizationFactors")
+        return torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=y.device)
+    if sizeFactors is not None:
+        raise ValueError("give sizeFactors or normalizationFactors, not both")
+    if weights is not None:
+        raise ValueError("observation weights together with normalization factors are not supported")
+    _check_positive_matrix(normalizationFactors, y, m, "normalizationFactors")
+    return normalizationFactors
 
 
 def _optim_fallback(ysrc, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, minmu, ll, useOptim=True,
@@ -329,6 +435,7 @@ def _optim_fallback(ysrc, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, 
     start = torch.where(usable[None, :], beta[:, rows], beta0[:, rows]).contiguous()
     start = torch.nan_to_num(start, nan=0.0)
     ysub = ysrc[rows].contiguous()
+    sfd = _rows(sfd, rows)
     asub = dispersion[rows].contiguous()
     wsub = None if weights is None else weights[rows].contiguous()
     o = D.beta_optim(ysub, xd, sfd, asub, lam, start, weights=wsub)
@@ -349,16 +456,19 @@ def _optim_fallback(ysrc, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, 
 
 
 def nbinomLRT_device(ynz, x_full, x_reduced, sizeFactors, dispersion, betaTol=1e-8, maxit=100, minmu=0.5,
-                     useOptim=True, weights=None):
+                     useOptim=True, weights=None, normalizationFactors=None):
     """nbinomLRT (R/core.R:1787-2012) on device tensors: two IRLS fits, LRT statistic 2 (logLike_full - logLike_reduced)
     (R/core.R:1877) and its chi-square p-value.  The log-likelihoods are evaluated at the UNCLAMPED fitted means
     nf * exp(x beta) as the reference does (R/fitNbinomGLMs.R:180-182) by b200nb_nb_loglik_dev -- NOT taken from the IRLS
     kernel's deviance, which is at the minmu-clamped mean and differs by several units when a design cell is all zeros.
     weights: gene-major (n, ld) float64 observation weights of the rows (raw or normalised): both fits, their
     log-likelihoods and the optim fallback are weighted, and an intercept-only reduced model takes the reference's
-    weighted closed form (R/fitNbinomGLMs.R:99-137) instead of an IRLS fit."""
+    weighted closed form (R/fitNbinomGLMs.R:99-137) instead of an IRLS fit.
+    normalizationFactors: gene-major (n, ld) float64 factors of the rows, in place of sizeFactors (None then); both
+    fits, their start values and log-likelihoods use them, and the intercept-only reduced model is an IRLS fit as on
+    the size-factor path."""
     dev = ynz.device
-    sfd = torch.as_tensor(np.asarray(sizeFactors, dtype=np.float64), device=dev)
+    sfd = _size_or_norm_factors(ynz, np.asarray(x_full).shape[0], sizeFactors, normalizationFactors, weights)
     wn = None if weights is None else normalize_weights(weights, ynz, np.asarray(x_full).shape[0])
     res = {}
     for name, x in (("full", x_full), ("reduced", x_reduced)):
@@ -367,7 +477,7 @@ def nbinomLRT_device(ynz, x_full, x_reduced, sizeFactors, dispersion, betaTol=1e
         if wn is not None and name == "reduced" and p == 1 and np.all(x == 1):
             res[name] = _intercept_only_weighted(ynz, sfd, dispersion, wn, m)
             continue
-        pr = prep(ynz, x, sizeFactors, minmu=minmu, want_mu=False)
+        pr = prep(ynz, x, sizeFactors, minmu=minmu, want_mu=False, normalizationFactors=normalizationFactors)
         contrast = torch.zeros(p, dtype=F64, device=dev)
         contrast[0] = 1.0
         lam = torch.full((p,), 1e-6 / LN2 ** 2, dtype=F64, device=dev)
@@ -401,15 +511,17 @@ def _intercept_only_weighted(ynz, sfd, dispersion, wn, m):
 
 
 def _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp, kappa_0, dispTol, maxit, betaTol,
-                minmu, outlierSD, useOptim=True):
+                minmu, outlierSD, useOptim=True, normalizationFactors=None):
     """The per-gene chain of DESeq_device (GeneEst -> MAP -> Wald) on a subset of rows with the dispersion trend and
     prior already known: what refitWithoutOutliers (R/core.R:2500-2528) does with objectSub.  Fresh tensors, no
-    shared workspace: the subset is small."""
+    shared workspace: the subset is small.  normalizationFactors: the subset's rows; xim is then over them, as R's
+    estimateDispersionsGeneEst(objectSub) computes it (R/core.R:2503-2510)."""
     dev = ysub.device
     m, p = x.shape
     maxDisp = float(max(10, m))
     linearMu = modelMatrixGroups(x) == p
-    pr = prep(ysub, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu)
+    pr = prep(ysub, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu,
+              normalizationFactors=normalizationFactors)
     xd, sfd, bm, alpha0, beta0 = pr["xd"], pr["sfd"], pr["baseMean"], pr["alpha0"], pr["beta0"]
     if linearMu:
         mu = pr["mu_lin"].clone()
@@ -457,7 +569,8 @@ def _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp,
 
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
                  outlierSD=2.0, minReplicatesForReplace=np.inf, allgather=None, useOptim=True, betaPrior=False,
-                 factors=None, weights=None, weightThreshold=1e-2):
+                 factors=None, weights=None, weightThreshold=1e-2, normalizationFactors=None, avgTxLength=None,
+                 nfXim=None):
     """y: gene-major (N, ld) device tensor of counts (int32 or float64).  Returns a dict of device tensors over the
     rows with a non-zero sum (`idx` maps them back to the N input rows) plus the trend / prior scalars.
     sizeFactors=None estimates them on the device first (median of ratios, R/core.R:535-578; returned under
@@ -483,10 +596,27 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     ("weightsFail", over the N input rows; a warning as in R) are dropped with the all-zero rows.  baseMean / baseVar
     use the raw weights; mu comes from a weighted GLM fit (no linear mu); the gene-wise fitDisp / fitDispGrid get
     max(w, 1e-6), every other fit the normalised weights, returned under "weights" for the rows in idx.  Weights are
-    not supported with betaPrior=True or outlier replacement (ValueError)."""
+    not supported with betaPrior=True or outlier replacement (ValueError).
+    normalizationFactors: gene-specific normalization factors (the "normalizationFactors" assay) as a gene-major
+    (N, ld) float64 device tensor aligned with y, finite and > 0 in the first m columns; they take the place of the size
+    factors everywhere (getSizeOrNormFactors): baseMean / baseVar, rough dispersion, linear mu and start values of
+    K/nf, xim = mean(1 / colMeans(nf)) over the non-all-zero rows, and the nf rows of idx in every fit, Cook's
+    distances and outlier replacement.  avgTxLength (same layout, instead of normalizationFactors): the factors are
+    estimated first by normalization_factors, as DESeq() -> estimateSizeFactors does for a tximport dataset.  Returned
+    under "normalizationFactors" (rows in idx).  Not with sizeFactors or weights (ValueError).  nfXim: xim computed
+    by the caller (the sharded driver, over every rank's rows)."""
     dev = y.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
+    if avgTxLength is not None:
+        if normalizationFactors is not None:
+            raise ValueError("give normalizationFactors or avgTxLength, not both")
+        if sizeFactors is not None:
+            raise ValueError("avgTxLength estimates normalization factors: sizeFactors must be None")
+        normalizationFactors = normalization_factors(y, m, avgTxLength=avgTxLength)["normalizationFactors"]
+    nf = normalizationFactors
+    if nf is not None:
+        _size_or_norm_factors(y, m, sizeFactors, nf, weights)
     if weights is not None:
         _check_weights_tensor(weights, y)
         if betaPrior:
@@ -502,7 +632,7 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             raise ValueError("betaPrior=True: x must be the standard model matrix of the factors, factorDesign(factors)[0]")
         if np.isfinite(minReplicatesForReplace):
             raise ValueError("outlier replacement (finite minReplicatesForReplace) is not supported with betaPrior=True")
-    estimated = sizeFactors is None
+    estimated = sizeFactors is None and nf is None
     if estimated:
         sizeFactors = size_factors(y, m)["sizeFactors"].cpu().numpy()
     import os
@@ -525,7 +655,9 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
         # rows with a zero sum are dropped before anything else (R/core.R:706), so every later array is aligned
         idx = torch.nonzero(y[:, :m].sum(dim=1) != 0).squeeze(1)
         ynz = y if idx.numel() == y.shape[0] else y[idx].contiguous()
-        pr = prep(ynz, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu)
+        nfz = None if nf is None else (nf if idx.numel() == y.shape[0] else nf[idx].contiguous())
+        pr = prep(ynz, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu, normalizationFactors=nfz,
+                  xim=nfXim)
         bm = pr["baseMean"]
         alpha0 = pr["alpha0"]
         beta0 = pr["beta0"]
@@ -664,7 +796,8 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     from .pipeline import nOrMoreInCell
     do_replace = bool(np.isfinite(minReplicatesForReplace)) and bool(nOrMoreInCell(x, minReplicatesForReplace).any())
     mu_cooks = ll["mu"]
-    ck = cooks(ynz, mu_cooks, fb["hat_diagonals"], x, sizeFactors, want_matrix=do_replace)   # R/core.R:1457-1460
+    ck = cooks(ynz, mu_cooks, fb["hat_diagonals"], x, sizeFactors, want_matrix=do_replace,   # R/core.R:1457-1460
+               normalizationFactors=sfd if nf is not None else None)
     mark("wald_stats+cooks")
     res = {"stage_ms": stage_ms, "maxCooks": ck["maxCooks"], "idx": idx, "baseMean": bm, "dispGeneEst": dge, "dispFit": dispFit, "dispMAP": dispMAP,
             "dispersion": dispersion, "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": rm["iter"],
@@ -672,10 +805,13 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             "betaIter": fit["iter"], "betaConv": betaConv, "n_optim": n_optim, "deviance": -2.0 * fit_ll["logLike"], "mu": mu_cooks,
             "H": fb["hat_diagonals"], "trendCoefs": tr[:2], "varLogDispEsts": varLogDispEsts,
             "dispPriorVar": dispPriorVar, "n_refit_geneest": n_refit_geneest, "n_refit_map": int(gi2.numel()),
-            "n_input_rows": y.shape[0], "sizeFactors": np.asarray(sizeFactors, dtype=np.float64)}
+            "n_input_rows": y.shape[0],
+            "sizeFactors": None if nf is not None else np.asarray(sizeFactors, dtype=np.float64)}
     res.update(prior)
     if weights is not None:
         res["weightsFail"], res["weights"] = weightsFail, wn
+    if nf is not None:
+        res["normalizationFactors"] = sfd
     if do_replace and m > p:
         _replace_and_refit(res, ynz, ck["cooks"], x, sizeFactors, sfd, tr, varLogDispEsts, dispPriorVar,
                            minReplicatesForReplace, minDisp, kappa_0, dispTol, maxit, betaTol, minmu, outlierSD,
@@ -720,7 +856,9 @@ def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, varLogDispEsts
                        kappa_0, dispTol, maxit, betaTol, minmu, outlierSD, trim=0.2, useOptim=True):
     """replaceOutliers + refitWithoutOutliers (R/core.R:2069-2115, 2484-2565) on the device results `res` (in place).
     Only the flagged rows move: their counts are gathered, the outlying entries of replaceable samples become
-    as.integer(trimmed mean of the normalised counts * size factor), and the rows go through _refit_rows."""
+    as.integer(trimmed mean of the normalised counts * size factor), and the rows go through _refit_rows.
+    `sfd` is the size-factor vector or the nf matrix of ynz's rows: with nf the trimmed mean is of K/nf and the
+    replacement count trunc(trimmed mean * nf_ij) (R/core.R:2089-2096)."""
     from scipy import stats as _st
     from .pipeline import nOrMoreInCell
     dev = ynz.device
@@ -734,13 +872,14 @@ def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, varLogDispEsts
     if rows.numel() == 0:
         return
     ys = ynz[rows][:, :m].to(F64)
-    srt, _ = torch.sort(ys / sfd[None, :], dim=1)
+    nfm = sfd[rows][:, :m] if sfd.dim() == 2 else sfd[None, :]
+    srt, _ = torch.sort(ys / nfm, dim=1)
     lo = int(np.floor(m * trim))
     tbm = srt[:, lo:m - lo].mean(dim=1)
-    replacement = torch.trunc(tbm[:, None] * sfd[None, :])
+    replacement = torch.trunc(tbm[:, None] * nfm)
     new = torch.where(over[rows] & replaceable[None, :], replacement, ys)
     res["baseMean"] = res["baseMean"].clone()
-    res["baseMean"][rows] = (new / sfd[None, :]).mean(dim=1)        # getBaseMeansAndVariances on the new counts
+    res["baseMean"][rows] = (new / nfm).mean(dim=1)                 # getBaseMeansAndVariances on the new counts
     newAllZero = new.sum(dim=1) == 0
     keep = ~newAllZero
     rr = rows[keep]
@@ -748,7 +887,8 @@ def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, varLogDispEsts
         ysub = torch.zeros((rr.numel(), ynz.shape[1]), dtype=F64, device=dev)
         ysub[:, :m] = new[keep]
         sub = _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp, kappa_0, dispTol, maxit,
-                          betaTol, minmu, outlierSD, useOptim=useOptim)
+                          betaTol, minmu, outlierSD, useOptim=useOptim,
+                          normalizationFactors=sfd[rr].contiguous() if sfd.dim() == 2 else None)
         for k, v in sub.items():
             if k == "baseMean":
                 continue

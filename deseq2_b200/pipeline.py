@@ -26,6 +26,9 @@ numpy, one function per R function, same names, so the engine can be driven and 
 
 Observation weights (a "weights" assay) go through every step above that takes them in the reference, except
 betaPrior=TRUE and outlier replacement, which raise with weights.
+Gene-specific normalization factors (estimateNormFactors, R/core.R:2159-2163, or a user matrix): every function that
+takes `sizeFactors` also takes an (n, m) matrix of the same rows, as getSizeOrNormFactors (R/core.R:2221-2228) hands
+either to the code; DESeq(normalizationFactors=...) threads it through every step.
 
 `engine` is any object with fitDisp / fitDispGrid / fitBeta taking the reference's argument names
 (deseq2_b200.wrappers is the product engine and the default; tests and the bench's CPU baseline pass the
@@ -58,10 +61,50 @@ def estimateSizeFactorsForMatrix(counts):
     return sf
 
 
+def _div(sizeFactors):
+    """getSizeOrNormFactors: the (m,) size factors as a (1, m) row, or an (n, m) normalization-factor matrix as is."""
+    sf = np.asarray(sizeFactors, dtype=np.float64)
+    return sf if sf.ndim == 2 else sf[None, :]
+
+
+def estimateNormFactors(counts, normMatrix, type="ratio"):
+    """R/core.R:2159-2163 as estimateSizeFactors calls it (R/methods.R:377-402), in the reference's formula order:
+    the median-of-ratios size factors of counts / normMatrix -- for type "poscounts" with the geoMeans of the raw
+    counts, log(exp(sum(log K[K > 0]) / m)), and the incoming-geoMeans rescaling sf / exp(mean(log sf))
+    (R/core.R:573-576) -- then nf = normMatrix * sf divided by its row geometric mean."""
+    if type not in ("ratio", "poscounts"):
+        raise ValueError("type must be 'ratio' or 'poscounts'")
+    counts = np.asarray(counts, dtype=np.float64)
+    nm = np.asarray(normMatrix, dtype=np.float64)
+    if nm.shape != counts.shape or not np.all(np.isfinite(nm) & (nm > 0)):
+        raise ValueError("normMatrix must be finite, positive and of the counts' shape")
+    cnts = counts / nm
+    m = counts.shape[1]
+    with np.errstate(divide="ignore"):
+        if type == "poscounts":
+            pos = counts > 0
+            s = np.where(pos, np.log(np.where(pos, counts, 1.0)), 0.0).sum(axis=1)
+            geoMeans = np.where(pos.any(axis=1), np.exp(s / m), 0.0)
+            loggeomeans = np.log(geoMeans)
+        else:
+            loggeomeans = np.log(cnts).mean(axis=1)
+        if np.all(np.isinf(loggeomeans)):
+            raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
+        ok = np.isfinite(loggeomeans)
+        sf = np.empty(m)
+        for j in range(m):
+            sel = ok & (cnts[:, j] > 0)
+            sf[j] = np.exp(np.median(np.log(cnts[sel, j]) - loggeomeans[sel]))
+    if type == "poscounts":
+        sf = sf / np.exp(np.mean(np.log(sf)))
+    nf = nm * sf[None, :]
+    return nf / np.exp(np.log(nf).mean(axis=1))[:, None]
+
+
 def getBaseMeansAndVariances(counts, sizeFactors, weights=None):
     """R/core.R:2138-2157.  With weights: mean and variance of the RAW weights times the normalised counts; allZero
-    stays the unweighted row sum."""
-    norm = np.asarray(counts, dtype=np.float64) / sizeFactors[None, :]
+    stays the unweighted row sum.  sizeFactors: (m,) or an (n, m) normalization-factor matrix."""
+    norm = np.asarray(counts, dtype=np.float64) / _div(sizeFactors)
     if weights is not None:
         norm = np.asarray(weights, dtype=np.float64) * norm
     return {"baseMean": norm.mean(axis=1), "baseVar": norm.var(axis=1, ddof=1),
@@ -155,8 +198,9 @@ def roughDispEstimate(y, x):
 
 
 def momentsDispEstimate(baseMean, baseVar, sizeFactors):
-    """R/core.R:2439-2448."""
-    xim = np.mean(1.0 / sizeFactors)
+    """R/core.R:2439-2448; with an (n, m) normalization-factor matrix xim = mean(1 / colMeans(nf)) over its rows."""
+    sizeFactors = np.asarray(sizeFactors, dtype=np.float64)
+    xim = np.mean(1.0 / (sizeFactors.mean(axis=0) if sizeFactors.ndim == 2 else sizeFactors))
     return (baseVar - xim * baseMean) / baseMean ** 2
 
 
@@ -209,7 +253,7 @@ def estimateDispersionsGeneEst(counts, sizeFactors, x, engine=None, minDisp=1e-8
     p = x.shape[1]
     if mv is None:
         mv = getBaseMeansAndVariances(counts, sizeFactors)      # with weights the caller passes the weighted pair
-    norm = counts / sizeFactors[None, :]
+    norm = counts / _div(sizeFactors)
     useWeights = weights is not None
     wdisp = np.maximum(weights, 1e-6) if useWeights else None
     roughDisp = roughDispEstimate(norm, x)
@@ -218,7 +262,7 @@ def estimateDispersionsGeneEst(counts, sizeFactors, x, engine=None, minDisp=1e-8
     maxDisp = max(10, m)
     alpha_hat = alpha_init = np.minimum(np.maximum(minDisp, alpha_hat), maxDisp)
     linearMu = modelMatrixGroups(x) == p and not useWeights
-    nf = np.broadcast_to(sizeFactors[None, :], (n, m))
+    nf = np.broadcast_to(_div(sizeFactors), (n, m))
     if not linearMu:
         fit = fitNbinomGLMs(counts, nf, x, alpha_hat, engine=engine, weights=weights)
         fitMu = fit["mu"]
@@ -560,7 +604,7 @@ def trimmedVariance(x):
 
 def robustMethodOfMomentsDisp(counts, sizeFactors, x):
     """R/core.R:2277-2300."""
-    cnts = np.asarray(counts, dtype=np.float64) / sizeFactors[None, :]
+    cnts = np.asarray(counts, dtype=np.float64) / _div(sizeFactors)
     cells, sizes = designCells(x)
     three = sizes[cells] >= 3
     if three.any():
@@ -596,7 +640,7 @@ def nOrMoreInCell(x, n):
 
 
 def replaceOutliers(counts, cooks, sizeFactors, x, trim=0.2, cooksCutoff=None, minReplicates=7):
-    """R/core.R:2069-2115 (size factors, no normalisation-factor matrix).  Returns (counts with the outlying entries of
+    """R/core.R:2069-2115 (size factors or an (n, m) normalization-factor matrix).  Returns (counts with the outlying entries of
     replaceable samples set to as.integer(trimmed mean of the normalised counts * size factor), per-gene `replace`
     flag, per-sample `replaceable` flag).  Like the reference, `replace` is raised by an outlier in ANY sample."""
     from scipy import stats as _st
@@ -612,8 +656,8 @@ def replaceOutliers(counts, cooks, sizeFactors, x, trim=0.2, cooksCutoff=None, m
     with np.errstate(invalid="ignore"):
         over = cooks > cooksCutoff                      # NA > cutoff is NA in R and drops out of which()/any()
     replace = over.any(axis=1)
-    trimBaseMean = _r_trimmed_mean(counts / sizeFactors[None, :], trim)
-    replacementCounts = np.trunc(trimBaseMean[:, None] * sizeFactors[None, :]).astype(counts.dtype)   # as.integer
+    trimBaseMean = _r_trimmed_mean(counts / _div(sizeFactors), trim)
+    replacementCounts = np.trunc(trimBaseMean[:, None] * _div(sizeFactors)).astype(counts.dtype)   # as.integer
     newCounts = counts.copy()
     newCounts[over] = replacementCounts[over]
     whichSamples = nOrMoreInCell(x, minReplicates)
@@ -808,7 +852,7 @@ def fitGLMsWithPrior(counts, nf, factors, dispersion, baseMean, dispFit, engine=
 
 
 def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.inf, useOptim=True, betaPrior=False,
-          factors=None, weights=None, weightThreshold=1e-2, minmu=0.5):
+          factors=None, weights=None, weightThreshold=1e-2, minmu=0.5, normalizationFactors=None):
     """R/core.R:280-432 with test='Wald', fitType='parametric', betaPrior=FALSE by default.
     minReplicatesForReplace: the reference's default is 7 (outlier replacement + refit whenever a design cell has >= 7
     samples, R/core.R:419-426, refitWithoutOutliers :2484-2565); the default here is Inf = off, which is what the
@@ -823,6 +867,9 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     rows (NaN results) and reported in `weightsFail`.  baseMean / baseVar use the raw weights, every fit the
     normalised ones.  Not supported with betaPrior=True or outlier replacement (ValueError).
     minmu: the lower bound on the fitted mean (R's minmu; 1e-6 is the usual single-cell setting).
+    normalizationFactors: an (N, m) matrix of gene-specific normalization factors in place of sizeFactors, used by
+    every step (getSizeOrNormFactors); the moments dispersion's xim is over the non-all-zero rows.  Returned under
+    `normalizationFactors`.  Not with sizeFactors or weights (ValueError).
     Returns per-gene vectors over ALL rows; all-zero rows carry NaN (buildDataFrameWithNARows, R/core.R:2232)."""
     engine = engine or _default_engine
     counts = np.asarray(counts)
@@ -844,8 +891,15 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
             raise ValueError("observation weights are not supported with outlier replacement "
                              "(finite minReplicatesForReplace)")
         wnAll, weightsFail = getAndCheckWeights(weights, x, weightThreshold)
+    if normalizationFactors is not None:
+        if sizeFactors is not None or weights is not None:
+            raise ValueError("normalizationFactors are not supported together with sizeFactors or weights")
+        sizeFactors = np.asarray(normalizationFactors, dtype=np.float64)
+        if sizeFactors.shape != counts.shape or not np.all(np.isfinite(sizeFactors) & (sizeFactors > 0)):
+            raise ValueError("normalizationFactors must be finite, positive and of the counts' shape")
     if sizeFactors is None:
         sizeFactors = estimateSizeFactorsForMatrix(counts)
+    sizeFactors = np.asarray(sizeFactors, dtype=np.float64)
     mvAll = getBaseMeansAndVariances(counts, sizeFactors, weights)
     nz = ~mvAll["allZero"]
     wnz = None
@@ -858,6 +912,9 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
                           "estimation, producing a degenerate design matrix. These rows have been flagged in "
                           "weightsFail and treated as if the row contained all zeros.")
     cnz = counts[nz]
+    sfAll = sizeFactors
+    if sizeFactors.ndim == 2:
+        sizeFactors = sizeFactors[nz]                                   # the nf rows of the non-all-zero genes
     mv = {k: v[nz] for k, v in mvAll.items()}
     ge = estimateDispersionsGeneEst(cnz, sizeFactors, x, engine=engine, mv=mv, weights=wnz,
                                     weightThreshold=weightThreshold, minmu=minmu)
@@ -865,7 +922,7 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     dispPriorVar = estimateDispersionsPriorVar(tf["varLogDispEsts"], m, p, ge["dispGeneEst"], tf["dispFit"])
     mp = estimateDispersionsMAP(cnz, x, ge["mu"], ge["dispGeneEst"], tf["dispFit"], dispPriorVar,
                                 tf["varLogDispEsts"], engine=engine, weights=wnz, weightThreshold=weightThreshold)
-    nf = np.broadcast_to(sizeFactors[None, :], cnz.shape)
+    nf = np.broadcast_to(_div(sizeFactors), cnz.shape)
     prior = {}
     if betaPrior:
         gp = fitGLMsWithPrior(cnz, nf, factors, mp["dispersion"], mv["baseMean"], tf["dispFit"], engine=engine,
@@ -900,11 +957,12 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
         if nrefit > 0 and nrefit > int(newAllZero.sum()):
             rr = replace & ~newAllZero
             sub = newc[rr]
-            ge2 = estimateDispersionsGeneEst(sub, sizeFactors, x, engine=engine)
+            sfSub = sizeFactors[rr] if sizeFactors.ndim == 2 else sizeFactors
+            ge2 = estimateDispersionsGeneEst(sub, sfSub, x, engine=engine)
             dispFit2 = tf["coefs"][0] + tf["coefs"][1] / ge2["baseMean"]       # dispersionFunction(object)(baseMean)
             mp2 = estimateDispersionsMAP(sub, x, ge2["mu"], ge2["dispGeneEst"], dispFit2, dispPriorVar,
                                          tf["varLogDispEsts"], engine=engine)
-            wt2 = nbinomWaldTest(sub, np.broadcast_to(sizeFactors[None, :], sub.shape), x, mp2["dispersion"],
+            wt2 = nbinomWaldTest(sub, np.broadcast_to(_div(sfSub), sub.shape), x, mp2["dispersion"],
                                  engine=engine, useOptim=useOptim)
             upd = {"dispGeneEst": ge2["dispGeneEst"], "dispFit": dispFit2, "dispMAP": mp2["dispMAP"],
                    "dispersion": mp2["dispersion"], "dispOutlier": mp2["dispOutlier"].astype(float),
@@ -935,7 +993,7 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
         return out
 
     res = {k: full(np.asarray(v, dtype=np.float64)) for k, v in per_gene.items()}
-    res.update({"sizeFactors": sizeFactors, "allZero": mvAll["allZero"], "dispPriorVar": dispPriorVar,
+    res.update({"sizeFactors": None if sfAll.ndim == 2 else sfAll, "allZero": mvAll["allZero"], "dispPriorVar": dispPriorVar,
                 "trendCoefs": tf["coefs"], "varLogDispEsts": tf["varLogDispEsts"], "n_refit_geneest": ge["n_refit"],
                 "n_refit_map": mp["n_refit"]})
     res["baseMean"] = np.where(nz, res["baseMean"], 0.0)
@@ -943,6 +1001,9 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
         res["baseMean"] = np.where(mvAll["allZero"], 0.0, mvAll["baseMean"])    # weightsFail rows keep theirs
         res["weightsFail"] = weightsFail
         res["weights"] = wnz
+        res["idx"] = np.flatnonzero(nz)
+    if sfAll.ndim == 2:
+        res["normalizationFactors"] = sfAll
         res["idx"] = np.flatnonzero(nz)
     res.update(extra)
     return res

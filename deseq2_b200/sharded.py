@@ -128,7 +128,7 @@ def allgather_1d(t: torch.Tensor) -> torch.Tensor:
     return PackedGather(t.numel(), t.device)(t)
 
 
-def sharded_DESeq_device(y_local, x, sizeFactors, **kw):
+def sharded_DESeq_device(y_local, x, sizeFactors=None, **kw):
     """Device-resident DESeq() on this rank's gene shard (y_local: gene-major counts of the shard, on the rank's GPU)
     with the reference's global step on all genes (dispersion trend + prior variance, R/parallel.R:25-28).  The whole run
     issues TWO per-gene collectives: one packed all-gather of (baseMean, dispGeneEst) for the global step and ONE packed
@@ -139,9 +139,37 @@ def sharded_DESeq_device(y_local, x, sizeFactors, **kw):
     (R/parallel.R:39-40) through ONE more packed all-gather of the p - 1 non-intercept MLE columns; the gathered
     results then carry the expanded matrix's columns.
     weights=w_local (passed on to DESeq_device): this shard's rows of the observation weights, gene-major like
-    y_local; no collective is added (the global step's gather carries the weighted baseMean)."""
+    y_local; no collective is added (the global step's gather carries the weighted baseMean).
+    normalizationFactors=nf_local (passed on to DESeq_device): this shard's rows of the normalization factors,
+    gene-major like y_local.  The moments dispersion's xim = mean(1 / colMeans(nf)) is over the non-all-zero rows of
+    ALL ranks, as a serial DESeq() computes it: ONE more all-gather carries each rank's m column sums and its row count
+    (m + 1 doubles), summed on every rank in rank order, so xim does not depend on the number of ranks (the reference's
+    DESeqParallel uses each chunk's own xim instead, R/parallel.R:18-20).  Not supported with finite
+    minReplicatesForReplace (the refitted rows' xim would need another collective) or avgTxLength (estimating the
+    factors needs a global median): estimate them on one device or pass them."""
     from . import device_pipeline as DP
     pg = PackedGather(y_local.shape[0], y_local.device)
+    nf = kw.get("normalizationFactors")
+    if kw.get("avgTxLength") is not None:
+        raise ValueError("sharded runs do not estimate normalization factors: estimate them on one device "
+                         "(normalization_factors) or pass normalizationFactors")
+    if nf is not None:
+        if np.isfinite(kw.get("minReplicatesForReplace", np.inf)):
+            raise ValueError("sharded normalization factors are not supported with outlier replacement "
+                             "(finite minReplicatesForReplace)")
+        m = np.asarray(x).shape[0]
+        DP._check_positive_matrix(nf, y_local, m, "normalizationFactors")
+        nz = y_local[:, :m].sum(dim=1) != 0
+        colsum, count = DP.nf_column_sums(nf[nz], m)
+        mine = torch.cat([colsum, torch.tensor([float(count)], dtype=torch.float64, device=colsum.device)])
+        allr = torch.empty(pg.world * (m + 1), dtype=torch.float64, device=mine.device)
+        dist.all_gather_into_tensor(allr, mine.contiguous())
+        allr = allr.view(pg.world, m + 1)
+        pg.collectives += 1
+        tot = allr[0].clone()
+        for r in range(1, pg.world):                # rank order: the same bits on every rank
+            tot = tot + allr[r]
+        kw["nfXim"] = DP.nf_xim(tot[:m], tot[m])
     res = DP.DESeq_device(y_local, x, sizeFactors, allgather=pg, **kw)
     p = res["betaMatrix"].shape[1]
     cols = [res["dispersion"]] + [res["betaMatrix"][:, k] for k in range(p)] \

@@ -151,6 +151,14 @@ int b200nb_prep_weighted_dev(const void* y, int y_type, const double* x, const d
                              int32_t* all_zero, double* alpha0, double* mu_lin, double* beta0, const double* weights,
                              double weight_threshold, double* out_weights_norm, int32_t* out_weights_fail,
                              int32_t* out_status, void* stream);
+/* b200nb_prep_nf_dev: b200nb_prep_dev with gene-specific normalization factors nf (gene-major n x ld, positive) in
+ * place of the size-factor vector: base_mean / base_var of K/nf, the rough dispersion and beta0 from K/nf,
+ * mu_lin = linearModelMu(K/nf) * nf clamped at minmu (linearModelMuNormalized, R/core.R:2465-2471).  xim is
+ * mean(1 / colMeans(nf)) over the rows the moments estimate is for (R/core.R:2439-2448), computed by the caller. */
+int b200nb_prep_nf_dev(const void* y, int y_type, const double* x, const double* proj, const double* nf, double xim,
+                       double min_disp, double max_disp, double minmu, int n, int m, int p, long long ld,
+                       double* base_mean, double* base_var, int32_t* all_zero, double* alpha0, double* mu_lin,
+                       double* beta0, void* stream);
 
 /* b200nb_cooks_dev: calculateCooksDistance + recordMaxCooks + robustMethodOfMomentsDisp (R/core.R:2277-2359).
  * cells = distinct design rows: cell_ptr (ncell+1) / cell_samples (m, sample indices grouped by cell), device ints.
@@ -158,6 +166,11 @@ int b200nb_prep_weighted_dev(const void* y, int y_type, const double* x, const d
 int b200nb_cooks_dev(const void* y, int y_type, const double* mu, const double* hat, const double* size_factors,
                      const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n, int m, int p,
                      long long ld, double* cooks, double* max_cooks, double* robust_disp, void* stream);
+/* b200nb_cooks_nf_dev: b200nb_cooks_dev with normalization factors nf (gene-major n x ld) in place of the size
+ * factors: the robust dispersion and the trimmed cell means work on K/nf; mu already carries nf. */
+int b200nb_cooks_nf_dev(const void* y, int y_type, const double* mu, const double* hat, const double* nf,
+                        const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n, int m, int p,
+                        long long ld, double* cooks, double* max_cooks, double* robust_disp, void* stream);
 
 /* b200nb_size_factors_dev: estimateSizeFactorsForMatrix (R/core.R:535-578; locfunc = median, no geoMeans /
  * controlGenes).  poscounts = 0 is type "ratio", 1 is type "poscounts".  y gene-major (n x ld); loggeomeans[n] and
@@ -168,6 +181,14 @@ int b200nb_cooks_dev(const void* y, int y_type, const double* mu, const double* 
 int b200nb_size_factors_dev(const void* y, int y_type, int poscounts, int n, int m, long long ld,
                             double* loggeomeans, double* scratch_gm, double* scratch_cm, double* size_factors,
                             int32_t* n_finite, void* stream);
+/* b200nb_size_factors_norm_dev: the size factors of K / d for a positive divisor matrix d (gene-major n x ld), the
+ * first step of estimateNormFactors (R/core.R:2159-2163).  Ratios log(K/d) - loggeomean over the entries with K > 0;
+ * poscounts = 0: loggeomean = mean log(K/d) (type "ratio"); 1: loggeomean = log(geoMeanNZ(K)) of the RAW counts, the
+ * geoMeans that estimateSizeFactors passes for type "poscounts" (R/methods.R:377-390).  The caller applies the
+ * incoming-geoMeans rescaling sf / exp(mean(log sf)) (R/core.R:573-576) for poscounts.  Other arguments as above. */
+int b200nb_size_factors_norm_dev(const void* y, int y_type, const double* divisor, int poscounts, int n, int m,
+                                 long long ld, double* loggeomeans, double* scratch_gm, double* scratch_cm,
+                                 double* size_factors, int32_t* n_finite, void* stream);
 
 /* b200nb_beta_prior_quantile_dev: the weighted upper quantile of estimateBetaPriorVar (betaPriorMethod "weighted",
  * R/core.R:1601-1689, 2416-2419; Hmisc.wtd.quantile with normwt = TRUE, :2762-2900).  For each of the k columns
