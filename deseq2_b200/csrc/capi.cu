@@ -47,7 +47,7 @@ std::mutex g_arena_mu;   // guards the (re)allocation of the shared device arena
 // ---------------------------------------------------------------- device workspace of the host entry points
 // grow-only slots (one set per process; calls are serialised)
 enum Slot {
-  S_RAW, S_SMALL_IN, S_SMALL_OUT, S_NF, S_H, S_MUO, S_HC, S_NSLOTS
+  S_RAW, S_SMALL_IN, S_SMALL_OUT, S_NF, S_H, S_MUO, S_HC, S_SFI, S_NSLOTS
 };
 constexpr int kMaxChunks = 8;
 struct Workspace {
@@ -1423,6 +1423,40 @@ int b200nb_size_factors_norm_dev(const void* y, int y_type, const double* diviso
   if (divisor == nullptr) return fail("size_factors_norm needs the divisor matrix");
   return size_factors_common(y, y_type, divisor, poscounts, n, m, ld, loggeomeans, scratch_gm, scratch_cm,
                              size_factors, n_finite, stream);
+}
+
+// The objective tiles of b200nb_sf_iterate_objective_dev: the grow-only workspace slot S_SFI (taken under g_call_mu,
+// which also serialises it against the host entry points).  128 MB of gene log-likelihoods per tile by default: one
+// tile up to 50 000 genes x 335 objective columns.
+constexpr size_t kSfiTileBytes = (size_t)128 << 20;
+
+int b200nb_sf_iterate_objective_dev(const void* y, int y_type, const double* q, const double* alpha,
+                                    const double* par, double h, double Q, int n, int m, long long ld,
+                                    int max_tile_cols, double* out, void* stream) {
+  if (n < 1 || m < 1) return fail("sf_iterate_objective: bad dimensions n=%d m=%d (both must be >= 1)", n, m);
+  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+  if (!(h > 0.0 && h < HUGE_VAL)) return fail("sf_iterate_objective: h=%g must be finite and > 0", h);
+  if (!(Q >= 0.0 && Q < 1.0)) return fail("sf_iterate_objective: Q=%g must lie in [0, 1)", Q);
+  if (max_tile_cols < 0) return fail("sf_iterate_objective: max_tile_cols=%d must be >= 0", max_tile_cols);
+  if (!y || !q || !alpha || !par || !out) return fail("sf_iterate_objective: null pointer argument");
+  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
+  if (check_device()) return 1;
+  const int cols = 2 * m + 1;
+  long long tile = (long long)(kSfiTileBytes / ((size_t)n * sizeof(double)));
+  if (max_tile_cols > 0 && tile > max_tile_cols) tile = max_tile_cols;
+  tile = std::max(1LL, std::min(tile, (long long)cols));
+  std::lock_guard<std::mutex> lk(g_call_mu);
+  void* ws = nullptr;
+  if (ws_get(S_SFI, ((size_t)3 + (size_t)tile) * (size_t)n * sizeof(double), &ws)) return 1;
+  nb::SfIterateArgs a{};
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.q = q; a.alpha = alpha; a.par = par; a.h = h; a.Q = Q;
+  a.n = n; a.m = m; a.ld = ld; a.tile = (int)tile;
+  a.abc = static_cast<double*>(ws);
+  a.ll = a.abc + (size_t)3 * n;
+  a.out = out;
+  CU(nb::launch_sf_iterate_objective(a, (cudaStream_t)stream));
+  g_launches += 2 * ((cols + tile - 1) / tile);
+  return 0;
 }
 
 /* ------------------------------------------------------------------ host entry points */

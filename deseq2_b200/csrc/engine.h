@@ -223,6 +223,24 @@ struct BetaPriorQArgs {
 };
 cudaError_t launch_beta_prior_quantile(const BetaPriorQArgs& a, cudaStream_t stream);
 
+// estimateSizeFactorsIterate's objective at par and its 2m central-difference points (sf_iterate.cuh, launched from
+// size_factors.cu)
+struct SfIterateArgs {
+  const void* y;
+  int y_is_f64;
+  const double* q;             // gene-major n x ld: mu / s
+  const double* alpha;         // n
+  const double* par;           // m: log size factors
+  double h, Q;                 // optim's ndeps, the trimmed quantile
+  int n, m;
+  long long ld;
+  int tile;                    // objective columns per tile (>= 1)
+  double* abc;                 // 3n scratch: the row sums at the scales 1, e^{-h/m}, e^{+h/m}
+  double* ll;                  // n x tile column-major scratch
+  double* out;                 // 2m + 1 (out)
+};
+cudaError_t launch_sf_iterate_objective(const SfIterateArgs& a, cudaStream_t stream);
+
 // Cook's distances (pipeline_kernels.cu)
 struct CooksArgs {
   const void* y;

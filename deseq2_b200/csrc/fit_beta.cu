@@ -19,6 +19,7 @@
 //   * log(mu/nf) is never formed: mu = exp(eta + log nf) so log(mu/nf) = eta unless the minmu clamp bites.
 #include "deseq_rules.cuh"
 #include "engine.h"
+#include "nb_logdens.cuh"
 #include "smallp.cuh"
 
 namespace nb {
@@ -32,29 +33,6 @@ struct BetaRow {
   const double* x;     // shared, column-major stride mpad
   int m, mpad;
 };
-
-// lgamma(y + r) - lgamma(r), accurate for large r (no catastrophic cancellation)
-__device__ __forceinline__ double lgamma_diff(double y, double r, double lg_r) {
-  if (r >= kShift) {
-    const double xr = y + r;
-    const double ixr = rcp_fast(xr), ir = rcp_fast(r);
-    const double tail = stirling_tail(ixr, ixr * ixr) - stirling_tail(ir, ir * ir);
-    return fma(y, log_pos(xr), fma(r - 0.5, log1p_pos(y * ir), -y)) + tail;
-  }
-  return lgamma_pos(y + r) - lg_r;
-}
-
-// lgamma(y + 1) for the mu-independent part of the deviance.  Counts
-// below 256 read log(y!) from a per-CTA shared table filled once with the very same lgamma_pos(k + 1), so the value --
-// and every result -- is bit-identical while one Stirling evaluation per sample and gene is saved.
-__shared__ double s_lfact[256];
-__device__ __forceinline__ void init_lfact_table() {   // call before the first log_factorial; contains a __syncthreads
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) s_lfact[i] = lgamma_pos((double)i + 1.0);
-  __syncthreads();
-}
-__device__ __forceinline__ double log_factorial(double y) {
-  return (y < 256.0 && y == floor(y)) ? s_lfact[(int)y] : lgamma_pos(y + 1.0);
-}
 
 constexpr int pow2_ceil_b(int n) { int p = 1; while (p < n) p <<= 1; return p; }
 

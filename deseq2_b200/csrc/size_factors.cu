@@ -12,7 +12,9 @@
 //                     order-preserving 64-bit image of the doubles (8 histogram passes + one pass for the upper
 //                     middle element when the count is even) -- no sort, no scratch beyond 256 shared counters.
 // The same one-CTA-per-column radix refinement computes estimateBetaPriorVar's weighted upper quantiles
-// (beta_prior_quantile_kernel, beta_prior.cuh); both kernels start through launch_per_column.
+// (beta_prior_quantile_kernel, beta_prior.cuh) and the trimmed sums of estimateSizeFactorsIterate's objective
+// (iterate_trim_sum_kernel, sf_iterate.cuh, whose per-gene kernel starts the same way); all start through
+// launch_per_column.
 #include "engine.h"
 #include "beta_prior.cuh"
 #include "nbmath.cuh"
@@ -29,6 +31,54 @@ __device__ __forceinline__ unsigned long long key_of(double v) {
 __device__ __forceinline__ double value_of(unsigned long long k) {
   const unsigned long long b = (k >> 63) ? (k & 0x7fffffffffffffffull) : ~k;
   return __longlong_as_double((long long)b);
+}
+
+// Column order statistics for the one-CTA-per-column kernels (every thread of the CTA calls these; the shared
+// variables are the caller's; s_prefix must be 0 on entry).  select_key: the key of 0-based rank `rank` among key_of(col[0..n)), by an MSB-first
+// 8-bit radix select (8 histogram passes, 256 shared counters).  next_key: the key of rank rank + 1 given that of rank
+// `rank`: k1 again if more than rank + 1 keys are <= k1, otherwise the smallest key above k1.
+__device__ __forceinline__ unsigned long long select_key(const double* col, int n, unsigned int rank,
+                                                         unsigned int* hist, unsigned long long& s_prefix,
+                                                         unsigned int& s_k) {
+  const int tid = threadIdx.x;
+  if (tid == 0) s_k = rank;
+  for (int pass = 7; pass >= 0; pass--) {
+    for (int b = tid; b < 256; b += blockDim.x) hist[b] = 0;
+    __syncthreads();
+    const unsigned long long prefix = s_prefix;
+    const unsigned long long mask = (pass == 7) ? 0ull : (~0ull << (8 * (pass + 1)));
+    for (int i = tid; i < n; i += blockDim.x) {
+      const unsigned long long k = key_of(col[i]);
+      if ((k & mask) == prefix) atomicAdd(&hist[(unsigned int)(k >> (8 * pass)) & 255u], 1u);
+    }
+    __syncthreads();
+    if (tid == 0) {
+      unsigned int k = s_k, b = 0;
+      while (b < 255u && k >= hist[b]) { k -= hist[b]; b++; }   // k < number of keys under this prefix; b is bounded anyway
+      s_k = k;
+      s_prefix = prefix | ((unsigned long long)b << (8 * pass));
+    }
+    __syncthreads();
+  }
+  return s_prefix;
+}
+__device__ __forceinline__ unsigned long long next_key(const double* col, int n, unsigned int rank,
+                                                       unsigned long long k1, unsigned int& s_le,
+                                                       unsigned long long& s_next) {
+  const int tid = threadIdx.x;
+  if (tid == 0) { s_le = 0; s_next = ~0ull; }
+  __syncthreads();
+  unsigned int le = 0;
+  unsigned long long nxt = ~0ull;
+  for (int i = tid; i < n; i += blockDim.x) {
+    const unsigned long long k = key_of(col[i]);
+    le += k <= k1;
+    if (k > k1 && k < nxt) nxt = k;
+  }
+  if (le) atomicAdd(&s_le, le);
+  atomicMin(&s_next, nxt);
+  __syncthreads();
+  return (s_le > rank + 1u) ? k1 : s_next;
 }
 
 // DIV: the ratios of K / divisor (estimateNormFactors, R/core.R:2160): log(K/d) - loggeomean, where loggeomean is the
@@ -102,46 +152,20 @@ __global__ void __launch_bounds__(512) sf_median_kernel(const double* __restrict
     if (tid == 0) size_factors[blockIdx.x] = __longlong_as_double(0x7ff8000000000000ll);
     return;
   }
-  if (tid == 0) s_k = (nv - 1) / 2;                          // lower middle element (0-based rank)
-  for (int pass = 7; pass >= 0; pass--) {
-    for (int b = tid; b < 256; b += blockDim.x) hist[b] = 0;
-    __syncthreads();
-    const unsigned long long prefix = s_prefix;
-    const unsigned long long mask = (pass == 7) ? 0ull : (~0ull << (8 * (pass + 1)));
-    for (int i = tid; i < n; i += blockDim.x) {
-      const unsigned long long k = key_of(col[i]);
-      if ((k & mask) == prefix) atomicAdd(&hist[(unsigned int)(k >> (8 * pass)) & 255u], 1u);
-    }
-    __syncthreads();
-    if (tid == 0) {
-      unsigned int k = s_k, b = 0;
-      while (b < 255u && k >= hist[b]) { k -= hist[b]; b++; }   // k < number of keys under this prefix; b is bounded anyway
-      s_k = k;
-      s_prefix = prefix | ((unsigned long long)b << (8 * pass));
-    }
-    __syncthreads();
-  }
-  const unsigned long long k1 = s_prefix;
+  const unsigned int rank = (nv - 1) / 2;                    // lower middle element (0-based rank)
+  const unsigned long long k1 = select_key(col, n, rank, hist, s_prefix, s_k);
   double med = value_of(k1);
-  if ((nv & 1u) == 0) {
-    // upper middle element: k1 again if enough copies of it exist, otherwise the smallest key above k1
-    if (tid == 0) { s_le = 0; s_next = ~0ull; }
-    __syncthreads();
-    unsigned int le = 0;
-    unsigned long long nxt = ~0ull;
-    for (int i = tid; i < n; i += blockDim.x) {
-      const unsigned long long k = key_of(col[i]);
-      le += k <= k1;
-      if (k > k1 && k < nxt) nxt = k;
-    }
-    if (le) atomicAdd(&s_le, le);
-    atomicMin(&s_next, nxt);
-    __syncthreads();
-    const unsigned long long k2 = (s_le > nv / 2) ? k1 : s_next;
-    med = 0.5 * (med + value_of(k2));
-  }
+  if ((nv & 1u) == 0) med = 0.5 * (med + value_of(next_key(col, n, rank, k1, s_le, s_next)));   // upper middle
   if (tid == 0) size_factors[blockIdx.x] = exp(med);
 }
+
+}  // namespace
+}  // namespace nb
+
+#include "sf_iterate.cuh"
+
+namespace nb {
+namespace {
 
 // One CTA per column with static shared memory only: the launch site of the column-select kernels of this file.
 template <class... P, class... A>
@@ -168,6 +192,18 @@ cudaError_t launch_size_factors(const SizeFactorArgs& a, cudaStream_t stream) {
 cudaError_t launch_beta_prior_quantile(const BetaPriorQArgs& a, cudaStream_t stream) {
   if (a.k == 0) return cudaSuccess;
   return launch_per_column(beta_prior_quantile_kernel, a.k, kBpThreads, stream, a);
+}
+
+cudaError_t launch_sf_iterate_objective(const SfIterateArgs& a, cudaStream_t stream) {
+  const int cols = 2 * a.m + 1;
+  for (int c0 = 0; c0 < cols; c0 += a.tile) {
+    const int t = cols - c0 < a.tile ? cols - c0 : a.tile;
+    cudaError_t e = launch_per_column(iterate_loglik_kernel, (a.n + 7) / 8, kItLlThreads, stream, a, c0, t);
+    if (e != cudaSuccess) return e;
+    e = launch_per_column(iterate_trim_sum_kernel, t, kItSumThreads, stream, a, c0);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 }  // namespace nb

@@ -23,6 +23,11 @@ getContrast_device take gene-specific normalization factors (the "normalizationF
 Cook's distances are the nf instantiations of their kernels (b200nb_prep_nf_dev, b200nb_cooks_nf_dev), and every fit
 gets the nf rows of its genes, which the engine's fitBeta / log-likelihood / optim entry points take in place of the
 size-factor vector.
+DESeq_device(sfType="iterate") estimates the size factors with size_factors_iterate (estimateSizeFactorsIterate,
+R/core.R:2589-2622): the dispersion chain for ~1 with fitType "mean" on the device, and scipy's L-BFGS-B over the log
+size factors whose every objective call (value and central differences) is b200nb_sf_iterate_objective_dev
+(csrc/sf_iterate.cuh).  DESeq_device(fitType="mean") replaces the parametric trend by the trimmed mean of the
+gene-wise estimates (mean_disp).
 """
 from __future__ import annotations
 
@@ -81,6 +86,37 @@ def size_factors(y, m, type="ratio"):
     if int(nfin.item()) == 0:
         raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
     return out
+
+
+def sf_iterate_objective(y, q, alpha, par, m, h=1e-3, Q=0.05, max_tile_cols=0, out=None):
+    """b200nb_sf_iterate_objective_dev: estimateSizeFactorsIterate's objective at the log size factors `par` and at
+    the 2m points of optim's central differences, as a (2m + 1,) device tensor in the column order of
+    pipeline.iterateObjective.  y: gene-major (n, ld) counts; q: gene-major (n, ld) float64 mu / s; alpha: (n,)
+    dispersions; par: (m,) float64 device tensor.  max_tile_cols bounds the objective columns per tile (0: the
+    library's default).  Enqueue only."""
+    L = _lib.lib()
+    n, ld = y.shape
+    if out is None:
+        out = torch.empty(2 * m + 1, dtype=F64, device=y.device)
+    _lib.check(L.b200nb_sf_iterate_objective_dev(_p(y), 1 if y.dtype == F64 else 0, _p(q), _p(alpha), _p(par),
+                                                 float(h), float(Q), n, m, ld, int(max_tile_cols), _p(out),
+                                                 _stream()), "sf_iterate_objective")
+    return out
+
+
+def mean_disp(dge, minDisp=1e-8):
+    """fitType = "mean" (R/core.R:900-905) on a device tensor: mean(dge[dge > 10 minDisp], trim = 0.001) with
+    mean.default's bounds floor(n trim) + 1 .. n - floor(n trim) and .Internal(mean)'s residual correction.  Raises
+    ValueError, as estimateDispersionsFit does, when no estimate exceeds 100 minDisp (one host read).  Returns a
+    0-d device tensor."""
+    if not bool((dge > 100 * minDisp).any()):
+        raise ValueError("all gene-wise dispersion estimates are within 2 orders of magnitude from the minimum value")
+    v, _ = torch.sort(dge[dge > 10 * minDisp])
+    n = v.numel()
+    lo = int(np.floor(n * 0.001))
+    v = v[lo:n - lo]
+    s = v.sum() / v.numel()
+    return s + (v - s).sum() / v.numel()
 
 
 def _check_positive_matrix(t, y, m, name):
@@ -567,10 +603,95 @@ def _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp,
             "betaIter": fb["iter"], "betaConv": betaConv, "deviance": fb["deviance"]}
 
 
+def _dispersions_intercept_mean(ynz, m, sf, minDisp, kappa_0, dispTol, maxit, minmu, outlierSD):
+    """estimateDispersions(design ~1, fitType = "mean") as estimateSizeFactorsIterate runs it (R/core.R:2594-2597):
+    the prep kernel's clamped linear mu, the gene-wise fitDisp with its rules and grid refit, the trimmed-mean fit,
+    varLogDispEsts as dispersionFunction<- computes it (R/methods.R:142-190), estimateDispersionsPriorVar, the MAP
+    fitDisp with its grid refit and the dispersion-outlier rule.  The same steps as DESeq_device's, for x = 1.
+    Returns (q = mu / sf as a fresh gene-major tensor, final dispersions, dispGeneEst, meanDisp, dispPriorVar)."""
+    dev = ynz.device
+    x = np.ones((m, 1))
+    maxDisp = float(max(10, m))
+    min_log_alpha = float(np.log(minDisp / 10))
+    pr = prep(ynz, x, sf, minDisp=minDisp, minmu=minmu, want_mu=True, want_beta0=False)
+    xd, alpha0, mu = pr["xd"], pr["alpha0"], pr["mu_lin"]
+    la0 = torch.log(alpha0)
+    r = D.fit_disp(ynz, xd, mu, la0, la0, 1.0, min_log_alpha, kappa_0, dispTol, maxit, False)
+    dge = torch.clamp(torch.exp(r["log_alpha"]), max=maxDisp)
+    dge = torch.where(r["last_lp"] < r["initial_lp"] + r["initial_lp"].abs() / 1e6, alpha0, dge)
+    conv = (r["iter"] < maxit) & (r["iter"] != 1)
+    gi, ga = _grid_refit(ynz, xd, mu, (~conv) & (dge > minDisp * 10), m, None, 1.0, False)
+    if ga is not None:
+        dge[gi] = ga
+    dge = torch.clamp(dge, minDisp, maxDisp)
+    meanDisp = mean_disp(dge, minDisp)
+    dispFit = meanDisp.expand(dge.shape)
+    above = dge >= minDisp * 100
+    resid = (torch.log(dge) - torch.log(meanDisp))[above]
+    med = _median(resid)
+    varLogDispEsts = (1.4826 * _median((resid - med).abs())) ** 2
+    if m - 1 <= 3:
+        from .pipeline import estimateDispersionsPriorVar
+        dispPriorVar = estimateDispersionsPriorVar(float(varLogDispEsts.item()), m, 1, dge.cpu().numpy(),
+                                                   dispFit.cpu().numpy(), minDisp)
+    else:
+        expVar = torch.special.polygamma(1, torch.tensor((m - 1) / 2.0, dtype=F64, device=dev))
+        dispPriorVar = float(torch.clamp(varLogDispEsts - expVar, min=0.25).item())
+    logFit = torch.log(dispFit).contiguous()
+    dispInit = torch.where(dge > 0.1 * dispFit, dge, dispFit)
+    rm = D.fit_disp(ynz, xd, mu, torch.log(dispInit), logFit, dispPriorVar, min_log_alpha, kappa_0, dispTol, maxit,
+                    True)
+    dispMAP = torch.exp(rm["log_alpha"])
+    gi2, ga2 = _grid_refit(ynz, xd, mu, rm["iter"] >= maxit, m, logFit, dispPriorVar, True)
+    if ga2 is not None:
+        dispMAP[gi2] = ga2
+    dispMAP = torch.clamp(dispMAP, minDisp, maxDisp)
+    dispOutlier = torch.log(dge) > logFit + outlierSD * torch.sqrt(varLogDispEsts)
+    dispersion = torch.where(dispOutlier, dge, dispMAP).contiguous()
+    q = torch.ones_like(mu)
+    q[:, :m] = mu[:, :m] / torch.as_tensor(np.asarray(sf, dtype=np.float64), device=dev)[None, :]
+    return q, dispersion, dge, meanDisp, dispPriorVar
+
+
+def size_factors_iterate(y, m, niter=10, Q=0.05, minDisp=1e-8, minmu=0.5, kappa_0=1.0, dispTol=1e-6, maxit=100,
+                         outlierSD=2.0, h=1e-3, max_tile_cols=0):
+    """estimateSizeFactorsIterate (R/core.R:2589-2622) on the device: the rows of y (gene-major (N, ld) counts) with
+    a positive sum, s = 1 to start; each outer iteration runs the dispersion chain for design ~1 with fitType "mean"
+    (_dispersions_intercept_mean) and maximises the trimmed total log-likelihood over the log size factors with
+    pipeline.optimizeLogSizeFactors (scipy's L-BFGS-B with optim's settings, the host mirror's driver): every
+    objective call is one b200nb_sf_iterate_objective_dev launch sequence and one D2H copy of 2m + 1 doubles.  R's
+    stops raise ValueError (see pipeline.iterateSizeFactors; niter = 1 always stops, as in R).
+    Returns {"sizeFactors": (m,) numpy, "iterations", "evaluations": objective calls per iteration, "dispersion",
+    "dispGeneEst", "meanDisp", "dispPriorVar" of the last iteration (device tensors / floats), "idx": kept rows}."""
+    from .pipeline import iterateSizeFactors
+    dev = y.device
+    idx = torch.nonzero(y[:, :m].sum(dim=1) > 0).squeeze(1)
+    ynz = y if idx.numel() == y.shape[0] else y[idx].contiguous()
+    out = torch.empty(2 * m + 1, dtype=F64, device=dev)
+
+    def step(sf):
+        q, disp, dge, meanDisp, dpv = _dispersions_intercept_mean(ynz, m, sf, minDisp, kappa_0, dispTol, maxit, minmu,
+                                                                  outlierSD)
+
+        def evaluate(par):
+            pd = torch.as_tensor(np.asarray(par, dtype=np.float64), device=dev)
+            return sf_iterate_objective(ynz, q, disp, pd, m, h=h, Q=Q, max_tile_cols=max_tile_cols,
+                                        out=out).cpu().numpy()
+
+        return evaluate, {"dispersion": disp, "dispGeneEst": dge, "meanDisp": float(meanDisp.item()),
+                          "dispPriorVar": dpv, "q": q}
+
+    r = iterateSizeFactors(m, step, niter=niter, h=h)
+    res = {"sizeFactors": r["sizeFactors"], "iterations": r["iterations"], "evaluations": r["evaluations"],
+           "idx": idx}
+    res.update(r["last"])
+    return res
+
+
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
                  outlierSD=2.0, minReplicatesForReplace=np.inf, allgather=None, useOptim=True, betaPrior=False,
                  factors=None, weights=None, weightThreshold=1e-2, normalizationFactors=None, avgTxLength=None,
-                 nfXim=None):
+                 nfXim=None, sfType="ratio", fitType="parametric"):
     """y: gene-major (N, ld) device tensor of counts (int32 or float64).  Returns a dict of device tensors over the
     rows with a non-zero sum (`idx` maps them back to the N input rows) plus the trend / prior scalars.
     sizeFactors=None estimates them on the device first (median of ratios, R/core.R:535-578; returned under
@@ -604,10 +725,26 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     distances and outlier replacement.  avgTxLength (same layout, instead of normalizationFactors): the factors are
     estimated first by normalization_factors, as DESeq() -> estimateSizeFactors does for a tximport dataset.  Returned
     under "normalizationFactors" (rows in idx).  Not with sizeFactors or weights (ValueError).  nfXim: xim computed
-    by the caller (the sharded driver, over every rank's rows)."""
+    by the caller (the sharded driver, over every rank's rows).
+    sfType: the estimator used when none of sizeFactors, normalizationFactors and avgTxLength is given: "ratio" (the
+    default), "poscounts", or "iterate" (size_factors_iterate with its defaults, whatever minmu / minDisp this call
+    uses, as DESeq() -> estimateSizeFactors does; its iteration and objective-call counts are returned under
+    "sfIterate").  "iterate" with weights, normalizationFactors or avgTxLength raises ValueError.
+    fitType: "parametric" (the default; "trendCoefs") or "mean": dispFit is the trimmed mean of the gathered
+    gene-wise estimates (mean_disp, no extra collective), reported under "meanDisp" instead of "trendCoefs".  Both
+    are reported under "fitType"."""
     dev = y.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
+    if sfType not in ("ratio", "poscounts", "iterate"):
+        raise ValueError("sfType must be 'ratio', 'poscounts' or 'iterate'")
+    if fitType not in ("parametric", "mean"):
+        raise ValueError("fitType must be 'parametric' or 'mean'")
+    if sfType == "iterate" and sizeFactors is None and (weights is not None or normalizationFactors is not None
+                                                        or avgTxLength is not None):
+        raise ValueError("sfType='iterate' is not supported with observation weights, normalizationFactors or "
+                         "avgTxLength")
+    sfIterate = None
     if avgTxLength is not None:
         if normalizationFactors is not None:
             raise ValueError("give normalizationFactors or avgTxLength, not both")
@@ -634,7 +771,16 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             raise ValueError("outlier replacement (finite minReplicatesForReplace) is not supported with betaPrior=True")
     estimated = sizeFactors is None and nf is None
     if estimated:
-        sizeFactors = size_factors(y, m)["sizeFactors"].cpu().numpy()
+        if sfType == "iterate":
+            # DESeq() passes none of its dispersion / fit arguments to estimateSizeFactors: the iterate estimator's
+            # estimateDispersions call runs with its own defaults (minmu = 0.5, R/core.R:388, 2596, 662)
+            sfIterate = size_factors_iterate(y, m)
+            sizeFactors = sfIterate["sizeFactors"]
+        elif sfType == "poscounts":
+            sf = size_factors(y, m, type="poscounts")["sizeFactors"]
+            sizeFactors = (sf / torch.exp(torch.log(sf).mean())).cpu().numpy()   # incoming geoMeans (R/core.R:573-576)
+        else:
+            sizeFactors = size_factors(y, m)["sizeFactors"].cpu().numpy()
     import os
     import time
     stage_ms = {}
@@ -731,7 +877,13 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     # ---- estimateDispersionsFit + dispersionFunction<- + PriorVar (R/core.R:864-940, R/methods.R:142-190, R/core.R:1135-1208)
     # ONE packed collective for the two vectors the global step needs (sharded.PackedGather accepts a list)
     bm_all, dge_all = allgather([bm, dge]) if allgather is not None else (bm, dge)
-    tr = trend_fit(bm_all, dge_all, minDisp)
+    if fitType == "mean":
+        # dispersionFunction(means) = meanDisp: (meanDisp, 0) in the trend's slots keeps every a + b / baseMean below
+        # (here, in the MAP prior and in the outlier refit) equal to meanDisp
+        tr = torch.zeros(4, dtype=F64, device=dev)
+        tr[0] = mean_disp(dge_all, minDisp)
+    else:
+        tr = trend_fit(bm_all, dge_all, minDisp)
     dispFit = tr[0] + tr[1] / bm
     above = dge_all >= minDisp * 100
     resid = (torch.log(dge_all) - torch.log(tr[0] + tr[1] / bm_all))[above]
@@ -803,10 +955,16 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             "dispersion": dispersion, "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": rm["iter"],
             "betaMatrix": betaMatrix.T, "betaSE": betaSE.T, "WaldStatistic": stat.T, "WaldPvalue": pval.T,
             "betaIter": fit["iter"], "betaConv": betaConv, "n_optim": n_optim, "deviance": -2.0 * fit_ll["logLike"], "mu": mu_cooks,
-            "H": fb["hat_diagonals"], "trendCoefs": tr[:2], "varLogDispEsts": varLogDispEsts,
+            "H": fb["hat_diagonals"], "varLogDispEsts": varLogDispEsts,
             "dispPriorVar": dispPriorVar, "n_refit_geneest": n_refit_geneest, "n_refit_map": int(gi2.numel()),
             "n_input_rows": y.shape[0],
-            "sizeFactors": None if nf is not None else np.asarray(sizeFactors, dtype=np.float64)}
+            "sizeFactors": None if nf is not None else np.asarray(sizeFactors, dtype=np.float64), "fitType": fitType}
+    if fitType == "mean":
+        res["meanDisp"] = float(tr[0].item())
+    else:
+        res["trendCoefs"] = tr[:2]
+    if sfIterate is not None:
+        res["sfIterate"] = {"iterations": sfIterate["iterations"], "evaluations": sfIterate["evaluations"]}
     res.update(prior)
     if weights is not None:
         res["weightsFail"], res["weights"] = weightsFail, wn

@@ -5,10 +5,12 @@ image, so the steps that prepare the inputs of fitDisp / fitBeta and consume the
 numpy, one function per R function, same names, so the engine can be driven and measured end to end:
 
   estimateSizeFactorsForMatrix   R/core.R:535-578   (type="ratio")
+  estimateSizeFactorsIterate     R/core.R:2589-2622 (sfType="iterate"; optim's L-BFGS-B on scipy's implementation)
   getBaseMeansAndVariances       R/core.R:2138-2157
   linearModelMu / roughDispEstimate / momentsDispEstimate   R/core.R:2454-2459, 2422-2437, 2439-2448
   estimateDispersionsGeneEst     R/core.R:657-860
   parametricDispersionFit        R/core.R:2166-2189  (Gamma GLM, identity link, glm.fit IRLS restated)
+  fitType = "mean"               R/core.R:900-905    (trimmed mean of the gene-wise estimates)
   dispersionFunction<-           R/methods.R:142-190 (dispFit, varLogDispEsts = mad^2)
   estimateDispersionsPriorVar    R/core.R:1135-1208  (incl. the Monte-Carlo branch for 1..3 residual df, own RNG)
   estimateDispersionsMAP         R/core.R:943-1131
@@ -32,7 +34,7 @@ either to the code; DESeq(normalizationFactors=...) threads it through every ste
 
 `engine` is any object with fitDisp / fitDispGrid / fitBeta taking the reference's argument names
 (deseq2_b200.wrappers is the product engine and the default; tests and the bench's CPU baseline pass the
-oracle).  Not restated (out of scope, SURVEY.md section 8f): local / mean trend fits, results()/lfcShrink().
+oracle).  Not restated (out of scope, SURVEY.md section 8f): the local trend fit, results()/lfcShrink().
 """
 from __future__ import annotations
 
@@ -45,12 +47,22 @@ from .wrappers import fitBetaWrapper, fitDispGridWrapper, fitDispWrapper
 LN2 = np.log(2.0)
 
 
-def estimateSizeFactorsForMatrix(counts):
-    """R/core.R:535-578, type='ratio', locfunc=median."""
+def estimateSizeFactorsForMatrix(counts, type="ratio"):
+    """R/core.R:535-578, locfunc=median.  type "ratio": loggeomeans = rowMeans(log K).  type "poscounts" (as
+    estimateSizeFactors calls it, R/methods.R:377-390): geoMeans = geoMeanNZ per row, log(exp(sum(log K[K > 0]) / m))
+    (0 for an all-zero row), passed as incoming geoMeans, so the factors are rescaled to geometric mean 1 (:573-576)."""
+    if type not in ("ratio", "poscounts"):
+        raise ValueError("type must be 'ratio' or 'poscounts'")
     counts = np.asarray(counts, dtype=np.float64)
     with np.errstate(divide="ignore"):
         logc = np.log(counts)
-    loggeomeans = logc.mean(axis=1)
+    if type == "poscounts":
+        pos = counts > 0
+        s = np.where(pos, logc, 0.0).sum(axis=1)
+        with np.errstate(divide="ignore"):
+            loggeomeans = np.log(np.where(pos.any(axis=1), np.exp(s / counts.shape[1]), 0.0))
+    else:
+        loggeomeans = logc.mean(axis=1)
     if np.all(np.isinf(loggeomeans)):
         raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
     ok = np.isfinite(loggeomeans)
@@ -58,7 +70,100 @@ def estimateSizeFactorsForMatrix(counts):
     for j in range(counts.shape[1]):
         sel = ok & (counts[:, j] > 0)
         sf[j] = np.exp(np.median(logc[sel, j] - loggeomeans[sel]))
+    if type == "poscounts":
+        sf = sf / np.exp(np.mean(np.log(sf)))
     return sf
+
+
+def iterateObjective(counts, q, disps, par, h=1e-3, Q=0.05):
+    """The objective of estimateSizeFactorsIterate (R/core.R:2598-2604) evaluated directly at par and at the 2m points
+    of optim's central differences, in the column order of b200nb_sf_iterate_objective_dev: [fn(par), fn(par + h e_k)
+    for k < m, fn(par - h e_k) for k < m], with fn(p) = sum(gene.ll[gene.ll > quantile(gene.ll, Q)]),
+    gene.ll = nbinomLogLike(counts, q * exp(p - mean(p)), disps) -- 2m + 1 full log-likelihood sums."""
+    counts = np.asarray(counts, dtype=np.float64)
+    par = np.asarray(par, dtype=np.float64)
+    m = len(par)
+    pts = [par] + [par + h * np.eye(m)[k] for k in range(m)] + [par - h * np.eye(m)[k] for k in range(m)]
+    out = np.empty(2 * m + 1)
+    for c, p in enumerate(pts):
+        ll = nbinomLogLike(counts, q * np.exp(p - np.mean(p))[None, :], disps)
+        out[c] = ll[ll > np.quantile(ll, Q, method="linear")].sum()
+    return out
+
+
+def optimizeLogSizeFactors(evaluate, par0, h=1e-3):
+    """optim(par0, fn, control = list(fnscale = -1), method = "L-BFGS-B") as estimateSizeFactorsIterate calls it
+    (R/core.R:2605), on scipy's L-BFGS-B (not R's lbfgsb.c): minimise -fn with optim's defaults lmm = 5,
+    factr = 1e7 (ftol = factr * eps), pgtol = 0, maxit = 100, no bounds, and optim's finite-difference gradient
+    (fmingr, ndeps = h): -(fn(par + h e_k) - fn(par - h e_k)) / (2 h).  `evaluate(par)` returns the 2m + 1 values of
+    iterateObjective's column order, one call per point.  Raises ValueError where optim stops on a non-finite value.
+    Returns scipy's OptimizeResult (status 0 = converged; `nfev` = objective calls)."""
+    from scipy import optimize as _so
+    m = len(par0)
+
+    def fg(p):
+        v = np.asarray(evaluate(p), dtype=np.float64)
+        if not np.isfinite(v[0]):
+            raise ValueError("L-BFGS-B needs finite values of 'fn'")
+        g = -(v[1:m + 1] - v[m + 1:]) / (2.0 * h)
+        if not np.all(np.isfinite(g)):
+            raise ValueError(f"non-finite finite-difference value [{int(np.flatnonzero(~np.isfinite(g))[0]) + 1}]")
+        return -v[0], g
+
+    return _so.minimize(fg, np.asarray(par0, dtype=np.float64), jac=True, method="L-BFGS-B",
+                        options={"maxcor": 5, "ftol": 1e7 * np.finfo(float).eps, "gtol": 0.0, "maxiter": 100})
+
+
+def iterateSizeFactors(m, step, niter=10, h=1e-3):
+    """The outer loop of estimateSizeFactorsIterate (R/core.R:2589-2622), shared by the host mirror and the device
+    path: `step(sf)` runs the dispersion chain at the size factors sf and returns (evaluate, info), the objective
+    evaluator for optimizeLogSizeFactors and whatever the caller wants kept from the last iteration.  R's stops: the
+    optimiser's status != 0, and niter iterations without sum((log sf_old - log sf)^2) < 1e-4 (tested from the second
+    iteration on, so niter = 1 always stops).  Returns sizeFactors, iterations, evaluations (objective calls per
+    iteration) and the last info."""
+    sf = np.ones(m)
+    evals = []
+    info = None
+    for i in range(1, niter + 1):
+        evaluate, info = step(sf)
+        sf_old = sf
+        o = optimizeLogSizeFactors(evaluate, np.log(sf_old), h)
+        evals.append(int(o.nfev))
+        if o.status != 0:
+            raise ValueError("iterative size factor normalization did not converge within an iteration")
+        sf = np.exp(o.x - np.mean(o.x))
+        if i > 1 and np.sum((np.log(sf_old) - np.log(sf)) ** 2) < 1e-4:
+            break
+        if i == niter:
+            raise ValueError("iterative size factor normalization did not converge")
+    return {"sizeFactors": sf, "iterations": i, "evaluations": evals, "last": info}
+
+
+def estimateSizeFactorsIterate(counts, niter=10, Q=0.05, engine=None, minDisp=1e-8, minmu=0.5):
+    """R/core.R:2589-2622: design ~1; each iteration estimateDispersions(fitType = "mean") at the current size
+    factors, q = mu / sf of the gene-wise fit, and optim over the log size factors of the trimmed total
+    log-likelihood (iterateObjective, evaluated directly).  Rows with a zero sum are left out.  Returns
+    iterateSizeFactors' dict; "last" holds the last iteration's q and dispersions (and the dispersion results)."""
+    counts = np.asarray(counts)
+    cts = counts[counts.sum(axis=1) > 0]
+    m = cts.shape[1]
+    x = np.ones((m, 1))
+
+    def step(sf):
+        mv = getBaseMeansAndVariances(cts, sf)
+        ge = estimateDispersionsGeneEst(cts, sf, x, engine=engine, mv=mv, minmu=minmu, minDisp=minDisp)
+        tf = estimateDispersionsFit(ge["dispGeneEst"], ge["baseMean"], minDisp=minDisp, fitType="mean")
+        dispPriorVar = estimateDispersionsPriorVar(tf["varLogDispEsts"], m, 1, ge["dispGeneEst"], tf["dispFit"],
+                                                   minDisp)
+        mp = estimateDispersionsMAP(cts, x, ge["mu"], ge["dispGeneEst"], tf["dispFit"], dispPriorVar,
+                                    tf["varLogDispEsts"], engine=engine, minDisp=minDisp)
+        q = ge["mu"] / sf[None, :]
+        disps = mp["dispersion"]
+        info = {"q": q, "dispersion": disps, "dispGeneEst": ge["dispGeneEst"], "meanDisp": tf["meanDisp"],
+                "dispPriorVar": dispPriorVar}
+        return (lambda par: iterateObjective(cts, q, disps, par, Q=Q)), info
+
+    return iterateSizeFactors(m, step, niter=niter)
 
 
 def _div(sizeFactors):
@@ -339,17 +444,45 @@ def _mad(x):
     return 1.4826 * np.median(np.abs(x - np.median(x)))
 
 
-def estimateDispersionsFit(dispGeneEst, baseMean, minDisp=1e-8):
-    """R/core.R:864-940 (fitType='parametric') + dispersionFunction<- (R/methods.R:142-190)."""
+def r_trimmed_mean(v, trim):
+    """R's mean(v, trim = trim) for 0 < trim < 0.5 (mean.default): the order statistics floor(n trim) + 1 ..
+    n - floor(n trim), averaged as .Internal(mean) does, a sum over n plus the mean of the residuals."""
+    v = np.sort(np.asarray(v, dtype=np.float64))
+    n = len(v)
+    lo = int(np.floor(n * trim))
+    v = v[lo:n - lo]
+    s = v.sum() / len(v)
+    return float(s + (v - s).sum() / len(v))
+
+
+def meanDispersionFit(dispGeneEst, minDisp=1e-8):
+    """fitType = "mean" (R/core.R:900-905): mean(dispGeneEst[dispGeneEst > 10 minDisp], trim = 0.001)."""
+    d = np.asarray(dispGeneEst, dtype=np.float64)
+    return r_trimmed_mean(d[d > 10 * minDisp], 0.001)
+
+
+def estimateDispersionsFit(dispGeneEst, baseMean, minDisp=1e-8, fitType="parametric"):
+    """R/core.R:864-940 (fitType 'parametric' or 'mean') + dispersionFunction<- (R/methods.R:142-190).  For "mean"
+    `coefs` is (meanDisp, 0), so coefs[0] + coefs[1] / baseMean is the constant fit, and `meanDisp` is added."""
+    if fitType not in ("parametric", "mean"):
+        raise ValueError("fitType must be 'parametric' or 'mean'")
     useForFit = dispGeneEst > 100 * minDisp
     if useForFit.sum() == 0:
         raise ValueError("all gene-wise dispersion estimates are within 2 orders of magnitude from the minimum value")
-    coefs = parametricDispersionFit(baseMean[useForFit], dispGeneEst[useForFit])
-    dispFit = coefs[0] + coefs[1] / baseMean
+    if fitType == "mean":
+        meanDisp = meanDispersionFit(dispGeneEst, minDisp)
+        coefs = np.array([meanDisp, 0.0])
+        dispFit = np.full(len(baseMean), meanDisp)
+    else:
+        coefs = parametricDispersionFit(baseMean[useForFit], dispGeneEst[useForFit])
+        dispFit = coefs[0] + coefs[1] / baseMean
     aboveMinDisp = dispGeneEst >= minDisp * 100
     dispResiduals = np.log(dispGeneEst) - np.log(dispFit)
     varLogDispEsts = _mad(dispResiduals[aboveMinDisp]) ** 2
-    return {"dispFit": dispFit, "coefs": coefs, "varLogDispEsts": varLogDispEsts}
+    out = {"dispFit": dispFit, "coefs": coefs, "varLogDispEsts": varLogDispEsts}
+    if fitType == "mean":
+        out["meanDisp"] = coefs[0]
+    return out
 
 
 def _loess_quadratic(xg, yg, xnew, span):
@@ -852,7 +985,8 @@ def fitGLMsWithPrior(counts, nf, factors, dispersion, baseMean, dispFit, engine=
 
 
 def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.inf, useOptim=True, betaPrior=False,
-          factors=None, weights=None, weightThreshold=1e-2, minmu=0.5, normalizationFactors=None):
+          factors=None, weights=None, weightThreshold=1e-2, minmu=0.5, normalizationFactors=None, sfType="ratio",
+          fitType="parametric"):
     """R/core.R:280-432 with test='Wald', fitType='parametric', betaPrior=FALSE by default.
     minReplicatesForReplace: the reference's default is 7 (outlier replacement + refit whenever a design cell has >= 7
     samples, R/core.R:419-426, refitWithoutOutliers :2484-2565); the default here is Inf = off, which is what the
@@ -870,11 +1004,23 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     normalizationFactors: an (N, m) matrix of gene-specific normalization factors in place of sizeFactors, used by
     every step (getSizeOrNormFactors); the moments dispersion's xim is over the non-all-zero rows.  Returned under
     `normalizationFactors`.  Not with sizeFactors or weights (ValueError).
+    sfType: the estimator used when neither sizeFactors nor normalizationFactors is given: "ratio" (the default),
+    "poscounts" or "iterate" (estimateSizeFactorsIterate; not with weights: ValueError).  The iterate run's outer
+    iteration and objective-call counts are returned under `sfIterate`.
+    fitType: "parametric" (the default; `trendCoefs`) or "mean" (R/core.R:900-905; `meanDisp` instead of
+    `trendCoefs`).  Both are reported under `fitType`.
     Returns per-gene vectors over ALL rows; all-zero rows carry NaN (buildDataFrameWithNARows, R/core.R:2232)."""
     engine = engine or _default_engine
     counts = np.asarray(counts)
     N, m = counts.shape
     p = x.shape[1]
+    if sfType not in ("ratio", "poscounts", "iterate"):
+        raise ValueError("sfType must be 'ratio', 'poscounts' or 'iterate'")
+    if fitType not in ("parametric", "mean"):
+        raise ValueError("fitType must be 'parametric' or 'mean'")
+    if sfType == "iterate" and sizeFactors is None and (weights is not None or normalizationFactors is not None):
+        raise ValueError("sfType='iterate' is not supported with observation weights or normalization factors")
+    sfIterate = None
     if betaPrior:
         if factors is None:
             raise ValueError("betaPrior=True needs the design factors (factors=...)")
@@ -898,7 +1044,13 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
         if sizeFactors.shape != counts.shape or not np.all(np.isfinite(sizeFactors) & (sizeFactors > 0)):
             raise ValueError("normalizationFactors must be finite, positive and of the counts' shape")
     if sizeFactors is None:
-        sizeFactors = estimateSizeFactorsForMatrix(counts)
+        if sfType == "iterate":
+            sfIterate = estimateSizeFactorsIterate(counts, engine=engine)
+            sizeFactors = sfIterate["sizeFactors"]
+        elif sfType == "poscounts":
+            sizeFactors = estimateSizeFactorsForMatrix(counts, type="poscounts")
+        else:
+            sizeFactors = estimateSizeFactorsForMatrix(counts)
     sizeFactors = np.asarray(sizeFactors, dtype=np.float64)
     mvAll = getBaseMeansAndVariances(counts, sizeFactors, weights)
     nz = ~mvAll["allZero"]
@@ -918,7 +1070,7 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     mv = {k: v[nz] for k, v in mvAll.items()}
     ge = estimateDispersionsGeneEst(cnz, sizeFactors, x, engine=engine, mv=mv, weights=wnz,
                                     weightThreshold=weightThreshold, minmu=minmu)
-    tf = estimateDispersionsFit(ge["dispGeneEst"], ge["baseMean"])
+    tf = estimateDispersionsFit(ge["dispGeneEst"], ge["baseMean"], fitType=fitType)
     dispPriorVar = estimateDispersionsPriorVar(tf["varLogDispEsts"], m, p, ge["dispGeneEst"], tf["dispFit"])
     mp = estimateDispersionsMAP(cnz, x, ge["mu"], ge["dispGeneEst"], tf["dispFit"], dispPriorVar,
                                 tf["varLogDispEsts"], engine=engine, weights=wnz, weightThreshold=weightThreshold)
@@ -994,8 +1146,14 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
 
     res = {k: full(np.asarray(v, dtype=np.float64)) for k, v in per_gene.items()}
     res.update({"sizeFactors": None if sfAll.ndim == 2 else sfAll, "allZero": mvAll["allZero"], "dispPriorVar": dispPriorVar,
-                "trendCoefs": tf["coefs"], "varLogDispEsts": tf["varLogDispEsts"], "n_refit_geneest": ge["n_refit"],
-                "n_refit_map": mp["n_refit"]})
+                "varLogDispEsts": tf["varLogDispEsts"], "n_refit_geneest": ge["n_refit"],
+                "n_refit_map": mp["n_refit"], "fitType": fitType})
+    if fitType == "mean":
+        res["meanDisp"] = tf["meanDisp"]
+    else:
+        res["trendCoefs"] = tf["coefs"]
+    if sfIterate is not None:
+        res["sfIterate"] = {"iterations": sfIterate["iterations"], "evaluations": sfIterate["evaluations"]}
     res["baseMean"] = np.where(nz, res["baseMean"], 0.0)
     if weights is not None:
         res["baseMean"] = np.where(mvAll["allZero"], 0.0, mvAll["baseMean"])    # weightsFail rows keep theirs

@@ -148,6 +148,9 @@ def sharded_DESeq_device(y_local, x, sizeFactors=None, **kw):
     minReplicatesForReplace (the refitted rows' xim would need another collective) or avgTxLength (estimating the
     factors needs a global median): estimate them on one device or pass them."""
     from . import device_pipeline as DP
+    if kw.get("sfType") == "iterate":
+        raise ValueError("sharded runs do not estimate iterate size factors (every perturbation needs a quantile over "
+                         "all genes): estimate them on one device (size_factors_iterate) and pass sizeFactors")
     pg = PackedGather(y_local.shape[0], y_local.device)
     nf = kw.get("normalizationFactors")
     if kw.get("avgTxLength") is not None:

@@ -201,6 +201,20 @@ int b200nb_beta_prior_quantile_dev(const double* beta_log2, int n, int p, const 
                                    const double* disp_fit, const int32_t* col_a, const int32_t* col_b, int k,
                                    double prob, double* out_q, void* stream);
 
+/* b200nb_sf_iterate_objective_dev: the objective of estimateSizeFactorsIterate (R/core.R:2589-2622) at the log size
+ * factors par[m] and at the 2m points optim's finite-difference gradient needs (ndeps = h):
+ *   fn(p) = sum(gene.ll[gene.ll > quantile(gene.ll, Q)]),  gene.ll_i = sum_j log dnbinom(K_ij; q_ij s_j, 1/alpha_i),
+ *   s = exp(p - mean(p)),  quantile type 7.
+ * out[0] = fn(par), out[1 + k] = fn(par + h e_k), out[1 + m + k] = fn(par - h e_k), k < m.  y: counts, gene-major
+ * (n x ld, int32 or f64); q: gene-major n x ld, mu / s of the dispersion fit; alpha: n dispersions.  Needs n, m >= 1,
+ * finite h > 0, 0 <= Q < 1 and no NULL pointer.  The gene log-likelihoods are formed for tiles of at most
+ * max_tile_cols objective columns (0: as many as 128 MB of workspace hold) in a workspace the library keeps per
+ * process, shared with the host entry points (calls on different streams must not overlap).  Enqueue only;
+ * deterministic: two calls on the same input give the same bits. */
+int b200nb_sf_iterate_objective_dev(const void* y, int y_type, const double* q, const double* alpha,
+                                    const double* par, double h, double Q, int n, int m, long long ld,
+                                    int max_tile_cols, double* out, void* stream);
+
 /* ---- housekeeping */
 const char* b200nb_last_error(void);
 int b200nb_device_count(void);            /* number of visible CUDA devices (0 if none / no driver) */
