@@ -8,7 +8,8 @@ mirror of the reference's R callers needed to drive and measure it:
   wrappers.py   fitDisp / fitDispGrid / fitBeta + the *Wrapper functions (R/wrappers.R, R/RcppExports.R)
   device.py     the same three calls on device-resident torch tensors (gene-major layout)
   device_pipeline.py  the whole Wald / LRT analysis device-resident: size factors, pre-steps, trend fit, Cook's distances,
-                outlier replacement + refit and getContrast as kernels / tensor glue around the three calls
+                outlier replacement + refit and getContrast as kernels / tensor glue around the three calls; vst(),
+                varianceStabilizingTransformation() and normTransform() (R/vst.R) with one transform kernel
   pipeline.py   host glue of DESeq()'s Wald path that feeds/consumes the kernels (R/core.R, R/fitNbinomGLMs.R)
   synth.py      makeExampleDESeqDataSet-style synthetic counts (R/core.R:459-498)
   sharded.py    gene-sharded multi-GPU drivers, host glue and device-resident (R/parallel.R:6-74 is the blueprint)

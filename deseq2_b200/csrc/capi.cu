@@ -1459,6 +1459,44 @@ int b200nb_sf_iterate_objective_dev(const void* y, int y_type, const double* q, 
   return 0;
 }
 
+int b200nb_transform_dev(const void* y, int y_type, const double* size_factors, const double* nf, int n, int m,
+                         long long ld, int mode, double c0, double c1, double* out, long long ld_out, void* stream) {
+  if (n < 0 || m < 0) return fail("transform: bad dimensions n=%d m=%d (both must be >= 0)", n, m);
+  if (ld < m || ld_out < m) return fail("transform: ld=%lld and ld_out=%lld must be >= m=%d", ld, ld_out, m);
+  if ((size_factors == nullptr) == (nf == nullptr))
+    return fail("transform: give exactly one of size_factors and nf");
+  if (!y || !out) return fail("transform: null pointer argument");
+  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
+  const auto finite_pos = [](double v) { return v > 0.0 && v < HUGE_VAL; };
+  nb::TransformArgs a{};
+  a.mode = mode;
+  a.ln2 = log(2.0);
+  switch (mode) {
+    case B200NB_TRANSFORM_VST_PARAMETRIC:
+      if (!finite_pos(c0) || !finite_pos(c1))
+        return fail("transform: asymptDisp=%g and extraPois=%g must be finite and > 0", c0, c1);
+      a.c0 = c0; a.c1 = 1.0 + c1; a.c2 = 2.0 * c0; a.c3 = 4.0 * c0;
+      break;
+    case B200NB_TRANSFORM_VST_MEAN:
+      if (!finite_pos(c0)) return fail("transform: alpha=%g must be finite and > 0", c0);
+      a.c0 = c0; a.c1 = log(c0); a.c2 = log(4.0);
+      break;
+    case B200NB_TRANSFORM_LOG2:
+      if (!(c0 >= 0.0 && c0 < HUGE_VAL)) return fail("transform: pc=%g must be finite and >= 0", c0);
+      a.c0 = c0;
+      break;
+    default:
+      return fail("transform: bad mode %d", mode);
+  }
+  if (n == 0 || m == 0) return 0;
+  if (check_device()) return 1;
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.size_factors = size_factors; a.nf = nf;
+  a.n = n; a.m = m; a.ld = ld; a.ld_out = ld_out; a.out = out;
+  CU(nb::launch_transform(a, (cudaStream_t)stream));
+  g_launches++;
+  return 0;
+}
+
 /* ------------------------------------------------------------------ host entry points */
 /* Each entry point runs at most twice: attempt 0 may launch on resident copies of its input matrices before their
  * content has been verified (CallInputs::validate, overlapped with the kernels); if a verification fails the launch

@@ -241,6 +241,21 @@ struct SfIterateArgs {
 };
 cudaError_t launch_sf_iterate_objective(const SfIterateArgs& a, cudaStream_t stream);
 
+// The transforms of the normalized counts (transform.cuh, launched from size_factors.cu): VST for fitType "parametric" / "mean", log2(q + pc)
+enum TransformMode { kTfVstParametric = 0, kTfVstMean = 1, kTfLog2 = 2 };
+struct TransformArgs {
+  const void* y;
+  int y_is_f64;
+  const double* size_factors;  // m, or nullptr when nf is given
+  const double* nf;            // gene-major n x ld normalization factors, or nullptr
+  int n, m;
+  long long ld, ld_out;
+  int mode;                    // TransformMode
+  double c0, c1, c2, c3, ln2;  // per-mode constants, see transform.cuh
+  double* out;                 // gene-major n x ld_out (out)
+};
+cudaError_t launch_transform(const TransformArgs& a, cudaStream_t stream);
+
 // Cook's distances (pipeline_kernels.cu)
 struct CooksArgs {
   const void* y;

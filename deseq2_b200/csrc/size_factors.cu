@@ -14,7 +14,8 @@
 // The same one-CTA-per-column radix refinement computes estimateBetaPriorVar's weighted upper quantiles
 // (beta_prior_quantile_kernel, beta_prior.cuh) and the trimmed sums of estimateSizeFactorsIterate's objective
 // (iterate_trim_sum_kernel, sf_iterate.cuh, whose per-gene kernel starts the same way); all start through
-// launch_per_column.
+// launch_per_column, as does the transform of the normalized counts (transform_kernel, transform.cuh: VST and
+// normTransform), one CTA per block of rows.
 #include "engine.h"
 #include "beta_prior.cuh"
 #include "nbmath.cuh"
@@ -163,11 +164,13 @@ __global__ void __launch_bounds__(512) sf_median_kernel(const double* __restrict
 }  // namespace nb
 
 #include "sf_iterate.cuh"
+#include "transform.cuh"
 
 namespace nb {
 namespace {
 
-// One CTA per column with static shared memory only: the launch site of the column-select kernels of this file.
+// One CTA per column (or per block of rows) with static shared memory only: the launch site of the kernels of this
+// file and its headers.
 template <class... P, class... A>
 cudaError_t launch_per_column(void (*kern)(P...), int columns, int threads, cudaStream_t stream, A... args) {
   kern<<<columns, threads, 0, stream>>>(args...);
@@ -204,6 +207,13 @@ cudaError_t launch_sf_iterate_objective(const SfIterateArgs& a, cudaStream_t str
     if (e != cudaSuccess) return e;
   }
   return cudaSuccess;
+}
+
+cudaError_t launch_transform(const TransformArgs& a, cudaStream_t stream) {
+  if (a.n == 0 || a.m == 0) return cudaSuccess;
+  const int rows = transform_rows_per_cta(a.m);
+  return launch_per_column(transform_kernel_for(a), (int)(((long long)a.n + rows - 1) / rows), kTfThreads, stream, a,
+                           rows);
 }
 
 }  // namespace nb

@@ -28,6 +28,9 @@ R/core.R:2589-2622): the dispersion chain for ~1 with fitType "mean" on the devi
 size factors whose every objective call (value and central differences) is b200nb_sf_iterate_objective_dev
 (csrc/sf_iterate.cuh).  DESeq_device(fitType="mean") replaces the parametric trend by the trimmed mean of the
 gene-wise estimates (mean_disp).
+vst_device, varianceStabilizingTransformation_device, vst_transform and normTransform_device (R/vst.R,
+R/helper.R:421-435) fit the dispersion function with DESeq_device's GeneEst block and trend, and transform the n x m
+matrix with one kernel (b200nb_transform_dev, csrc/transform.cuh).
 """
 from __future__ import annotations
 
@@ -688,6 +691,67 @@ def size_factors_iterate(y, m, niter=10, Q=0.05, minDisp=1e-8, minmu=0.5, kappa_
     return res
 
 
+def _gene_est(ynz, xd, sfd, alpha0, beta0, mu_lin, m, minDisp, kappa_0, dispTol, maxit, betaTol, minmu, wn=None,
+              wdisp=None, weightThreshold=1e-2, mark=lambda name: None):
+    """estimateDispersionsGeneEst (R/core.R:657-860) after the pre-steps: the gene-wise mean (mu_lin, the prep
+    kernel's linear mu, when it is given; else a GLM fit, weighted with R's defaults when the normalised weights wn
+    are given), the fitDisp MLE, the noIncrease rule, the grid refit of the unconverged genes and the clamps.  sfd:
+    the size-factor vector or the nf rows of ynz; alpha0 / beta0: the prep kernel's start values; wdisp:
+    pmax(wn, 1e-6).  Returns (mu, the fitDisp result, dispGeneEst, number of grid refits)."""
+    dev = ynz.device
+    p = beta0.shape[0]
+    maxDisp = float(max(10, m))
+    contrast = torch.zeros(p, dtype=F64, device=dev)
+    contrast[0] = 1.0
+    lam = torch.full((p,), 1e-6 / LN2 ** 2, dtype=F64, device=dev)
+    min_log_alpha = float(np.log(minDisp / 10))
+    if mu_lin is not None:
+        mu = mu_lin
+    elif wn is not None:
+        # fitNbinomGLMs with the normalised weights, its defaults minmu = 0.5 and useOptim = TRUE (R/core.R:752-755
+        # passes neither), its unclamped mean nf exp(x beta) (R/fitNbinomGLMs.R:180; the optim rows' own, :383)
+        # bounded at minmu (:764)
+        fb0 = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=0.5, weights=wn,
+                         want_hat=False, want_mu=False)
+        ll0 = D.nb_loglik(ynz, xd, sfd, alpha0, fb0["beta_mat"], weights=wn,
+                          out_mu=_ws("mu_glm", tuple(ynz.shape), F64, dev))
+        _optim_fallback(ynz, xd, sfd, alpha0, fb0, beta0, lam, contrast, maxit, 0.5, ll0, useOptim=True, weights=wn)
+        mu = ll0["mu"].clamp_(min=minmu)
+    else:
+        nn0 = ynz.shape[0]
+        vec = lambda: torch.empty(nn0, dtype=F64, device=dev)
+        out0 = {"beta_mat": torch.empty((p, nn0), dtype=F64, device=dev),
+                "beta_var_mat": torch.empty((p, nn0), dtype=F64, device=dev), "iter": vec(), "contrast_num": vec(),
+                "contrast_denom": vec(), "deviance": vec(), "hat_diagonals": None,
+                "mu": _ws("mu_glm", tuple(ynz.shape), F64, dev)}
+        mu = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=minmu, out=out0)["mu"]
+    la0 = torch.log(alpha0)
+    mark("mu")
+    r = D.fit_disp(ynz, xd, mu, la0, la0, 1.0, min_log_alpha, kappa_0, dispTol, maxit, False, weights=wdisp,
+                   weightThreshold=weightThreshold)
+    mark("fit_disp_mle")
+    dge = torch.clamp(torch.exp(r["log_alpha"]), max=maxDisp)
+    noIncrease = r["last_lp"] < r["initial_lp"] + r["initial_lp"].abs() / 1e6
+    dge = torch.where(noIncrease, alpha0, dge)
+    conv = (r["iter"] < maxit) & (r["iter"] != 1)
+    gi, ga = _grid_refit(ynz, xd, mu, (~conv) & (dge > minDisp * 10), m, None, 1.0, False, wdisp, weightThreshold)
+    if ga is not None:
+        dge[gi] = ga
+    dge = torch.clamp(dge, minDisp, maxDisp)
+    return mu, r, dge, int(gi.numel())
+
+
+def _dispersion_trend(baseMean, dge, fitType, minDisp=1e-8):
+    """estimateDispersionsFit's fit (R/core.R:864-940) as a 4-vector (a, b, status, rounds) with dispFit = a + b /
+    baseMean: parametricDispersionFit on the device (trend_fit), or for fitType "mean" (mean_disp, 0, 0, 0), so that
+    every a + b / baseMean downstream (the MAP prior, the outlier refit) equals meanDisp."""
+    if fitType == "mean":
+        tr = torch.zeros(4, dtype=F64, device=dge.device)
+        tr[0] = mean_disp(dge, minDisp)
+        return tr
+    return trend_fit(baseMean, dge, minDisp)
+
+
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
                  outlierSD=2.0, minReplicatesForReplace=np.inf, allgather=None, useOptim=True, betaPrior=False,
                  factors=None, weights=None, weightThreshold=1e-2, normalizationFactors=None, avgTxLength=None,
@@ -838,52 +902,15 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     min_log_alpha = float(np.log(minDisp / 10))
 
     # ---- estimateDispersionsGeneEst (R/core.R:657-860)
-    if linearMu:
-        mu = pr["mu_lin"]
-    elif weights is not None:
-        # fitNbinomGLMs with the normalised weights, its defaults minmu = 0.5 and useOptim = TRUE (R/core.R:752-755
-        # passes neither), its unclamped mean nf exp(x beta) (R/fitNbinomGLMs.R:180; the optim rows' own, :383)
-        # bounded at minmu (:764)
-        fb0 = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=0.5, weights=wn,
-                         want_hat=False, want_mu=False)
-        ll0 = D.nb_loglik(ynz, xd, sfd, alpha0, fb0["beta_mat"], weights=wn,
-                          out_mu=_ws("mu_glm", tuple(ynz.shape), F64, dev))
-        _optim_fallback(ynz, xd, sfd, alpha0, fb0, beta0, lam, contrast, maxit, 0.5, ll0, useOptim=True, weights=wn)
-        mu = ll0["mu"].clamp_(min=minmu)
-    else:
-        nn0 = ynz.shape[0]
-        vec = lambda: torch.empty(nn0, dtype=F64, device=dev)
-        out0 = {"beta_mat": torch.empty((p, nn0), dtype=F64, device=dev),
-                "beta_var_mat": torch.empty((p, nn0), dtype=F64, device=dev), "iter": vec(), "contrast_num": vec(),
-                "contrast_denom": vec(), "deviance": vec(), "hat_diagonals": None,
-                "mu": _ws("mu_glm", tuple(ynz.shape), F64, dev)}
-        mu = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=minmu, out=out0)["mu"]
-    la0 = torch.log(alpha0)
-    mark("mu")
-    r = D.fit_disp(ynz, xd, mu, la0, la0, 1.0, min_log_alpha, kappa_0, dispTol, maxit, False, weights=wdisp,
-                   weightThreshold=weightThreshold)
-    mark("fit_disp_mle")
-    dge = torch.clamp(torch.exp(r["log_alpha"]), max=maxDisp)
-    noIncrease = r["last_lp"] < r["initial_lp"] + r["initial_lp"].abs() / 1e6
-    dge = torch.where(noIncrease, alpha0, dge)
-    conv = (r["iter"] < maxit) & (r["iter"] != 1)
-    gi, ga = _grid_refit(ynz, xd, mu, (~conv) & (dge > minDisp * 10), m, None, 1.0, False, wdisp, weightThreshold)
-    if ga is not None:
-        dge[gi] = ga
-    dge = torch.clamp(dge, minDisp, maxDisp)
-    n_refit_geneest = int(gi.numel())
+    mu, r, dge, n_refit_geneest = _gene_est(ynz, xd, sfd, alpha0, beta0, pr["mu_lin"] if linearMu else None, m,
+                                            minDisp, kappa_0, dispTol, maxit, betaTol, minmu, wn=wn, wdisp=wdisp,
+                                            weightThreshold=weightThreshold, mark=mark)
     mark("rules+grid_mle")
 
     # ---- estimateDispersionsFit + dispersionFunction<- + PriorVar (R/core.R:864-940, R/methods.R:142-190, R/core.R:1135-1208)
     # ONE packed collective for the two vectors the global step needs (sharded.PackedGather accepts a list)
     bm_all, dge_all = allgather([bm, dge]) if allgather is not None else (bm, dge)
-    if fitType == "mean":
-        # dispersionFunction(means) = meanDisp: (meanDisp, 0) in the trend's slots keeps every a + b / baseMean below
-        # (here, in the MAP prior and in the outlier refit) equal to meanDisp
-        tr = torch.zeros(4, dtype=F64, device=dev)
-        tr[0] = mean_disp(dge_all, minDisp)
-    else:
-        tr = trend_fit(bm_all, dge_all, minDisp)
+    tr = _dispersion_trend(bm_all, dge_all, fitType, minDisp)
     dispFit = tr[0] + tr[1] / bm
     above = dge_all >= minDisp * 100
     resid = (torch.log(dge_all) - torch.log(tr[0] + tr[1] / bm_all))[above]
@@ -1064,3 +1091,190 @@ def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, varLogDispEsts
             rc[:, replaceable] = 0.0
             res["maxCooks"] = (rc[:, forCooks].max(dim=1).values if bool(forCooks.any())
                                else torch.full_like(res["maxCooks"], float("nan")))
+
+
+# ---------------------------------------------------------------- transforms: vst(), varianceStabilizingTransformation(),
+# normTransform() (R/vst.R, R/helper.R:421-435)
+
+_TRANSFORM_MODE = {"parametric": 0, "mean": 1, "log2": 2}     # B200NB_TRANSFORM_* of include/b200nb.h
+
+
+def transform(y, m, mode, c0, c1, sfd):
+    """b200nb_transform_dev: a fresh contiguous (N, m) float64 device tensor of the transformed normalized counts
+    K / s_j (sfd: the (m,) size-factor device vector) or K / nf_ij (sfd: the gene-major (N, ld) nf matrix) of all N
+    rows of y.  mode "parametric" (c0 = asymptDisp, c1 = extraPois), "mean" (c0 = the mean dispersion) or "log2"
+    (c0 = the pseudocount).  Enqueue only."""
+    if y.dim() != 2 or y.dtype not in (torch.int32, F64) or not y.is_contiguous():
+        raise ValueError("y must be a contiguous gene-major int32 or float64 tensor")
+    L = _lib.lib()
+    n, ld = y.shape
+    out = torch.empty((n, m), dtype=F64, device=y.device)
+    sf, nf = (None, sfd) if sfd.dim() == 2 else (sfd, None)
+    _lib.check(L.b200nb_transform_dev(_p(y), 1 if y.dtype == F64 else 0, _p(sf), _p(nf), n, m, ld,
+                                      _TRANSFORM_MODE[mode], float(c0), float(c1), _p(out), m, _stream()),
+               "transform_dev")
+    return out
+
+
+def _vst_constants(dispersionFunction):
+    """(mode, c0, c1) of b200nb_transform_dev for a dispersion function given as DESeq_device returns it."""
+    fitType = dispersionFunction.get("fitType")
+    if fitType == "parametric":
+        a = dispersionFunction["trendCoefs"]
+        a = a.cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a, dtype=np.float64)
+        return "parametric", float(a[0]), float(a[1])
+    if fitType == "mean":
+        return "mean", float(dispersionFunction["meanDisp"]), 0.0
+    raise ValueError(f"fitType {fitType!r}: only 'parametric' and 'mean' dispersion functions have a variance "
+                     "stabilizing transformation here (there is no 'local' trend fit)")
+
+
+def _check_vst_fit_type(fitType):
+    if fitType not in ("parametric", "mean"):
+        raise ValueError(f"fitType must be 'parametric' or 'mean' (there is no 'local' trend fit), got {fitType!r}")
+
+
+def _factors(y, m, sizeFactors, normalizationFactors, avgTxLength=None):
+    """The normalization of R's transforms: normalizationFactors, or those estimated from avgTxLength (as DESeq_device
+    does), or sizeFactors (numpy or a device tensor), or, when none is given, the median-of-ratios size factors
+    (estimateSizeFactors).  Returns (size factors as numpy or None, nf matrix or None, the factors as sfd for
+    transform / the fits)."""
+    if avgTxLength is not None:
+        if normalizationFactors is not None:
+            raise ValueError("give normalizationFactors or avgTxLength, not both")
+        if sizeFactors is not None:
+            raise ValueError("avgTxLength estimates normalization factors: sizeFactors must be None")
+        normalizationFactors = normalization_factors(y, m, avgTxLength=avgTxLength)["normalizationFactors"]
+    if sizeFactors is None and normalizationFactors is None:
+        sizeFactors = size_factors(y, m)["sizeFactors"]
+    if sizeFactors is not None:
+        sizeFactors = (sizeFactors.cpu().numpy() if isinstance(sizeFactors, torch.Tensor)
+                       else np.asarray(sizeFactors, dtype=np.float64))
+        if sizeFactors.shape != (m,):
+            raise ValueError(f"sizeFactors must have one value per sample ({m}), got shape {sizeFactors.shape}")
+    sfd = _size_or_norm_factors(y, m, sizeFactors, normalizationFactors, None)
+    return sizeFactors, normalizationFactors, sfd
+
+
+def _vst_design(x, m, blind):
+    """~1 when blind, else the given design (m rows)."""
+    if blind:
+        return np.ones((m, 1))
+    x = np.asarray(x, dtype=np.float64)
+    if x.ndim != 2 or x.shape[0] != m:
+        raise ValueError(f"x must be a design matrix with one row per sample ({m}), got shape {x.shape}")
+    return x
+
+
+def _dispersion_function(ynz, x, sizeFactors, nfz, fitType, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100,
+                         betaTol=1e-8, minmu=0.5):
+    """estimateDispersionsGeneEst + estimateDispersionsFit with their defaults on the rows of ynz (none of them
+    all-zero; nfz: their nf rows, xim is taken over them): the pre-step kernel, _gene_est and _dispersion_trend, as in
+    DESeq_device.  Returns {"fitType", "trendCoefs" (device (2,)) or "meanDisp" (float)}.  A failed parametric fit
+    raises FloatingPointError (R would fall back to the local fit)."""
+    m, p = x.shape
+    linearMu = modelMatrixGroups(x) == p
+    pr = prep(ynz, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu, normalizationFactors=nfz)
+    _, _, dge, _ = _gene_est(ynz, pr["xd"], pr["sfd"], pr["alpha0"], pr["beta0"], pr["mu_lin"], m, minDisp, kappa_0,
+                             dispTol, maxit, betaTol, minmu)
+    tr = _dispersion_trend(pr["baseMean"], dge, fitType, minDisp)
+    if fitType == "mean":
+        return {"fitType": "mean", "meanDisp": float(tr[0].item())}
+    status = tr[2].item()
+    if status != 0:
+        raise FloatingPointError(f"parametric dispersion fit failed on device (status {int(status)})")
+    return {"fitType": "parametric", "trendCoefs": tr[:2].clone()}
+
+
+def _vst_result(y, m, fn, sizeFactors, nf, sfd):
+    mode, c0, c1 = _vst_constants(fn)
+    res = {"vst": transform(y, m, mode, c0, c1, sfd), "fitType": fn["fitType"]}
+    res.update({k: fn[k] for k in ("trendCoefs", "meanDisp") if k in fn})
+    if nf is not None:
+        res["normalizationFactors"] = nf
+    else:
+        res["sizeFactors"] = sizeFactors
+    return res
+
+
+def vst_transform(y, m, dispersionFunction, sizeFactors=None, normalizationFactors=None):
+    """getVarianceStabilizedData (R/vst.R:145-196) on the device: the VST of the normalized counts of all N rows of y
+    (gene-major (N, ld), int32 or float64) as a fresh contiguous (N, m) float64 device tensor; all-zero rows too.
+    dispersionFunction: a dict as DESeq_device or the VST functions return it, {"fitType": "parametric",
+    "trendCoefs": (asymptDisp, extraPois)} or {"fitType": "mean", "meanDisp": alpha}.  Applying the function of one
+    analysis to other samples (any m) is R's frozen VST (R/vst.R:69-76).  Exactly one of sizeFactors ((m,) numpy or
+    device tensor) and normalizationFactors (gene-major (N, ld) float64 device tensor) is needed.  Any other fitType
+    ("local") raises ValueError."""
+    mode, c0, c1 = _vst_constants(dispersionFunction)
+    if isinstance(sizeFactors, torch.Tensor):
+        sizeFactors = sizeFactors.cpu().numpy()
+    sfd = _size_or_norm_factors(y, m, sizeFactors, normalizationFactors, None)
+    return transform(y, m, mode, c0, c1, sfd)
+
+
+def varianceStabilizingTransformation_device(y, m, x=None, blind=True, fitType="parametric", sizeFactors=None,
+                                             normalizationFactors=None, avgTxLength=None, dispersionFunction=None):
+    """varianceStabilizingTransformation (R/vst.R:112-142) on the device, for y gene-major (N, ld) counts of m samples.
+    The size factors are estimated (median of ratios) when none of sizeFactors / normalizationFactors / avgTxLength is
+    given; avgTxLength estimates the nf as DESeq_device does.  With blind=True (the design is ~1) or without a
+    dispersionFunction, estimateDispersionsGeneEst + estimateDispersionsFit (fitType "parametric" or "mean") run on
+    the rows with a non-zero sum, with design x when blind=False; otherwise dispersionFunction is used as it is and
+    fitType is ignored, as in R.  Returns {"vst": (N, m) device tensor, "fitType", "trendCoefs" or "meanDisp",
+    "sizeFactors" or "normalizationFactors"}; the dispersion keys can be passed back as a frozen dispersionFunction.
+    blind=False without x or dispersionFunction raises ValueError; a failed parametric fit raises FloatingPointError."""
+    refit = blind or dispersionFunction is None
+    if refit:
+        if not blind and x is None:
+            raise ValueError("blind=False needs the design x or a dispersionFunction")
+        _check_vst_fit_type(fitType)
+        x = _vst_design(x, m, blind)
+    sizeFactors, nf, sfd = _factors(y, m, sizeFactors, normalizationFactors, avgTxLength)
+    if refit:
+        idx = torch.nonzero(y[:, :m].sum(dim=1) != 0).squeeze(1)
+        whole = idx.numel() == y.shape[0]
+        ynz = y if whole else y[idx].contiguous()
+        nfz = None if nf is None else (nf if whole else nf[idx].contiguous())
+        dispersionFunction = _dispersion_function(ynz, x, sizeFactors, nfz, fitType)
+    return _vst_result(y, m, dispersionFunction, sizeFactors, nf, sfd)
+
+
+def vst_device(y, m, x=None, blind=True, nsub=1000, fitType="parametric", sizeFactors=None,
+               normalizationFactors=None, avgTxLength=None):
+    """vst (R/vst.R:219-267) on the device: the dispersion function is fitted on nsub genes only, then the VST runs
+    over all N rows of y (gene-major (N, ld) counts of m samples).  Factors as in
+    varianceStabilizingTransformation_device.  The genes: baseMean (the pre-step kernel's row mean of the normalized
+    counts) > 5, in the order of a stable sort of baseMean, at the positions pipeline.vstSubsetPositions(L, nsub);
+    estimateDispersionsGeneEst + estimateDispersionsFit run on them in that order, with design ~1 when blind and x
+    otherwise (xim over the subset's nf rows).  R's two stops raise ValueError.  Returns the dict of
+    varianceStabilizingTransformation_device plus "subset": the nsub row indices into y, in fit order."""
+    from .pipeline import vstSubsetPositions
+    if y.shape[0] < nsub:
+        raise ValueError("less than 'nsub' rows, it is recommended to use varianceStabilizingTransformation directly")
+    if not blind and x is None:
+        raise ValueError("blind=False needs the design x")
+    _check_vst_fit_type(fitType)
+    x = _vst_design(x, m, blind)
+    sizeFactors, nf, sfd = _factors(y, m, sizeFactors, normalizationFactors, avgTxLength)
+    # rowMeans(counts(normalized = TRUE)) over all rows: the pre-step kernel's baseMean for x = 1 (xim is not used)
+    bm = prep(y, np.ones((m, 1)), sizeFactors, want_mu=False, want_beta0=False, normalizationFactors=nf,
+              xim=1.0)["baseMean"]
+    cand = torch.nonzero(bm > 5).squeeze(1)
+    L = cand.numel()
+    if L < nsub:
+        raise ValueError("less than 'nsub' rows with mean normalized count > 5, it is recommended to use "
+                         "varianceStabilizingTransformation directly")
+    _, o = torch.sort(bm[cand], stable=True)
+    subset = cand[o[torch.as_tensor(vstSubsetPositions(L, nsub), device=y.device)]]
+    ysub = y[subset].contiguous()
+    nfsub = None if nf is None else nf[subset].contiguous()
+    res = _vst_result(y, m, _dispersion_function(ysub, x, sizeFactors, nfsub, fitType), sizeFactors, nf, sfd)
+    res["subset"] = subset
+    return res
+
+
+def normTransform_device(y, m, sizeFactors=None, normalizationFactors=None, pc=1.0):
+    """normTransform(f = log2) (R/helper.R:421-435) on the device: log2(normalized counts + pc) of all N rows of y as a
+    fresh (N, m) float64 device tensor; the size factors are estimated (median of ratios) when neither sizeFactors
+    nor normalizationFactors is given."""
+    _, _, sfd = _factors(y, m, sizeFactors, normalizationFactors)
+    return transform(y, m, "log2", pc, 0.0, sfd)

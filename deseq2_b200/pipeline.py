@@ -23,6 +23,8 @@ numpy, one function per R function, same names, so the engine can be driven and 
   fitGLMsWithPrior / estimateBetaPriorVar / Hmisc.wtd.quantile / addAllContrasts / averagePriorsOverLevels /
   makeExpandedModelMatrix (additive factor designs)   R/fitNbinomGLMs.R:242-337, R/core.R:1601-1689, 2762-2803, R/expanded.R
   DESeq                          R/core.R:280-432    (test="Wald", fitType="parametric", betaPrior=FALSE or TRUE)
+  vst / varianceStabilizingTransformation / getVarianceStabilizedData / normTransform   R/vst.R, R/helper.R:421-435
+                                 (fitType "parametric" / "mean"; vst's gene subset is vstSubsetPositions)
   getAndCheckWeights             R/core.R:2697-2752  (observation weights: row-max normalisation, two rank tests per
                                  gene with a restatement of LINPACK dqrdc2, the rank routine of R's qr())
 
@@ -1165,3 +1167,108 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
         res["idx"] = np.flatnonzero(nz)
     res.update(extra)
     return res
+
+
+def vstSubsetPositions(L, nsub):
+    """The 0-based positions, into order(baseMean) of the L genes with baseMean > 5, of the nsub genes vst() fits its
+    dispersion function on (R/vst.R:244-247): round(seq(from = 1, to = L, length.out = nsub)).  seq.default gives
+    c(1, 1 + k ((L - 1) / (nsub - 1)) for k = 1 .. nsub - 2, L) (c(1, L) for nsub = 2, 1 for nsub = 1), and round()
+    rounds half to even (L = 4, nsub = 3: 1, 2.5, 4 -> 1, 2, 4).  The one statement of this rule: the host mirror and
+    the device path both use it."""
+    L, nsub = int(L), int(nsub)
+    if not 1 <= nsub <= L:
+        raise ValueError(f"nsub={nsub} must lie in [1, {L}]")
+    if nsub == 1:
+        pos = np.array([1.0])
+    elif nsub == 2:
+        pos = np.array([1.0, float(L)])
+    else:
+        pos = np.r_[1.0, 1.0 + np.arange(1, nsub - 1) * ((L - 1.0) / (nsub - 1.0)), float(L)]
+    return np.round(pos).astype(np.int64) - 1
+
+
+def getVarianceStabilizedData(counts, sizeFactors, dispersionFunction):
+    """R/vst.R:145-196 for fitType "parametric" ({"fitType", "trendCoefs": (asymptDisp, extraPois)}) and "mean"
+    ({"fitType", "meanDisp"}), in R's operand order, on counts / sizeFactors (an (m,) vector or an (n, m) nf
+    matrix).  "local" has no trend fit here: ValueError."""
+    q = np.asarray(counts, dtype=np.float64) / _div(sizeFactors)
+    fitType = dispersionFunction.get("fitType")
+    if fitType == "parametric":
+        a0, a1 = (float(v) for v in np.asarray(dispersionFunction["trendCoefs"], dtype=np.float64)[:2])
+        return np.log((1 + a1 + 2 * a0 * q + 2 * np.sqrt(a0 * q * (1 + a1 + a0 * q))) / (4 * a0)) / np.log(2)
+    if fitType == "mean":
+        alpha = float(dispersionFunction["meanDisp"])
+        return (2 * np.arcsinh(np.sqrt(alpha * q)) - np.log(alpha) - np.log(4)) / np.log(2)
+    raise ValueError(f"fitType {fitType!r}: only 'parametric' and 'mean' dispersion functions are supported")
+
+
+def _fitDispersionFunction(counts, sizeFactors, x, fitType, engine):
+    """estimateDispersionsGeneEst + estimateDispersionsFit (quiet, defaults) on rows none of which is all zero."""
+    ge = estimateDispersionsGeneEst(counts, sizeFactors, x, engine=engine)
+    tf = estimateDispersionsFit(ge["dispGeneEst"], ge["baseMean"], fitType=fitType)
+    if fitType == "mean":
+        return {"fitType": "mean", "meanDisp": float(tf["meanDisp"])}
+    return {"fitType": "parametric", "trendCoefs": tf["coefs"]}
+
+
+def _vstDesign(x, m, blind):
+    if blind:
+        return np.ones((m, 1))
+    if x is None:
+        raise ValueError("blind=False needs the design x or a dispersionFunction")
+    x = np.asarray(x, dtype=np.float64)
+    if x.ndim != 2 or x.shape[0] != m:
+        raise ValueError(f"x must be a design matrix with one row per sample ({m}), got shape {x.shape}")
+    return x
+
+
+def _vstResult(counts, sizeFactors, fn):
+    return dict(fn, vst=getVarianceStabilizedData(counts, sizeFactors, fn), sizeFactors=sizeFactors)
+
+
+def varianceStabilizingTransformation(counts, x=None, blind=True, fitType="parametric", sizeFactors=None,
+                                      dispersionFunction=None, engine=None):
+    """R/vst.R:112-142.  sizeFactors: (m,) or an (n, m) nf matrix; estimated (ratio) when None.  The dispersion
+    function is fitted on the non-all-zero rows (design ~1 when blind, x otherwise) unless blind=False and
+    dispersionFunction is given.  Returns {"vst", the dispersion keys, "sizeFactors"}."""
+    counts = np.asarray(counts)
+    m = counts.shape[1]
+    if sizeFactors is None:
+        sizeFactors = estimateSizeFactorsForMatrix(counts)
+    if blind or dispersionFunction is None:
+        x = _vstDesign(x, m, blind)
+        nz = counts.sum(axis=1) > 0
+        sf = np.asarray(sizeFactors, dtype=np.float64)
+        dispersionFunction = _fitDispersionFunction(counts[nz], sf[nz] if sf.ndim == 2 else sf, x, fitType, engine)
+    return _vstResult(counts, sizeFactors, dispersionFunction)
+
+
+def vst(counts, x=None, blind=True, nsub=1000, fitType="parametric", sizeFactors=None, engine=None):
+    """R/vst.R:219-267: the dispersion function fitted on nsub genes with baseMean > 5 (vstSubsetPositions of a stable
+    ordering of baseMean, in that row order), then the VST of all rows.  Returns varianceStabilizingTransformation's
+    dict plus "subset" (the row indices, in fit order)."""
+    counts = np.asarray(counts)
+    n, m = counts.shape
+    if n < nsub:
+        raise ValueError("less than 'nsub' rows, it is recommended to use varianceStabilizingTransformation directly")
+    if sizeFactors is None:
+        sizeFactors = estimateSizeFactorsForMatrix(counts)
+    sf = np.asarray(sizeFactors, dtype=np.float64)
+    baseMean = (counts / _div(sf)).mean(axis=1)
+    keep = np.flatnonzero(baseMean > 5)
+    if len(keep) < nsub:
+        raise ValueError("less than 'nsub' rows with mean normalized count > 5, it is recommended to use "
+                         "varianceStabilizingTransformation directly")
+    o = np.argsort(baseMean[keep], kind="stable")
+    subset = keep[o[vstSubsetPositions(len(keep), nsub)]]
+    fn = _fitDispersionFunction(counts[subset], sf[subset] if sf.ndim == 2 else sf, _vstDesign(x, m, blind),
+                                fitType, engine)
+    return dict(_vstResult(counts, sizeFactors, fn), subset=subset)
+
+
+def normTransform(counts, sizeFactors=None, pc=1.0):
+    """R/helper.R:421-435 with f = log2: log2(counts / sizeFactors + pc); sizeFactors (m,) or (n, m), estimated
+    (ratio) when None."""
+    if sizeFactors is None:
+        sizeFactors = estimateSizeFactorsForMatrix(counts)
+    return np.log2(np.asarray(counts, dtype=np.float64) / _div(sizeFactors) + pc)

@@ -38,6 +38,9 @@ extern "C" {
 #define B200NB_MAX_P 32
 #define B200NB_Y_INT32 0
 #define B200NB_Y_F64 1
+#define B200NB_TRANSFORM_VST_PARAMETRIC 0
+#define B200NB_TRANSFORM_VST_MEAN 1
+#define B200NB_TRANSFORM_LOG2 2
 
 /* ---- fitDisp: src/DESeq2.cpp:164.  Outputs = list members at :268-276 (length n each). */
 int b200nb_fit_disp(const void* y, int y_type, const double* x, const double* mu_hat, const double* log_alpha,
@@ -214,6 +217,21 @@ int b200nb_beta_prior_quantile_dev(const double* beta_log2, int n, int p, const 
 int b200nb_sf_iterate_objective_dev(const void* y, int y_type, const double* q, const double* alpha,
                                     const double* par, double h, double Q, int n, int m, long long ld,
                                     int max_tile_cols, double* out, void* stream);
+
+/* b200nb_transform_dev: a transform of the normalized counts q = K / s_j (size_factors[m]) or K / nf_ij (nf, gene-major
+ * n x ld): exactly one of the two is non-NULL.  y: counts, gene-major (n x ld, int32 or f64); out: gene-major n x ld_out
+ * float64, columns >= m untouched.  mode and its constants c0, c1:
+ *   B200NB_TRANSFORM_VST_PARAMETRIC  getVarianceStabilizedData for fitType "parametric" (R/vst.R:153-155),
+ *     c0 = asymptDisp, c1 = extraPois (both finite and > 0):
+ *     log((1 + c1 + 2 c0 q + 2 sqrt(c0 q (1 + c1 + c0 q))) / (4 c0)) / log(2)
+ *   B200NB_TRANSFORM_VST_MEAN  fitType "mean" (R/vst.R:185-189), c0 = alpha (finite and > 0), c1 unused:
+ *     (2 asinh(sqrt(c0 q)) - log(c0) - log(4)) / log(2)
+ *   B200NB_TRANSFORM_LOG2  normTransform(f = log2, pc = c0) (R/helper.R:421-435), c0 finite and >= 0, c1 unused:
+ *     log2(q + c0)
+ * q is an IEEE division and the formulas are evaluated in R's operand order without contraction.  Needs n, m >= 0,
+ * ld >= m, ld_out >= m and no NULL pointer.  Enqueue only. */
+int b200nb_transform_dev(const void* y, int y_type, const double* size_factors, const double* nf, int n, int m,
+                         long long ld, int mode, double c0, double c1, double* out, long long ld_out, void* stream);
 
 /* ---- housekeeping */
 const char* b200nb_last_error(void);
