@@ -58,6 +58,8 @@ SIGNATURES = {
     "b200nb_beta_prior_quantile_dev": [vp, _I, _I, vp, vp, vp, vp, _I, _D, vp, vp],
     "b200nb_sf_iterate_objective_dev": [vp, _I, vp, vp, vp, _D, _D, _I, _I, _LL, _I, vp, vp],
     "b200nb_transform_dev": [vp, _I, vp, vp, _I, _I, _LL, _I, _D, _D, vp, _LL, vp],
+    "b200nb_rlog_fit_dev": [vp, _I, vp, vp, vp, vp, _I, _I, _LL, _D, _D, _I, _D, vp, _LL, vp, vp, vp],
+    "b200nb_rlog_prior_var_dev": [vp, _I, vp, vp, vp, vp, _I, _I, _LL, vp, vp],
     "b200nb_last_error": [],
     "b200nb_device_count": [],
     "b200nb_kernel_launches": [],

@@ -28,6 +28,61 @@ namespace {
 constexpr int kBpThreads = 128;
 constexpr int kBpDigits = 16;                                  // 4-bit digits, 16 passes over 64 bits
 
+// ---- the steps of the refinement, shared with rlog's prior variance (rlog.cuh), which runs them over many CTAs
+// Hmisc's order statistics for N kept entries: frac and the cumulative-weight targets of x_(low) and x_(high), in the
+// host restatement's arithmetic, unfused (nvcc would contract these into FMAs)
+__device__ __forceinline__ void bp_targets(double dN, double prob, double& frac, double& t_low, double& t_high) {
+  const double order = __dadd_rn(1.0, __dmul_rn(dN - 1.0, prob));
+  const double low = fmax(floor(order), 1.0);
+  const double high = fmin(low + 1.0, dN);
+  frac = order - floor(order);
+  t_low = __dadd_rn(low, -__dmul_rn(1e-12, fmax(1.0, low)));
+  t_high = __dadd_rn(high, -__dmul_rn(1e-12, fmax(1.0, high)));
+}
+
+// one entry into the calling thread's histogram column hl (row stride kBpThreads): digit `shift` of its bit pattern,
+// for each target whose prefix it shares
+__device__ __forceinline__ void bp_hist_add(double* hl, unsigned long long bits, double wn, int shift,
+                                            unsigned long long mask, unsigned long long p0, unsigned long long p1,
+                                            int& md0, int& md1) {
+  const int d = (int)(bits >> shift) & (kBpDigits - 1);
+  const unsigned long long hi = bits & mask;
+  if (hi == p0) { hl[d * kBpThreads] += wn; md0 = max(md0, d); }
+  if (hi == p1) { hl[(kBpDigits + d) * kBpThreads] += wn; md1 = max(md1, d); }
+}
+
+// bucket totals of the 2 x kBpDigits x kBpThreads histogram: warp w sums the rows w, w + 4, ...; each lane 4
+// consecutive columns, then a fixed tree
+__device__ __forceinline__ void bp_bucket_totals(const double* s_hist, double (*bucket)[kBpDigits], int warp,
+                                                 int lane) {
+  for (int row = warp; row < 2 * kBpDigits; row += kBpThreads / 32) {
+    const double* col = s_hist + row * kBpThreads + lane * (kBpThreads / 32);
+    double v = 0.0;
+    for (int k = 0; k < kBpThreads / 32; k++) v += col[k];
+    v = warp_allreduce_sum(v);
+    if (lane == 0) bucket[row / kBpDigits][row % kBpDigits] = v;
+  }
+}
+
+// the digit of one target: the first whose cumulative weight reaches it; none (rounding, or the target lies beyond the
+// total weight: rule = 2) -> the largest digit present under the prefix (maxd).  Advances below and prefix.
+__device__ __forceinline__ void bp_pick_digit(const double* bucket, const int& maxd, double target, int shift,
+                                              double& below, unsigned long long& prefix) {
+  double b = below;
+  int pick = -1;
+  for (int d = 0; d < kBpDigits; d++) {
+    if (b + bucket[d] >= target) { pick = d; break; }
+    b += bucket[d];
+  }
+  if (pick < 0) {
+    pick = max(maxd, 0);
+    b = below;
+    for (int d = 0; d < pick; d++) b += bucket[d];
+  }
+  below = b;
+  prefix |= (unsigned long long)pick << shift;
+}
+
 // one entry of column (a, b): its |x| bit pattern and weight; false if the entry does not take part
 __device__ __forceinline__ bool bp_entry(const BetaPriorQArgs& A, int a, int b, int i, unsigned long long& bits,
                                          double& w) {
@@ -70,13 +125,8 @@ __global__ void __launch_bounds__(kBpThreads) beta_prior_quantile_kernel(const B
   double S = 0.0;
   for (int k = 0; k < kBpThreads / 32; k++) S += s_red[k];
   const double dN = (double)N;
-  // the host restatement's arithmetic, unfused (nvcc would contract these into FMAs)
-  const double order = __dadd_rn(1.0, __dmul_rn(dN - 1.0, A.prob));
-  const double low = fmax(floor(order), 1.0);
-  const double high = fmin(low + 1.0, dN);
-  const double frac = order - floor(order);
-  const double t_low = __dadd_rn(low, -__dmul_rn(1e-12, fmax(1.0, low)));
-  const double t_high = __dadd_rn(high, -__dmul_rn(1e-12, fmax(1.0, high)));
+  double frac, t_low, t_high;
+  bp_targets(dN, A.prob, frac, t_low, t_high);
 
   // ---- 16 refinement passes, both order statistics at once
   double* hl = s_hist + tid;
@@ -90,42 +140,14 @@ __global__ void __launch_bounds__(kBpThreads) beta_prior_quantile_kernel(const B
     int md0 = -1, md1 = -1;
     for (int i = tid; i < A.n; i += kBpThreads) {
       if (!bp_entry(A, a, b, i, bits, w)) continue;
-      const double wn = (w * dN) / S;                           // normwt, as w * length(x) / sum(w)
-      const int d = (int)(bits >> shift) & (kBpDigits - 1);
-      const unsigned long long hi = bits & mask;
-      if (hi == p0) { hl[d * kBpThreads] += wn; md0 = max(md0, d); }
-      if (hi == p1) { hl[(kBpDigits + d) * kBpThreads] += wn; md1 = max(md1, d); }
+      bp_hist_add(hl, bits, (w * dN) / S, shift, mask, p0, p1, md0, md1);   // normwt, as w * length(x) / sum(w)
     }
     if (md0 >= 0) atomicMax(&s_maxd[0], md0);
     if (md1 >= 0) atomicMax(&s_maxd[1], md1);
     __syncthreads();
-    // bucket totals: warp w sums the histogram rows w, w + 4, ...; each lane 4 consecutive columns, then a fixed tree
-    for (int row = warp; row < 2 * kBpDigits; row += kBpThreads / 32) {
-      const double* col = s_hist + row * kBpThreads + lane * (kBpThreads / 32);
-      double v = 0.0;
-      for (int k = 0; k < kBpThreads / 32; k++) v += col[k];
-      v = warp_allreduce_sum(v);
-      if (lane == 0) s_bucket[row / kBpDigits][row % kBpDigits] = v;
-    }
+    bp_bucket_totals(s_hist, s_bucket, warp, lane);
     __syncthreads();
-    if (tid < 2) {
-      // first digit whose cumulative weight reaches the target; none (rounding, or the target lies beyond the total
-      // weight: rule = 2) -> the largest digit present under the prefix
-      const double target = tid ? t_high : t_low;
-      double below = s_below[tid];
-      int pick = -1;
-      for (int d = 0; d < kBpDigits; d++) {
-        if (below + s_bucket[tid][d] >= target) { pick = d; break; }
-        below += s_bucket[tid][d];
-      }
-      if (pick < 0) {
-        pick = max(s_maxd[tid], 0);
-        below = s_below[tid];
-        for (int d = 0; d < pick; d++) below += s_bucket[tid][d];
-      }
-      s_below[tid] = below;
-      s_prefix[tid] |= (unsigned long long)pick << shift;
-    }
+    if (tid < 2) bp_pick_digit(s_bucket[tid], s_maxd[tid], tid ? t_high : t_low, shift, s_below[tid], s_prefix[tid]);
     __syncthreads();
   }
   if (tid == 0) {

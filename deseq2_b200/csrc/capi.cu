@@ -47,7 +47,7 @@ std::mutex g_arena_mu;   // guards the (re)allocation of the shared device arena
 // ---------------------------------------------------------------- device workspace of the host entry points
 // grow-only slots (one set per process; calls are serialised)
 enum Slot {
-  S_RAW, S_SMALL_IN, S_SMALL_OUT, S_NF, S_H, S_MUO, S_HC, S_SFI, S_NSLOTS
+  S_RAW, S_SMALL_IN, S_SMALL_OUT, S_NF, S_H, S_MUO, S_HC, S_SFI, S_RLOG, S_NSLOTS
 };
 constexpr int kMaxChunks = 8;
 struct Workspace {
@@ -1494,6 +1494,71 @@ int b200nb_transform_dev(const void* y, int y_type, const double* size_factors, 
   a.n = n; a.m = m; a.ld = ld; a.ld_out = ld_out; a.out = out;
   CU(nb::launch_transform(a, (cudaStream_t)stream));
   g_launches++;
+  return 0;
+}
+
+// qnorm(1 - 0.05 / 2): the normal quantile rlog's weighted upper quantile is matched to (R/core.R:2416-2419)
+constexpr double kRlogSdScale = 1.959963984540054;
+
+static int rlog_common_checks(const char* what, const void* y, int y_type, const double* size_factors,
+                              const double* nf, int m, long long ld) {
+  if (ld < m) return fail("%s: ld=%lld must be >= m=%d", what, ld, m);
+  if ((size_factors == nullptr) == (nf == nullptr)) return fail("%s: give exactly one of size_factors and nf", what);
+  if (!y) return fail("%s: null pointer argument", what);
+  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
+  return 0;
+}
+
+int b200nb_rlog_fit_dev(const void* y, int y_type, const double* size_factors, const double* nf,
+                        const double* intercept, const double* disp_fit, int n, int m, long long ld,
+                        double beta_prior_var, double tol, int maxit, double minmu, double* out, long long ld_out,
+                        double* out_intercept, double* out_iter, void* stream) {
+  if (n < 0 || m < 1) return fail("rlog_fit: bad dimensions n=%d m=%d (n >= 0, m >= 1)", n, m);
+  if (ld_out < m) return fail("rlog_fit: ld_out=%lld must be >= m=%d", ld_out, m);
+  if (rlog_common_checks("rlog_fit", y, y_type, size_factors, nf, m, ld)) return 1;
+  const auto finite_pos = [](double v) { return v > 0.0 && v < HUGE_VAL; };
+  if (!finite_pos(beta_prior_var)) return fail("rlog_fit: betaPriorVar=%g must be finite and > 0", beta_prior_var);
+  if (!finite_pos(tol)) return fail("rlog_fit: tol=%g must be finite and > 0", tol);
+  if (!finite_pos(minmu)) return fail("rlog_fit: minmu=%g must be finite and > 0", minmu);
+  if (maxit < 1) return fail("rlog_fit: maxit=%d must be >= 1", maxit);
+  if (!disp_fit || !out || !out_iter || (!intercept && !out_intercept))
+    return fail("rlog_fit: null pointer argument");
+  if (n == 0) return 0;
+  if (check_device()) return 1;
+  const double ln2 = log(2.0);
+  nb::RlogFitArgs a{};
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.size_factors = size_factors; a.nf = nf; a.intercept = intercept;
+  a.disp_fit = disp_fit;
+  // fitNbinomGLMs' lambda / log(2)^2 (R/fitNbinomGLMs.R:160) of rlogData's lambda = 1 / betaPriorVar, 1e-6 (:243-247)
+  a.lambda = (1.0 / beta_prior_var) / (ln2 * ln2);
+  a.lambda0 = 1e-6 / (ln2 * ln2);
+  a.tol = tol; a.maxit = maxit; a.minmu = minmu; a.log_minmu = log(minmu); a.ln2 = ln2;
+  a.n = n; a.m = m; a.ld = ld; a.ld_out = ld_out; a.out = out; a.out_intercept = intercept ? nullptr : out_intercept;
+  a.iter = out_iter;
+  CU(nb::launch_rlog_fit(a, (cudaStream_t)stream));
+  g_launches++;
+  return 0;
+}
+
+// The per-CTA partials of b200nb_rlog_prior_var_dev: the grow-only workspace slot S_RLOG (taken under g_call_mu, as
+// S_SFI; a few hundred KB)
+int b200nb_rlog_prior_var_dev(const void* y, int y_type, const double* size_factors, const double* nf,
+                              const double* base_mean, const double* disp_fit, int n, int m, long long ld,
+                              double* out_var, void* stream) {
+  if (n < 1 || m < 1) return fail("rlog_prior_var: bad dimensions n=%d m=%d (both must be >= 1)", n, m);
+  if (rlog_common_checks("rlog_prior_var", y, y_type, size_factors, nf, m, ld)) return 1;
+  if (!base_mean || !disp_fit || !out_var) return fail("rlog_prior_var: null pointer argument");
+  if (check_device()) return 1;
+  std::lock_guard<std::mutex> lk(g_call_mu);
+  void* ws = nullptr;
+  if (ws_get(S_RLOG, nb::rlog_prior_scratch_bytes(n, m), &ws)) return 1;
+  nb::RlogPriorArgs a{};
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.size_factors = size_factors; a.nf = nf; a.base_mean = base_mean;
+  a.disp_fit = disp_fit; a.n = n; a.m = m; a.ld = ld; a.prob = 0.95; a.sd_scale = kRlogSdScale;
+  a.st = static_cast<nb::RlogPriorState*>(ws);
+  a.out_var = out_var;
+  CU(nb::launch_rlog_prior_var(a, (cudaStream_t)stream));
+  g_launches += 2 * (1 + 16);
   return 0;
 }
 

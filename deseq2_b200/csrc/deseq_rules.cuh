@@ -133,8 +133,10 @@ struct IrlsProgress {
   __device__ __forceinline__ void start_iteration() { it += 1.0; }
   __device__ __forceinline__ void diverged(int maxit) { it = (double)maxit; }
 
-  // dv + devc: the log-likelihood sum of the pass (mu-dependent and mu-independent parts)
-  __device__ __forceinline__ bool stop_after_pass(double dv, double devc, const BetaArgs& A) {
+  // dv + devc: the log-likelihood sum of the pass (mu-dependent and mu-independent parts); Args: BetaArgs, or any
+  // argument block with the same tol and maxit (RlogFitArgs)
+  template <class Args>
+  __device__ __forceinline__ bool stop_after_pass(double dv, double devc, const Args& A) {
     dev = -2.0 * (dv + devc);
     const double conv_test = fabs(dev - dev_old) / (fabs(dev) + 0.1);
     if (isnan(conv_test)) {

@@ -256,6 +256,51 @@ struct TransformArgs {
 };
 cudaError_t launch_transform(const TransformArgs& a, cudaStream_t stream);
 
+// rlog (rlog.cuh, launched from size_factors.cu): the IRLS fit of rlogData's design [1 | I_m] (or I_m with a frozen
+// intercept) and the prior variance of its sample coefficients
+struct RlogFitArgs {
+  const void* y;
+  int y_is_f64;
+  const double* size_factors;  // m, or nullptr when nf is given
+  const double* nf;            // gene-major n x ld normalization factors, or nullptr
+  const double* intercept;     // n frozen log2 intercepts, or nullptr (fit [1 | I_m])
+  const double* disp_fit;      // n
+  double lambda, lambda0;      // natural-log-scale ridge of the sample columns and of the intercept
+  double tol, minmu, log_minmu, ln2;
+  int maxit;
+  int n, m;
+  long long ld, ld_out;
+  double* out;                 // gene-major n x ld_out: the rlog values (the sample coefficients while fitting)
+  double* out_intercept;       // n fitted log2 intercepts, or nullptr (not written with a frozen intercept)
+  double* iter;                // n
+};
+cudaError_t launch_rlog_fit(const RlogFitArgs& a, cudaStream_t stream);
+
+// Per-CTA partials and running state of the multi-CTA weighted quantile (rlog.cuh)
+struct RlogPriorState {
+  unsigned long long prefix[2];
+  double below[2];
+  double dN, S, frac, t_low, t_high;
+};
+struct RlogPriorArgs {
+  const void* y;
+  int y_is_f64;
+  const double* size_factors;  // m, or nullptr when nf is given
+  const double* nf;            // gene-major n x ld, or nullptr
+  const double* base_mean;     // n
+  const double* disp_fit;      // n
+  int n, m;
+  long long ld;
+  double prob, sd_scale;       // quantile probability; the normal quantile the upper quantile is matched to
+  RlogPriorState* st;          // rlog_prior_scratch_bytes(n, m) of device scratch (the state, then per-CTA partials)
+  double* out_var;             // 1
+  // set by the launcher: the histogram grid (fixed by n and m, so the partials are summed in the same order)
+  int ctas, rows_per_block;
+  double* part;
+};
+cudaError_t launch_rlog_prior_var(const RlogPriorArgs& a, cudaStream_t stream);
+size_t rlog_prior_scratch_bytes(int n, int m);
+
 // Cook's distances (pipeline_kernels.cu)
 struct CooksArgs {
   const void* y;

@@ -15,7 +15,8 @@
 // (beta_prior_quantile_kernel, beta_prior.cuh) and the trimmed sums of estimateSizeFactorsIterate's objective
 // (iterate_trim_sum_kernel, sf_iterate.cuh, whose per-gene kernel starts the same way); all start through
 // launch_per_column, as does the transform of the normalized counts (transform_kernel, transform.cuh: VST and
-// normTransform), one CTA per block of rows.
+// normTransform), one CTA per block of rows, and rlog's fit and prior variance (rlog.cuh: one CTA per block of genes;
+// a fixed grid of histogram CTAs and one picking CTA per refinement pass).
 #include "engine.h"
 #include "beta_prior.cuh"
 #include "nbmath.cuh"
@@ -165,6 +166,7 @@ __global__ void __launch_bounds__(512) sf_median_kernel(const double* __restrict
 
 #include "sf_iterate.cuh"
 #include "transform.cuh"
+#include "rlog.cuh"
 
 namespace nb {
 namespace {
@@ -214,6 +216,33 @@ cudaError_t launch_transform(const TransformArgs& a, cudaStream_t stream) {
   const int rows = transform_rows_per_cta(a.m);
   return launch_per_column(transform_kernel_for(a), (int)(((long long)a.n + rows - 1) / rows), kTfThreads, stream, a,
                            rows);
+}
+
+cudaError_t launch_rlog_fit(const RlogFitArgs& a, cudaStream_t stream) {
+  if (a.n == 0 || a.m == 0) return cudaSuccess;
+  const int genes = rlog_genes_per_cta(a.m);
+  return launch_per_column(rlog_fit_kernel_for(a), (int)(((long long)a.n + genes - 1) / genes), kRlThreads, stream, a);
+}
+
+size_t rlog_prior_scratch_bytes(int n, int m) {
+  int rows = 0, ctas = 0;
+  rlog_prior_grid(n, m, rows, ctas);
+  return sizeof(RlogPriorState) + (size_t)ctas * kRpPart * sizeof(double);
+}
+
+// the scratch (rlog_prior_scratch_bytes) starts at a.st; the partials follow the state
+cudaError_t launch_rlog_prior_var(const RlogPriorArgs& a, cudaStream_t stream) {
+  RlogPriorArgs b = a;
+  rlog_prior_grid(a.n, a.m, b.rows_per_block, b.ctas);
+  b.part = reinterpret_cast<double*>(b.st + 1);
+  const auto hist = rlog_prior_hist_for(b);
+  for (int pass = -1; pass < kBpDigits; pass++) {
+    cudaError_t e = launch_per_column(hist, b.ctas, kBpThreads, stream, b, pass);
+    if (e != cudaSuccess) return e;
+    e = launch_per_column(rlog_prior_pick_kernel, 1, kBpThreads, stream, b, pass);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 }  // namespace nb

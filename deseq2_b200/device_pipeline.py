@@ -31,6 +31,8 @@ gene-wise estimates (mean_disp).
 vst_device, varianceStabilizingTransformation_device, vst_transform and normTransform_device (R/vst.R,
 R/helper.R:421-435) fit the dispersion function with DESeq_device's GeneEst block and trend, and transform the n x m
 matrix with one kernel (b200nb_transform_dev, csrc/transform.cuh).
+rlog_device (R/rlog.R) fits the dispersion function the same way, then runs rlogData's prior variance
+(b200nb_rlog_prior_var_dev) and its per-gene fit of the design [1 | I_m] (b200nb_rlog_fit_dev, csrc/rlog.cuh).
 """
 from __future__ import annotations
 
@@ -1278,3 +1280,149 @@ def normTransform_device(y, m, sizeFactors=None, normalizationFactors=None, pc=1
     nor normalizationFactors is given."""
     _, _, sfd = _factors(y, m, sizeFactors, normalizationFactors)
     return transform(y, m, "log2", pc, 0.0, sfd)
+
+
+# ---------------------------------------------------------------- rlog() (R/rlog.R)
+
+def rlog_prior_var(y, m, sfd, baseMean, dispFit):
+    """b200nb_rlog_prior_var_dev: rlogData's betaPriorVar (R/rlog.R:233-240) over every entry of the N rows of y
+    (gene-major (N, ld) int32 or float64): the weighted 95 % quantile of |log2(K / s + 0.5) - log2(baseMean + 0.5)| with
+    weights 1 / (1 / baseMean + dispFit), matched to a normal.  sfd: the (m,) size-factor device vector or a gene-major
+    (N, ld) nf matrix; baseMean, dispFit: (N,) device tensors.  Rows whose weight is NaN or 0 (all-zero rows) do not
+    take part.  Returns a 0-d device tensor (NaN when no entry takes part).  Enqueue only."""
+    L = _lib.lib()
+    n, ld = y.shape
+    out = torch.empty(1, dtype=F64, device=y.device)
+    sf, nf = (None, sfd) if sfd.dim() == 2 else (sfd, None)
+    _lib.check(L.b200nb_rlog_prior_var_dev(_p(y), 1 if y.dtype == F64 else 0, _p(sf), _p(nf), _p(baseMean),
+                                           _p(dispFit), n, m, ld, _p(out), _stream()), "rlog_prior_var_dev")
+    return out[0]
+
+
+def rlog_fit(y, m, sfd, dispFit, betaPriorVar, intercept=None, betaTol=1e-4, maxit=100, minmu=0.5):
+    """b200nb_rlog_fit_dev: rlogData's fitNbinomGLMs call (R/rlog.R:249-253) for all N rows of y (gene-major (N, ld)
+    int32 or float64): the design [1 | I_m], or I_m on nf 2^intercept when `intercept` ((N,) float64 device tensor of
+    log2 intercepts) is given.  sfd as for rlog_prior_var; dispFit: (N,) device tensor.  Returns {"rlog": fresh (N, m)
+    device tensor on the log2 scale, "intercept": (N,) fitted log2 intercepts (-Inf for all-zero rows; None with a
+    frozen intercept), "betaIter": (N,)}.  Rows R leaves out (all-zero; a non-finite frozen intercept) are 0 with
+    betaIter 0.  Enqueue only."""
+    if y.dim() != 2 or y.dtype not in (torch.int32, F64) or not y.is_contiguous():
+        raise ValueError("y must be a contiguous gene-major int32 or float64 tensor")
+    L = _lib.lib()
+    n, ld = y.shape
+    dev = y.device
+    out = torch.empty((n, m), dtype=F64, device=dev)
+    icpt = None if intercept is not None else torch.empty(n, dtype=F64, device=dev)
+    it = torch.empty(n, dtype=F64, device=dev)
+    sf, nf = (None, sfd) if sfd.dim() == 2 else (sfd, None)
+    _lib.check(L.b200nb_rlog_fit_dev(_p(y), 1 if y.dtype == F64 else 0, _p(sf), _p(nf), _p(intercept), _p(dispFit),
+                                     n, m, ld, float(betaPriorVar), float(betaTol), int(maxit), float(minmu), _p(out),
+                                     m, _p(icpt), _p(it), _stream()), "rlog_fit_dev")
+    return {"rlog": out, "intercept": icpt, "betaIter": it}
+
+
+def _sparse_test(q, rs, p=0.9, t1=100, t2=0.1):
+    """sparseTest (R/rlog.R:274-287) on the normalized counts q (N, m) with row sums rs: warns when, among the rows
+    whose sum exceeds t1, more than a fraction t2 have one sample holding more than p of the row sum."""
+    import warnings
+    rmx = q.amax(dim=1)
+    sel = rs > t1
+    if not bool(sel.any()):
+        return
+    total = float(((rmx[sel] / rs[sel]) > p).to(F64).mean().item())
+    if total > t2:
+        warnings.warn("the rlog assumes that data is close to a negative binomial distribution, an assumption which is "
+                      "sometimes not compatible with datasets where many genes have many zero counts despite a few "
+                      f"very large counts.  In this data, for {round(total, 3) * 100}% of genes with a sum of "
+                      f"normalized counts above {t1}, it was the case that a single sample's normalized count made up "
+                      f"more than {p * 100}% of the sum over all samples.  The threshold for this warning is "
+                      f"{t2 * 100}% of genes.  We recommend instead using the varianceStabilizingTransformation or "
+                      "shifted log.", stacklevel=3)
+
+
+def _row_vector(v, n, dev, name):
+    """An (n,) float64 device tensor from a numpy array or tensor; ValueError for another length."""
+    t = torch.as_tensor(v, dtype=F64, device=dev).reshape(-1)
+    if t.numel() != n:
+        raise ValueError(f"{name} should be as long as the number of rows of object ({n}), got {t.numel()}")
+    return t.contiguous()
+
+
+def rlog_device(y, m, x=None, blind=True, intercept=None, betaPriorVar=None, fitType="parametric", sizeFactors=None,
+                normalizationFactors=None, avgTxLength=None, dispFit=None):
+    """rlog / rlogData (R/rlog.R:108-272) on the device for y gene-major (N, ld) counts of m samples, in R's order:
+    the factors (_factors: estimated size factors, sizeFactors, normalizationFactors or avgTxLength); sparseTest as a
+    warning when no intercept is given; with blind=True or without dispFit, estimateDispersionsGeneEst +
+    estimateDispersionsFit (fitType "parametric" or "mean") on the non-zero rows with design ~1 when blind and x
+    otherwise, and dispFit = the trend at baseMean; else dispFit ((N,) device tensor aligned with y's rows, R's
+    mcols(object)$dispFit) as given.  betaPriorVar, when not given, by rlog_prior_var; then one rlog_fit.
+    With intercept ((N,) log2, R's rlogIntercept of an earlier call), the frozen rlog: design I_m on nf 2^intercept,
+    rows with a non-finite intercept left out (0) and the intercept added back.
+    Returns {"rlog": (N, m) device tensor, "betaPriorVar": float, "intercept": (N,) device tensor (None when frozen),
+    "dispFit", "fitType" and "trendCoefs" / "meanDisp" (when estimated), "sizeFactors" / "normalizationFactors",
+    "betaIter", "n_nonfinite"}.  Rows whose fit is not finite (R's rowStable would send them to optim) are counted in
+    n_nonfinite with a warning, not refitted.  R's stops raise ValueError (intercept length, dispFit missing or not
+    finite and positive on a fitted row); a failed parametric trend raises FloatingPointError."""
+    import warnings
+    dev = y.device
+    n = y.shape[0]
+    if intercept is not None:
+        intercept = _row_vector(intercept, n, dev, "intercept")
+    refit = blind or dispFit is None
+    if refit:
+        if not blind and x is None:
+            raise ValueError("blind=False needs the design x or dispFit")
+        _check_vst_fit_type(fitType)
+        x = _vst_design(x, m, blind)
+    sizeFactors, nf, sfd = _factors(y, m, sizeFactors, normalizationFactors, avgTxLength)
+    # the normalized counts of sparseTest and getBaseMeansAndVariances' baseMean = rowMeans (any m, also 1)
+    q = y[:, :m].to(F64) / (sfd[:, :m] if sfd.dim() == 2 else sfd)
+    rs = q.sum(dim=1)
+    if intercept is None:
+        _sparse_test(q, rs)
+    del q
+    bm = rs / m
+    res = {}
+    if refit:
+        idx = torch.nonzero(bm > 0).squeeze(1)
+        whole = idx.numel() == n
+        ynz = y if whole else y[idx].contiguous()
+        nfz = None if nf is None else (nf if whole else nf[idx].contiguous())
+        fn = _dispersion_function(ynz, x, sizeFactors, nfz, fitType)
+        res.update(fn)
+        if fitType == "mean":
+            dispFit = torch.full((n,), fn["meanDisp"], dtype=F64, device=dev)
+        else:
+            dispFit = fn["trendCoefs"][0] + fn["trendCoefs"][1] / bm
+    else:
+        dispFit = _row_vector(dispFit, n, dev, "dispFit")
+    fit_rows = torch.isfinite(intercept) if intercept is not None else bm > 0
+    d = dispFit[fit_rows]
+    if not bool(torch.all(torch.isfinite(d) & (d > 0))):
+        raise ValueError("dispFit must be finite and positive on every row the rlog fits")
+    if betaPriorVar is None:
+        if intercept is None:
+            bpv = rlog_prior_var(y, m, sfd, bm, dispFit)
+        else:
+            # the entries of the rows with a finite intercept, normalized by nf 2^intercept (R/rlog.R:219, :234)
+            keep = torch.nonzero(fit_rows).squeeze(1)
+            ysub = y[keep].contiguous()
+            base = sfd[keep][:, :m] if sfd.dim() == 2 else sfd[None, :]
+            nfp = torch.ones(ysub.shape, dtype=F64, device=dev)
+            nfp[:, :m] = base * torch.pow(2.0, intercept[keep])[:, None]
+            bpv = rlog_prior_var(ysub, m, nfp, bm[keep].contiguous(), dispFit[keep].contiguous())
+        betaPriorVar = float(bpv.item())
+        if not (np.isfinite(betaPriorVar) and betaPriorVar > 0):
+            raise ValueError(f"the estimated betaPriorVar ({betaPriorVar}) is not finite and positive")
+    fit = rlog_fit(y, m, sfd, dispFit, betaPriorVar, intercept=intercept)
+    bad = int((~torch.isfinite(fit["rlog"])).any(dim=1).sum().item())
+    if bad:
+        warnings.warn(f"{bad} rows of the rlog fit are not finite (R would refit them with optim); they are returned "
+                      "as they are", stacklevel=2)
+    res.update({"rlog": fit["rlog"], "betaPriorVar": betaPriorVar, "intercept": fit["intercept"], "dispFit": dispFit,
+                "betaIter": fit["betaIter"], "n_nonfinite": bad})
+    if nf is not None:
+        res["normalizationFactors"] = nf
+    else:
+        res["sizeFactors"] = sizeFactors
+    return res

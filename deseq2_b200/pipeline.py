@@ -25,6 +25,7 @@ numpy, one function per R function, same names, so the engine can be driven and 
   DESeq                          R/core.R:280-432    (test="Wald", fitType="parametric", betaPrior=FALSE or TRUE)
   vst / varianceStabilizingTransformation / getVarianceStabilizedData / normTransform   R/vst.R, R/helper.R:421-435
                                  (fitType "parametric" / "mean"; vst's gene subset is vstSubsetPositions)
+  rlog / rlogData / sparseTest   R/rlog.R  (the design [1 | I_m], or I_m with a frozen intercept, through fitNbinomGLMs)
   getAndCheckWeights             R/core.R:2697-2752  (observation weights: row-max normalisation, two rank tests per
                                  gene with a restatement of LINPACK dqrdc2, the rank routine of R's qr())
 
@@ -1272,3 +1273,103 @@ def normTransform(counts, sizeFactors=None, pc=1.0):
     if sizeFactors is None:
         sizeFactors = estimateSizeFactorsForMatrix(counts)
     return np.log2(np.asarray(counts, dtype=np.float64) / _div(sizeFactors) + pc)
+
+
+def sparseTest(normCounts, p=0.9, t1=100, t2=0.1):
+    """R/rlog.R:274-287: warns when, among the rows whose sum of normalized counts exceeds t1, more than a fraction t2
+    have one sample holding more than p of the row sum."""
+    import warnings
+    rs = normCounts.sum(axis=1)
+    rmx = normCounts.max(axis=1)
+    if np.all(rs <= t1):
+        return
+    total = np.mean((rmx / rs)[rs > t1] > p)
+    if total > t2:
+        warnings.warn(f"the rlog assumes that data is close to a negative binomial distribution: for "
+                      f"{round(total, 3) * 100}% of genes with a sum of normalized counts above {t1}, a single "
+                      f"sample's normalized count made up more than {p * 100}% of the sum", stacklevel=3)
+
+
+def rlogData(counts, sizeFactors, dispFit, baseMean, intercept=None, betaPriorVar=None, engine=None):
+    """R/rlog.R:172-272.  sizeFactors: (m,) or an (n, m) nf matrix; dispFit, baseMean: (n,).  The design is
+    [1 | I_m] with lambda = (1e-6, 1 / betaPriorVar, ...) or, with a frozen intercept (n log2 values), I_m on
+    nf 2^intercept; rows that are all zero (or whose intercept is not finite) are left out and get 0.  betaPriorVar,
+    when None, is matchWeightedUpperQuantileForVariance of the log fold changes over an intercept.  One fitNbinomGLMs
+    call (betaTol = 1e-4, useQR, useOptim = FALSE).  Returns {"rlog", "betaPriorVar", "intercept" (None when frozen),
+    "betaIter"}."""
+    counts = np.asarray(counts)
+    n, m = counts.shape
+    nf = np.broadcast_to(_div(sizeFactors), (n, m)).astype(np.float64)
+    dispFit = np.asarray(dispFit, dtype=np.float64)
+    baseMean = np.asarray(baseMean, dtype=np.float64)
+    if intercept is None:
+        allZero = counts.sum(axis=1) == 0
+        x = np.c_[np.ones(m), np.eye(m)]            # model.matrix(~samples)[-1, ] with a "null_level" row first
+    else:
+        intercept = np.array(intercept, dtype=np.float64).reshape(-1)
+        if len(intercept) != n:
+            raise ValueError("intercept should be as long as the number of rows of object")
+        infiniteIntercept = ~np.isfinite(intercept)
+        intercept[infiniteIntercept] = -10.0
+        nf = nf * 2.0 ** intercept[:, None]
+        allZero = infiniteIntercept
+        x = np.eye(m)
+    nz = ~allZero
+    if np.any(np.isnan(dispFit[nz])):
+        raise ValueError("dispFit is NA on a row the rlog fits")
+    if betaPriorVar is None:
+        logFoldChangeMatrix = np.log2(counts[nz] / nf[nz] + 0.5) - np.log2(baseMean[nz] + 0.5)[:, None]
+        weights = 1.0 / (1.0 / baseMean[nz] + dispFit[nz])
+        betaPriorVar = matchWeightedUpperQuantileForVariance(logFoldChangeMatrix.ravel(order="F"), np.tile(weights, m))
+    lam = np.full(x.shape[1], 1.0 / betaPriorVar)
+    if intercept is None:
+        lam[0] = 1e-6
+    fit = fitNbinomGLMs(counts[nz], nf[nz], x, dispFit[nz], lambda_=lam, engine=engine, betaTol=1e-4, useQR=True,
+                        useOptim=False)
+    out = np.zeros((n, m))
+    out[nz] = fit["betaMatrix"] @ x.T
+    it = np.zeros(n)
+    it[nz] = fit["betaIter"]
+    res = {"betaPriorVar": betaPriorVar, "betaIter": it, "intercept": None}
+    if intercept is not None:
+        out = out + np.where(allZero, 0.0, intercept)[:, None]
+    else:
+        icpt = np.full(n, -np.inf)
+        icpt[nz] = fit["betaMatrix"][:, 0]
+        res["intercept"] = icpt
+    res["rlog"] = out
+    return res
+
+
+def rlog(counts, x=None, blind=True, intercept=None, betaPriorVar=None, fitType="parametric", sizeFactors=None,
+         dispFit=None, engine=None):
+    """R/rlog.R:108-164 for a count matrix.  sizeFactors: (m,) or an (n, m) nf matrix, estimated (ratio) when None.
+    sparseTest runs when no intercept is given.  With blind=True or without dispFit, the dispersion function is
+    fitted on the non-all-zero rows (design ~1 when blind, x otherwise) and dispFit is it at baseMean.  Returns
+    rlogData's dict plus "dispFit", "sizeFactors" and the dispersion keys when they were estimated."""
+    counts = np.asarray(counts)
+    m = counts.shape[1]
+    if sizeFactors is None:
+        sizeFactors = estimateSizeFactorsForMatrix(counts)
+    sf = np.asarray(sizeFactors, dtype=np.float64)
+    norm = counts / _div(sf)
+    if intercept is None:
+        sparseTest(norm)
+    baseMean = norm.mean(axis=1)
+    extra = {}
+    if blind or dispFit is None:
+        if not blind and x is None:
+            raise ValueError("blind=False needs the design x or dispFit")
+        nz = counts.sum(axis=1) > 0
+        extra = _fitDispersionFunction(counts[nz], sf[nz] if sf.ndim == 2 else sf, _vstDesign(x, m, blind), fitType,
+                                       engine)
+        with np.errstate(divide="ignore"):
+            if fitType == "mean":
+                dispFit = np.full(len(counts), extra["meanDisp"])
+            else:
+                a = np.asarray(extra["trendCoefs"], dtype=np.float64)
+                dispFit = a[0] + a[1] / baseMean
+    res = rlogData(counts, sf, dispFit, baseMean, intercept=intercept, betaPriorVar=betaPriorVar, engine=engine)
+    res.update(extra)
+    res.update(dispFit=np.asarray(dispFit, dtype=np.float64), sizeFactors=sizeFactors)
+    return res

@@ -233,6 +233,34 @@ int b200nb_sf_iterate_objective_dev(const void* y, int y_type, const double* q, 
 int b200nb_transform_dev(const void* y, int y_type, const double* size_factors, const double* nf, int n, int m,
                          long long ld, int mode, double c0, double c1, double* out, long long ld_out, void* stream);
 
+/* b200nb_rlog_fit_dev: rlogData's fitNbinomGLMs call (R/rlog.R:249-253: betaTol = tol, useQR, no optim) for every row
+ * of y (gene-major n x ld, int32 or f64 counts), with exactly one of size_factors[m] and nf (gene-major n x ld):
+ *   intercept == NULL: the design [1 | I_m], ridge 1e-6 on the intercept and 1 / beta_prior_var on the samples (log2
+ *     scale); start beta0 = log(rowMeans(K / nf)), beta_j = 0.  out_ij = (beta0 + beta_j) / log(2) and
+ *     out_intercept_i = beta0 / log(2); an all-zero row gets out = 0 and out_intercept = -Inf.
+ *   intercept != NULL (n log2 intercepts, the frozen rlog): the design I_m on nf' = nf 2^intercept, start
+ *     log(K / nf' + 0.1); out_ij = beta_j / log(2) + intercept_i; a row with a non-finite intercept gets out = 0.
+ *     out_intercept is not written (may be NULL).
+ * disp_fit: n dispersions (R's dispFit); a fitted row whose dispersion is not finite and > 0 gets NaN in out,
+ * out_intercept and out_iter.  out: gene-major n x ld_out, columns >= m untouched; out_iter: n IRLS iterations (maxit
+ * for a diverged row, |beta| > 30; 0 for a row left out).  Needs n >= 0, m >= 1, ld >= m, ld_out >= m, finite
+ * beta_prior_var > 0, tol > 0 and minmu > 0, maxit >= 1 and no NULL pointer among y, disp_fit, out, out_iter (and
+ * out_intercept without an intercept).  Enqueue only. */
+int b200nb_rlog_fit_dev(const void* y, int y_type, const double* size_factors, const double* nf,
+                        const double* intercept, const double* disp_fit, int n, int m, long long ld,
+                        double beta_prior_var, double tol, int maxit, double minmu, double* out, long long ld_out,
+                        double* out_intercept, double* out_iter, void* stream);
+
+/* b200nb_rlog_prior_var_dev: rlogData's betaPriorVar (R/rlog.R:233-240) over the n x m entries of y (gene-major n x
+ * ld) with exactly one of size_factors[m] and nf (gene-major n x ld):
+ *   x_ij = log2(K_ij / s_ij + 0.5) - log2(base_mean_i + 0.5), weight 1 / (1 / base_mean_i + disp_fit_i)
+ *   *out_var = (Hmisc weighted quantile of |x| at 0.95, normwt = TRUE, / qnorm(0.975))^2
+ * Entries whose weight is NaN or 0 (an all-zero row: base_mean 0) do not take part; NaN when none does.  Two calls
+ * give the same bits.  Needs n, m >= 1, ld >= m and no NULL pointer.  Enqueue only. */
+int b200nb_rlog_prior_var_dev(const void* y, int y_type, const double* size_factors, const double* nf,
+                              const double* base_mean, const double* disp_fit, int n, int m, long long ld,
+                              double* out_var, void* stream);
+
 /* ---- housekeeping */
 const char* b200nb_last_error(void);
 int b200nb_device_count(void);            /* number of visible CUDA devices (0 if none / no driver) */
