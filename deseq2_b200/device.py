@@ -112,9 +112,10 @@ def fit_disp_grid(y, x, mu_hat, disp_grid, log_alpha_prior_mean, log_alpha_prior
 
 
 def fit_beta(y, x, nf, alpha_hat, contrast, beta_mat, lambda_, tol, maxit, useQR=True, minmu=0.5, weights=None,
-             want_hat=True, want_mu=True, out=None):
+             want_hat=True, want_mu=True, out=None, out_mu=None):
     """fitBeta on device tensors (src/DESeq2.cpp:283).  nf: (m,) size-factor vector or gene-major (n, ld) matrix.
-    beta_mat: (p, n) contiguous (= column-major n x p)."""
+    beta_mat: (p, n) contiguous (= column-major n x p).  out_mu: an (n, ld) buffer for the fitted mean (when out is
+    not given)."""
     L = _lib.lib()
     n, ld = y.shape
     xd = _x_dev(x, y.device)
@@ -133,7 +134,8 @@ def fit_beta(y, x, nf, alpha_hat, contrast, beta_mat, lambda_, tol, maxit, useQR
                "contrast_denom": torch.empty(n, dtype=F64, device=dev),
                "deviance": torch.empty(n, dtype=F64, device=dev),
                "hat_diagonals": torch.empty((n, ld), dtype=F64, device=dev) if want_hat else None,
-               "mu": torch.empty((n, ld), dtype=F64, device=dev) if want_mu else None}
+               "mu": out_mu if out_mu is not None else (torch.empty((n, ld), dtype=F64, device=dev) if want_mu
+                                                        else None)}
     rc = L.b200nb_fit_beta_dev(_p(y), _ytype(y), _p(xd), _p(nf), nf_is_vector, _p(alpha_hat), _p(contrast),
                                _p(beta_mat), _p(lam), _p(weights), int(weights is not None), float(tol), int(maxit),
                                int(bool(useQR)), float(minmu), n, m, p, ld, _p(out["beta_mat"]),

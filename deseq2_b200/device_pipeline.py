@@ -519,15 +519,12 @@ def nbinomLRT_device(ynz, x_full, x_reduced, sizeFactors, dispersion, betaTol=1e
             res[name] = _intercept_only_weighted(ynz, sfd, dispersion, wn, m)
             continue
         pr = prep(ynz, x, sizeFactors, minmu=minmu, want_mu=False, normalizationFactors=normalizationFactors)
-        contrast = torch.zeros(p, dtype=F64, device=dev)
-        contrast[0] = 1.0
-        lam = torch.full((p,), 1e-6 / LN2 ** 2, dtype=F64, device=dev)
-        res[name] = D.fit_beta(ynz, pr["xd"], sfd, dispersion, contrast, pr["beta0"], lam, betaTol, maxit, minmu=minmu,
-                               weights=wn, want_hat=(name == "full"), want_mu=False)
-        ll = D.nb_loglik(ynz, pr["xd"], sfd, dispersion, res[name]["beta_mat"], weights=wn, want_mu=(name == "full"))
-        res[name]["conv"], _ = _optim_fallback(ynz, pr["xd"], sfd, dispersion, res[name], pr["beta0"], lam, contrast,
-                                               maxit, minmu, ll, useOptim=useOptim, weights=wn)
-        res[name]["logLike"], res[name]["mu"] = ll["logLike"], ll["mu"]
+        contrast, lam = _mle_penalty(p, dev)
+        fit, ll, conv, _ = _glm_fit(ynz, pr["xd"], sfd, dispersion, contrast, pr["beta0"], lam, betaTol=betaTol,
+                                    maxit=maxit, minmu=minmu, useOptim=useOptim, weights=wn,
+                                    want_hat=(name == "full"), want_mu=(name == "full"))
+        fit["conv"], fit["logLike"], fit["mu"] = conv, ll["logLike"], ll["mu"]
+        res[name] = fit
     df = x_full.shape[1] - x_reduced.shape[1]
     stat = 2.0 * (res["full"]["logLike"] - res["reduced"]["logLike"])
     pval = torch.special.gammaincc(torch.tensor(df / 2.0, dtype=F64, device=dev), torch.clamp(stat, min=0.0) / 2.0)
@@ -551,111 +548,24 @@ def _intercept_only_weighted(ynz, sfd, dispersion, wn, m):
             "conv": torch.ones(ynz.shape[0], dtype=torch.bool, device=dev)}
 
 
-def _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp, kappa_0, dispTol, maxit, betaTol,
-                minmu, outlierSD, useOptim=True, normalizationFactors=None):
-    """The per-gene chain of DESeq_device (GeneEst -> MAP -> Wald) on a subset of rows with the dispersion trend and
-    prior already known: what refitWithoutOutliers (R/core.R:2500-2528) does with objectSub.  Fresh tensors, no
-    shared workspace: the subset is small.  normalizationFactors: the subset's rows; xim is then over them, as R's
-    estimateDispersionsGeneEst(objectSub) computes it (R/core.R:2503-2510)."""
-    dev = ysub.device
-    m, p = x.shape
-    maxDisp = float(max(10, m))
-    linearMu = modelMatrixGroups(x) == p
-    pr = prep(ysub, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu,
-              normalizationFactors=normalizationFactors)
-    xd, sfd, bm, alpha0, beta0 = pr["xd"], pr["sfd"], pr["baseMean"], pr["alpha0"], pr["beta0"]
-    if linearMu:
-        mu = pr["mu_lin"].clone()
-    n = ysub.shape[0]
-    contrast = torch.zeros(p, dtype=F64, device=dev)
-    contrast[0] = 1.0
-    lam = torch.full((p,), 1e-6 / LN2 ** 2, dtype=F64, device=dev)
-    min_log_alpha = float(np.log(minDisp / 10))
-    if not linearMu:
-        mu = D.fit_beta(ysub, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=minmu, want_hat=False,
-                        want_mu=True)["mu"]
-    la0 = torch.log(alpha0)
-    r = D.fit_disp(ysub, xd, mu, la0, la0, 1.0, min_log_alpha, kappa_0, dispTol, maxit, False)
-    dge = torch.clamp(torch.exp(r["log_alpha"]), max=maxDisp)
-    dge = torch.where(r["last_lp"] < r["initial_lp"] + r["initial_lp"].abs() / 1e6, alpha0, dge)
-    conv = (r["iter"] < maxit) & (r["iter"] != 1)
-    gi, ga = _grid_refit(ysub, xd, mu, (~conv) & (dge > minDisp * 10), m, None, 1.0, False)
-    if ga is not None:
-        dge[gi] = ga
-    dge = torch.clamp(dge, minDisp, maxDisp)
-    dispFit = tr[0] + tr[1] / bm
-    logFit = torch.log(dispFit)
-    dispInit = torch.where(dge > 0.1 * dispFit, dge, dispFit)
-    rm = D.fit_disp(ysub, xd, mu, torch.log(dispInit), logFit, dispPriorVar, min_log_alpha, kappa_0, dispTol, maxit, True)
-    dispMAP = torch.exp(rm["log_alpha"])
-    gi2, ga2 = _grid_refit(ysub, xd, mu, rm["iter"] >= maxit, m, logFit, dispPriorVar, True)
-    if ga2 is not None:
-        dispMAP[gi2] = ga2
-    dispMAP = torch.clamp(dispMAP, minDisp, maxDisp)
-    dispOutlier = torch.log(dge) > logFit + outlierSD * torch.sqrt(varLogDispEsts)
-    dispersion = torch.where(dispOutlier, dge, dispMAP)
-    fb = D.fit_beta(ysub, xd, sfd, dispersion, contrast, beta0, lam, betaTol, maxit, minmu=minmu, want_hat=False,
-                    want_mu=False)
-    ll = D.nb_loglik(ysub, xd, sfd, dispersion, fb["beta_mat"], want_mu=False)
-    betaConv, _ = _optim_fallback(ysub, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, minmu, ll, useOptim=useOptim)
-    betaMatrix = fb["beta_mat"] / LN2
-    betaSE = torch.sqrt(torch.clamp(fb["beta_var_mat"], min=0.0)) / LN2
-    stat = betaMatrix / betaSE
-    fb["deviance"] = -2.0 * ll["logLike"]
-    return {"baseMean": bm, "dispGeneEst": dge, "dispFit": dispFit, "dispMAP": dispMAP, "dispersion": dispersion,
-            "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": rm["iter"], "betaMatrix": betaMatrix.T,
-            "betaSE": betaSE.T, "WaldStatistic": stat.T, "WaldPvalue": (2.0 * torch.special.ndtr(-stat.abs())).T,
-            "betaIter": fb["iter"], "betaConv": betaConv, "deviance": fb["deviance"]}
-
-
-def _dispersions_intercept_mean(ynz, m, sf, minDisp, kappa_0, dispTol, maxit, minmu, outlierSD):
+def _dispersions_intercept_mean(ynz, m, sf, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, minmu=0.5,
+                                outlierSD=2.0):
     """estimateDispersions(design ~1, fitType = "mean") as estimateSizeFactorsIterate runs it (R/core.R:2594-2597):
-    the prep kernel's clamped linear mu, the gene-wise fitDisp with its rules and grid refit, the trimmed-mean fit,
-    varLogDispEsts as dispersionFunction<- computes it (R/methods.R:142-190), estimateDispersionsPriorVar, the MAP
-    fitDisp with its grid refit and the dispersion-outlier rule.  The same steps as DESeq_device's, for x = 1.
-    Returns (q = mu / sf as a fresh gene-major tensor, final dispersions, dispGeneEst, meanDisp, dispPriorVar)."""
-    dev = ynz.device
-    x = np.ones((m, 1))
-    maxDisp = float(max(10, m))
-    min_log_alpha = float(np.log(minDisp / 10))
-    pr = prep(ynz, x, sf, minDisp=minDisp, minmu=minmu, want_mu=True, want_beta0=False)
-    xd, alpha0, mu = pr["xd"], pr["alpha0"], pr["mu_lin"]
-    la0 = torch.log(alpha0)
-    r = D.fit_disp(ynz, xd, mu, la0, la0, 1.0, min_log_alpha, kappa_0, dispTol, maxit, False)
-    dge = torch.clamp(torch.exp(r["log_alpha"]), max=maxDisp)
-    dge = torch.where(r["last_lp"] < r["initial_lp"] + r["initial_lp"].abs() / 1e6, alpha0, dge)
-    conv = (r["iter"] < maxit) & (r["iter"] != 1)
-    gi, ga = _grid_refit(ynz, xd, mu, (~conv) & (dge > minDisp * 10), m, None, 1.0, False)
-    if ga is not None:
-        dge[gi] = ga
-    dge = torch.clamp(dge, minDisp, maxDisp)
-    meanDisp = mean_disp(dge, minDisp)
-    dispFit = meanDisp.expand(dge.shape)
-    above = dge >= minDisp * 100
-    resid = (torch.log(dge) - torch.log(meanDisp))[above]
-    med = _median(resid)
-    varLogDispEsts = (1.4826 * _median((resid - med).abs())) ** 2
-    if m - 1 <= 3:
-        from .pipeline import estimateDispersionsPriorVar
-        dispPriorVar = estimateDispersionsPriorVar(float(varLogDispEsts.item()), m, 1, dge.cpu().numpy(),
-                                                   dispFit.cpu().numpy(), minDisp)
-    else:
-        expVar = torch.special.polygamma(1, torch.tensor((m - 1) / 2.0, dtype=F64, device=dev))
-        dispPriorVar = float(torch.clamp(varLogDispEsts - expVar, min=0.25).item())
-    logFit = torch.log(dispFit).contiguous()
-    dispInit = torch.where(dge > 0.1 * dispFit, dge, dispFit)
-    rm = D.fit_disp(ynz, xd, mu, torch.log(dispInit), logFit, dispPriorVar, min_log_alpha, kappa_0, dispTol, maxit,
-                    True)
-    dispMAP = torch.exp(rm["log_alpha"])
-    gi2, ga2 = _grid_refit(ynz, xd, mu, rm["iter"] >= maxit, m, logFit, dispPriorVar, True)
-    if ga2 is not None:
-        dispMAP[gi2] = ga2
-    dispMAP = torch.clamp(dispMAP, minDisp, maxDisp)
-    dispOutlier = torch.log(dge) > logFit + outlierSD * torch.sqrt(varLogDispEsts)
-    dispersion = torch.where(dispOutlier, dge, dispMAP).contiguous()
+    the pre-step kernel's clamped linear mu, then DESeq_device's stages for x = 1: _gene_est, the trimmed-mean trend,
+    _disp_prior_var and _disp_map.  Returns (q = mu / sf as a fresh gene-major tensor, final dispersions, dispGeneEst,
+    meanDisp, dispPriorVar)."""
+    pr = prep(ynz, np.ones((m, 1)), sf, minDisp=minDisp, minmu=minmu, want_mu=True, want_beta0=False)
+    xd, bm, mu = pr["xd"], pr["baseMean"], pr["mu_lin"]
+    _, _, dge, _ = _gene_est(ynz, xd, pr["sfd"], pr["alpha0"], None, mu, m, minDisp=minDisp, kappa_0=kappa_0,
+                             dispTol=dispTol, maxit=maxit, minmu=minmu)
+    tr = _dispersion_trend(bm, dge, "mean", minDisp)
+    dispFit = tr[0] + tr[1] / bm
+    varLogDispEsts, dispPriorVar = _disp_prior_var(dge, dispFit, m, 1, minDisp)
+    _, dispersion, _, _, _ = _disp_map(ynz, xd, mu, dge, dispFit, varLogDispEsts, dispPriorVar, m, minDisp=minDisp,
+                                       kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, outlierSD=outlierSD)
     q = torch.ones_like(mu)
-    q[:, :m] = mu[:, :m] / torch.as_tensor(np.asarray(sf, dtype=np.float64), device=dev)[None, :]
-    return q, dispersion, dge, meanDisp, dispPriorVar
+    q[:, :m] = mu[:, :m] / pr["sfd"][None, :]
+    return q, dispersion, dge, tr[0], dispPriorVar
 
 
 def size_factors_iterate(y, m, niter=10, Q=0.05, minDisp=1e-8, minmu=0.5, kappa_0=1.0, dispTol=1e-6, maxit=100,
@@ -675,8 +585,9 @@ def size_factors_iterate(y, m, niter=10, Q=0.05, minDisp=1e-8, minmu=0.5, kappa_
     out = torch.empty(2 * m + 1, dtype=F64, device=dev)
 
     def step(sf):
-        q, disp, dge, meanDisp, dpv = _dispersions_intercept_mean(ynz, m, sf, minDisp, kappa_0, dispTol, maxit, minmu,
-                                                                  outlierSD)
+        q, disp, dge, meanDisp, dpv = _dispersions_intercept_mean(ynz, m, sf, minDisp=minDisp, kappa_0=kappa_0,
+                                                                  dispTol=dispTol, maxit=maxit, minmu=minmu,
+                                                                  outlierSD=outlierSD)
 
         def evaluate(par):
             pd = torch.as_tensor(np.asarray(par, dtype=np.float64), device=dev)
@@ -693,44 +604,43 @@ def size_factors_iterate(y, m, niter=10, Q=0.05, minDisp=1e-8, minmu=0.5, kappa_
     return res
 
 
-def _gene_est(ynz, xd, sfd, alpha0, beta0, mu_lin, m, minDisp, kappa_0, dispTol, maxit, betaTol, minmu, wn=None,
-              wdisp=None, weightThreshold=1e-2, mark=lambda name: None):
+def _mle_penalty(p, dev):
+    """fitNbinomGLMs' maximum-likelihood fit (R/fitNbinomGLMs.R:29-236): the contrast e1 and lambda = 1e-6 on the
+    log2 scale, as (contrast, lam) device tensors."""
+    contrast = torch.zeros(p, dtype=F64, device=dev)
+    contrast[0] = 1.0
+    return contrast, torch.full((p,), 1e-6 / LN2 ** 2, dtype=F64, device=dev)
+
+
+def _gene_est(ynz, xd, sfd, alpha0, beta0, mu_lin, m, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100,
+              betaTol=1e-8, minmu=0.5, wn=None, wdisp=None, weightThreshold=1e-2, mu_out=None, penalty=None,
+              mark=lambda name: None):
     """estimateDispersionsGeneEst (R/core.R:657-860) after the pre-steps: the gene-wise mean (mu_lin, the prep
     kernel's linear mu, when it is given; else a GLM fit, weighted with R's defaults when the normalised weights wn
     are given), the fitDisp MLE, the noIncrease rule, the grid refit of the unconverged genes and the clamps.  sfd:
     the size-factor vector or the nf rows of ynz; alpha0 / beta0: the prep kernel's start values; wdisp:
-    pmax(wn, 1e-6).  Returns (mu, the fitDisp result, dispGeneEst, number of grid refits)."""
-    dev = ynz.device
-    p = beta0.shape[0]
+    pmax(wn, 1e-6).  The GLM mean is written to mu_out, an (n, ld) buffer, or to a fresh tensor; penalty: the
+    (contrast, lam) of that fit, _mle_penalty's when not given.  Returns (mu, the fitDisp result, dispGeneEst, number
+    of grid refits)."""
     maxDisp = float(max(10, m))
-    contrast = torch.zeros(p, dtype=F64, device=dev)
-    contrast[0] = 1.0
-    lam = torch.full((p,), 1e-6 / LN2 ** 2, dtype=F64, device=dev)
-    min_log_alpha = float(np.log(minDisp / 10))
     if mu_lin is not None:
         mu = mu_lin
-    elif wn is not None:
-        # fitNbinomGLMs with the normalised weights, its defaults minmu = 0.5 and useOptim = TRUE (R/core.R:752-755
-        # passes neither), its unclamped mean nf exp(x beta) (R/fitNbinomGLMs.R:180; the optim rows' own, :383)
-        # bounded at minmu (:764)
-        fb0 = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=0.5, weights=wn,
-                         want_hat=False, want_mu=False)
-        ll0 = D.nb_loglik(ynz, xd, sfd, alpha0, fb0["beta_mat"], weights=wn,
-                          out_mu=_ws("mu_glm", tuple(ynz.shape), F64, dev))
-        _optim_fallback(ynz, xd, sfd, alpha0, fb0, beta0, lam, contrast, maxit, 0.5, ll0, useOptim=True, weights=wn)
-        mu = ll0["mu"].clamp_(min=minmu)
     else:
-        nn0 = ynz.shape[0]
-        vec = lambda: torch.empty(nn0, dtype=F64, device=dev)
-        out0 = {"beta_mat": torch.empty((p, nn0), dtype=F64, device=dev),
-                "beta_var_mat": torch.empty((p, nn0), dtype=F64, device=dev), "iter": vec(), "contrast_num": vec(),
-                "contrast_denom": vec(), "deviance": vec(), "hat_diagonals": None,
-                "mu": _ws("mu_glm", tuple(ynz.shape), F64, dev)}
-        mu = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=minmu, out=out0)["mu"]
+        contrast, lam = penalty if penalty is not None else _mle_penalty(beta0.shape[0], ynz.device)
+        if wn is not None:
+            # fitNbinomGLMs with the normalised weights, its defaults minmu = 0.5 and useOptim = TRUE (R/core.R:752-755
+            # passes neither), its unclamped mean nf exp(x beta) (R/fitNbinomGLMs.R:180; the optim rows' own, :383)
+            # bounded at minmu (:764)
+            _, ll0, _, _ = _glm_fit(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol=betaTol, maxit=maxit, minmu=0.5,
+                                    weights=wn, want_hat=False, out_mu=mu_out)
+            mu = ll0["mu"].clamp_(min=minmu)
+        else:
+            mu = D.fit_beta(ynz, xd, sfd, alpha0, contrast, beta0, lam, betaTol, maxit, minmu=minmu, want_hat=False,
+                            out_mu=mu_out)["mu"]
     la0 = torch.log(alpha0)
     mark("mu")
-    r = D.fit_disp(ynz, xd, mu, la0, la0, 1.0, min_log_alpha, kappa_0, dispTol, maxit, False, weights=wdisp,
-                   weightThreshold=weightThreshold)
+    r = D.fit_disp(ynz, xd, mu, la0, la0, 1.0, float(np.log(minDisp / 10)), kappa_0, dispTol, maxit, False,
+                   weights=wdisp, weightThreshold=weightThreshold)
     mark("fit_disp_mle")
     dge = torch.clamp(torch.exp(r["log_alpha"]), max=maxDisp)
     noIncrease = r["last_lp"] < r["initial_lp"] + r["initial_lp"].abs() / 1e6
@@ -746,12 +656,85 @@ def _gene_est(ynz, xd, sfd, alpha0, beta0, mu_lin, m, minDisp, kappa_0, dispTol,
 def _dispersion_trend(baseMean, dge, fitType, minDisp=1e-8):
     """estimateDispersionsFit's fit (R/core.R:864-940) as a 4-vector (a, b, status, rounds) with dispFit = a + b /
     baseMean: parametricDispersionFit on the device (trend_fit), or for fitType "mean" (mean_disp, 0, 0, 0), so that
-    every a + b / baseMean downstream (the MAP prior, the outlier refit) equals meanDisp."""
+    every a + b / baseMean downstream (the MAP prior, the outlier refit) equals meanDisp.  A failed parametric fit
+    raises FloatingPointError (one host read; R would fall back to the local fit)."""
     if fitType == "mean":
         tr = torch.zeros(4, dtype=F64, device=dge.device)
         tr[0] = mean_disp(dge, minDisp)
         return tr
-    return trend_fit(baseMean, dge, minDisp)
+    tr = trend_fit(baseMean, dge, minDisp)
+    status = tr[2].item()
+    if status != 0:
+        raise FloatingPointError(f"parametric dispersion fit failed on device (status {int(status)})")
+    return tr
+
+
+def _disp_prior_var(dge_all, dispFit_all, m, p, minDisp=1e-8):
+    """varLogDispEsts as dispersionFunction<- computes it (R/methods.R:142-190: the squared MAD of the log residuals of
+    the estimates >= 100 minDisp) and estimateDispersionsPriorVar (R/core.R:1135-1208), over all genes.  Returns
+    (varLogDispEsts as a 0-d device tensor, dispPriorVar as a float)."""
+    above = dge_all >= minDisp * 100
+    resid = (torch.log(dge_all) - torch.log(dispFit_all))[above]
+    med = _median(resid)
+    varLogDispEsts = (1.4826 * _median((resid - med).abs())) ** 2
+    if m - p <= 3 and m > p:
+        # 2-vs-2 / 3-vs-2 experiments: the reference's Monte-Carlo KL match (R/core.R:1157-1193) is host glue (numpy);
+        # it needs the log-dispersion residuals of all genes: one D2H of two doubles per gene
+        from .pipeline import estimateDispersionsPriorVar
+        dispPriorVar = estimateDispersionsPriorVar(float(varLogDispEsts.item()), m, p, dge_all.cpu().numpy(),
+                                                   dispFit_all.cpu().numpy(), minDisp)
+    elif m > p:
+        expVar = torch.special.polygamma(1, torch.tensor((m - p) / 2.0, dtype=F64, device=dge_all.device))
+        dispPriorVar = float(torch.clamp(varLogDispEsts - expVar, min=0.25).item())
+    else:
+        dispPriorVar = float(varLogDispEsts.item())
+    return varLogDispEsts, dispPriorVar
+
+
+def _disp_map(ynz, xd, mu, dge, dispFit, varLogDispEsts, dispPriorVar, m, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6,
+              maxit=100, outlierSD=2.0, wn=None, weightThreshold=1e-2, mark=lambda name: None):
+    """estimateDispersionsMAP (R/core.R:943-1131): dispInit, the fitDisp MAP with the log trend as prior mean, the
+    grid refit of the genes at maxit, the clamps and the dispersion-outlier rule.  wn: the normalised weights.
+    Returns (dispMAP, dispersion, dispOutlier, dispIter, number of grid refits)."""
+    maxDisp = float(max(10, m))
+    dispInit = torch.where(dge > 0.1 * dispFit, dge, dispFit)
+    logFit = torch.log(dispFit)
+    rm = D.fit_disp(ynz, xd, mu, torch.log(dispInit), logFit, dispPriorVar, float(np.log(minDisp / 10)), kappa_0,
+                    dispTol, maxit, True, weights=wn, weightThreshold=weightThreshold)
+    mark("fit_disp_map")
+    dispMAP = torch.exp(rm["log_alpha"])
+    gi, ga = _grid_refit(ynz, xd, mu, rm["iter"] >= maxit, m, logFit, dispPriorVar, True, wn, weightThreshold)
+    if ga is not None:
+        dispMAP[gi] = ga
+    dispMAP = torch.clamp(dispMAP, minDisp, maxDisp)
+    dispOutlier = torch.log(dge) > logFit + outlierSD * torch.sqrt(varLogDispEsts)
+    dispersion = torch.where(dispOutlier, dge, dispMAP)
+    return dispMAP, dispersion, dispOutlier, rm["iter"], int(gi.numel())
+
+
+def _glm_fit(y, xd, sfd, dispersion, contrast, beta0, lam, betaTol=1e-8, maxit=100, minmu=0.5, useOptim=True,
+             weights=None, out=None, want_hat=True, out_mu=None, want_mu=True, mark=lambda name: None):
+    """fitNbinomGLMs (R/fitNbinomGLMs.R:29-236): the IRLS fit (out / want_hat: its buffers or its hat diagonals), the
+    log-likelihood at the UNCLAMPED fitted mean nf * exp(x beta) that R recomputes right after the native call
+    (:180-182; out_mu / want_mu: that mean's buffer or whether it is wanted), then the optim fallback (:186-227).
+    Returns (the fitBeta result, the log-likelihood result, betaConv, number of optim rows)."""
+    fb = D.fit_beta(y, xd, sfd, dispersion, contrast, beta0, lam, betaTol, maxit, minmu=minmu, weights=weights,
+                    want_hat=want_hat, want_mu=False, out=out)
+    mark("fit_beta")
+    ll = D.nb_loglik(y, xd, sfd, dispersion, fb["beta_mat"], weights=weights, want_mu=want_mu, out_mu=out_mu)
+    betaConv, n_optim = _optim_fallback(y, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, minmu, ll,
+                                        useOptim=useOptim, weights=weights)
+    return fb, ll, betaConv, n_optim
+
+
+def _wald_stats(fit):
+    """nbinomWaldTest's betaMatrix, betaSE, WaldStatistic and WaldPvalue (n, p) on the log2 scale from a fitBeta
+    result."""
+    betaMatrix = fit["beta_mat"] / LN2                     # (p, n)
+    betaSE = torch.sqrt(torch.clamp(fit["beta_var_mat"], min=0.0)) / LN2
+    stat = betaMatrix / betaSE
+    return {"betaMatrix": betaMatrix.T, "betaSE": betaSE.T, "WaldStatistic": stat.T,
+            "WaldPvalue": (2.0 * torch.special.ndtr(-stat.abs())).T}
 
 
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
@@ -860,7 +843,6 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             stage_ms[name] = round((now - _t[0]) * 1e3, 3)
             _t[0] = now
 
-    maxDisp = float(max(10, m))
     linearMu = modelMatrixGroups(x) == p and weights is None
     wn = wdisp = weightsFail = None
     if weights is None:
@@ -897,56 +879,28 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             beta0, wn = pr["beta0"][:, idx].contiguous(), pr["weightsNorm"][idx].contiguous()
         wdisp = torch.clamp(wn, min=1e-6)                   # pmax(weights, 1e-6) for the gene-wise estimate (:702)
     xd, sfd = pr["xd"], pr["sfd"]
-    n = idx.numel()
-    contrast = torch.zeros(p, dtype=F64, device=dev)
-    contrast[0] = 1.0
-    lam = torch.full((p,), 1e-6 / LN2 ** 2, dtype=F64, device=dev)
-    min_log_alpha = float(np.log(minDisp / 10))
+    contrast, lam = _mle_penalty(p, dev)
 
     # ---- estimateDispersionsGeneEst (R/core.R:657-860)
-    mu, r, dge, n_refit_geneest = _gene_est(ynz, xd, sfd, alpha0, beta0, pr["mu_lin"] if linearMu else None, m,
-                                            minDisp, kappa_0, dispTol, maxit, betaTol, minmu, wn=wn, wdisp=wdisp,
-                                            weightThreshold=weightThreshold, mark=mark)
+    mu_glm = None if linearMu else _ws("mu_glm", tuple(ynz.shape), F64, dev)
+    mu, r, dge, n_refit_geneest = _gene_est(ynz, xd, sfd, alpha0, beta0, pr["mu_lin"], m, minDisp=minDisp,
+                                            kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, betaTol=betaTol,
+                                            minmu=minmu, wn=wn, wdisp=wdisp, weightThreshold=weightThreshold,
+                                            mu_out=mu_glm, penalty=(contrast, lam), mark=mark)
     mark("rules+grid_mle")
 
     # ---- estimateDispersionsFit + dispersionFunction<- + PriorVar (R/core.R:864-940, R/methods.R:142-190, R/core.R:1135-1208)
     # ONE packed collective for the two vectors the global step needs (sharded.PackedGather accepts a list)
     bm_all, dge_all = allgather([bm, dge]) if allgather is not None else (bm, dge)
     tr = _dispersion_trend(bm_all, dge_all, fitType, minDisp)
-    dispFit = tr[0] + tr[1] / bm
-    above = dge_all >= minDisp * 100
-    resid = (torch.log(dge_all) - torch.log(tr[0] + tr[1] / bm_all))[above]
-    med = _median(resid)
-    varLogDispEsts = (1.4826 * _median((resid - med).abs())) ** 2
-    if m - p <= 3 and m > p:
-        # 2-vs-2 / 3-vs-2 experiments: the reference's Monte-Carlo KL match (R/core.R:1157-1193) is host glue (numpy);
-        # it needs the log-dispersion residuals of all genes: one D2H of two doubles per gene
-        from .pipeline import estimateDispersionsPriorVar
-        dispPriorVar = estimateDispersionsPriorVar(float(varLogDispEsts.item()), m, p, dge_all.cpu().numpy(),
-                                                   (tr[0] + tr[1] / bm_all).cpu().numpy(), minDisp)
-    elif m > p:
-        expVar = torch.special.polygamma(1, torch.tensor((m - p) / 2.0, dtype=F64, device=dev))
-        dispPriorVar = float(torch.clamp(varLogDispEsts - expVar, min=0.25).item())
-    else:
-        dispPriorVar = float(varLogDispEsts.item())
-    status = tr[2].item()
-    if status != 0:
-        raise FloatingPointError(f"parametric dispersion fit failed on device (status {int(status)})")
+    dispFit, dispFit_all = tr[0] + tr[1] / bm, tr[0] + tr[1] / bm_all
+    varLogDispEsts, dispPriorVar = _disp_prior_var(dge_all, dispFit_all, m, p, minDisp)
     mark("trend+priorvar")
 
     # ---- estimateDispersionsMAP (R/core.R:943-1131)
-    dispInit = torch.where(dge > 0.1 * dispFit, dge, dispFit)
-    logFit = torch.log(dispFit)
-    rm = D.fit_disp(ynz, xd, mu, torch.log(dispInit), logFit, dispPriorVar, min_log_alpha, kappa_0, dispTol, maxit, True,
-                    weights=wn, weightThreshold=weightThreshold)
-    mark("fit_disp_map")
-    dispMAP = torch.exp(rm["log_alpha"])
-    gi2, ga2 = _grid_refit(ynz, xd, mu, rm["iter"] >= maxit, m, logFit, dispPriorVar, True, wn, weightThreshold)
-    if ga2 is not None:
-        dispMAP[gi2] = ga2
-    dispMAP = torch.clamp(dispMAP, minDisp, maxDisp)
-    dispOutlier = torch.log(dge) > logFit + outlierSD * torch.sqrt(varLogDispEsts)
-    dispersion = torch.where(dispOutlier, dge, dispMAP)
+    dispMAP, dispersion, dispOutlier, dispIter, n_refit_map = _disp_map(
+        ynz, xd, mu, dge, dispFit, varLogDispEsts, dispPriorVar, m, minDisp=minDisp, kappa_0=kappa_0, dispTol=dispTol,
+        maxit=maxit, outlierSD=outlierSD, wn=wn, weightThreshold=weightThreshold, mark=mark)
     mark("rules+grid_map")
 
     # ---- nbinomWaldTest (R/core.R:1332-1565) via fitNbinomGLMs (R/fitNbinomGLMs.R:29-236)
@@ -955,25 +909,18 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             "iter": torch.empty(nn, dtype=F64, device=dev), "contrast_num": torch.empty(nn, dtype=F64, device=dev),
             "contrast_denom": torch.empty(nn, dtype=F64, device=dev), "deviance": torch.empty(nn, dtype=F64, device=dev),
             "hat_diagonals": _ws("H", (nn, ldd), F64, dev), "mu": None}
-    fb = D.fit_beta(ynz, xd, sfd, dispersion, contrast, beta0, lam, betaTol, maxit, minmu=minmu, weights=wn, out=outb)
-    mark("fit_beta")
     # Cook's distances and the reported deviance use the UNCLAMPED fitted mean nf * exp(x beta) and the log-likelihood
-    # at it, which the reference recomputes in R right after the native call (R/fitNbinomGLMs.R:180-182): one small
-    # kernel (b200nb_nb_loglik_dev); the IRLS kernel's fused mean / deviance are at the minmu clamp.
-    ll = D.nb_loglik(ynz, xd, sfd, dispersion, fb["beta_mat"], weights=wn, out_mu=_ws("mu_cooks", (nn, ldd), F64, dev))
-    # rows the IRLS could not fit go to the box-constrained maximiser (R/fitNbinomGLMs.R:203-227, useOptim = TRUE)
-    betaConv, n_optim = _optim_fallback(ynz, xd, sfd, dispersion, fb, beta0, lam, contrast, maxit, minmu, ll,
-                                        useOptim=useOptim, weights=wn)
+    # at it (one small kernel, b200nb_nb_loglik_dev); the IRLS kernel's fused mean / deviance are at the minmu clamp.
+    # Rows the IRLS could not fit go to the box-constrained maximiser (R/fitNbinomGLMs.R:203-227, useOptim = TRUE).
+    fb, ll, betaConv, n_optim = _glm_fit(ynz, xd, sfd, dispersion, contrast, beta0, lam, betaTol=betaTol, maxit=maxit,
+                                         minmu=minmu, useOptim=useOptim, weights=wn, out=outb,
+                                         out_mu=_ws("mu_cooks", (nn, ldd), F64, dev), mark=mark)
     mark("loglik+optim")
     fit, fit_ll, prior = fb, ll, {}
     if betaPrior:
-        fit, fit_ll, betaConv, prior = _fit_with_prior(ynz, factors, sfd, dispersion, fb, bm, bm_all, tr, allgather,
-                                                       betaTol, maxit, minmu, useOptim)
+        fit, fit_ll, betaConv, prior = _fit_with_prior(ynz, factors, sfd, dispersion, fb, bm, bm_all, dispFit_all,
+                                                       allgather, betaTol, maxit, minmu, useOptim)
         mark("beta_prior_var+fit_beta_map")
-    betaMatrix = fit["beta_mat"] / LN2                     # (p, n)
-    betaSE = torch.sqrt(torch.clamp(fit["beta_var_mat"], min=0.0)) / LN2
-    stat = betaMatrix / betaSE
-    pval = 2.0 * torch.special.ndtr(-stat.abs())
     from .pipeline import nOrMoreInCell
     do_replace = bool(np.isfinite(minReplicatesForReplace)) and bool(nOrMoreInCell(x, minReplicatesForReplace).any())
     mu_cooks = ll["mu"]
@@ -981,11 +928,11 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
                normalizationFactors=sfd if nf is not None else None)
     mark("wald_stats+cooks")
     res = {"stage_ms": stage_ms, "maxCooks": ck["maxCooks"], "idx": idx, "baseMean": bm, "dispGeneEst": dge, "dispFit": dispFit, "dispMAP": dispMAP,
-            "dispersion": dispersion, "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": rm["iter"],
-            "betaMatrix": betaMatrix.T, "betaSE": betaSE.T, "WaldStatistic": stat.T, "WaldPvalue": pval.T,
+            "dispersion": dispersion, "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": dispIter,
+            **_wald_stats(fit),
             "betaIter": fit["iter"], "betaConv": betaConv, "n_optim": n_optim, "deviance": -2.0 * fit_ll["logLike"], "mu": mu_cooks,
             "H": fb["hat_diagonals"], "varLogDispEsts": varLogDispEsts,
-            "dispPriorVar": dispPriorVar, "n_refit_geneest": n_refit_geneest, "n_refit_map": int(gi2.numel()),
+            "dispPriorVar": dispPriorVar, "n_refit_geneest": n_refit_geneest, "n_refit_map": n_refit_map,
             "n_input_rows": y.shape[0],
             "sizeFactors": None if nf is not None else np.asarray(sizeFactors, dtype=np.float64), "fitType": fitType}
     if fitType == "mean":
@@ -1000,13 +947,14 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     if nf is not None:
         res["normalizationFactors"] = sfd
     if do_replace and m > p:
-        _replace_and_refit(res, ynz, ck["cooks"], x, sizeFactors, sfd, tr, varLogDispEsts, dispPriorVar,
-                           minReplicatesForReplace, minDisp, kappa_0, dispTol, maxit, betaTol, minmu, outlierSD,
-                           useOptim=useOptim)
+        _replace_and_refit(res, ynz, ck["cooks"], x, sizeFactors, sfd, tr, minReplicatesForReplace, minDisp=minDisp,
+                           kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, betaTol=betaTol, minmu=minmu,
+                           outlierSD=outlierSD, useOptim=useOptim)
     return res
 
 
-def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, tr, allgather, betaTol, maxit, minmu, useOptim):
+def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, dispFit_all, allgather, betaTol, maxit, minmu,
+                    useOptim):
     """The betaPrior half of fitGLMsWithPrior (R/fitNbinomGLMs.R:242-337) after the MLE fit `mle`: prior variance
     over all genes, then the MAP fit on the expanded matrix, its log-likelihood and the optim fallback with the same
     lambda.  Returns (fit, loglik, betaConv, extra result entries)."""
@@ -1020,7 +968,7 @@ def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, tr, allgathe
         beta_all = torch.stack([torch.zeros_like(g[0])] + list(g))
     else:
         beta_all = mleBeta
-    pv = estimate_beta_prior_var(beta_all.T, factors, bm_all, tr[0] + tr[1] / bm_all)
+    pv = estimate_beta_prior_var(beta_all.T, factors, bm_all, dispFit_all)
     x_exp = factorDesign(factors, expanded=True)[0]
     pe = x_exp.shape[1]
     xe = D.x_to_device(x_exp, dev)
@@ -1030,22 +978,20 @@ def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, tr, allgathe
     # the expanded matrix is rank deficient: start at (log baseMean, 0, ..., 0) (R/fitNbinomGLMs.R:146-151)
     beta0 = torch.zeros((pe, ynz.shape[0]), dtype=F64, device=dev)
     beta0[0] = torch.log(bm)
-    fit = D.fit_beta(ynz, xe, sfd, dispersion, contrast, beta0, lam, betaTol, maxit, minmu=minmu, want_hat=False,
-                     want_mu=False)
-    ll = D.nb_loglik(ynz, xe, sfd, dispersion, fit["beta_mat"], want_mu=False)
-    betaConv, n_optim = _optim_fallback(ynz, xe, sfd, dispersion, fit, beta0, lam, contrast, maxit, minmu, ll,
-                                        useOptim=useOptim)
+    fit, ll, betaConv, n_optim = _glm_fit(ynz, xe, sfd, dispersion, contrast, beta0, lam, betaTol=betaTol, maxit=maxit,
+                                          minmu=minmu, useOptim=useOptim, want_hat=False, want_mu=False)
     return fit, ll, betaConv, {"mleBetaMatrix": mleBeta.T, "betaPriorVar": pv.cpu().numpy(), "modelMatrix": x_exp,
                                "n_optim_map": n_optim}
 
 
-def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, varLogDispEsts, dispPriorVar, minReplicates, minDisp,
-                       kappa_0, dispTol, maxit, betaTol, minmu, outlierSD, trim=0.2, useOptim=True):
+def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, minReplicates, minDisp=1e-8, kappa_0=1.0,
+                       dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5, outlierSD=2.0, useOptim=True, trim=0.2):
     """replaceOutliers + refitWithoutOutliers (R/core.R:2069-2115, 2484-2565) on the device results `res` (in place).
     Only the flagged rows move: their counts are gathered, the outlying entries of replaceable samples become
-    as.integer(trimmed mean of the normalised counts * size factor), and the rows go through _refit_rows.
-    `sfd` is the size-factor vector or the nf matrix of ynz's rows: with nf the trimmed mean is of K/nf and the
-    replacement count trunc(trimmed mean * nf_ij) (R/core.R:2089-2096)."""
+    as.integer(trimmed mean of the normalised counts * size factor), and the rows go through DESeq_device's stages
+    (GeneEst -> MAP -> Wald) with the trend `tr` and res's prior variance, as refitWithoutOutliers does with
+    objectSub.  `sfd` is the size-factor vector or the nf matrix of ynz's rows: with nf the trimmed mean is of K/nf
+    and the replacement count trunc(trimmed mean * nf_ij) (R/core.R:2089-2096)."""
     from scipy import stats as _st
     from .pipeline import nOrMoreInCell
     dev = ynz.device
@@ -1073,12 +1019,25 @@ def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, varLogDispEsts
     if rr.numel() > 0:
         ysub = torch.zeros((rr.numel(), ynz.shape[1]), dtype=F64, device=dev)
         ysub[:, :m] = new[keep]
-        sub = _refit_rows(ysub, x, sizeFactors, tr, varLogDispEsts, dispPriorVar, minDisp, kappa_0, dispTol, maxit,
-                          betaTol, minmu, outlierSD, useOptim=useOptim,
-                          normalizationFactors=sfd[rr].contiguous() if sfd.dim() == 2 else None)
+        # no mu_out: a GLM mean of the subset goes to a fresh tensor, not into the full-size "mu_glm" workspace; with
+        # nf, xim is over the subset's rows, as estimateDispersionsGeneEst(objectSub) computes it (R/core.R:2503-2510)
+        pr = prep(ysub, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=modelMatrixGroups(x) == p,
+                  normalizationFactors=sfd[rr].contiguous() if sfd.dim() == 2 else None)
+        xd, sfs, beta0 = pr["xd"], pr["sfd"], pr["beta0"]
+        contrast, lam = _mle_penalty(p, dev)
+        mu, r, dge, _ = _gene_est(ysub, xd, sfs, pr["alpha0"], beta0, pr["mu_lin"], m, minDisp=minDisp,
+                                  kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, betaTol=betaTol, minmu=minmu,
+                                  penalty=(contrast, lam))
+        dispFit = tr[0] + tr[1] / pr["baseMean"]
+        dispMAP, dispersion, dispOutlier, dispIter, _ = _disp_map(
+            ysub, xd, mu, dge, dispFit, res["varLogDispEsts"], res["dispPriorVar"], m, minDisp=minDisp,
+            kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, outlierSD=outlierSD)
+        fb, ll, betaConv, _ = _glm_fit(ysub, xd, sfs, dispersion, contrast, beta0, lam, betaTol=betaTol, maxit=maxit,
+                                       minmu=minmu, useOptim=useOptim, want_hat=False, want_mu=False)
+        sub = {"dispGeneEst": dge, "dispFit": dispFit, "dispMAP": dispMAP, "dispersion": dispersion,
+               "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": dispIter, **_wald_stats(fb),
+               "betaIter": fb["iter"], "betaConv": betaConv, "deviance": -2.0 * ll["logLike"]}
         for k, v in sub.items():
-            if k == "baseMean":
-                continue
             res[k] = res[k].clone()
             res[k][rr] = v.to(res[k].dtype)
         for k in ("betaMatrix", "betaSE", "WaldStatistic", "WaldPvalue", "deviance"):
@@ -1177,14 +1136,13 @@ def _dispersion_function(ynz, x, sizeFactors, nfz, fitType, minDisp=1e-8, kappa_
     m, p = x.shape
     linearMu = modelMatrixGroups(x) == p
     pr = prep(ynz, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu, normalizationFactors=nfz)
-    _, _, dge, _ = _gene_est(ynz, pr["xd"], pr["sfd"], pr["alpha0"], pr["beta0"], pr["mu_lin"], m, minDisp, kappa_0,
-                             dispTol, maxit, betaTol, minmu)
+    mu_glm = None if linearMu else _ws("mu_glm", tuple(ynz.shape), F64, ynz.device)
+    _, _, dge, _ = _gene_est(ynz, pr["xd"], pr["sfd"], pr["alpha0"], pr["beta0"], pr["mu_lin"], m, minDisp=minDisp,
+                             kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, betaTol=betaTol, minmu=minmu,
+                             mu_out=mu_glm)
     tr = _dispersion_trend(pr["baseMean"], dge, fitType, minDisp)
     if fitType == "mean":
         return {"fitType": "mean", "meanDisp": float(tr[0].item())}
-    status = tr[2].item()
-    if status != 0:
-        raise FloatingPointError(f"parametric dispersion fit failed on device (status {int(status)})")
     return {"fitType": "parametric", "trendCoefs": tr[:2].clone()}
 
 

@@ -48,7 +48,7 @@ def main():
         # objective calls at the first iteration's q / dispersions
         keep = d["counts"].sum(axis=1) > 0
         ynz = y[torch.as_tensor(np.flatnonzero(keep), device=dev)].contiguous()
-        q, disp, *_ = DP._dispersions_intercept_mean(ynz, m, np.ones(m), 1e-8, 1.0, 1e-6, 100, 0.5, 2.0)
+        q, disp, *_ = DP._dispersions_intercept_mean(ynz, m, np.ones(m))
         par = torch.zeros(m, dtype=torch.float64, device=dev)
         out = torch.empty(2 * m + 1, dtype=torch.float64, device=dev)
         for _ in range(3):

@@ -289,12 +289,14 @@ def test_device_pipeline_mean_matches_host(emu_dev, oracle, design):
 
 def test_device_pipeline_mean_with_replacement_and_iterate(emu_dev, oracle):
     from deseq2_b200 import synth
-    x = synth.design_condition(16)
-    d = synth.make_example_counts(240, 16, x=x, seed=33, betaSD=0.3)
-    counts = d["counts"].copy()
-    counts[[10, 20, 30, 40], [1, 2, 9, 12]] = 40 * counts[[10, 20, 30, 40]].max(axis=1) + 200
-    host, dv = _compare_mean(oracle, counts, x, "cpu", minReplicatesForReplace=7, sizeFactors=d["sizeFactors"])
-    assert dv["n_replaced"] == int(host["replace"].sum()) > 0
+    # batch x condition at 48 samples: 8 per cell, so every sample is replaceable, and the gene-wise mean of the refit
+    # comes from a GLM fit (fewer coefficients than design groups)
+    for x in (synth.design_batch_condition(48, 3), synth.design_condition(16)):
+        d = synth.make_example_counts(240, x.shape[0], x=x, seed=33, betaSD=0.3)
+        counts = d["counts"].copy()
+        counts[[10, 20, 30, 40], [1, 2, 9, 12]] = 40 * counts[[10, 20, 30, 40]].max(axis=1) + 200
+        host, dv = _compare_mean(oracle, counts, x, "cpu", minReplicatesForReplace=7, sizeFactors=d["sizeFactors"])
+        assert dv["n_replaced"] == int(host["replace"].sum()) > 0
     host, dv = _compare_mean(oracle, counts, x, "cpu", sfType="iterate")
     assert np.max(rel_err(dv["sizeFactors"], host["sizeFactors"])) < 1e-4
     assert dv["sfIterate"]["iterations"] == host["sfIterate"]["iterations"]
