@@ -60,6 +60,12 @@ SIGNATURES = {
     "b200nb_transform_dev": [vp, _I, vp, vp, _I, _I, _LL, _I, _D, _D, vp, _LL, vp],
     "b200nb_rlog_fit_dev": [vp, _I, vp, vp, vp, vp, _I, _I, _LL, _D, _D, _I, _D, vp, _LL, vp, vp, vp],
     "b200nb_rlog_prior_var_dev": [vp, _I, vp, vp, vp, vp, _I, _I, _LL, vp, vp],
+    "b200nb_results_gene_dev": [vp, _I, _I, _I, _LL, vp, vp, vp, vp, _I, vp, _I, _I, _D, vp, _D, vp, vp, vp, vp, vp,
+                                vp, vp, vp],
+    "b200nb_results_heuristic_dev": [vp, _I, vp, _I, _I, _LL, vp, _LL, vp, vp],
+    "b200nb_filter_cutoffs_dev": [vp, _I, vp, _I, vp, vp],
+    "b200nb_filter_numrej_dev": [vp, vp, _I, vp, _I, _I, _D, vp, vp],
+    "b200nb_padj_dev": [vp, vp, vp, _I, vp, _I, _I, vp, vp],
     "b200nb_last_error": [],
     "b200nb_device_count": [],
     "b200nb_kernel_launches": [],

@@ -1562,6 +1562,98 @@ int b200nb_rlog_prior_var_dev(const void* y, int y_type, const double* size_fact
   return 0;
 }
 
+static bool padj_method_ok(int method) { return method >= B200NB_PADJ_BH && method <= B200NB_PADJ_NONE; }
+
+int b200nb_results_gene_dev(const void* y, int y_type, int n, int m, long long ld, const double* lfc, const double* se,
+                            const double* stat, const double* pvalue, int negate, const int32_t* zero_mask, int lrt,
+                            int alt, double lfc_threshold, const double* max_cooks, double cooks_cutoff,
+                            const int32_t* keep, const int32_t* replace, const double* base_mean, double* out_lfc,
+                            double* out_se, double* out_stat, double* out_pvalue, void* stream) {
+  if (n < 0 || m < 1) return fail("results_gene: bad dimensions n=%d m=%d (n >= 0, m >= 1)", n, m);
+  if (ld < m) return fail("results_gene: ld=%lld must be >= m=%d", ld, m);
+  if (alt < B200NB_ALT_NONE || alt > B200NB_ALT_LESS) return fail("results_gene: unknown altHypothesis code %d", alt);
+  if (!(lfc_threshold >= 0.0 && lfc_threshold < HUGE_VAL))
+    return fail("results_gene: lfcThreshold=%g must be finite and >= 0", lfc_threshold);
+  if (!lfc || !se || !stat || !pvalue || !out_lfc || !out_se || !out_stat || !out_pvalue || (zero_mask && !y) ||
+      (replace && !base_mean))
+    return fail("results_gene: null pointer argument");
+  if (zero_mask && y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
+  if (n == 0) return 0;
+  if (check_device()) return 1;
+  nb::ResultsGeneArgs a{};
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.n = n; a.m = m; a.ld = ld;
+  a.lfc = lfc; a.se = se; a.stat = stat; a.pvalue = pvalue; a.negate = negate != 0; a.lrt = lrt != 0; a.alt = alt;
+  a.zero_mask = zero_mask; a.lfc_threshold = lfc_threshold; a.cooks_cutoff = cooks_cutoff; a.max_cooks = max_cooks;
+  a.keep = keep; a.replace = replace; a.base_mean = base_mean;
+  a.out_lfc = out_lfc; a.out_se = out_se; a.out_stat = out_stat; a.out_pvalue = out_pvalue;
+  CU(nb::launch_results_gene(a, (cudaStream_t)stream));
+  g_launches++;
+  return 0;
+}
+
+int b200nb_results_heuristic_dev(const void* y, int y_type, const int64_t* rows, int k, int m, long long ld,
+                                 const double* cooks, long long ld_cooks, int32_t* keep, void* stream) {
+  if (k < 0 || m < 1) return fail("results_heuristic: bad dimensions k=%d m=%d (k >= 0, m >= 1)", k, m);
+  if (ld < m || ld_cooks < m) return fail("results_heuristic: ld=%lld and ld_cooks=%lld must be >= m=%d", ld, ld_cooks, m);
+  if (!y || !rows || !cooks || !keep) return fail("results_heuristic: null pointer argument");
+  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
+  if (k == 0) return 0;
+  if (check_device()) return 1;
+  nb::ResultsHeuristicArgs a{};
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.rows = rows; a.k = k; a.m = m; a.ld = ld; a.ld_cooks = ld_cooks;
+  a.cooks = cooks; a.keep = keep;
+  CU(nb::launch_results_heuristic(a, (cudaStream_t)stream));
+  g_launches++;
+  return 0;
+}
+
+// one CTA per probability: the grid's x dimension bound kept well inside every launch limit
+constexpr int kMaxTheta = 65535;
+
+int b200nb_filter_cutoffs_dev(const double* filter, int n, const double* theta, int n_theta, double* out,
+                              void* stream) {
+  if (n < 1) return fail("filter_cutoffs: n=%d must be >= 1", n);
+  if (n_theta < 1 || n_theta > kMaxTheta) return fail("filter_cutoffs: n_theta=%d must be in [1, %d]", n_theta, kMaxTheta);
+  if (!filter || !theta || !out) return fail("filter_cutoffs: null pointer argument");
+  if (check_device()) return 1;
+  nb::FilterCutoffArgs a{};
+  a.filter = filter; a.n = n; a.theta = theta; a.out = out;
+  CU(nb::launch_filter_cutoffs(a, n_theta, (cudaStream_t)stream));
+  g_launches++;
+  return 0;
+}
+
+int b200nb_filter_numrej_dev(const double* p_sorted, const double* filter_sorted, int n, const double* cutoffs,
+                             int n_theta, int method, double alpha, int32_t* out_numrej, void* stream) {
+  if (n < 1) return fail("filter_numrej: n=%d must be >= 1", n);
+  if (n_theta < 1 || n_theta > kMaxTheta) return fail("filter_numrej: n_theta=%d must be in [1, %d]", n_theta, kMaxTheta);
+  if (!padj_method_ok(method)) return fail("filter_numrej: unknown p.adjust method code %d", method);
+  if (!(alpha > 0.0 && alpha < 1.0)) return fail("filter_numrej: alpha=%g must be in (0, 1)", alpha);
+  if (!p_sorted || !filter_sorted || !cutoffs || !out_numrej) return fail("filter_numrej: null pointer argument");
+  if (check_device()) return 1;
+  nb::PadjArgs a{};
+  a.p_sorted = p_sorted; a.filter_sorted = filter_sorted; a.n = n; a.cutoffs = cutoffs; a.method = method;
+  a.alpha = alpha; a.out_numrej = out_numrej;
+  CU(nb::launch_filter_numrej(a, n_theta, (cudaStream_t)stream));
+  g_launches++;
+  return 0;
+}
+
+int b200nb_padj_dev(const double* p_sorted, const double* filter_sorted, const int64_t* order, int n,
+                    const double* cutoffs, int j, int method, double* out, void* stream) {
+  if (n < 1) return fail("padj: n=%d must be >= 1", n);
+  if (j < 0) return fail("padj: j=%d must be >= 0", j);
+  if (!padj_method_ok(method)) return fail("padj: unknown p.adjust method code %d", method);
+  if (!p_sorted || !filter_sorted || !order || !out) return fail("padj: null pointer argument");
+  if (check_device()) return 1;
+  nb::PadjArgs a{};
+  a.p_sorted = p_sorted; a.filter_sorted = filter_sorted; a.order = order; a.n = n; a.cutoffs = cutoffs; a.j = j;
+  a.method = method; a.out = out;
+  CU(nb::launch_padj(a, (cudaStream_t)stream));
+  g_launches++;
+  return 0;
+}
+
 /* ------------------------------------------------------------------ host entry points */
 /* Each entry point runs at most twice: attempt 0 may launch on resident copies of its input matrices before their
  * content has been verified (CallInputs::validate, overlapped with the kernels); if a verification fails the launch

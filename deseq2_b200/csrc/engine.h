@@ -301,6 +301,58 @@ struct RlogPriorArgs {
 cudaError_t launch_rlog_prior_var(const RlogPriorArgs& a, cudaStream_t stream);
 size_t rlog_prior_scratch_bytes(int n, int m);
 
+// results() and pvalueAdjustment() (results.cuh, launched from size_factors.cu)
+struct ResultsGeneArgs {
+  const void* y;               // gene-major n x ld original counts (read only with zero_mask)
+  int y_is_f64;
+  int n, m;
+  long long ld;
+  const double *lfc, *se, *stat, *pvalue;   // the selected column, n each
+  int negate, lrt, alt;        // alt: B200NB_ALT_*
+  const int32_t* zero_mask;    // m flags of contrastAllZero's samples, or nullptr
+  double lfc_threshold, cooks_cutoff;
+  const double* max_cooks;     // n, or nullptr: no Cook's cutoff
+  const int32_t* keep;         // n, or nullptr: the two-group heuristic's kept genes
+  const int32_t* replace;      // n, or nullptr
+  const double* base_mean;     // n (with replace)
+  double *out_lfc, *out_se, *out_stat, *out_pvalue;
+};
+cudaError_t launch_results_gene(const ResultsGeneArgs& a, cudaStream_t stream);
+
+struct ResultsHeuristicArgs {
+  const void* y;
+  int y_is_f64;
+  const int64_t* rows;         // k gene rows of y
+  int k, m;
+  long long ld, ld_cooks;
+  const double* cooks;         // gene-major k x ld_cooks
+  int32_t* keep;               // indexed by gene row
+};
+cudaError_t launch_results_heuristic(const ResultsHeuristicArgs& a, cudaStream_t stream);
+
+struct FilterCutoffArgs {
+  const double* filter;        // n
+  int n;
+  const double* theta;         // one CTA per probability
+  double* out;
+};
+cudaError_t launch_filter_cutoffs(const FilterCutoffArgs& a, int n_theta, cudaStream_t stream);
+
+// the p-values in ascending order (NaN last) and their filter values; a subset is {i : p not NaN, filter >= cutoff}
+struct PadjArgs {
+  const double* p_sorted;
+  const double* filter_sorted;
+  const int64_t* order;        // padj: gene position of sorted position i
+  int n;
+  const double* cutoffs;       // numrej: one per CTA; padj: cutoffs[j], or nullptr for every non-NaN p
+  int j, method;               // method: B200NB_PADJ_*
+  double alpha;
+  int32_t* out_numrej;
+  double* out;
+};
+cudaError_t launch_filter_numrej(const PadjArgs& a, int n_theta, cudaStream_t stream);
+cudaError_t launch_padj(const PadjArgs& a, cudaStream_t stream);
+
 // Cook's distances (pipeline_kernels.cu)
 struct CooksArgs {
   const void* y;

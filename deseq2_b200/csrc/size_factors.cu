@@ -15,8 +15,9 @@
 // (beta_prior_quantile_kernel, beta_prior.cuh) and the trimmed sums of estimateSizeFactorsIterate's objective
 // (iterate_trim_sum_kernel, sf_iterate.cuh, whose per-gene kernel starts the same way); all start through
 // launch_per_column, as does the transform of the normalized counts (transform_kernel, transform.cuh: VST and
-// normTransform), one CTA per block of rows, and rlog's fit and prior variance (rlog.cuh: one CTA per block of genes;
-// a fixed grid of histogram CTAs and one picking CTA per refinement pass).
+// normTransform), one CTA per block of rows, rlog's fit and prior variance (rlog.cuh: one CTA per block of genes;
+// a fixed grid of histogram CTAs and one picking CTA per refinement pass), and results()' per-gene steps, filter
+// cutoffs, rejection counts and adjusted p-values (results.cuh: one warp per gene, one CTA per theta).
 #include "engine.h"
 #include "beta_prior.cuh"
 #include "nbmath.cuh"
@@ -167,6 +168,7 @@ __global__ void __launch_bounds__(512) sf_median_kernel(const double* __restrict
 #include "sf_iterate.cuh"
 #include "transform.cuh"
 #include "rlog.cuh"
+#include "results.cuh"
 
 namespace nb {
 namespace {
@@ -243,6 +245,32 @@ cudaError_t launch_rlog_prior_var(const RlogPriorArgs& a, cudaStream_t stream) {
     if (e != cudaSuccess) return e;
   }
   return cudaSuccess;
+}
+
+cudaError_t launch_results_gene(const ResultsGeneArgs& a, cudaStream_t stream) {
+  if (a.n == 0) return cudaSuccess;
+  constexpr int genes = kRsThreads / 32;
+  return launch_per_column(a.y_is_f64 ? results_gene_kernel<double> : results_gene_kernel<int32_t>,
+                           (int)(((long long)a.n + genes - 1) / genes), kRsThreads, stream, a);
+}
+
+cudaError_t launch_results_heuristic(const ResultsHeuristicArgs& a, cudaStream_t stream) {
+  if (a.k == 0) return cudaSuccess;
+  constexpr int genes = kRsThreads / 32;
+  return launch_per_column(a.y_is_f64 ? results_heuristic_kernel<double> : results_heuristic_kernel<int32_t>,
+                           (a.k + genes - 1) / genes, kRsThreads, stream, a);
+}
+
+cudaError_t launch_filter_cutoffs(const FilterCutoffArgs& a, int n_theta, cudaStream_t stream) {
+  return launch_per_column(filter_cutoff_kernel, n_theta, kRsScanThreads, stream, a);
+}
+
+cudaError_t launch_filter_numrej(const PadjArgs& a, int n_theta, cudaStream_t stream) {
+  return launch_per_column(filter_numrej_kernel, n_theta, kRsScanThreads, stream, a);
+}
+
+cudaError_t launch_padj(const PadjArgs& a, cudaStream_t stream) {
+  return launch_per_column(padj_kernel, 1, kRsScanThreads, stream, a);
 }
 
 }  // namespace nb

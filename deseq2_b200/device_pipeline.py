@@ -984,6 +984,16 @@ def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, dispFit_all,
                                "n_optim_map": n_optim}
 
 
+def _replacement_counts(ys, nfm, over, replaceable, m, trim=0.2):
+    """replaceOutliers' new counts (R/core.R:2069-2115) of the rows ys ((k, m) float64 counts, nfm their factors):
+    the outlying entries (`over`) of replaceable samples become as.integer(trimmed mean of K / nf * nf)."""
+    srt, _ = torch.sort(ys / nfm, dim=1)
+    lo = int(np.floor(m * trim))
+    tbm = srt[:, lo:m - lo].mean(dim=1)
+    replacement = torch.trunc(tbm[:, None] * nfm)
+    return torch.where(over & replaceable[None, :], replacement, ys)
+
+
 def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, minReplicates, minDisp=1e-8, kappa_0=1.0,
                        dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5, outlierSD=2.0, useOptim=True, trim=0.2):
     """replaceOutliers + refitWithoutOutliers (R/core.R:2069-2115, 2484-2565) on the device results `res` (in place).
@@ -1006,11 +1016,7 @@ def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, minReplicates,
         return
     ys = ynz[rows][:, :m].to(F64)
     nfm = sfd[rows][:, :m] if sfd.dim() == 2 else sfd[None, :]
-    srt, _ = torch.sort(ys / nfm, dim=1)
-    lo = int(np.floor(m * trim))
-    tbm = srt[:, lo:m - lo].mean(dim=1)
-    replacement = torch.trunc(tbm[:, None] * nfm)
-    new = torch.where(over[rows] & replaceable[None, :], replacement, ys)
+    new = _replacement_counts(ys, nfm, over[rows], replaceable, m, trim)
     res["baseMean"] = res["baseMean"].clone()
     res["baseMean"][rows] = (new / nfm).mean(dim=1)                 # getBaseMeansAndVariances on the new counts
     newAllZero = new.sum(dim=1) == 0
@@ -1384,3 +1390,225 @@ def rlog_device(y, m, x=None, blind=True, intercept=None, betaPriorVar=None, fit
     else:
         res["sizeFactors"] = sizeFactors
     return res
+
+
+# ---------------------------------------------------------------- results() and pvalueAdjustment() (R/results.R)
+
+_ALT_CODE = {"greaterAbs": 1, "greaterAbs2014": 2, "lessAbs": 3, "greater": 4, "less": 5}     # B200NB_ALT_*
+_PADJ_CODE = {"BH": 0, "fdr": 0, "BY": 1, "holm": 2, "hochberg": 3, "bonferroni": 4, "none": 5}   # B200NB_PADJ_*
+
+
+def filter_cutoffs(filter, theta):
+    """b200nb_filter_cutoffs_dev: quantile(filter, theta, type = 7) of a (N,) float64 device tensor at the (T,) device
+    probabilities, one CTA per probability.  Enqueue only."""
+    L = _lib.lib()
+    out = torch.empty(theta.numel(), dtype=F64, device=filter.device)
+    _lib.check(L.b200nb_filter_cutoffs_dev(_p(filter), filter.numel(), _p(theta), theta.numel(), _p(out), _stream()),
+               "filter_cutoffs_dev")
+    return out
+
+
+def filter_numrej(p_sorted, filter_sorted, cutoffs, method, alpha):
+    """b200nb_filter_numrej_dev: numRej of pvalueAdjustment for every cutoff, from the p-values sorted ascending (NaN
+    last) and their filter values.  Returns a (T,) int32 device tensor.  Enqueue only."""
+    L = _lib.lib()
+    out = torch.empty(cutoffs.numel(), dtype=torch.int32, device=p_sorted.device)
+    _lib.check(L.b200nb_filter_numrej_dev(_p(p_sorted), _p(filter_sorted), p_sorted.numel(), _p(cutoffs),
+                                          cutoffs.numel(), _PADJ_CODE[method], float(alpha), _p(out), _stream()),
+               "filter_numrej_dev")
+    return out
+
+
+def padj_column(p_sorted, filter_sorted, order, method, cutoffs=None, j=0):
+    """b200nb_padj_dev: p.adjust(method) over the genes with filter >= cutoffs[j] (cutoffs None: every gene with a
+    p-value), as a (N,) device tensor in gene order with NaN for the others.  Enqueue only."""
+    L = _lib.lib()
+    out = torch.empty(p_sorted.numel(), dtype=F64, device=p_sorted.device)
+    _lib.check(L.b200nb_padj_dev(_p(p_sorted), _p(filter_sorted), _p(order), p_sorted.numel(), _p(cutoffs), int(j),
+                                 _PADJ_CODE[method], _p(out), _stream()), "padj_dev")
+    return out
+
+
+def p_value_adjustment(pvalue, filter, independentFiltering=True, theta=None, alpha=0.1, pAdjustMethod="BH"):
+    """pvalueAdjustment (R/results.R:638-718) on (N,) float64 device tensors: the p-values sorted once (torch.sort,
+    plumbing), then the cutoff, rejection-count and adjusted-column kernels.  theta: numpy probabilities, or None for
+    seq(mean(filter == 0), .95 or 1, length = 50) formed on the device.  The one host read is numRej (with theta and the
+    cutoffs), which lowess needs.  Returns (padj (N,) device tensor, metadata)."""
+    from .pipeline import filter_choose, lowess
+    dev = pvalue.device
+    meta = {"alpha": alpha}
+    ps, order = torch.sort(pvalue)                          # NaN last
+    fs = filter[order].contiguous()
+    if not independentFiltering:
+        return padj_column(ps, fs, order, pAdjustMethod), meta
+    if theta is None:
+        # divisors as device tensors: a division by a Python scalar becomes a multiplication by its reciprocal on the
+        # GPU, which is not R's rounding
+        cst = lambda v: torch.tensor(v, dtype=F64, device=dev)
+        lo = (filter == 0).to(F64).sum() / cst(float(filter.numel()))
+        hi = torch.where(lo < 0.95, cst(0.95), cst(1.0))
+        th = lo + torch.arange(50, dtype=F64, device=dev) * ((hi - lo) / cst(49.0))
+        th[49] = hi
+    else:
+        th = torch.as_tensor(theta, dtype=F64, device=dev)
+    cutoffs = filter_cutoffs(filter, th)
+    numRej = filter_numrej(ps, fs, cutoffs, pAdjustMethod, alpha)
+    host = torch.stack([numRej.to(F64), th, cutoffs]).cpu().numpy()
+    nr, theta, cut = host[0].astype(np.int64), host[1], host[2]
+    lo_fit = lowess(theta, nr, f=1.0 / 5.0)
+    j = filter_choose(nr, lo_fit["y"])
+    meta.update(filterThreshold=float(cut[j]), filterTheta=float(theta[j]),
+                filterNumRej={"theta": theta, "numRej": nr}, lo_fit=lo_fit, j=j, cutoffs=cut)
+    return padj_column(ps, fs, order, pAdjustMethod, cutoffs, j), meta
+
+
+def results_gene(ynz, m, lfc, se, stat, pvalue, negate=False, zero_mask=None, lrt=False, alt=0, lfcThreshold=0.0,
+                 maxCooks=None, cooksCutoff=0.0, keep=None, replace=None, baseMean=None):
+    """b200nb_results_gene_dev: results()' per-gene steps for the n rows of ynz (gene-major counts, read for
+    zero_mask only): swapped reference, contrastAllZero, threshold test, Cook's cutoff, now-all-zero rows.  Returns
+    (log2FoldChange, lfcSE, stat, pvalue) as fresh (n,) device tensors.  Enqueue only."""
+    L = _lib.lib()
+    n, ld = ynz.shape
+    out = [torch.empty(n, dtype=F64, device=ynz.device) for _ in range(4)]
+    _lib.check(L.b200nb_results_gene_dev(_p(ynz), 1 if ynz.dtype == F64 else 0, n, m, ld, _p(lfc), _p(se), _p(stat),
+                                         _p(pvalue), int(negate), _p(zero_mask), int(lrt), int(alt),
+                                         float(lfcThreshold), _p(maxCooks), float(cooksCutoff), _p(keep),
+                                         _p(replace), _p(baseMean), *(_p(t) for t in out), _stream()),
+               "results_gene_dev")
+    return out
+
+
+def results_heuristic(ynz, m, rows, cooks_rows, keep):
+    """b200nb_results_heuristic_dev: keep[rows[r]] = (at least 3 counts of the gene are above the count at which.max of
+    its Cook's row cooks_rows[r]).  Enqueue only."""
+    L = _lib.lib()
+    n, ld = ynz.shape
+    _lib.check(L.b200nb_results_heuristic_dev(_p(ynz), 1 if ynz.dtype == F64 else 0, _p(rows), rows.numel(), m, ld,
+                                              _p(cooks_rows), cooks_rows.shape[1], _p(keep), _stream()),
+               "results_heuristic_dev")
+
+
+def _first_fit_cooks(res, ynz, rows, x, sfd):
+    """The Cook's rows of `rows` from the first fit's mu / H (res["mu"] / res["H"], DESeq_device's workspace views: R
+    restores the first fit's Cook's distances after a refit, R/core.R:2556).  Raises ValueError when a later
+    DESeq_device call has since replaced the workspace."""
+    mu_ws, h_ws = _WS.get(("mu_cooks", str(ynz.device))), _WS.get(("H", str(ynz.device)))
+    if (mu_ws is None or h_ws is None or res["mu"].data_ptr() != mu_ws.data_ptr()
+            or res["H"].data_ptr() != h_ws.data_ptr() or tuple(res["mu"].shape) != tuple(ynz.shape)):
+        raise ValueError("res['mu'] / res['H'] are views of DESeq_device's workspace and a later DESeq_device call has "
+                         "replaced it: run results_device before the next DESeq_device call")
+    nf = sfd[rows].contiguous() if sfd.dim() == 2 else None
+    return cooks(ynz[rows].contiguous(), res["mu"][rows].contiguous(), res["H"][rows].contiguous(), x,
+                 res.get("sizeFactors"), normalizationFactors=nf)["cooks"]
+
+
+def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcThreshold=0, altHypothesis="greaterAbs",
+                   cooksCutoff=None, independentFiltering=True, alpha=0.1, filter=None, theta=None,
+                   pAdjustMethod="BH", factors=None, lrt=None, minmu=0.5, weights=None, allgather=None):
+    """results() + pvalueAdjustment() (R/results.R:298-740) on a DESeq_device result `res` for the gene-major (N, ld)
+    counts y it was run on and its design x.  Arguments as pipeline.results (the host mirror): name / contrast /
+    listValues select the column (pipeline.resultsSelection; list and numeric contrasts, factor-level contrasts that
+    involve no reference level and every betaPrior contrast go through getContrast_device, on the replaced counts
+    after an outlier refit); factors: the design's level-code vectors; lrt: an nbinomLRT_device result for the same
+    rows and full design.  The per-gene steps are one kernel (results_gene), the adjustment p_value_adjustment.
+    res["mu"] / res["H"] are DESeq_device's workspace views, valid until the next DESeq_device call: the two-group
+    heuristic and the replaced counts of a contrast after an outlier refit recompute Cook's rows from them.
+    weights: the raw observation weights DESeq_device was given (gene-major (N, ld)); a weights result needs them for
+    the baseMean of its weightsFail rows (mean of w K / s, as getBaseMeansAndVariances), which count in the filter.
+    Host reads: at most two small ones -- the number of genes the Cook's cutoff flags (only for a single two-level
+    factor) and numRej with theta and the cutoffs (only with independent filtering).  A `filter` given as a device
+    tensor is read once to check it for NaN; getContrast_device reads once to check weights.
+    Returns {"baseMean", "log2FoldChange", "lfcSE", "stat", "pvalue", "padj"}: (N,) device tensors over all input
+    rows (all-zero rows: baseMean 0; all-zero and weightsFail rows: NaN in the other columns; both count in the
+    filter), and "metadata".
+    allgather (sharded_results_device): concatenates a list of per-gene vectors over the ranks in rank order (one
+    collective); [filter, pvalue] of this rank's rows travel in it, the cutoffs, counts and adjusted column are
+    computed on all genes, and this rank keeps the padj of its own rows (sharded.shard_bounds)."""
+    from scipy import stats as _st
+    from .pipeline import check_filter_args, results_checks, resultsSelection
+    dev = y.device
+    x = np.asarray(x, dtype=np.float64)
+    m, p = x.shape
+    N = y.shape[0]
+    idx = res["idx"]
+    betaPrior = res.get("modelMatrix") is not None
+    thresholded = results_checks(lfcThreshold, altHypothesis, lrt is not None, betaPrior, alpha)
+    filter, theta = check_filter_args(N, filter, theta, alpha, pAdjustMethod)
+    sel = resultsSelection(x, name, contrast, listValues, factors, betaPrior, res.get("modelMatrix"))
+    wf = res.get("weightsFail")
+    if wf is not None and weights is None:
+        raise ValueError("a DESeq_device result with observation weights needs weights= (the raw weights it was given) "
+                         "for the baseMean of its weightsFail rows")
+    whole = idx.numel() == N
+    ynz = y if whole else y[idx].contiguous()
+    nf = res.get("normalizationFactors")
+    sfd = nf if nf is not None else torch.as_tensor(res["sizeFactors"], device=dev)
+    replace = res.get("replace") if res.get("n_replaced", 0) > 0 else None
+    # ---- the selected column (cleanContrast / getCoef)
+    if sel["kind"] == "coef":
+        k = sel["col"]
+        cols = [res[key][:, k].contiguous() for key in ("betaMatrix", "betaSE", "WaldStatistic", "WaldPvalue")]
+    else:
+        xf = res["modelMatrix"] if betaPrior else x
+        ycnt = ynz
+        if replace is not None:                            # getContrast reads replaceCounts (R/results.R:776-780)
+            rows = torch.nonzero_static(replace, size=res["n_replaced"]).squeeze(1)   # the count is known: no read
+            cutoff = float(_st.f.ppf(0.99, p, m - p))
+            ck = _first_fit_cooks(res, ynz, rows, x, sfd)
+            ys = ynz[rows][:, :m].to(F64)
+            nfm = sfd[rows][:, :m] if sfd.dim() == 2 else sfd[None, :]
+            ycnt = ynz.to(F64).clone()
+            ycnt[rows, :m] = _replacement_counts(ys, nfm, ck[:, :m] > cutoff, res["replaceable"], m)
+        g = getContrast_device(ycnt, xf, None if nf is not None else res["sizeFactors"], res["dispersion"],
+                               res["betaMatrix"], sel["vec"], betaPriorVar=res.get("betaPriorVar"), minmu=minmu,
+                               weights=res.get("weights"), normalizationFactors=nf)
+        cols = [g[key].contiguous() for key in ("log2FoldChange", "lfcSE", "stat")]
+        # getContrast's 2 pnorm(|stat|, lower.tail = FALSE) (R/results.R:822) as erfc(|stat| / sqrt 2): torch's ndtr
+        # loses relative accuracy in the far tail on the CPU
+        cols.append(torch.erfc(cols[2].abs() * 0.7071067811865476))
+    if lrt is not None:
+        cols[2], cols[3] = lrt["LRTStatistic"].contiguous(), lrt["LRTPvalue"].contiguous()
+    mask = None if sel["mask"] is None else torch.as_tensor(sel["mask"].astype(np.int32), device=dev)
+    # ---- Cook's cutoff and the two-group heuristic
+    maxCooks, keep, cutoff = None, None, 0.0
+    if cooksCutoff is not False:
+        cutoff = float(_st.f.ppf(0.99, p, m - p)) if cooksCutoff is None or cooksCutoff is True else float(cooksCutoff)
+        maxCooks = res["maxCooks"].contiguous()
+        if factors is not None and len(factors) == 1 and int(np.max(factors[0])) == 1:
+            rows = torch.nonzero(maxCooks > cutoff).squeeze(1)
+            if rows.numel() > 0:
+                keep = torch.zeros(ynz.shape[0], dtype=torch.int32, device=dev)
+                results_heuristic(ynz, m, rows, _first_fit_cooks(res, ynz, rows, x, sfd), keep)
+    alt = _ALT_CODE[altHypothesis] if thresholded else 0
+    lfc, se, stat, pv = results_gene(ynz, m, *cols, negate=sel.get("negate", False), zero_mask=mask,
+                                     lrt=lrt is not None, alt=alt, lfcThreshold=lfcThreshold, maxCooks=maxCooks,
+                                     cooksCutoff=cutoff, keep=keep,
+                                     replace=None if replace is None else replace.to(torch.int32),
+                                     baseMean=res["baseMean"])
+    # ---- all N rows (buildDataFrameWithNARows), then pvalueAdjustment
+    out = {"baseMean": torch.zeros(N, dtype=F64, device=dev)}
+    out["baseMean"][idx] = res["baseMean"]
+    if wf is not None:                                  # the weightsFail rows keep their weighted baseMean
+        sf = torch.as_tensor(res["sizeFactors"], device=dev)
+        wbm = (weights[:, :m] * (y[:, :m].to(F64) / sf)).mean(dim=1)
+        out["baseMean"] = torch.where(wf, wbm, out["baseMean"])
+    for key, v in (("log2FoldChange", lfc), ("lfcSE", se), ("stat", stat), ("pvalue", pv)):
+        out[key] = torch.full((N,), float("nan"), dtype=F64, device=dev)
+        out[key][idx] = v
+    filt = out["baseMean"] if filter is None else torch.as_tensor(filter, device=dev)
+    if allgather is None:
+        out["padj"], meta = p_value_adjustment(out["pvalue"], filt, independentFiltering, theta, alpha,
+                                               pAdjustMethod)
+    else:
+        import torch.distributed as dist
+        from .sharded import shard_bounds
+        fa, pa = allgather([filt, out["pvalue"]])
+        lo, hi = shard_bounds(pa.numel(), dist.get_world_size(), dist.get_rank())
+        if hi - lo != N:
+            raise ValueError(f"this rank holds {N} rows where shard_bounds gives it {hi - lo}: split the rows as "
+                             "sharded.shard_bounds does")
+        padj, meta = p_value_adjustment(pa, fa, independentFiltering, theta, alpha, pAdjustMethod)
+        out["padj"] = padj[lo:hi]
+    meta["lfcThreshold"] = lfcThreshold
+    out["metadata"] = meta
+    return out

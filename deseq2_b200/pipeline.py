@@ -1373,3 +1373,488 @@ def rlog(counts, x=None, blind=True, intercept=None, betaPriorVar=None, fitType=
     res.update(extra)
     res.update(dispFit=np.asarray(dispFit, dtype=np.float64), sizeFactors=sizeFactors)
     return res
+
+
+# ---------------------------------------------------------------- results() and pvalueAdjustment() (R/results.R)
+
+P_ADJUST_METHODS = ("BH", "fdr", "BY", "holm", "hochberg", "bonferroni", "none")
+ALT_HYPOTHESES = ("greaterAbs", "lessAbs", "greater", "less", "greaterAbs2014")
+
+
+def quantile7(x, probs):
+    """quantile(x, probs, type = 7) (R's quantile.default): index = 1 + (n - 1) p, lo = floor(index); x[lo], replaced by
+    (1 - h) x[lo] + h x[hi] (h = index - lo, hi = ceiling(index)) only where index > lo and x[hi] != x[lo].  numpy's
+    default lerp is another formula.  x must not contain NaN (R stops)."""
+    x = np.sort(np.asarray(x, dtype=np.float64))
+    probs = np.atleast_1d(np.asarray(probs, dtype=np.float64))
+    n = len(x)
+    index = 1.0 + max(n - 1, 0) * probs
+    lo = np.floor(index)
+    hi = np.ceil(index)
+    qs = x[lo.astype(np.int64) - 1]
+    xhi = x[hi.astype(np.int64) - 1]
+    i = (index > lo) & (xhi != qs)
+    h = (index - lo)[i]
+    qs = qs.copy()
+    qs[i] = (1.0 - h) * qs[i] + h * xhi[i]
+    return qs
+
+
+def p_adjust(p, method="BH"):
+    """R's p.adjust(p, method) restated literally (stats/R/p.adjust.R).  NaN is NA: it stays NaN and does not count;
+    n = the number of non-NA p-values (the lazy default n = length(p) is forced after the NAs are dropped).  hommel is
+    not supported (ValueError)."""
+    if method == "fdr":
+        method = "BH"
+    if method not in ("BH", "BY", "holm", "hochberg", "bonferroni", "none"):
+        raise ValueError(f"p.adjust method {method!r} is not supported (BH/fdr, BY, holm, hochberg, bonferroni, none)")
+    p0 = np.array(p, dtype=np.float64)
+    nna = ~np.isnan(p0)
+    p = p0[nna]
+    lp = len(p)
+    n = lp
+    if n <= 1:
+        return p0
+    with np.errstate(over="ignore"):
+        if method == "bonferroni":
+            v = np.minimum(1.0, n * p)
+        elif method == "holm":
+            i = np.arange(1, lp + 1)
+            o = np.argsort(p, kind="stable")
+            v = np.empty(lp)
+            v[o] = np.minimum(1.0, np.maximum.accumulate((n - i + 1) * p[o]))
+        elif method in ("hochberg", "BH", "BY"):
+            i = np.arange(lp, 0, -1)
+            o = np.argsort(-p, kind="stable")                     # order(p, decreasing = TRUE)
+            if method == "hochberg":
+                t = (n + 1 - i) * p[o]
+            elif method == "BH":
+                t = n / i * p[o]
+            else:
+                q = float(np.sum(1.0 / np.arange(1, n + 1)))
+                t = q * n / i * p[o]
+            v = np.empty(lp)
+            v[o] = np.minimum(1.0, np.minimum.accumulate(t))
+        else:
+            v = p
+    p0[nna] = v
+    return p0
+
+
+def _lowest(x, y, n, xs, nleft, nright, w, userw, rw):
+    """clowess' local fit at xs from the points nleft..nright (1-based, ties on the right picked up); returns (ys, ok)."""
+    rng = x[n] - x[1]
+    h = max(xs - x[nleft], x[nright] - xs)
+    h9, h1 = 0.999 * h, 0.001 * h
+    a = 0.0
+    j = nleft
+    while j <= n:
+        w[j] = 0.0
+        r = abs(x[j] - xs)
+        if r <= h9:
+            w[j] = 1.0 if r <= h1 else (1.0 - (r / h) ** 3) ** 3
+            if userw:
+                w[j] *= rw[j]
+            a += w[j]
+        elif x[j] > xs:
+            break
+        j += 1
+    nrt = j - 1
+    if a <= 0.0:
+        return 0.0, False
+    for j in range(nleft, nrt + 1):
+        w[j] /= a
+    if h > 0.0:
+        a = 0.0
+        for j in range(nleft, nrt + 1):
+            a += w[j] * x[j]
+        b = xs - a
+        c = 0.0
+        for j in range(nleft, nrt + 1):
+            c += w[j] * (x[j] - a) * (x[j] - a)
+        if np.sqrt(c) > 0.001 * rng:
+            b /= c
+            for j in range(nleft, nrt + 1):
+                w[j] *= (b * (x[j] - a) + 1.0)
+    ys = 0.0
+    for j in range(nleft, nrt + 1):
+        ys += w[j] * y[j]
+    return ys, True
+
+
+def lowess(x, y, f=2.0 / 3.0, iter=3, delta=None):
+    """R's lowess(x, y, f, iter, delta = 0.01 * diff(range(x))): the points sorted by x, then clowess (Cleveland 1979,
+    R's src/library/stats/src/lowess.c) restated: tricube-weighted local linear fits over the ns = max(2, min(n,
+    floor(f n + 1e-7))) nearest points, points within delta of the last fit interpolated, and `iter` robustness
+    passes with bisquare weights of the residuals over 6 MAD.  Returns {"x": sorted x, "y": fitted values}."""
+    x = np.asarray(x, dtype=np.float64)
+    y = np.asarray(y, dtype=np.float64)
+    o = np.argsort(x, kind="stable")
+    x, y = x[o], y[o]
+    n = len(x)
+    if delta is None:
+        delta = 0.01 * (x[-1] - x[0]) if n else 0.0
+    if n < 2:
+        return {"x": x, "y": y.copy()}
+    X = np.r_[0.0, x]                                           # 1-based, as the C code
+    Y = np.r_[0.0, y]
+    ys = np.zeros(n + 1)
+    rw = np.zeros(n + 1)
+    res = np.zeros(n + 1)
+    ns = max(2, min(n, int(f * n + 1e-7)))
+    it = 1
+    while it <= iter + 1:
+        nleft, nright, last, i = 1, ns, 0, 1
+        while True:
+            if nright < n:
+                d1 = X[i] - X[nleft]
+                d2 = X[nright + 1] - X[i]
+                if d1 > d2:
+                    nleft += 1
+                    nright += 1
+                    continue
+            v, ok = _lowest(X, Y, n, X[i], nleft, nright, res, it > 1, rw)
+            ys[i] = v if ok else Y[i]
+            if last < i - 1:
+                denom = X[i] - X[last]
+                for j in range(last + 1, i):
+                    alpha = (X[j] - X[last]) / denom
+                    ys[j] = alpha * ys[i] + (1.0 - alpha) * ys[last]
+            last = i
+            cut = X[last] + delta
+            i = last + 1
+            while i <= n:
+                if X[i] > cut:
+                    break
+                if X[i] == X[last]:
+                    ys[i] = ys[last]
+                    last = i
+                i += 1
+            i = max(last + 1, i - 1)
+            if last >= n:
+                break
+        res[1:] = Y[1:] - ys[1:]
+        sc = float(np.sum(np.abs(res[1:]))) / n
+        if it > iter:
+            break
+        r = np.abs(res[1:])
+        s = np.sort(r)
+        m1 = n // 2
+        cmad = 3.0 * (s[m1] + s[n - m1 - 1]) if n % 2 == 0 else 6.0 * s[m1]
+        if cmad < 1e-7 * sc:
+            break
+        c9, c1 = 0.999 * cmad, 0.001 * cmad
+        with np.errstate(divide="ignore", invalid="ignore"):     # cmad = 0: every r <= c1, the quotient is unused
+            rw[1:] = np.where(r <= c1, 1.0, np.where(r <= c9, (1.0 - (r / cmad) ** 2) ** 2, 0.0))
+        it += 1
+    return {"x": x, "y": ys[1:].copy()}
+
+
+def filtered_p(filter, test, theta, method="none"):
+    """filtered_p (R/results.R:721-740) with a filter vector: the n x len(theta) matrix of p.adjust over the genes with
+    filter >= quantile(filter, theta[i]) (NA elsewhere)."""
+    filter = np.asarray(filter, dtype=np.float64)
+    test = np.asarray(test, dtype=np.float64)
+    cutoffs = quantile7(filter, theta)
+    result = np.full((len(filter), len(cutoffs)), np.nan)
+    for i, c in enumerate(cutoffs):
+        use = filter >= c
+        if use.any():
+            result[use, i] = p_adjust(test[use], method)
+    return result
+
+
+def filter_default_theta(filter):
+    """pvalueAdjustment's default theta: seq(mean(filter == 0), .95 or 1, length = 50), R's seq.default: the end
+    points exact, the interior lo + k * ((hi - lo) / 49)."""
+    lo = float(np.mean(np.asarray(filter) == 0))
+    hi = 0.95 if lo < 0.95 else 1.0
+    by = (hi - lo) / 49.0
+    theta = lo + np.arange(50) * by
+    theta[-1] = hi
+    return theta
+
+
+def filter_choose(numRej, fit_y):
+    """pvalueAdjustment's choice of the theta index j (R/results.R:662-692), 0-based."""
+    numRej = np.asarray(numRej, dtype=np.float64)
+    if np.max(numRej) <= 10:
+        return 0
+    residual = 0.0 if np.all(numRej == 0) else numRej[numRej > 0] - fit_y[numRej > 0]
+    maxFit = np.max(fit_y)
+    rmse = np.sqrt(np.mean(np.asarray(residual) ** 2))
+    thresh = maxFit - rmse
+    for cond in (numRej > thresh, numRej > 0.9 * maxFit, numRej > 0.8 * maxFit):
+        if cond.any():
+            return int(np.flatnonzero(cond)[0])
+    return 0
+
+
+def check_filter_args(N, filter, theta, alpha, pAdjustMethod):
+    """pvalueAdjustment's stops and this restatement's limits, shared by the host mirror and the device path.  Returns
+    (filter as float64 numpy or None, theta as float64 numpy or None)."""
+    if not (0.0 < alpha < 1.0):
+        raise ValueError("alpha must be in (0, 1)")
+    if pAdjustMethod not in P_ADJUST_METHODS:
+        raise ValueError(f"pAdjustMethod {pAdjustMethod!r} is not supported (hommel and others are out of scope): "
+                         f"use one of {', '.join(P_ADJUST_METHODS)}")
+    if callable(filter):
+        raise ValueError("a filter function is not supported: pass the filter values")
+    if filter is not None:
+        filter = np.asarray(filter.cpu() if hasattr(filter, "cpu") else filter, dtype=np.float64).reshape(-1)
+        if len(filter) != N:
+            raise ValueError(f"filter must have one value per row ({N}), got {len(filter)}")
+        if np.isnan(filter).any():
+            raise ValueError("missing values are not allowed in the filter")
+    if theta is not None:
+        theta = np.asarray(theta, dtype=np.float64).reshape(-1)
+        if len(theta) < 2:
+            raise ValueError("theta must have length > 1")
+        if not np.all((theta >= 0) & (theta <= 1)):
+            raise ValueError("theta must be probabilities in [0, 1]")
+    return filter, theta
+
+
+def pvalueAdjustment(pvalue, baseMean, independentFiltering=True, filter=None, theta=None, alpha=0.1,
+                     pAdjustMethod="BH"):
+    """pvalueAdjustment (R/results.R:638-718): returns (padj, metadata)."""
+    N = len(pvalue)
+    filter, theta = check_filter_args(N, filter, theta, alpha, pAdjustMethod)
+    meta = {"alpha": alpha}
+    if not independentFiltering:
+        return p_adjust(pvalue, pAdjustMethod), meta
+    if filter is None:
+        filter = np.asarray(baseMean, dtype=np.float64)
+    if theta is None:
+        theta = filter_default_theta(filter)
+    filtPadj = filtered_p(filter, pvalue, theta, pAdjustMethod)
+    numRej = np.sum(filtPadj < alpha, axis=0)
+    lo_fit = lowess(theta, numRej, f=1.0 / 5.0)
+    j = filter_choose(numRej, lo_fit["y"])
+    cutoffs = quantile7(filter, theta)
+    meta.update(filterThreshold=float(cutoffs[j]), filterTheta=float(theta[j]), filterNumRej={"theta": theta,
+                "numRej": numRej.astype(np.int64)}, lo_fit=lo_fit, j=j, cutoffs=cutoffs)
+    return filtPadj[:, j].copy(), meta
+
+
+def _column_names(x, factors, expanded):
+    if factors is None:
+        return None
+    return factorDesign(factors, expanded=expanded)[1]
+
+
+def _col_index(name, names, p):
+    if isinstance(name, (bool, np.bool_)) or not isinstance(name, (int, np.integer, str)):
+        raise ValueError("the argument 'name' should be a column index or one column name")
+    if isinstance(name, str):
+        if names is None or name not in names:
+            raise ValueError(f"name {name!r} is not a column of the model matrix")
+        return names.index(name)
+    if not 0 <= int(name) < p:
+        raise ValueError(f"column index {name} out of range (p = {p})")
+    return int(name)
+
+
+def resultsSelection(x, name=None, contrast=None, listValues=(1, -1), factors=None, betaPrior=False,
+                     modelMatrix=None):
+    """cleanContrast / getCoef (R/results.R:389-463, 832-1040): which column results() reports.  Returns a dict:
+    {"kind": "coef", "col": k, "negate": bool} (a coefficient of the fitted matrix, negated when the numerator is the
+    reference level) or {"kind": "contrast", "vec": numeric contrast over the fitted matrix's columns}, each with
+    "mask": the samples of contrastAllZero (a bool (m,) array) or None.  Contrasts: `(k, num, den)` (a tuple of three
+    ints: factor k of `factors`, numerator and denominator level codes), a list `[numerator names, denominator names]`
+    (column names of factorDesign, weighted by listValues), or a numeric vector.  With betaPrior the fitted matrix is
+    `modelMatrix` (the expanded one) and, without name and contrast, the default is the last factor's last level vs its
+    first."""
+    x = np.asarray(x, dtype=np.float64)
+    xf = np.asarray(modelMatrix, dtype=np.float64) if betaPrior else x
+    p = xf.shape[1]
+    names = _column_names(x, factors, betaPrior)
+    lv = np.asarray(listValues, dtype=np.float64)
+    if lv.shape != (2,) or not (lv[0] > 0 and lv[1] < 0):
+        raise ValueError("listValues must be two numbers, the first positive and the second negative")
+    if betaPrior and contrast is None and name is None:
+        f = np.asarray(factors[-1])
+        contrast = (len(factors) - 1, int(f.max()), 0)
+    if contrast is None:
+        k = p - 1 if name is None else _col_index(name, names, p)
+        return {"kind": "coef", "col": k, "negate": False, "mask": None}
+    if isinstance(contrast, tuple) and len(contrast) == 3 and all(isinstance(v, (int, np.integer)) for v in contrast):
+        if factors is None:
+            raise ValueError("a factor-level contrast needs the design factors (factors=...)")
+        k, num, den = (int(v) for v in contrast)
+        if not 0 <= k < len(factors):
+            raise ValueError(f"{k} should be the index of a factor of the design")
+        f = np.asarray(factors[k])
+        nlev = int(f.max()) + 1
+        if num == den:
+            raise ValueError(f"{num} and {den} should be different level names")
+        if not (0 <= num < nlev and 0 <= den < nlev):
+            raise ValueError(f"{num} and {den} should be levels of factor {k}")
+        mask = np.isin(f, (num, den))
+        _, _, fidx, lvl = factorDesign(factors, expanded=betaPrior)
+        col = {int(l): c for c, (fi, l) in enumerate(zip(fidx, lvl)) if fi == k}
+        if not betaPrior and den == 0:
+            return {"kind": "coef", "col": col[num], "negate": False, "mask": mask}
+        if not betaPrior and num == 0:
+            return {"kind": "coef", "col": col[den], "negate": True, "mask": mask}
+        vec = np.zeros(p)
+        vec[col[num]] = 1.0
+        vec[col[den]] = -1.0
+        return {"kind": "contrast", "vec": vec, "mask": mask}
+    if isinstance(contrast, list):
+        if len(contrast) == 1:
+            contrast = [contrast[0], []]
+        if len(contrast) != 2:
+            raise ValueError("'contrast', as a list, should have length 2, or, if length 1, an empty vector will be "
+                             "added for the second element")
+        num, den = ([v] if isinstance(v, str) else list(v) for v in contrast)
+        if not all(isinstance(v, str) for v in num + den):
+            raise ValueError("'contrast', as a list of length 2, should have column names as elements")
+        if names is None or not all(v in names for v in num + den):
+            raise ValueError("all elements of the contrast as a list of length 2 should be column names of the model "
+                             "matrix")
+        if set(num) & set(den):
+            raise ValueError("elements in the contrast list should only appear in the numerator or the denominator, "
+                             "but not both")
+        if not num + den:
+            raise ValueError("one of the two elements in the list should be a character vector of non-zero length")
+        vec = np.zeros(p)
+        vec[[names.index(v) for v in num]] = lv[0]
+        vec[[names.index(v) for v in den]] = lv[1]
+    else:
+        if isinstance(contrast, (bool, np.bool_, str)) or isinstance(contrast, tuple):
+            raise ValueError("'contrast' should be a (factor, numerator level, denominator level) tuple, a list of "
+                             "two lists of column names, or a numeric vector")
+        vec = np.asarray(contrast, dtype=np.float64).reshape(-1)
+        if len(vec) != p:
+            raise ValueError("numeric contrast vector should have one element for every column of the model matrix")
+        if np.all(vec == 0):
+            raise ValueError("numeric contrast vector cannot have all elements equal to 0")
+    mask = None
+    if not (np.all(vec >= 0) or np.all(vec <= 0)):          # contrastAllZeroNumeric (R/results.R:1248-1270)
+        mask = (xf @ (vec != 0).astype(np.float64)) != 0
+    return {"kind": "contrast", "vec": vec, "mask": mask}
+
+
+def results_checks(lfcThreshold, altHypothesis, lrt, betaPrior, alpha, useT=False):
+    """results()' stops (R/results.R:318-345, 465-470) and this restatement's limits."""
+    if useT:
+        raise ValueError("useT is not supported (there are no t degrees of freedom)")
+    if altHypothesis not in ALT_HYPOTHESES:
+        raise ValueError(f"altHypothesis must be one of {', '.join(ALT_HYPOTHESES)}")
+    if not (np.isfinite(lfcThreshold) and lfcThreshold >= 0):
+        raise ValueError("lfcThreshold must be finite and >= 0")
+    if not (0.0 < alpha < 1.0):
+        raise ValueError("alpha must be in (0, 1)")
+    if lfcThreshold == 0 and altHypothesis == "lessAbs":
+        raise ValueError("when testing altHypothesis='lessAbs', set the argument lfcThreshold to a positive value")
+    thresholded = not (lfcThreshold == 0 and altHypothesis == "greaterAbs")
+    if thresholded and lrt:
+        raise ValueError("tests of log fold change above or below a theshold must be Wald tests")
+    if thresholded and altHypothesis == "lessAbs" and betaPrior:
+        raise ValueError("testing altHypothesis='lessAbs' requires setting the DESeq() argument betaPrior=FALSE")
+    return thresholded
+
+
+def r_pnorm_upper(q):
+    """pnorm(q, lower.tail = FALSE)."""
+    from scipy import stats as _st
+    return _st.norm.sf(q)
+
+
+def thresholdTest(LFC, SE, T, altHypothesis):
+    """results()' lfcThreshold / altHypothesis step (R/results.R:464-518, pnorm; pnorm(q, sd = se) = pnorm(q / se)).
+    Returns (stat, pvalue)."""
+    from scipy import stats as _st
+    up = r_pnorm_upper
+    with np.errstate(divide="ignore", invalid="ignore"):
+        if altHypothesis == "greaterAbs":
+            return LFC / SE, _st.norm.cdf((-np.abs(LFC) + T) / SE) + _st.norm.cdf((-np.abs(LFC) - T) / SE)
+        if altHypothesis == "greaterAbs2014":
+            q = (np.abs(LFC) - T) / SE
+            return np.sign(LFC) * np.maximum(q, 0), np.minimum(1.0, 2.0 * up(q))
+        if altHypothesis == "lessAbs":
+            qa, qb = (T - LFC) / SE, (LFC + T) / SE
+            return np.minimum(np.maximum(qa, 0), np.maximum(qb, 0)), np.maximum(up(qa), up(qb))
+        if altHypothesis == "greater":
+            q = (LFC - T) / SE
+            return np.maximum(q, 0), up(q)
+        return np.minimum((LFC + T) / SE, 0), up((-T - LFC) / SE)
+
+
+def results(dds, counts, x, name=None, contrast=None, listValues=(1, -1), lfcThreshold=0.0,
+            altHypothesis="greaterAbs", cooksCutoff=None, independentFiltering=True, alpha=0.1, filter=None, theta=None,
+            pAdjustMethod="BH", factors=None, lrt=None, minmu=0.5, cooks=None, engine=None, useT=False):
+    """results() + pvalueAdjustment() (R/results.R:298-740) on a pipeline.DESeq result `dds` (per-gene arrays over all
+    N rows, NaN for all-zero rows) for the (N, m) counts it was run on and its design x.  Arguments as R's (see
+    resultsSelection for name / contrast / listValues); factors: the design's level-code vectors (names, factor-level
+    contrasts, betaPrior results, the two-group Cook's heuristic); lrt: a nbinomLRT result (full-length LRTStatistic /
+    LRTPvalue) whose stat and p replace the Wald ones; cooks: the (N, m) Cook's distances of the first fit, needed by
+    the two-group heuristic (a single factor with two levels) when a gene is flagged.  Returns {"baseMean",
+    "log2FoldChange", "lfcSE", "stat", "pvalue", "padj"} over all N rows, and "metadata" (filterThreshold,
+    filterTheta, filterNumRej, lo_fit, alpha, lfcThreshold, the cutoffs and the chosen index j)."""
+    from scipy import stats as _st
+    engine = engine or _default_engine
+    counts = np.asarray(counts)
+    N, m = counts.shape
+    x = np.asarray(x, dtype=np.float64)
+    p = x.shape[1]
+    betaPrior = "betaPriorVar" in dds and dds.get("modelMatrix") is not None
+    thresholded = results_checks(lfcThreshold, altHypothesis, lrt is not None, betaPrior, alpha, useT)
+    check_filter_args(N, filter, theta, alpha, pAdjustMethod)
+    sel = resultsSelection(x, name, contrast, listValues, factors, betaPrior, dds.get("modelMatrix"))
+    nz = ~np.asarray(dds["allZero"], bool)
+    if "weightsFail" in dds:
+        nz = nz & ~np.asarray(dds["weightsFail"], bool)
+    if sel["kind"] == "coef":
+        k = sel["col"]
+        lfc, se = dds["betaMatrix"][:, k].copy(), dds["betaSE"][:, k].copy()
+        stat, pv = dds["WaldStatistic"][:, k].copy(), dds["WaldPvalue"][:, k].copy()
+        if sel["negate"]:
+            lfc = -lfc
+            stat = -stat
+    else:
+        xf = dds["modelMatrix"] if betaPrior else x
+        cts = dds["replaceCounts"] if "replaceCounts" in dds else counts
+        if dds.get("normalizationFactors") is not None:
+            nf = np.asarray(dds["normalizationFactors"])[nz]
+        else:
+            nf = np.broadcast_to(dds["sizeFactors"], (int(nz.sum()), m))
+        g = getContrast(cts[nz], nf, xf, dds["dispersion"][nz], dds["betaMatrix"][nz], sel["vec"],
+                        betaPriorVar=dds.get("betaPriorVar"), engine=engine, minmu=minmu, weights=dds.get("weights"))
+        lfc, se, stat, pv = (np.full(N, np.nan) for _ in range(4))
+        lfc[nz], se[nz], stat[nz], pv[nz] = g["log2FoldChange"], g["lfcSE"], g["stat"], g["pvalue"]
+    if sel["mask"] is not None:
+        az = nz & (counts[:, sel["mask"]].sum(axis=1) == 0)
+        lfc[az] = 0.0
+        stat[az] = 0.0
+        pv[az] = 1.0
+    if lrt is not None:
+        stat = np.asarray(lrt["LRTStatistic"], dtype=np.float64).copy()
+        pv = np.asarray(lrt["LRTPvalue"], dtype=np.float64).copy()
+    if thresholded:
+        stat, pv = thresholdTest(lfc, se, lfcThreshold, altHypothesis)
+    if cooksCutoff is None or cooksCutoff is True:
+        cooksCutoff = float(_st.f.ppf(0.99, p, m - p))              # the dispersion design's p and m
+    if cooksCutoff is not False:
+        with np.errstate(invalid="ignore"):
+            out = dds["maxCooks"] > float(cooksCutoff)
+        if out.any() and factors is not None and len(factors) == 1 and int(np.max(factors[0])) == 1:
+            if cooks is None:
+                raise ValueError("the two-group Cook's heuristic needs the Cook's distances (cooks=...)")
+            for ii in np.flatnonzero(out):
+                row = np.asarray(cooks[ii], dtype=np.float64)
+                if np.all(np.isnan(row)):
+                    continue
+                outCount = counts[ii, int(np.nanargmax(row))]
+                if np.sum(counts[ii] > outCount) >= 3:
+                    out[ii] = False
+        pv[out] = np.nan
+    if "replace" in dds and np.nansum(dds["replace"]) > 0:
+        nowZero = np.asarray(dds["replace"], bool) & (dds["baseMean"] == 0)
+        lfc[nowZero] = se[nowZero] = stat[nowZero] = 0.0
+        pv[nowZero] = 1.0
+    padj, meta = pvalueAdjustment(pv, dds["baseMean"], independentFiltering, filter, theta, alpha, pAdjustMethod)
+    meta["lfcThreshold"] = lfcThreshold
+    return {"baseMean": np.asarray(dds["baseMean"], dtype=np.float64), "log2FoldChange": lfc, "lfcSE": se,
+            "stat": stat, "pvalue": pv, "padj": padj, "metadata": meta}

@@ -196,3 +196,16 @@ def sharded_nbinomLRT_device(y_local, x_full, x_reduced, sizeFactors, dispersion
     res["gathered"] = {"LRTStatistic": g[0], "LRTPvalue": g[1], "betaMatrix": torch.stack(g[2:2 + p], dim=1)}
     res["collectives"] = pg.collectives
     return res
+
+
+def sharded_results_device(res_local, y_local, x, **kw):
+    """results() on this rank's shard of a sharded_DESeq_device run (y_local: the shard's rows as shard_bounds splits
+    them; res_local: its result).  The per-gene steps stay local; ONE packed all-gather carries [filter, pvalue] of
+    every gene, and every rank runs the cutoff, rejection-count and adjusted-column kernels on all genes, then keeps
+    its own rows.  Keyword arguments as device_pipeline.results_device (a custom `filter` holds this shard's rows);
+    returns its dict for the shard, whose metadata is that of all genes, plus "collectives"."""
+    from . import device_pipeline as DP
+    pg = PackedGather(y_local.shape[0], y_local.device)
+    out = DP.results_device(res_local, y_local, x, allgather=pg, **kw)
+    out["collectives"] = pg.collectives
+    return out

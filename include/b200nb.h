@@ -41,6 +41,20 @@ extern "C" {
 #define B200NB_TRANSFORM_VST_PARAMETRIC 0
 #define B200NB_TRANSFORM_VST_MEAN 1
 #define B200NB_TRANSFORM_LOG2 2
+/* results(): altHypothesis (B200NB_ALT_NONE: lfcThreshold = 0 with "greaterAbs", the columns pass unchanged) */
+#define B200NB_ALT_NONE 0
+#define B200NB_ALT_GREATER_ABS 1
+#define B200NB_ALT_GREATER_ABS_2014 2
+#define B200NB_ALT_LESS_ABS 3
+#define B200NB_ALT_GREATER 4
+#define B200NB_ALT_LESS 5
+/* p.adjust methods ("fdr" is BH) */
+#define B200NB_PADJ_BH 0
+#define B200NB_PADJ_BY 1
+#define B200NB_PADJ_HOLM 2
+#define B200NB_PADJ_HOCHBERG 3
+#define B200NB_PADJ_BONFERRONI 4
+#define B200NB_PADJ_NONE 5
 
 /* ---- fitDisp: src/DESeq2.cpp:164.  Outputs = list members at :268-276 (length n each). */
 int b200nb_fit_disp(const void* y, int y_type, const double* x, const double* mu_hat, const double* log_alpha,
@@ -260,6 +274,53 @@ int b200nb_rlog_fit_dev(const void* y, int y_type, const double* size_factors, c
 int b200nb_rlog_prior_var_dev(const void* y, int y_type, const double* size_factors, const double* nf,
                               const double* base_mean, const double* disp_fit, int n, int m, long long ld,
                               double* out_var, void* stream);
+
+/* b200nb_results_gene_dev: results()' per-gene steps (R/results.R:298-575) for n genes, in R's order, from the selected
+ * column lfc, se, stat, pvalue (n each):
+ *   negate != 0 (the numerator is the reference level): LFC negated, and stat too unless lrt != 0;
+ *   zero_mask (m int32 flags, or NULL): contrastAllZero -- when the counts of y (gene-major n x ld, int32 or f64: the
+ *     original counts) at the flagged samples are all zero, LFC = 0 and, unless lrt != 0, stat = 0 and p = 1;
+ *   alt (B200NB_ALT_*) with lfc_threshold T >= 0: the thresholded stat and p (pnorm);
+ *   max_cooks (n, or NULL: no Cook's cutoff): p = NaN where max_cooks > cooks_cutoff, unless keep (n int32, or NULL)
+ *     is non-zero there;
+ *   replace (n int32, or NULL) with base_mean (n): where replace != 0 and base_mean == 0, LFC, SE, stat = 0, p = 1.
+ * Writes out_lfc, out_se, out_stat, out_pvalue (n each; may alias the inputs).  Needs n >= 0, m >= 1, ld >= m, a known
+ * alt, finite T >= 0, and no NULL pointer among the column inputs and outputs (y with zero_mask, base_mean with
+ * replace).  Enqueue only. */
+int b200nb_results_gene_dev(const void* y, int y_type, int n, int m, long long ld, const double* lfc, const double* se,
+                            const double* stat, const double* pvalue, int negate, const int32_t* zero_mask, int lrt,
+                            int alt, double lfc_threshold, const double* max_cooks, double cooks_cutoff,
+                            const int32_t* keep, const int32_t* replace, const double* base_mean, double* out_lfc,
+                            double* out_se, double* out_stat, double* out_pvalue, void* stream);
+
+/* b200nb_results_heuristic_dev: results()' two-group Cook's heuristic (R/results.R:538-556) for k flagged genes:
+ * rows (k gene indices into y, gene-major n x ld counts), cooks (gene-major k x ld_cooks: row r holds the Cook's
+ * distances of gene rows[r]).  outCount = y[rows[r], which.max(cooks row)] (first maximum, NaN skipped);
+ * keep[rows[r]] = (at least 3 counts of the gene are > outCount).  Other entries of keep are not written.  Needs
+ * k >= 0, m >= 1, ld >= m, ld_cooks >= m and no NULL pointer.  Enqueue only. */
+int b200nb_results_heuristic_dev(const void* y, int y_type, const int64_t* rows, int k, int m, long long ld,
+                                 const double* cooks, long long ld_cooks, int32_t* keep, void* stream);
+
+/* b200nb_filter_cutoffs_dev: quantile(filter, theta, type = 7) (R/results.R:725) of the n filter values (none NaN) at
+ * n_theta probabilities in [0, 1], one CTA per probability by radix select.  Needs n >= 1, 1 <= n_theta <= 65535 and
+ * no NULL pointer.  Enqueue only. */
+int b200nb_filter_cutoffs_dev(const double* filter, int n, const double* theta, int n_theta, double* out,
+                              void* stream);
+
+/* b200nb_filter_numrej_dev: numRej of pvalueAdjustment (R/results.R:652): for every cutoff c_t (n_theta of them) the
+ * number of genes with filter >= c_t whose p.adjust(method) over that subset is < alpha.  p_sorted: the n p-values in
+ * ascending order, NaN last (NaN never belongs to a subset); filter_sorted: their filter values.  out_numrej: n_theta
+ * int32.  Needs n >= 1, 1 <= n_theta <= 65535, a known method, 0 < alpha < 1 and no NULL pointer.  Enqueue only. */
+int b200nb_filter_numrej_dev(const double* p_sorted, const double* filter_sorted, int n, const double* cutoffs,
+                             int n_theta, int method, double alpha, int32_t* out_numrej, void* stream);
+
+/* b200nb_padj_dev: the adjusted p-values of one subset: p.adjust(method) over the genes with filter >= cutoffs[j]
+ * (cutoffs == NULL: every gene with a p-value), written to out[order[i]] for the gene at sorted position i; the
+ * others get NaN.  p_sorted, filter_sorted as for b200nb_filter_numrej_dev; order: the n gene positions (0 <= order[i]
+ * < n_out, each once).  Needs n >= 1, j >= 0, a known method and no NULL pointer among p_sorted, filter_sorted,
+ * order, out.  Enqueue only. */
+int b200nb_padj_dev(const double* p_sorted, const double* filter_sorted, const int64_t* order, int n,
+                    const double* cutoffs, int j, int method, double* out, void* stream);
 
 /* ---- housekeeping */
 const char* b200nb_last_error(void);
