@@ -13,6 +13,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <initializer_list>
 #include <memory>
 #include <mutex>
 #include <thread>
@@ -942,12 +943,42 @@ int check_device() {
   return 0;
 }
 
+// Argument checks of the entry points: each returns 0, or 1 with the reason in g_err.  They touch no device, so a bad
+// argument is refused before any CUDA call; every entry point calls check_device() itself before its first launch.
 int check_dims(int n, int m, int p) {
   if (n < 0 || m < 1 || p < 1) return fail("bad dimensions n=%d m=%d p=%d", n, m, p);
   if (p > nb::kMaxP) return fail("p=%d not supported (max %d design columns)", p, nb::kMaxP);
-  if (n > 0 && check_device()) return 1;
   return 0;
 }
+
+// y_type is a known code (anything else would be read as int32), and y is given when there are rows to read
+int check_y(const char* what, const void* y, int y_type, long long n) {
+  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("%s: bad y_type %d", what, y_type);
+  if (n > 0 && !y) return fail("%s: y == NULL", what);
+  return 0;
+}
+
+// the row stride `name` of a gene-major matrix: >= m, and a multiple of 4 where the kernels read rows with 16-byte
+// vector loads (aligned)
+int check_ld(const char* what, const char* name, long long ld, int m, bool aligned) {
+  if (ld < m || (aligned && (ld & 3)))
+    return fail("%s: %s=%lld must be >= m=%d%s", what, name, ld, m, aligned ? " and a multiple of 4" : "");
+  return 0;
+}
+
+int check_factors(const char* what, const double* size_factors, const double* nf) {
+  if ((size_factors == nullptr) == (nf == nullptr)) return fail("%s: give exactly one of size_factors and nf", what);
+  return 0;
+}
+
+// the pointers a call with n > 0 rows of work reads or writes
+int check_ptrs(const char* what, long long n, std::initializer_list<const void*> ptrs) {
+  for (const void* q : ptrs)
+    if (n > 0 && !q) return fail("%s: null pointer argument", what);
+  return 0;
+}
+
+bool finite_pos(double v) { return v > 0.0 && v < HUGE_VAL; }
 
 // B200NB_HOST_TIMING=1: the host entry points print where their wall time goes (hashing + upload incl. layout
 // conversion / kernels / download) to stderr; it adds a stream synchronisation between the phases, so it is a
@@ -1104,9 +1135,12 @@ int b200nb_fit_disp_dev(const void* y, int y_type, const double* x, const double
                         double* out_log_alpha, int32_t* out_iter, int32_t* out_iter_accept,
                         double* out_last_change, double* out_initial_lp, double* out_initial_dlp,
                         double* out_last_lp, double* out_last_dlp, double* out_last_d2lp, void* stream) {
-  if (check_dims(n, m, p)) return 1;
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+  if (check_dims(n, m, p) || check_y("fit_disp", y, y_type, n) || check_ld("fit_disp", "ld", ld, m, true)) return 1;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
+  if (check_ptrs("fit_disp", n, {x, mu_hat, log_alpha, log_alpha_prior_mean, out_log_alpha, out_iter, out_iter_accept,
+                                 out_last_change, out_initial_lp, out_initial_dlp, out_last_lp, out_last_dlp,
+                                 out_last_d2lp}))
+    return 1;
   nb::DispArgs a{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.mu = mu_hat; a.w = use_weights ? weights : nullptr; a.x = x;
   a.log_alpha_in = log_alpha; a.prior_mean = log_alpha_prior_mean;
@@ -1117,7 +1151,7 @@ int b200nb_fit_disp_dev(const void* y, int y_type, const double* x, const double
   a.initial_lp = out_initial_lp; a.initial_dlp = out_initial_dlp; a.last_lp = out_last_lp; a.last_dlp = out_last_dlp;
   a.last_d2lp = out_last_d2lp; a.grid = nullptr; a.grid_n = 0;
   if (n == 0) return 0;
-  if (next_scratch(nb::disp_scratch_bytes(n), &a.scratch)) return 1;
+  if (check_device() || next_scratch(nb::disp_scratch_bytes(n), &a.scratch)) return 1;
   if (use_generic(p) || long_rows(m, use_weights)) {
     DesignDev dd;
     if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
@@ -1138,8 +1172,9 @@ int b200nb_fit_disp_grid_dev(const void* y, int y_type, const double* x, const d
                              double log_alpha_prior_sigmasq, int use_prior, const double* weights, int use_weights,
                              double weight_threshold, int use_cr, int n, int m, int p, long long ld,
                              double* out_log_alpha, void* stream) {
-  if (check_dims(n, m, p)) return 1;
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+  if (check_dims(n, m, p) || check_y("fit_disp_grid", y, y_type, n) || check_ld("fit_disp_grid", "ld", ld, m, true) ||
+      check_ptrs("fit_disp_grid", n, {x, mu_hat, disp_grid, log_alpha_prior_mean, out_log_alpha}))
+    return 1;
   if (disp_grid_n < 2) return fail("disp_grid needs at least 2 points");
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   nb::DispArgs a{};
@@ -1148,7 +1183,7 @@ int b200nb_fit_disp_grid_dev(const void* y, int y_type, const double* x, const d
   a.use_prior = use_prior; a.use_weights = use_weights; a.use_cr = use_cr; a.weight_threshold = weight_threshold;
   a.n = n; a.m = m; a.p = p; a.ld = ld; a.log_alpha = out_log_alpha; a.grid = disp_grid; a.grid_n = disp_grid_n;
   if (n == 0) return 0;
-  if (next_scratch(nb::disp_scratch_bytes(n), &a.scratch)) return 1;
+  if (check_device() || next_scratch(nb::disp_scratch_bytes(n), &a.scratch)) return 1;
   if (use_generic(p)) {
     DesignDev dd;
     if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
@@ -1169,12 +1204,14 @@ int b200nb_fit_beta_dev(const void* y, int y_type, const double* x, const double
                         double* out_beta_var_mat, double* out_iter, double* out_hat_diagonals,
                         double* out_contrast_num, double* out_contrast_denom, double* out_deviance, double* out_mu,
                         void* stream) {
-  if (check_dims(n, m, p)) return 1;
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+  if (check_dims(n, m, p) || check_y("fit_beta", y, y_type, n) || check_ld("fit_beta", "ld", ld, m, true)) return 1;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   if (maxit < 0) return fail("maxit must be >= 0");
   unsigned int* ctr;
-  if (next_counter(&ctr)) return 1;
+  if (check_ptrs("fit_beta", n, {x, nf, alpha_hat, contrast, beta_mat, lambda, out_beta_mat, out_beta_var_mat, out_iter,
+                                 out_contrast_num, out_contrast_denom, out_deviance}) ||
+      (n > 0 && check_device()) || next_counter(&ctr))
+    return 1;
   nb::BetaArgs a{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.nf = nf; a.nf_is_vector = nf_is_vector;
   a.w = use_weights ? weights : nullptr; a.x = x; a.alpha_hat = alpha_hat; a.contrast = contrast; a.beta_in = beta_mat;
@@ -1202,10 +1239,10 @@ int b200nb_nb_loglik_dev(const void* y, int y_type, const double* x, const doubl
                          const double* alpha_hat, const double* beta_mat, const double* weights, int use_weights,
                          double minmu, int n, int m, int p, long long ld, double* out_loglik, double* out_mu,
                          void* stream) {
-  if (check_dims(n, m, p)) return 1;
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+  if (check_dims(n, m, p) || check_y("nb_loglik", y, y_type, n) || check_ld("nb_loglik", "ld", ld, m, true)) return 1;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   if (!out_loglik) return fail("out_loglik == NULL");
+  if (check_ptrs("nb_loglik", n, {x, nf, alpha_hat, beta_mat}) || (n > 0 && check_device())) return 1;
   nb::LogLikArgs a{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.x = x; a.nf = nf; a.nf_is_vector = nf_is_vector;
   a.alpha = alpha_hat; a.beta = beta_mat; a.w = use_weights ? weights : nullptr; a.n = n; a.m = m; a.p = p; a.ld = ld;
@@ -1219,10 +1256,12 @@ int b200nb_beta_optim_dev(const void* y, int y_type, const double* x, const doub
                           const double* alpha_hat, const double* lambda, const double* beta_start,
                           const double* weights, int use_weights, int maxit, int n, int m, int p, long long ld,
                           double* out_beta_mat, int32_t* out_converged, int32_t* out_iter, void* stream) {
-  if (check_dims(n, m, p)) return 1;
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+  if (check_dims(n, m, p) || check_y("beta_optim", y, y_type, n) || check_ld("beta_optim", "ld", ld, m, true)) return 1;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   if (maxit < 1) return fail("maxit must be >= 1");
+  if (check_ptrs("beta_optim", n, {x, nf, alpha_hat, lambda, beta_start, out_beta_mat, out_converged, out_iter}) ||
+      (n > 0 && check_device()))
+    return 1;
   nb::OptimArgs a{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.x = x; a.nf = nf; a.nf_is_vector = nf_is_vector;
   a.alpha = alpha_hat; a.lambda = lambda; a.beta_in = beta_start; a.w = use_weights ? weights : nullptr;
@@ -1234,27 +1273,35 @@ int b200nb_beta_optim_dev(const void* y, int y_type, const double* x, const doub
 }
 
 int b200nb_to_gene_major_dev(const void* src, void* dst, int n, int m, long long ld, int elem_size, void* stream) {
+  if (elem_size != 4 && elem_size != 8) return fail("to_gene_major: elem_size=%d must be 4 or 8", elem_size);
+  if (check_ld("to_gene_major", "ld", ld, m, false) || check_ptrs("to_gene_major", n, {src, dst})) return 1;
+  if (n > 0 && check_device()) return 1;
   CU(nb::launch_to_gene_major(src, dst, n, m, ld, elem_size, (cudaStream_t)stream));
   g_launches++;
   return 0;
 }
 
 int b200nb_to_col_major_dev(const double* src, double* dst, int n, int m, long long ld, void* stream) {
+  if (check_ld("to_col_major", "ld", ld, m, false) || check_ptrs("to_col_major", n, {src, dst})) return 1;
+  if (n > 0 && check_device()) return 1;
   CU(nb::launch_to_col_major(src, dst, n, m, ld, (cudaStream_t)stream));
   g_launches++;
   return 0;
 }
 
-static int prep_args(nb::PrepArgs& a, const void* y, int y_type, const double* x, const double* proj,
-                     const double* size_factors, double xim, double min_disp, double max_disp, double minmu, int n,
-                     int m, int p, long long ld, double* base_mean, double* base_var, int32_t* all_zero,
-                     double* alpha0, double* mu_lin, double* beta0) {
-  if (check_dims(n, m, p)) return 1;
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+// the checks and arguments the three prep variants share; exactly one of size_factors and nf is read
+static int prep_args(const char* what, nb::PrepArgs& a, const void* y, int y_type, const double* x, const double* proj,
+                     const double* size_factors, const double* nf, double xim, double min_disp, double max_disp,
+                     double minmu, int n, int m, int p, long long ld, double* base_mean, double* base_var,
+                     int32_t* all_zero, double* alpha0, double* mu_lin, double* beta0) {
+  if (check_dims(n, m, p) || check_y(what, y, y_type, n) || check_ld(what, "ld", ld, m, true)) return 1;
   if (m <= p) return fail("prep needs m > p (m=%d, p=%d)", m, p);
+  if (check_ptrs(what, n, {x, proj, size_factors ? size_factors : nf, base_mean, base_var, all_zero, alpha0}) ||
+      (n > 0 && check_device()))
+    return 1;
   a = nb::PrepArgs{};
-  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.x = x; a.proj = proj; a.size_factors = size_factors; a.xim = xim;
-  a.min_disp = min_disp; a.max_disp = max_disp; a.minmu = minmu; a.n = n; a.m = m; a.p = p; a.ld = ld;
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.x = x; a.proj = proj; a.size_factors = size_factors; a.nf = nf;
+  a.xim = xim; a.min_disp = min_disp; a.max_disp = max_disp; a.minmu = minmu; a.n = n; a.m = m; a.p = p; a.ld = ld;
   a.base_mean = base_mean; a.base_var = base_var; a.all_zero = all_zero; a.alpha0 = alpha0; a.mu_lin = mu_lin;
   a.beta0 = beta0;
   a.gid = nullptr; a.xg = nullptr; a.G = 0;
@@ -1279,8 +1326,8 @@ int b200nb_prep_dev(const void* y, int y_type, const double* x, const double* pr
                     double* base_mean, double* base_var, int32_t* all_zero, double* alpha0, double* mu_lin,
                     double* beta0, void* stream) {
   nb::PrepArgs a;
-  if (prep_args(a, y, y_type, x, proj, size_factors, xim, min_disp, max_disp, minmu, n, m, p, ld, base_mean, base_var,
-                all_zero, alpha0, mu_lin, beta0))
+  if (prep_args("prep", a, y, y_type, x, proj, size_factors, nullptr, xim, min_disp, max_disp, minmu, n, m, p, ld,
+                base_mean, base_var, all_zero, alpha0, mu_lin, beta0))
     return 1;
   return prep_launch(a, stream);
 }
@@ -1292,13 +1339,11 @@ int b200nb_prep_weighted_dev(const void* y, int y_type, const double* x, const d
                              double weight_threshold, double* out_weights_norm, int32_t* out_weights_fail,
                              int32_t* out_status, void* stream) {
   nb::PrepArgs a;
-  if (prep_args(a, y, y_type, x, proj, size_factors, xim, min_disp, max_disp, minmu, n, m, p, ld, base_mean, base_var,
-                all_zero, alpha0, mu_lin, beta0))
+  if (prep_args("prep_weighted", a, y, y_type, x, proj, size_factors, nullptr, xim, min_disp, max_disp, minmu, n, m, p,
+                ld, base_mean, base_var, all_zero, alpha0, mu_lin, beta0))
     return 1;
   if (p > 32) return fail("weighted prep supports p <= 32 (p=%d)", p);
-  if (n > 0 && (weights == nullptr || out_weights_norm == nullptr || out_weights_fail == nullptr ||
-                out_status == nullptr))
-    return fail("weighted prep needs weights, out_weights_norm, out_weights_fail and out_status");
+  if (check_ptrs("prep_weighted", n, {weights, out_weights_norm, out_weights_fail, out_status})) return 1;
   if (!(weight_threshold >= 0.0)) return fail("weight_threshold must be >= 0");
   a.weights = weights; a.weight_threshold = weight_threshold; a.weights_norm = out_weights_norm;
   a.weights_fail = out_weights_fail; a.status = out_status;
@@ -1311,49 +1356,31 @@ int b200nb_prep_nf_dev(const void* y, int y_type, const double* x, const double*
                        double* base_mean, double* base_var, int32_t* all_zero, double* alpha0, double* mu_lin,
                        double* beta0, void* stream) {
   nb::PrepArgs a;
-  if (prep_args(a, y, y_type, x, proj, nullptr, xim, min_disp, max_disp, minmu, n, m, p, ld, base_mean, base_var,
-                all_zero, alpha0, mu_lin, beta0))
+  if (prep_args("prep_nf", a, y, y_type, x, proj, nullptr, nf, xim, min_disp, max_disp, minmu, n, m, p, ld, base_mean,
+                base_var, all_zero, alpha0, mu_lin, beta0))
     return 1;
-  if (n > 0 && nf == nullptr) return fail("prep_nf needs the normalization factor matrix");
-  a.nf = nf;
   return prep_launch(a, stream);
 }
 
 int b200nb_trend_fit_dev(const double* means, const double* disps, int n, double min_disp, double* out4,
                          void* stream) {
   if (n < 1) return fail("trend fit needs at least one gene");
+  if (check_ptrs("trend_fit", n, {means, disps, out4}) || check_device()) return 1;
   CU(nb::launch_trend_fit(means, disps, n, min_disp, out4, (cudaStream_t)stream));
   g_launches++;
   return 0;
 }
 
-static int cooks_common(const void* y, int y_type, const double* mu, const double* hat, const double* size_factors,
-                        const double* nf, const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n,
-                        int m, int p, long long ld, double* cooks, double* max_cooks, double* robust_disp,
-                        void* stream);
-
-int b200nb_cooks_dev(const void* y, int y_type, const double* mu, const double* hat, const double* size_factors,
-                     const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n, int m, int p,
-                     long long ld, double* cooks, double* max_cooks, double* robust_disp, void* stream) {
-  return cooks_common(y, y_type, mu, hat, size_factors, nullptr, cell_ptr, cell_samples, ncell, n, m, p, ld, cooks,
-                      max_cooks, robust_disp, stream);
-}
-
-int b200nb_cooks_nf_dev(const void* y, int y_type, const double* mu, const double* hat, const double* nf,
-                        const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n, int m, int p,
-                        long long ld, double* cooks, double* max_cooks, double* robust_disp, void* stream) {
-  if (n > 0 && nf == nullptr) return fail("cooks_nf needs the normalization factor matrix");
-  return cooks_common(y, y_type, mu, hat, nullptr, nf, cell_ptr, cell_samples, ncell, n, m, p, ld, cooks, max_cooks,
-                      robust_disp, stream);
-}
-
-static int cooks_common(const void* y, int y_type, const double* mu, const double* hat, const double* size_factors,
-                        const double* nf, const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n,
-                        int m, int p, long long ld, double* cooks, double* max_cooks, double* robust_disp,
-                        void* stream) {
-  if (check_dims(n, m, p)) return 1;
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+// b200nb_cooks_dev and b200nb_cooks_nf_dev: exactly one of size_factors and nf is read
+static int cooks_common(const char* what, const void* y, int y_type, const double* mu, const double* hat,
+                        const double* size_factors, const double* nf, const int32_t* cell_ptr,
+                        const int32_t* cell_samples, int ncell, int n, int m, int p, long long ld, double* cooks,
+                        double* max_cooks, double* robust_disp, void* stream) {
+  if (check_dims(n, m, p) || check_y(what, y, y_type, n) || check_ld(what, "ld", ld, m, true)) return 1;
   if (ncell < 1 || ncell > m) return fail("bad number of design cells %d", ncell);
+  if (check_ptrs(what, n, {mu, hat, size_factors ? size_factors : nf, cell_ptr, cell_samples, max_cooks, robust_disp}))
+    return 1;
+  if (n > 0 && check_device()) return 1;
   nb::CooksArgs a{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.mu = mu; a.hat = hat; a.size_factors = size_factors;
   a.cell_ptr = cell_ptr; a.cell_samples = cell_samples; a.ncell = ncell; a.n = n; a.m = m; a.p = p; a.ld = ld;
@@ -1372,12 +1399,28 @@ static int cooks_common(const void* y, int y_type, const double* mu, const doubl
   return 0;
 }
 
+int b200nb_cooks_dev(const void* y, int y_type, const double* mu, const double* hat, const double* size_factors,
+                     const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n, int m, int p,
+                     long long ld, double* cooks, double* max_cooks, double* robust_disp, void* stream) {
+  return cooks_common("cooks", y, y_type, mu, hat, size_factors, nullptr, cell_ptr, cell_samples, ncell, n, m, p, ld,
+                      cooks, max_cooks, robust_disp, stream);
+}
+
+int b200nb_cooks_nf_dev(const void* y, int y_type, const double* mu, const double* hat, const double* nf,
+                        const int32_t* cell_ptr, const int32_t* cell_samples, int ncell, int n, int m, int p,
+                        long long ld, double* cooks, double* max_cooks, double* robust_disp, void* stream) {
+  return cooks_common("cooks_nf", y, y_type, mu, hat, nullptr, nf, cell_ptr, cell_samples, ncell, n, m, p, ld, cooks,
+                      max_cooks, robust_disp, stream);
+}
+
 int b200nb_beta_prior_quantile_dev(const double* beta_log2, int n, int p, const double* base_mean,
                                    const double* disp_fit, const int32_t* col_a, const int32_t* col_b, int k,
                                    double prob, double* out_q, void* stream) {
   if (n < 1 || p < 1 || k < 0) return fail("bad dimensions n=%d p=%d k=%d", n, p, k);
   if (!(prob > 0.0 && prob < 1.0)) return fail("prob=%g must lie in (0, 1)", prob);
   if (k == 0) return 0;
+  if (check_ptrs("beta_prior_quantile", k, {beta_log2, base_mean, disp_fit, col_a, col_b, out_q}) || check_device())
+    return 1;
   // the column list is tiny (k <= a few hundred): fetch it once to check every index (one stream sync)
   std::vector<int32_t> ca((size_t)k), cb((size_t)k);
   CU(cudaMemcpyAsync(ca.data(), col_a, k * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
@@ -1395,12 +1438,13 @@ int b200nb_beta_prior_quantile_dev(const double* beta_log2, int n, int p, const 
   return 0;
 }
 
-static int size_factors_common(const void* y, int y_type, const double* divisor, int poscounts, int n, int m,
-                               long long ld, double* loggeomeans, double* scratch_gm, double* scratch_cm,
-                               double* size_factors, int32_t* n_finite, void* stream) {
-  if (check_dims(n, m, 1)) return 1;
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
+static int size_factors_common(const char* what, const void* y, int y_type, const double* divisor, int poscounts,
+                               int n, int m, long long ld, double* loggeomeans, double* scratch_gm,
+                               double* scratch_cm, double* size_factors, int32_t* n_finite, void* stream) {
   if (n < 1) return fail("size factors need at least one gene");
+  if (check_dims(n, m, 1) || check_y(what, y, y_type, n) || check_ld(what, "ld", ld, m, true) ||
+      check_ptrs(what, n, {loggeomeans, scratch_gm, scratch_cm, size_factors, n_finite}) || check_device())
+    return 1;
   nb::SizeFactorArgs a{};
   a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.poscounts = poscounts ? 1 : 0; a.n = n; a.m = m; a.ld = ld;
   a.loggeomeans = loggeomeans; a.ratios = scratch_gm; a.ratios_colmajor = scratch_cm; a.size_factors = size_factors;
@@ -1413,16 +1457,16 @@ static int size_factors_common(const void* y, int y_type, const double* divisor,
 int b200nb_size_factors_dev(const void* y, int y_type, int poscounts, int n, int m, long long ld,
                             double* loggeomeans, double* scratch_gm, double* scratch_cm, double* size_factors,
                             int32_t* n_finite, void* stream) {
-  return size_factors_common(y, y_type, nullptr, poscounts, n, m, ld, loggeomeans, scratch_gm, scratch_cm,
-                             size_factors, n_finite, stream);
+  return size_factors_common("size_factors", y, y_type, nullptr, poscounts, n, m, ld, loggeomeans, scratch_gm,
+                             scratch_cm, size_factors, n_finite, stream);
 }
 
 int b200nb_size_factors_norm_dev(const void* y, int y_type, const double* divisor, int poscounts, int n, int m,
                                  long long ld, double* loggeomeans, double* scratch_gm, double* scratch_cm,
                                  double* size_factors, int32_t* n_finite, void* stream) {
   if (divisor == nullptr) return fail("size_factors_norm needs the divisor matrix");
-  return size_factors_common(y, y_type, divisor, poscounts, n, m, ld, loggeomeans, scratch_gm, scratch_cm,
-                             size_factors, n_finite, stream);
+  return size_factors_common("size_factors_norm", y, y_type, divisor, poscounts, n, m, ld, loggeomeans, scratch_gm,
+                             scratch_cm, size_factors, n_finite, stream);
 }
 
 // The objective tiles of b200nb_sf_iterate_objective_dev: the grow-only workspace slot S_SFI (taken under g_call_mu,
@@ -1434,13 +1478,11 @@ int b200nb_sf_iterate_objective_dev(const void* y, int y_type, const double* q, 
                                     const double* par, double h, double Q, int n, int m, long long ld,
                                     int max_tile_cols, double* out, void* stream) {
   if (n < 1 || m < 1) return fail("sf_iterate_objective: bad dimensions n=%d m=%d (both must be >= 1)", n, m);
-  if (ld < m || (ld & 3)) return fail("ld=%lld must be >= m and a multiple of 4", ld);
-  if (!(h > 0.0 && h < HUGE_VAL)) return fail("sf_iterate_objective: h=%g must be finite and > 0", h);
+  if (check_ld("sf_iterate_objective", "ld", ld, m, true) || check_y("sf_iterate_objective", y, y_type, n)) return 1;
+  if (!finite_pos(h)) return fail("sf_iterate_objective: h=%g must be finite and > 0", h);
   if (!(Q >= 0.0 && Q < 1.0)) return fail("sf_iterate_objective: Q=%g must lie in [0, 1)", Q);
   if (max_tile_cols < 0) return fail("sf_iterate_objective: max_tile_cols=%d must be >= 0", max_tile_cols);
-  if (!y || !q || !alpha || !par || !out) return fail("sf_iterate_objective: null pointer argument");
-  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
-  if (check_device()) return 1;
+  if (check_ptrs("sf_iterate_objective", n, {q, alpha, par, out}) || check_device()) return 1;
   const int cols = 2 * m + 1;
   long long tile = (long long)(kSfiTileBytes / ((size_t)n * sizeof(double)));
   if (max_tile_cols > 0 && tile > max_tile_cols) tile = max_tile_cols;
@@ -1462,12 +1504,10 @@ int b200nb_sf_iterate_objective_dev(const void* y, int y_type, const double* q, 
 int b200nb_transform_dev(const void* y, int y_type, const double* size_factors, const double* nf, int n, int m,
                          long long ld, int mode, double c0, double c1, double* out, long long ld_out, void* stream) {
   if (n < 0 || m < 0) return fail("transform: bad dimensions n=%d m=%d (both must be >= 0)", n, m);
-  if (ld < m || ld_out < m) return fail("transform: ld=%lld and ld_out=%lld must be >= m=%d", ld, ld_out, m);
-  if ((size_factors == nullptr) == (nf == nullptr))
-    return fail("transform: give exactly one of size_factors and nf");
+  if (check_ld("transform", "ld", ld, m, false) || check_ld("transform", "ld_out", ld_out, m, false) ||
+      check_factors("transform", size_factors, nf) || check_y("transform", y, y_type, n))
+    return 1;
   if (!y || !out) return fail("transform: null pointer argument");
-  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
-  const auto finite_pos = [](double v) { return v > 0.0 && v < HUGE_VAL; };
   nb::TransformArgs a{};
   a.mode = mode;
   a.ln2 = log(2.0);
@@ -1500,28 +1540,19 @@ int b200nb_transform_dev(const void* y, int y_type, const double* size_factors, 
 // qnorm(1 - 0.05 / 2): the normal quantile rlog's weighted upper quantile is matched to (R/core.R:2416-2419)
 constexpr double kRlogSdScale = 1.959963984540054;
 
-static int rlog_common_checks(const char* what, const void* y, int y_type, const double* size_factors,
-                              const double* nf, int m, long long ld) {
-  if (ld < m) return fail("%s: ld=%lld must be >= m=%d", what, ld, m);
-  if ((size_factors == nullptr) == (nf == nullptr)) return fail("%s: give exactly one of size_factors and nf", what);
-  if (!y) return fail("%s: null pointer argument", what);
-  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
-  return 0;
-}
-
 int b200nb_rlog_fit_dev(const void* y, int y_type, const double* size_factors, const double* nf,
                         const double* intercept, const double* disp_fit, int n, int m, long long ld,
                         double beta_prior_var, double tol, int maxit, double minmu, double* out, long long ld_out,
                         double* out_intercept, double* out_iter, void* stream) {
   if (n < 0 || m < 1) return fail("rlog_fit: bad dimensions n=%d m=%d (n >= 0, m >= 1)", n, m);
-  if (ld_out < m) return fail("rlog_fit: ld_out=%lld must be >= m=%d", ld_out, m);
-  if (rlog_common_checks("rlog_fit", y, y_type, size_factors, nf, m, ld)) return 1;
-  const auto finite_pos = [](double v) { return v > 0.0 && v < HUGE_VAL; };
+  if (check_ld("rlog_fit", "ld", ld, m, false) || check_ld("rlog_fit", "ld_out", ld_out, m, false) ||
+      check_factors("rlog_fit", size_factors, nf) || check_y("rlog_fit", y, y_type, n))
+    return 1;
   if (!finite_pos(beta_prior_var)) return fail("rlog_fit: betaPriorVar=%g must be finite and > 0", beta_prior_var);
   if (!finite_pos(tol)) return fail("rlog_fit: tol=%g must be finite and > 0", tol);
   if (!finite_pos(minmu)) return fail("rlog_fit: minmu=%g must be finite and > 0", minmu);
   if (maxit < 1) return fail("rlog_fit: maxit=%d must be >= 1", maxit);
-  if (!disp_fit || !out || !out_iter || (!intercept && !out_intercept))
+  if (!y || !disp_fit || !out || !out_iter || (!intercept && !out_intercept))
     return fail("rlog_fit: null pointer argument");
   if (n == 0) return 0;
   if (check_device()) return 1;
@@ -1546,9 +1577,10 @@ int b200nb_rlog_prior_var_dev(const void* y, int y_type, const double* size_fact
                               const double* base_mean, const double* disp_fit, int n, int m, long long ld,
                               double* out_var, void* stream) {
   if (n < 1 || m < 1) return fail("rlog_prior_var: bad dimensions n=%d m=%d (both must be >= 1)", n, m);
-  if (rlog_common_checks("rlog_prior_var", y, y_type, size_factors, nf, m, ld)) return 1;
-  if (!base_mean || !disp_fit || !out_var) return fail("rlog_prior_var: null pointer argument");
-  if (check_device()) return 1;
+  if (check_ld("rlog_prior_var", "ld", ld, m, false) || check_factors("rlog_prior_var", size_factors, nf)) return 1;
+  if (check_ptrs("rlog_prior_var", n, {base_mean, disp_fit, out_var}) || check_y("rlog_prior_var", y, y_type, n) ||
+      check_device())
+    return 1;
   std::lock_guard<std::mutex> lk(g_call_mu);
   void* ws = nullptr;
   if (ws_get(S_RLOG, nb::rlog_prior_scratch_bytes(n, m), &ws)) return 1;
@@ -1570,14 +1602,14 @@ int b200nb_results_gene_dev(const void* y, int y_type, int n, int m, long long l
                             const int32_t* keep, const int32_t* replace, const double* base_mean, double* out_lfc,
                             double* out_se, double* out_stat, double* out_pvalue, void* stream) {
   if (n < 0 || m < 1) return fail("results_gene: bad dimensions n=%d m=%d (n >= 0, m >= 1)", n, m);
-  if (ld < m) return fail("results_gene: ld=%lld must be >= m=%d", ld, m);
+  if (check_ld("results_gene", "ld", ld, m, false)) return 1;
   if (alt < B200NB_ALT_NONE || alt > B200NB_ALT_LESS) return fail("results_gene: unknown altHypothesis code %d", alt);
   if (!(lfc_threshold >= 0.0 && lfc_threshold < HUGE_VAL))
     return fail("results_gene: lfcThreshold=%g must be finite and >= 0", lfc_threshold);
   if (!lfc || !se || !stat || !pvalue || !out_lfc || !out_se || !out_stat || !out_pvalue || (zero_mask && !y) ||
       (replace && !base_mean))
     return fail("results_gene: null pointer argument");
-  if (zero_mask && y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
+  if (zero_mask && check_y("results_gene", y, y_type, n)) return 1;
   if (n == 0) return 0;
   if (check_device()) return 1;
   nb::ResultsGeneArgs a{};
@@ -1594,9 +1626,10 @@ int b200nb_results_gene_dev(const void* y, int y_type, int n, int m, long long l
 int b200nb_results_heuristic_dev(const void* y, int y_type, const int64_t* rows, int k, int m, long long ld,
                                  const double* cooks, long long ld_cooks, int32_t* keep, void* stream) {
   if (k < 0 || m < 1) return fail("results_heuristic: bad dimensions k=%d m=%d (k >= 0, m >= 1)", k, m);
-  if (ld < m || ld_cooks < m) return fail("results_heuristic: ld=%lld and ld_cooks=%lld must be >= m=%d", ld, ld_cooks, m);
+  if (check_ld("results_heuristic", "ld", ld, m, false) ||
+      check_ld("results_heuristic", "ld_cooks", ld_cooks, m, false) || check_y("results_heuristic", y, y_type, k))
+    return 1;
   if (!y || !rows || !cooks || !keep) return fail("results_heuristic: null pointer argument");
-  if (y_type != B200NB_Y_INT32 && y_type != B200NB_Y_F64) return fail("bad y_type %d", y_type);
   if (k == 0) return 0;
   if (check_device()) return 1;
   nb::ResultsHeuristicArgs a{};
@@ -1614,8 +1647,7 @@ int b200nb_filter_cutoffs_dev(const double* filter, int n, const double* theta, 
                               void* stream) {
   if (n < 1) return fail("filter_cutoffs: n=%d must be >= 1", n);
   if (n_theta < 1 || n_theta > kMaxTheta) return fail("filter_cutoffs: n_theta=%d must be in [1, %d]", n_theta, kMaxTheta);
-  if (!filter || !theta || !out) return fail("filter_cutoffs: null pointer argument");
-  if (check_device()) return 1;
+  if (check_ptrs("filter_cutoffs", n, {filter, theta, out}) || check_device()) return 1;
   nb::FilterCutoffArgs a{};
   a.filter = filter; a.n = n; a.theta = theta; a.out = out;
   CU(nb::launch_filter_cutoffs(a, n_theta, (cudaStream_t)stream));
@@ -1629,8 +1661,7 @@ int b200nb_filter_numrej_dev(const double* p_sorted, const double* filter_sorted
   if (n_theta < 1 || n_theta > kMaxTheta) return fail("filter_numrej: n_theta=%d must be in [1, %d]", n_theta, kMaxTheta);
   if (!padj_method_ok(method)) return fail("filter_numrej: unknown p.adjust method code %d", method);
   if (!(alpha > 0.0 && alpha < 1.0)) return fail("filter_numrej: alpha=%g must be in (0, 1)", alpha);
-  if (!p_sorted || !filter_sorted || !cutoffs || !out_numrej) return fail("filter_numrej: null pointer argument");
-  if (check_device()) return 1;
+  if (check_ptrs("filter_numrej", n, {p_sorted, filter_sorted, cutoffs, out_numrej}) || check_device()) return 1;
   nb::PadjArgs a{};
   a.p_sorted = p_sorted; a.filter_sorted = filter_sorted; a.n = n; a.cutoffs = cutoffs; a.method = method;
   a.alpha = alpha; a.out_numrej = out_numrej;
@@ -1644,8 +1675,7 @@ int b200nb_padj_dev(const double* p_sorted, const double* filter_sorted, const i
   if (n < 1) return fail("padj: n=%d must be >= 1", n);
   if (j < 0) return fail("padj: j=%d must be >= 0", j);
   if (!padj_method_ok(method)) return fail("padj: unknown p.adjust method code %d", method);
-  if (!p_sorted || !filter_sorted || !order || !out) return fail("padj: null pointer argument");
-  if (check_device()) return 1;
+  if (check_ptrs("padj", n, {p_sorted, filter_sorted, order, out}) || check_device()) return 1;
   nb::PadjArgs a{};
   a.p_sorted = p_sorted; a.filter_sorted = filter_sorted; a.order = order; a.n = n; a.cutoffs = cutoffs; a.j = j;
   a.method = method; a.out = out;
@@ -1671,9 +1701,10 @@ int b200nb_fit_disp(const void* y, int y_type, const double* x, const double* mu
                     double* out_log_alpha, int32_t* out_iter, int32_t* out_iter_accept, double* out_last_change,
                     double* out_initial_lp, double* out_initial_dlp, double* out_last_lp, double* out_last_dlp,
                     double* out_last_d2lp) {
-  if (check_dims(n, m, p)) return 1;
+  if (check_dims(n, m, p) || check_y("fitDisp", y, y_type, n)) return 1;
   if (n == 0) return 0;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
+  if (check_ptrs("fitDisp", n, {x, mu_hat, log_alpha, log_alpha_prior_mean}) || check_device()) return 1;
   std::lock_guard<std::mutex> lk(g_call_mu);
   HostCallScope host_scope;   // the row-chunked path keeps the small-p kernels (see long_rows)
   g_call_seq++;
@@ -1774,10 +1805,11 @@ int b200nb_fit_disp_grid(const void* y, int y_type, const double* x, const doubl
                          int disp_grid_n, const double* log_alpha_prior_mean, double log_alpha_prior_sigmasq,
                          int use_prior, const double* weights, int use_weights, double weight_threshold, int use_cr,
                          int n, int m, int p, double* out_log_alpha) {
-  if (check_dims(n, m, p)) return 1;
+  if (check_dims(n, m, p) || check_y("fitDispGrid", y, y_type, n)) return 1;
   if (n == 0) return 0;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   if (disp_grid_n < 2) return fail("disp_grid needs at least 2 points");
+  if (check_ptrs("fitDispGrid", n, {x, mu_hat, disp_grid, log_alpha_prior_mean}) || check_device()) return 1;
   std::lock_guard<std::mutex> lk(g_call_mu);
   HostCallScope host_scope;   // the row-chunked path keeps the small-p kernels (see long_rows)
   g_call_seq++;
@@ -1853,9 +1885,10 @@ int b200nb_fit_beta(const void* y, int y_type, const double* x, const double* nf
                     int use_weights, double tol, int maxit, int use_qr, double minmu, int n, int m, int p,
                     double* out_beta_mat, double* out_beta_var_mat, double* out_iter, double* out_hat_diagonals,
                     double* out_contrast_num, double* out_contrast_denom, double* out_deviance, double* out_mu) {
-  if (check_dims(n, m, p)) return 1;
+  if (check_dims(n, m, p) || check_y("fitBeta", y, y_type, n)) return 1;
   if (n == 0) return 0;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
+  if (check_ptrs("fitBeta", n, {x, nf, alpha_hat, contrast, beta_mat, lambda}) || check_device()) return 1;
   std::lock_guard<std::mutex> lk(g_call_mu);
   HostCallScope host_scope;   // the row-chunked path keeps the small-p kernels (see long_rows)
   g_call_seq++;

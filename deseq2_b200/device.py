@@ -68,6 +68,12 @@ def _ytype(y):
     raise TypeError("y must be int32 or float64")
 
 
+def _split_factors(sfd):
+    """(size_factors, nf) for the entry points that take exactly one: sfd is the (m,) size-factor vector or the
+    gene-major (n, ld) normalization-factor matrix."""
+    return (None, sfd) if sfd.dim() == 2 else (sfd, None)
+
+
 def fit_disp(y, x, mu_hat, log_alpha, log_alpha_prior_mean, log_alpha_prior_sigmasq, min_log_alpha, kappa_0, tol,
              maxit, usePrior, weights=None, weightThreshold=1e-2, useCR=True, m=None, out=None):
     """fitDisp on device tensors (src/DESeq2.cpp:164).  x: (m, p) numpy or tensor (column-major on device).

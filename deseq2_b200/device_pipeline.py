@@ -36,25 +36,19 @@ rlog_device (R/rlog.R) fits the dispersion function the same way, then runs rlog
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 import torch
 
 from . import _lib
 from . import device as D
+# The call helpers live in device.py.  Their names stay importable from here for callers that use or replace
+# device_pipeline._p / ._stream; the bindings below call D._p and D._stream() at call time, so replacing
+# device._stream is what changes the stream they use.
+from .device import _p, _stream  # noqa: F401
 from .pipeline import modelMatrixGroups
 
 F64 = torch.float64
 LN2 = float(np.log(2.0))
-
-
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 _WS = {}
@@ -85,9 +79,9 @@ def size_factors(y, m, type="ratio"):
     nfin = torch.zeros(1, dtype=torch.int32, device=dev)
     gm = _ws("sf_ratios", (n, ld), F64, dev)
     cm = _ws("sf_ratios_cm", (n * m,), F64, dev)
-    _lib.check(L.b200nb_size_factors_dev(_p(y), 1 if y.dtype == F64 else 0, int(type == "poscounts"), n, m, ld,
-                                         _p(out["loggeomeans"]), _p(gm), _p(cm), _p(out["sizeFactors"]), _p(nfin),
-                                         _stream()), "size_factors")
+    _lib.check(L.b200nb_size_factors_dev(D._p(y), D._ytype(y), int(type == "poscounts"), n, m, ld,
+                                         D._p(out["loggeomeans"]), D._p(gm), D._p(cm), D._p(out["sizeFactors"]),
+                                         D._p(nfin), D._stream()), "size_factors")
     if int(nfin.item()) == 0:
         raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
     return out
@@ -103,9 +97,9 @@ def sf_iterate_objective(y, q, alpha, par, m, h=1e-3, Q=0.05, max_tile_cols=0, o
     n, ld = y.shape
     if out is None:
         out = torch.empty(2 * m + 1, dtype=F64, device=y.device)
-    _lib.check(L.b200nb_sf_iterate_objective_dev(_p(y), 1 if y.dtype == F64 else 0, _p(q), _p(alpha), _p(par),
-                                                 float(h), float(Q), n, m, ld, int(max_tile_cols), _p(out),
-                                                 _stream()), "sf_iterate_objective")
+    _lib.check(L.b200nb_sf_iterate_objective_dev(D._p(y), D._ytype(y), D._p(q), D._p(alpha), D._p(par),
+                                                 float(h), float(Q), n, m, ld, int(max_tile_cols), D._p(out),
+                                                 D._stream()), "sf_iterate_objective")
     return out
 
 
@@ -165,8 +159,8 @@ def normalization_factors(y, m, normMatrix=None, avgTxLength=None, type="ratio")
     nfin = torch.zeros(1, dtype=torch.int32, device=dev)
     gm = _ws("sf_ratios", (n, ld), F64, dev)
     cm = _ws("sf_ratios_cm", (n * m,), F64, dev)
-    _lib.check(L.b200nb_size_factors_norm_dev(_p(y), 1 if y.dtype == F64 else 0, _p(d), int(type == "poscounts"), n,
-                                              m, ld, _p(lg), _p(gm), _p(cm), _p(sf), _p(nfin), _stream()),
+    _lib.check(L.b200nb_size_factors_norm_dev(D._p(y), D._ytype(y), D._p(d), int(type == "poscounts"), n,
+                                              m, ld, D._p(lg), D._p(gm), D._p(cm), D._p(sf), D._p(nfin), D._stream()),
                "size_factors_norm")
     if int(nfin.item()) == 0:
         raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
@@ -247,13 +241,13 @@ def prep(y, x, sizeFactors, minDisp=1e-8, minmu=0.5, want_mu=True, want_beta0=Tr
            "allZero": torch.empty(n, dtype=torch.int32, device=dev), "alpha0": torch.empty(n, dtype=F64, device=dev),
            "mu_lin": _ws("mu_lin", (n, ld), F64, dev) if want_mu else None,
            "beta0": torch.empty((p, n), dtype=F64, device=dev) if want_beta0 else None}
-    args = (_p(y), 0 if y.dtype == torch.int32 else 1, _p(xd), _p(projd), _p(sfd), float(xim), float(minDisp),
-            float(max(10, m)), float(minmu), n, m, p, ld, _p(out["baseMean"]), _p(out["baseVar"]), _p(out["allZero"]),
-            _p(out["alpha0"]))
+    args = (D._p(y), D._ytype(y), D._p(xd), D._p(projd), D._p(sfd), float(xim), float(minDisp),
+            float(max(10, m)), float(minmu), n, m, p, ld, D._p(out["baseMean"]), D._p(out["baseVar"]),
+            D._p(out["allZero"]), D._p(out["alpha0"]))
     if nf is not None:
-        _lib.check(L.b200nb_prep_nf_dev(*args, _p(out["mu_lin"]), _p(out["beta0"]), _stream()), "prep_nf_dev")
+        _lib.check(L.b200nb_prep_nf_dev(*args, D._p(out["mu_lin"]), D._p(out["beta0"]), D._stream()), "prep_nf_dev")
     elif weights is None:
-        rc = L.b200nb_prep_dev(*args, _p(out["mu_lin"]), _p(out["beta0"]), _stream())
+        rc = L.b200nb_prep_dev(*args, D._p(out["mu_lin"]), D._p(out["beta0"]), D._stream())
         _lib.check(rc, "prep_dev")
     else:
         _check_weights_tensor(weights, y)
@@ -261,8 +255,9 @@ def prep(y, x, sizeFactors, minDisp=1e-8, minmu=0.5, want_mu=True, want_beta0=Tr
         out["weightsNorm"] = torch.empty((n, ld), dtype=F64, device=dev)
         out["weightsFail"] = torch.empty(n, dtype=torch.int32, device=dev)
         out["status"] = torch.zeros(1, dtype=torch.int32, device=dev)
-        rc = L.b200nb_prep_weighted_dev(*args, None, _p(out["beta0"]), _p(weights), float(weightThreshold),
-                                        _p(out["weightsNorm"]), _p(out["weightsFail"]), _p(out["status"]), _stream())
+        rc = L.b200nb_prep_weighted_dev(*args, None, D._p(out["beta0"]), D._p(weights), float(weightThreshold),
+                                        D._p(out["weightsNorm"]), D._p(out["weightsFail"]), D._p(out["status"]),
+                                        D._stream())
         _lib.check(rc, "prep_weighted_dev")
     out["xd"], out["sfd"] = xd, sfd
     return out
@@ -296,7 +291,7 @@ def trend_fit(means, disps, minDisp=1e-8):
     """parametricDispersionFit on device: returns a 4-vector tensor (asymptDisp, extraPois, status, rounds)."""
     L = _lib.lib()
     out = torch.empty(4, dtype=F64, device=means.device)
-    _lib.check(L.b200nb_trend_fit_dev(_p(means), _p(disps), means.numel(), float(minDisp), _p(out), _stream()),
+    _lib.check(L.b200nb_trend_fit_dev(D._p(means), D._p(disps), means.numel(), float(minDisp), D._p(out), D._stream()),
                "trend_fit_dev")
     return out
 
@@ -320,8 +315,8 @@ def cooks(y, mu, hat, x, sizeFactors, want_matrix=True, normalizationFactors=Non
     out = {"cooks": torch.empty((n, ld), dtype=F64, device=dev) if want_matrix else None,
            "maxCooks": torch.empty(n, dtype=F64, device=dev), "robustDisp": torch.empty(n, dtype=F64, device=dev)}
     entry = L.b200nb_cooks_nf_dev if nf is not None else L.b200nb_cooks_dev
-    rc = entry(_p(y), 0 if y.dtype == torch.int32 else 1, _p(mu), _p(hat), _p(sfd), _p(ptrd), _p(ordd),
-               len(sizes), n, m, p, ld, _p(out["cooks"]), _p(out["maxCooks"]), _p(out["robustDisp"]), _stream())
+    rc = entry(D._p(y), D._ytype(y), D._p(mu), D._p(hat), D._p(sfd), D._p(ptrd), D._p(ordd),
+               len(sizes), n, m, p, ld, D._p(out["cooks"]), D._p(out["maxCooks"]), D._p(out["robustDisp"]), D._stream())
     _lib.check(rc, "cooks_dev")
     return out
 
@@ -337,8 +332,9 @@ def beta_prior_quantile(beta, baseMean, dispFit, col_a, col_b, prob):
     ca = torch.as_tensor(np.asarray(col_a, dtype=np.int32), device=dev)
     cb = torch.as_tensor(np.asarray(col_b, dtype=np.int32), device=dev)
     out = torch.empty(ca.numel(), dtype=F64, device=dev)
-    _lib.check(L.b200nb_beta_prior_quantile_dev(_p(beta), n, p, _p(baseMean), _p(dispFit), _p(ca), _p(cb), ca.numel(),
-                                                float(prob), _p(out), _stream()), "beta_prior_quantile_dev")
+    _lib.check(L.b200nb_beta_prior_quantile_dev(D._p(beta), n, p, D._p(baseMean), D._p(dispFit), D._p(ca), D._p(cb),
+                                                ca.numel(), float(prob), D._p(out), D._stream()),
+               "beta_prior_quantile_dev")
     return out
 
 
@@ -1076,9 +1072,9 @@ def transform(y, m, mode, c0, c1, sfd):
     L = _lib.lib()
     n, ld = y.shape
     out = torch.empty((n, m), dtype=F64, device=y.device)
-    sf, nf = (None, sfd) if sfd.dim() == 2 else (sfd, None)
-    _lib.check(L.b200nb_transform_dev(_p(y), 1 if y.dtype == F64 else 0, _p(sf), _p(nf), n, m, ld,
-                                      _TRANSFORM_MODE[mode], float(c0), float(c1), _p(out), m, _stream()),
+    sf, nf = D._split_factors(sfd)
+    _lib.check(L.b200nb_transform_dev(D._p(y), D._ytype(y), D._p(sf), D._p(nf), n, m, ld,
+                                      _TRANSFORM_MODE[mode], float(c0), float(c1), D._p(out), m, D._stream()),
                "transform_dev")
     return out
 
@@ -1257,9 +1253,9 @@ def rlog_prior_var(y, m, sfd, baseMean, dispFit):
     L = _lib.lib()
     n, ld = y.shape
     out = torch.empty(1, dtype=F64, device=y.device)
-    sf, nf = (None, sfd) if sfd.dim() == 2 else (sfd, None)
-    _lib.check(L.b200nb_rlog_prior_var_dev(_p(y), 1 if y.dtype == F64 else 0, _p(sf), _p(nf), _p(baseMean),
-                                           _p(dispFit), n, m, ld, _p(out), _stream()), "rlog_prior_var_dev")
+    sf, nf = D._split_factors(sfd)
+    _lib.check(L.b200nb_rlog_prior_var_dev(D._p(y), D._ytype(y), D._p(sf), D._p(nf), D._p(baseMean),
+                                           D._p(dispFit), n, m, ld, D._p(out), D._stream()), "rlog_prior_var_dev")
     return out[0]
 
 
@@ -1278,10 +1274,10 @@ def rlog_fit(y, m, sfd, dispFit, betaPriorVar, intercept=None, betaTol=1e-4, max
     out = torch.empty((n, m), dtype=F64, device=dev)
     icpt = None if intercept is not None else torch.empty(n, dtype=F64, device=dev)
     it = torch.empty(n, dtype=F64, device=dev)
-    sf, nf = (None, sfd) if sfd.dim() == 2 else (sfd, None)
-    _lib.check(L.b200nb_rlog_fit_dev(_p(y), 1 if y.dtype == F64 else 0, _p(sf), _p(nf), _p(intercept), _p(dispFit),
-                                     n, m, ld, float(betaPriorVar), float(betaTol), int(maxit), float(minmu), _p(out),
-                                     m, _p(icpt), _p(it), _stream()), "rlog_fit_dev")
+    sf, nf = D._split_factors(sfd)
+    _lib.check(L.b200nb_rlog_fit_dev(D._p(y), D._ytype(y), D._p(sf), D._p(nf), D._p(intercept), D._p(dispFit),
+                                     n, m, ld, float(betaPriorVar), float(betaTol), int(maxit), float(minmu), D._p(out),
+                                     m, D._p(icpt), D._p(it), D._stream()), "rlog_fit_dev")
     return {"rlog": out, "intercept": icpt, "betaIter": it}
 
 
@@ -1403,8 +1399,8 @@ def filter_cutoffs(filter, theta):
     probabilities, one CTA per probability.  Enqueue only."""
     L = _lib.lib()
     out = torch.empty(theta.numel(), dtype=F64, device=filter.device)
-    _lib.check(L.b200nb_filter_cutoffs_dev(_p(filter), filter.numel(), _p(theta), theta.numel(), _p(out), _stream()),
-               "filter_cutoffs_dev")
+    _lib.check(L.b200nb_filter_cutoffs_dev(D._p(filter), filter.numel(), D._p(theta), theta.numel(), D._p(out),
+                                           D._stream()), "filter_cutoffs_dev")
     return out
 
 
@@ -1413,8 +1409,8 @@ def filter_numrej(p_sorted, filter_sorted, cutoffs, method, alpha):
     last) and their filter values.  Returns a (T,) int32 device tensor.  Enqueue only."""
     L = _lib.lib()
     out = torch.empty(cutoffs.numel(), dtype=torch.int32, device=p_sorted.device)
-    _lib.check(L.b200nb_filter_numrej_dev(_p(p_sorted), _p(filter_sorted), p_sorted.numel(), _p(cutoffs),
-                                          cutoffs.numel(), _PADJ_CODE[method], float(alpha), _p(out), _stream()),
+    _lib.check(L.b200nb_filter_numrej_dev(D._p(p_sorted), D._p(filter_sorted), p_sorted.numel(), D._p(cutoffs),
+                                          cutoffs.numel(), _PADJ_CODE[method], float(alpha), D._p(out), D._stream()),
                "filter_numrej_dev")
     return out
 
@@ -1424,8 +1420,8 @@ def padj_column(p_sorted, filter_sorted, order, method, cutoffs=None, j=0):
     p-value), as a (N,) device tensor in gene order with NaN for the others.  Enqueue only."""
     L = _lib.lib()
     out = torch.empty(p_sorted.numel(), dtype=F64, device=p_sorted.device)
-    _lib.check(L.b200nb_padj_dev(_p(p_sorted), _p(filter_sorted), _p(order), p_sorted.numel(), _p(cutoffs), int(j),
-                                 _PADJ_CODE[method], _p(out), _stream()), "padj_dev")
+    _lib.check(L.b200nb_padj_dev(D._p(p_sorted), D._p(filter_sorted), D._p(order), p_sorted.numel(), D._p(cutoffs),
+                                 int(j), _PADJ_CODE[method], D._p(out), D._stream()), "padj_dev")
     return out
 
 
@@ -1470,10 +1466,10 @@ def results_gene(ynz, m, lfc, se, stat, pvalue, negate=False, zero_mask=None, lr
     L = _lib.lib()
     n, ld = ynz.shape
     out = [torch.empty(n, dtype=F64, device=ynz.device) for _ in range(4)]
-    _lib.check(L.b200nb_results_gene_dev(_p(ynz), 1 if ynz.dtype == F64 else 0, n, m, ld, _p(lfc), _p(se), _p(stat),
-                                         _p(pvalue), int(negate), _p(zero_mask), int(lrt), int(alt),
-                                         float(lfcThreshold), _p(maxCooks), float(cooksCutoff), _p(keep),
-                                         _p(replace), _p(baseMean), *(_p(t) for t in out), _stream()),
+    _lib.check(L.b200nb_results_gene_dev(D._p(ynz), D._ytype(ynz), n, m, ld, D._p(lfc), D._p(se), D._p(stat),
+                                         D._p(pvalue), int(negate), D._p(zero_mask), int(lrt), int(alt),
+                                         float(lfcThreshold), D._p(maxCooks), float(cooksCutoff), D._p(keep),
+                                         D._p(replace), D._p(baseMean), *(D._p(t) for t in out), D._stream()),
                "results_gene_dev")
     return out
 
@@ -1483,8 +1479,8 @@ def results_heuristic(ynz, m, rows, cooks_rows, keep):
     its Cook's row cooks_rows[r]).  Enqueue only."""
     L = _lib.lib()
     n, ld = ynz.shape
-    _lib.check(L.b200nb_results_heuristic_dev(_p(ynz), 1 if ynz.dtype == F64 else 0, _p(rows), rows.numel(), m, ld,
-                                              _p(cooks_rows), cooks_rows.shape[1], _p(keep), _stream()),
+    _lib.check(L.b200nb_results_heuristic_dev(D._p(ynz), D._ytype(ynz), D._p(rows), rows.numel(), m, ld,
+                                              D._p(cooks_rows), cooks_rows.shape[1], D._p(keep), D._stream()),
                "results_heuristic_dev")
 
 

@@ -17,8 +17,14 @@
  *   - host entry points take HOST pointers, copy to the current CUDA device, run the kernels, copy the
  *     results back; they are synchronous.  Inputs are never modified.
  *   - *_dev entry points take DEVICE pointers in the engine's gene-major layout (one gene per row, sample
- *     axis contiguous, row stride ld elements, ld % 4 == 0, base 16-byte aligned) and enqueue on `stream`
- *     (a cudaStream_t passed as void*; NULL = legacy default stream) without synchronising.
+ *     axis contiguous, row stride ld >= m elements) and enqueue on `stream` (a cudaStream_t passed as void*;
+ *     NULL = legacy default stream) without synchronising.  The GLM, prep, Cook's, size-factor and
+ *     sf_iterate_objective entry points read rows with 16-byte loads: there ld % 4 == 0 and every matrix base is
+ *     16-byte aligned.  The layout helpers, transform, rlog_* and results_* entry points accept any ld >= m.
+ *   - arguments are checked before anything is enqueued: y_type is B200NB_Y_INT32 or B200NB_Y_F64, every ld
+ *     (ld_out, ld_cooks) is >= m, and no pointer an entry point reads or writes is NULL when it has work
+ *     (n > 0); the pointers documented as optional may be NULL.  A call with n == 0 that passes its checks
+ *     does nothing and succeeds, unless its entry point states that it needs n >= 1.
  *   - every function returns 0 on success, non-zero on failure; b200nb_last_error() then returns a
  *     message (thread-local).  Per-gene numerical failure is in-band exactly as in the reference
  *     (iter == maxit sentinel, NaN coefficients), never an error (src/DESeq2.cpp:357-360,375-378).

@@ -18,7 +18,7 @@ EMU = "libb200nb_emu" in os.environ.get("B200NB_LIB", "")   # dry run of this sc
 if EMU:
     import ctypes
     import time
-    D._stream = DP._stream = lambda: ctypes.c_void_p(0)
+    D._stream = lambda: ctypes.c_void_p(0)
 x = synth.design_factor(m, 10)
 d = synth.make_example_counts(n, m, x=x, seed=11, betaSD=0.5)
 dev = torch.device("cpu" if EMU else "cuda")

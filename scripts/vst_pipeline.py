@@ -64,11 +64,11 @@ def main():
             torch.cuda.synchronize()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             L = _lib.lib()
-            st = DP._stream()
+            st = D._stream()
             mcode = DP._TRANSFORM_MODE[mode]
             e0.record()
             for _ in range(200):
-                L.b200nb_transform_dev(DP._p(y), 0, DP._p(sf), None, n, m, y.shape[1], mcode, c0, c1, DP._p(out), m,
+                L.b200nb_transform_dev(D._p(y), 0, D._p(sf), None, n, m, y.shape[1], mcode, c0, c1, D._p(out), m,
                                        st)
             e1.record()
             torch.cuda.synchronize()

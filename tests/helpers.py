@@ -2,6 +2,7 @@
 import os
 
 import numpy as np
+import pytest
 
 from deseq2_b200 import pipeline, synth
 
@@ -10,6 +11,21 @@ from deseq2_b200 import pipeline, synth
 # pointers (tests/conftest.py then also replaces the CUDA stream getters of the torch wrappers by a null stream).
 EMULATED = "libb200nb_emu" in os.path.basename(os.environ.get("B200NB_LIB", ""))
 DEV = "cpu" if EMULATED else "cuda"
+
+
+@pytest.fixture(scope="module")
+def emu_dev(emu):
+    """The emulated engine with CPU tensors: device pointers are host pointers, there is no CUDA stream.  Every binding
+    takes its stream from deseq2_b200.device._stream at call time, so replacing that one getter covers them all."""
+    import ctypes as C
+    from deseq2_b200 import device as D
+    saved = D._stream
+    D._stream = lambda: C.c_void_p(0)
+    try:
+        yield emu
+    finally:
+        D._stream = saved
+
 
 DISP_KEYS = ("log_alpha", "last_change", "initial_lp", "initial_dlp", "last_lp", "last_dlp", "last_d2lp")
 

@@ -106,9 +106,7 @@ def emu_device(emu, monkeypatch):
     and there are no streams, so the torch plumbing runs unchanged with device = "cpu"."""
     import test_device_pipeline_gpu as TD
     from deseq2_b200 import device as D, device_pipeline as DP
-    null_stream = lambda: C.c_void_p(0)
-    monkeypatch.setattr(D, "_stream", null_stream)
-    monkeypatch.setattr(DP, "_stream", null_stream)
+    monkeypatch.setattr(D, "_stream", lambda: C.c_void_p(0))
     monkeypatch.setattr(TD, "DEV", "cpu")
     import test_size_factors_gpu as TS
     monkeypatch.setattr(TS, "DEV", "cpu")

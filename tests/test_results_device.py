@@ -10,21 +10,10 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DEV
+from helpers import DEV, emu_dev
 from deseq2_b200 import pipeline, synth
 
 NAN = np.nan
-
-
-@pytest.fixture(scope="module")
-def emu_dev(emu):
-    from deseq2_b200 import device as D, device_pipeline as DP
-    saved = D._stream, DP._stream
-    D._stream = DP._stream = lambda: C.c_void_p(0)
-    try:
-        yield emu
-    finally:
-        D._stream, DP._stream = saved
 
 
 # ---------------------------------------------------------------- host pieces
@@ -574,7 +563,7 @@ def _sharded_worker(rank, world, port, q, emu_lib):
     import torch.distributed as dist
     from deseq2_b200 import _lib, device as D, device_pipeline as DP, sharded
     _lib._SO, _lib._lib = emu_lib, None            # this module imported the package before B200NB_LIB was set
-    D._stream = DP._stream = lambda: C.c_void_p(0)
+    D._stream = lambda: C.c_void_p(0)
     dist.init_process_group("gloo", rank=rank, world_size=world)
     K, x, factors, sf = _sharded_case()
     lo, hi = sharded.shard_bounds(K.shape[0], world, rank)

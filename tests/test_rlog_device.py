@@ -10,21 +10,9 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DEV
+from helpers import DEV, emu_dev
 
 LN2 = np.log(2.0)
-
-
-@pytest.fixture(scope="module")
-def emu_dev(emu):
-    """The emulated engine with CPU tensors: device pointers are host pointers, there is no CUDA stream."""
-    from deseq2_b200 import device as D, device_pipeline as DP
-    saved = D._stream, DP._stream
-    D._stream = DP._stream = lambda: C.c_void_p(0)
-    try:
-        yield emu
-    finally:
-        D._stream, DP._stream = saved
 
 
 @pytest.fixture(scope="module")

@@ -91,8 +91,8 @@ def _device_worker(rank, world, port, q, emu_lib):
     import ctypes as C
     import torch
     import torch.distributed as dist
-    from deseq2_b200 import device as D, device_pipeline as DP, sharded, synth
-    D._stream = DP._stream = lambda: C.c_void_p(0)          # emulated engine: host pointers, no CUDA stream
+    from deseq2_b200 import device as D, sharded, synth
+    D._stream = lambda: C.c_void_p(0)          # emulated engine: host pointers, no CUDA stream
     dist.init_process_group("gloo", rank=rank, world_size=world)
     m = 12
     x = synth.design_condition(m)
@@ -127,15 +127,15 @@ def test_sharded_device_pipeline_equals_whole(emu):
     for p in procs:
         p.join(timeout=60)
         assert p.exitcode == 0
-    saved = D._stream, DP._stream
-    D._stream = DP._stream = lambda: C.c_void_p(0)
+    saved = D._stream
+    D._stream = lambda: C.c_void_p(0)
     try:
         m = 12
         x = synth.design_condition(m)
         d = synth.make_example_counts(400, m, x=x, seed=91)
         whole = DP.DESeq_device(D.to_gene_major(d["counts"], torch.device("cpu")), x, d["sizeFactors"])
     finally:
-        D._stream, DP._stream = saved
+        D._stream = saved
     assert np.array_equal(got["trend"], whole["trendCoefs"].numpy()) and got["priorVar"] == whole["dispPriorVar"]
     assert 0 < got["n_local"] < whole["idx"].numel()
     assert np.array_equal(got["disp"], whole["dispersion"].numpy())

@@ -10,22 +10,10 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, rel_err
+from helpers import DEV, emu_dev, rel_err
 
 LN2 = np.log(2.0)
 MODES = {"parametric": (0, 0.05, 2.0), "mean": (1, 0.07, 0.0), "log2": (2, 1.0, 0.0)}
-
-
-@pytest.fixture(scope="module")
-def emu_dev(emu):
-    """The emulated engine with CPU tensors: device pointers are host pointers, there is no CUDA stream."""
-    from deseq2_b200 import device as D, device_pipeline as DP
-    saved = D._stream, DP._stream
-    D._stream = DP._stream = lambda: C.c_void_p(0)
-    try:
-        yield emu
-    finally:
-        D._stream, DP._stream = saved
 
 
 def _gm(a, dev):

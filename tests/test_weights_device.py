@@ -15,21 +15,9 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, rel_err
+from helpers import DEV, emu_dev, rel_err
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def emu_dev(emu):
-    """The emulated engine with CPU tensors: device pointers are host pointers, there is no CUDA stream."""
-    from deseq2_b200 import device as D, device_pipeline as DP
-    saved = D._stream, DP._stream
-    D._stream = DP._stream = lambda: C.c_void_p(0)
-    try:
-        yield emu
-    finally:
-        D._stream, DP._stream = saved
 
 
 def _gm(a, dev):
@@ -435,7 +423,7 @@ def _sharded_worker(rank, world, port, q, emu_lib):
     import torch.distributed as dist
     from deseq2_b200 import _lib, device as D, device_pipeline as DP, sharded, synth
     _lib._SO, _lib._lib = emu_lib, None          # this module imported the package before B200NB_LIB was set
-    D._stream = DP._stream = lambda: C.c_void_p(0)
+    D._stream = lambda: C.c_void_p(0)
     warnings.simplefilter("ignore")
     dist.init_process_group("gloo", rank=rank, world_size=world)
     x = synth.design_batch_condition(12, 3)
