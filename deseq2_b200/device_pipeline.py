@@ -45,7 +45,7 @@ from . import device as D
 # device_pipeline._p / ._stream; the bindings below call D._p and D._stream() at call time, so replacing
 # device._stream is what changes the stream they use.
 from .device import _p, _stream  # noqa: F401
-from .pipeline import modelMatrixGroups
+from .pipeline import check_test_args, modelMatrixGroups
 
 F64 = torch.float64
 LN2 = float(np.log(2.0))
@@ -504,26 +504,15 @@ def nbinomLRT_device(ynz, x_full, x_reduced, sizeFactors, dispersion, betaTol=1e
     normalizationFactors: gene-major (n, ld) float64 factors of the rows, in place of sizeFactors (None then); both
     fits, their start values and log-likelihoods use them, and the intercept-only reduced model is an IRLS fit as on
     the size-factor path."""
-    dev = ynz.device
     sfd = _size_or_norm_factors(ynz, np.asarray(x_full).shape[0], sizeFactors, normalizationFactors, weights)
     wn = None if weights is None else normalize_weights(weights, ynz, np.asarray(x_full).shape[0])
     res = {}
     for name, x in (("full", x_full), ("reduced", x_reduced)):
-        x = np.asarray(x, dtype=np.float64)
-        m, p = x.shape
-        if wn is not None and name == "reduced" and p == 1 and np.all(x == 1):
-            res[name] = _intercept_only_weighted(ynz, sfd, dispersion, wn, m)
-            continue
-        pr = prep(ynz, x, sizeFactors, minmu=minmu, want_mu=False, normalizationFactors=normalizationFactors)
-        contrast, lam = _mle_penalty(p, dev)
-        fit, ll, conv, _ = _glm_fit(ynz, pr["xd"], sfd, dispersion, contrast, pr["beta0"], lam, betaTol=betaTol,
-                                    maxit=maxit, minmu=minmu, useOptim=useOptim, weights=wn,
-                                    want_hat=(name == "full"), want_mu=(name == "full"))
-        fit["conv"], fit["logLike"], fit["mu"] = conv, ll["logLike"], ll["mu"]
-        res[name] = fit
+        res[name] = _lrt_model_fit(ynz, x, sizeFactors, sfd, dispersion, wn, closed_form=wn is not None,
+                                   betaTol=betaTol, maxit=maxit, minmu=minmu, useOptim=useOptim,
+                                   normalizationFactors=normalizationFactors, full=(name == "full"))
     df = x_full.shape[1] - x_reduced.shape[1]
-    stat = 2.0 * (res["full"]["logLike"] - res["reduced"]["logLike"])
-    pval = torch.special.gammaincc(torch.tensor(df / 2.0, dtype=F64, device=dev), torch.clamp(stat, min=0.0) / 2.0)
+    stat, pval = _lrt_stats(res["full"]["logLike"], res["reduced"]["logLike"], df)
     return {"LRTStatistic": stat, "LRTPvalue": pval, "deviance": -2.0 * res["full"]["logLike"], "df": df,
             "betaMatrix": (res["full"]["beta_mat"] / LN2).T,
             "betaSE": (torch.sqrt(torch.clamp(res["full"]["beta_var_mat"], min=0.0)) / LN2).T,
@@ -531,13 +520,51 @@ def nbinomLRT_device(ynz, x_full, x_reduced, sizeFactors, dispersion, betaTol=1e
             "mu": res["full"]["mu"], "H": res["full"]["hat_diagonals"]}
 
 
-def _intercept_only_weighted(ynz, sfd, dispersion, wn, m):
-    """R/fitNbinomGLMs.R:99-137 with weights: beta = log2(sum(w K/s) / sum(w)), log-likelihood sum(w log dnbinom) at
-    mu = s 2^beta (b200nb_nb_loglik_dev with the weights); no IRLS."""
+def _is_intercept_only(x):
+    """fitNbinomGLMs' justIntercept for a model matrix (R/fitNbinomGLMs.R:99-103): one column, every entry 1."""
+    return x.shape[1] == 1 and bool(np.all(x == 1))
+
+
+def _lrt_model_fit(ynz, x, sizeFactors, sfd, dispersion, wn, closed_form, betaTol=1e-8, maxit=100, minmu=0.5,
+                   useOptim=True, normalizationFactors=None, full=False):
+    """One of nbinomLRT's two fitNbinomGLMs calls (R/core.R:1850-1873) on the rows of ynz: an intercept-only model by
+    R's closed form when closed_form is set (_intercept_only), else the pre-step kernel's start values and _glm_fit,
+    with the hat diagonals and the fitted mean only for the full model.  Returns the fitBeta result (the closed form:
+    "beta_mat" only) with "conv", "logLike" and "mu" added.  The start values need no xim: it is passed as 1 so that
+    the nf path makes no host read."""
+    x = np.asarray(x, dtype=np.float64)
+    m, p = x.shape
+    if closed_form and _is_intercept_only(x):
+        return _intercept_only(ynz, sfd, dispersion, wn, m)
+    pr = prep(ynz, x, sizeFactors, minmu=minmu, want_mu=False, normalizationFactors=normalizationFactors, xim=1.0)
+    contrast, lam = _mle_penalty(p, ynz.device)
+    fit, ll, conv, _ = _glm_fit(ynz, pr["xd"], sfd, dispersion, contrast, pr["beta0"], lam, betaTol=betaTol,
+                                maxit=maxit, minmu=minmu, useOptim=useOptim, weights=wn, want_hat=full, want_mu=full)
+    fit["conv"], fit["logLike"], fit["mu"] = conv, ll["logLike"], ll["mu"]
+    return fit
+
+
+def _lrt_stats(ll_full, ll_reduced, df):
+    """nbinomLRT's LRTStatistic = 2 (logLike_full - logLike_reduced) (R/core.R:1877) and its chi-square upper tail with
+    df degrees of freedom."""
+    stat = 2.0 * (ll_full - ll_reduced)
+    pval = torch.special.gammaincc(torch.tensor(df / 2.0, dtype=F64, device=stat.device),
+                                   torch.clamp(stat, min=0.0) / 2.0)
+    return stat, pval
+
+
+def _intercept_only(ynz, sfd, dispersion, wn, m):
+    """R/fitNbinomGLMs.R:99-137, no IRLS: beta = log(mean of K/nf), or log(sum(w K/nf) / sum(w)) with the normalised
+    weights wn, and the log-likelihood (weighted with wn) at mu = nf e^beta by b200nb_nb_loglik_dev.  sfd: the
+    size-factor vector or the gene-major nf rows of ynz."""
     dev = ynz.device
-    norm = ynz[:, :m].to(F64) / sfd[None, :]
-    w = wn[:, :m]
-    beta = torch.log((w * norm).sum(dim=1) / w.sum(dim=1))[None, :].contiguous()    # (1, n), natural-log scale
+    norm = ynz[:, :m].to(F64) / (sfd[:, :m] if sfd.dim() == 2 else sfd[None, :])
+    if wn is None:
+        beta = torch.log(norm.mean(dim=1))
+    else:
+        w = wn[:, :m]
+        beta = torch.log((w * norm).sum(dim=1) / w.sum(dim=1))
+    beta = beta[None, :].contiguous()                                                # (1, n), natural-log scale
     ones = torch.ones((1, m), dtype=F64, device=dev)
     ll = D.nb_loglik(ynz, ones, sfd, dispersion, beta, weights=wn, want_mu=False)
     return {"beta_mat": beta, "logLike": ll["logLike"], "mu": None,
@@ -736,7 +763,7 @@ def _wald_stats(fit):
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
                  outlierSD=2.0, minReplicatesForReplace=np.inf, allgather=None, useOptim=True, betaPrior=False,
                  factors=None, weights=None, weightThreshold=1e-2, normalizationFactors=None, avgTxLength=None,
-                 nfXim=None, sfType="ratio", fitType="parametric"):
+                 nfXim=None, sfType="ratio", fitType="parametric", test="Wald", reduced=None):
     """y: gene-major (N, ld) device tensor of counts (int32 or float64).  Returns a dict of device tensors over the
     rows with a non-zero sum (`idx` maps them back to the N input rows) plus the trend / prior scalars.
     sizeFactors=None estimates them on the device first (median of ratios, R/core.R:535-578; returned under
@@ -777,10 +804,22 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     "sfIterate").  "iterate" with weights, normalizationFactors or avgTxLength raises ValueError.
     fitType: "parametric" (the default; "trendCoefs") or "mean": dispFit is the trimmed mean of the gathered
     gene-wise estimates (mean_disp, no extra collective), reported under "meanDisp" instead of "trendCoefs".  Both
-    are reported under "fitType"."""
+    are reported under "fitType".
+    test="LRT", reduced=<(m, p_r) numpy model matrix nested in x>: DESeq(test = "LRT") with matrices (R/core.R:318-341,
+    nbinomLRT :1787-2012).  The dispersions and the fit on x are the Wald path's: that fit is nbinomLRT's full fit (the
+    same fitNbinomGLMs call), so its mu / H give the Cook's distances and the Wald columns stay, as R's
+    results(test = "Wald") derives them from an LRT object (makeWaldTest, R/results.R:1101-1116).  One more fit on the
+    same rows, dispersions, minmu, useOptim and weights is added: R's closed form when reduced is ~1
+    (R/fitNbinomGLMs.R:99-137, no IRLS), else the pre-step kernel's start values and an IRLS fit with the optim
+    fallback.  Adds "LRTStatistic" = 2 (logLike_full - logLike_reduced), "LRTPvalue" (chi-square upper tail, df = p -
+    p_r), "df", "fullBetaConv" (= betaConv), "reducedBetaConv" and "reducedModelMatrix".  With outlier replacement the
+    refitted rows get the reduced fit too and their LRT columns are overwritten (R/core.R:2530-2531).  R's stops
+    raise ValueError: no reduced, betaPrior=True, p_r >= p, a model matrix that is not full rank, and reduced with
+    test="Wald".  "test" reports the test ("Wald" or "LRT") for results_device."""
     dev = y.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
+    reduced = check_test_args(x, test, reduced, betaPrior)
     if sfType not in ("ratio", "poscounts", "iterate"):
         raise ValueError("sfType must be 'ratio', 'poscounts' or 'iterate'")
     if fitType not in ("parametric", "mean"):
@@ -923,6 +962,17 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     ck = cooks(ynz, mu_cooks, fb["hat_diagonals"], x, sizeFactors, want_matrix=do_replace,   # R/core.R:1457-1460
                normalizationFactors=sfd if nf is not None else None)
     mark("wald_stats+cooks")
+    lrt = {}
+    if test == "LRT":
+        # nbinomLRT (R/core.R:1850-1877): the fit above is its full fit; only the reduced model is fitted here
+        red = _lrt_model_fit(ynz, reduced, sizeFactors, sfd, dispersion, wn, closed_form=True, betaTol=betaTol,
+                             maxit=maxit, minmu=minmu, useOptim=useOptim, normalizationFactors=sfd if nf is not None
+                             else None)
+        df = p - reduced.shape[1]
+        stat, pval = _lrt_stats(fit_ll["logLike"], red["logLike"], df)
+        lrt = {"LRTStatistic": stat, "LRTPvalue": pval, "df": df, "reducedBetaConv": red["conv"],
+               "reducedModelMatrix": reduced}
+        mark("lrt_reduced_fit")
     res = {"stage_ms": stage_ms, "maxCooks": ck["maxCooks"], "idx": idx, "baseMean": bm, "dispGeneEst": dge, "dispFit": dispFit, "dispMAP": dispMAP,
             "dispersion": dispersion, "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": dispIter,
             **_wald_stats(fit),
@@ -930,7 +980,8 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
             "H": fb["hat_diagonals"], "varLogDispEsts": varLogDispEsts,
             "dispPriorVar": dispPriorVar, "n_refit_geneest": n_refit_geneest, "n_refit_map": n_refit_map,
             "n_input_rows": y.shape[0],
-            "sizeFactors": None if nf is not None else np.asarray(sizeFactors, dtype=np.float64), "fitType": fitType}
+            "sizeFactors": None if nf is not None else np.asarray(sizeFactors, dtype=np.float64), "fitType": fitType,
+            "test": test, **lrt}
     if fitType == "mean":
         res["meanDisp"] = float(tr[0].item())
     else:
@@ -945,7 +996,9 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     if do_replace and m > p:
         _replace_and_refit(res, ynz, ck["cooks"], x, sizeFactors, sfd, tr, minReplicatesForReplace, minDisp=minDisp,
                            kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, betaTol=betaTol, minmu=minmu,
-                           outlierSD=outlierSD, useOptim=useOptim)
+                           outlierSD=outlierSD, useOptim=useOptim, reduced=reduced if test == "LRT" else None)
+    if test == "LRT":
+        res["fullBetaConv"] = res["betaConv"]
     return res
 
 
@@ -991,13 +1044,16 @@ def _replacement_counts(ys, nfm, over, replaceable, m, trim=0.2):
 
 
 def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, minReplicates, minDisp=1e-8, kappa_0=1.0,
-                       dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5, outlierSD=2.0, useOptim=True, trim=0.2):
+                       dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5, outlierSD=2.0, useOptim=True, trim=0.2,
+                       reduced=None):
     """replaceOutliers + refitWithoutOutliers (R/core.R:2069-2115, 2484-2565) on the device results `res` (in place).
     Only the flagged rows move: their counts are gathered, the outlying entries of replaceable samples become
     as.integer(trimmed mean of the normalised counts * size factor), and the rows go through DESeq_device's stages
     (GeneEst -> MAP -> Wald) with the trend `tr` and res's prior variance, as refitWithoutOutliers does with
     objectSub.  `sfd` is the size-factor vector or the nf matrix of ynz's rows: with nf the trimmed mean is of K/nf
-    and the replacement count trunc(trimmed mean * nf_ij) (R/core.R:2089-2096)."""
+    and the replacement count trunc(trimmed mean * nf_ij) (R/core.R:2089-2096).  reduced (test="LRT"): the rows also
+    get the reduced fit and their LRT columns are overwritten, as nbinomLRT(objectSub) does (R/core.R:2530-2531).
+    Every fit here takes DESeq_device's minmu, where R's refit passes none (0.5)."""
     from scipy import stats as _st
     from .pipeline import nOrMoreInCell
     dev = ynz.device
@@ -1039,10 +1095,18 @@ def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, minReplicates,
         sub = {"dispGeneEst": dge, "dispFit": dispFit, "dispMAP": dispMAP, "dispersion": dispersion,
                "dispOutlier": dispOutlier, "dispGeneIter": r["iter"], "dispIter": dispIter, **_wald_stats(fb),
                "betaIter": fb["iter"], "betaConv": betaConv, "deviance": -2.0 * ll["logLike"]}
+        results_cols = ["betaMatrix", "betaSE", "WaldStatistic", "WaldPvalue", "deviance"]
+        if reduced is not None:
+            red = _lrt_model_fit(ysub, reduced, sizeFactors, sfs, dispersion, None, closed_form=True, betaTol=betaTol,
+                                 maxit=maxit, minmu=minmu, useOptim=useOptim,
+                                 normalizationFactors=sfs if sfd.dim() == 2 else None)
+            sub["LRTStatistic"], sub["LRTPvalue"] = _lrt_stats(ll["logLike"], red["logLike"], res["df"])
+            sub["reducedBetaConv"] = red["conv"]
+            results_cols += ["LRTStatistic", "LRTPvalue"]
         for k, v in sub.items():
             res[k] = res[k].clone()
             res[k][rr] = v.to(res[k].dtype)
-        for k in ("betaMatrix", "betaSE", "WaldStatistic", "WaldPvalue", "deviance"):
+        for k in results_cols:
             res[k][rows[newAllZero]] = float("nan")
         if bool(replaceable.all()):
             res["maxCooks"] = torch.full_like(res["maxCooks"], float("nan"))
@@ -1500,7 +1564,7 @@ def _first_fit_cooks(res, ynz, rows, x, sfd):
 
 def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcThreshold=0, altHypothesis="greaterAbs",
                    cooksCutoff=None, independentFiltering=True, alpha=0.1, filter=None, theta=None,
-                   pAdjustMethod="BH", factors=None, lrt=None, minmu=0.5, weights=None, allgather=None):
+                   pAdjustMethod="BH", factors=None, lrt=None, minmu=0.5, weights=None, allgather=None, test=None):
     """results() + pvalueAdjustment() (R/results.R:298-740) on a DESeq_device result `res` for the gene-major (N, ld)
     counts y it was run on and its design x.  Arguments as pipeline.results (the host mirror): name / contrast /
     listValues select the column (pipeline.resultsSelection; list and numeric contrasts, factor-level contrasts that
@@ -1519,13 +1583,28 @@ def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcT
     filter), and "metadata".
     allgather (sharded_results_device): concatenates a list of per-gene vectors over the ranks in rank order (one
     collective); [filter, pvalue] of this rank's rows travel in it, the cutoffs, counts and adjusted column are
-    computed on all genes, and this rank keeps the padj of its own rows (sharded.shard_bounds)."""
+    computed on all genes, and this rank keeps the padj of its own rows (sharded.shard_bounds).
+    test: as R's results(test =), by default the test DESeq_device ran (res["test"]).  An LRT result
+    (DESeq_device(test="LRT")) gives its LRTStatistic / LRTPvalue with the selected column's log2FoldChange / lfcSE;
+    test="Wald" on it gives the Wald columns (makeWaldTest).  test="LRT" on a Wald result, and lrt= with an LRT result,
+    raise ValueError."""
     from scipy import stats as _st
     from .pipeline import check_filter_args, results_checks, resultsSelection
     dev = y.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
     N = y.shape[0]
+    ran = res.get("test", "Wald")
+    test = ran if test is None else test
+    if test not in ("Wald", "LRT"):
+        raise ValueError("test must be 'Wald' or 'LRT'")
+    if test == "LRT" and ran == "Wald":
+        raise ValueError("the LRT requires the user run nbinomLRT or DESeq(dds,test='LRT')")
+    if ran == "LRT":
+        if lrt is not None:
+            raise ValueError("this DESeq_device result holds its own LRT: lrt= is for a Wald result")
+        if test == "LRT":
+            lrt = {"LRTStatistic": res["LRTStatistic"], "LRTPvalue": res["LRTPvalue"]}
     idx = res["idx"]
     betaPrior = res.get("modelMatrix") is not None
     thresholded = results_checks(lfcThreshold, altHypothesis, lrt is not None, betaPrior, alpha)

@@ -264,6 +264,31 @@ def dqrdc2_rank(z, tol=1e-7):
     return min(k - 1, n)
 
 
+def check_test_args(x, test, reduced, betaPrior):
+    """DESeq()'s checks of test / reduced for model matrices (R/core.R:318-344; checkFullRank :2624-2644 with R's qr
+    rank).  Raises ValueError as R stops; returns reduced as a float64 matrix (None for the Wald test)."""
+    if test not in ("Wald", "LRT"):
+        raise ValueError("test must be 'Wald' or 'LRT'")
+    if test == "Wald":
+        if reduced is not None:
+            raise ValueError("'reduced' ignored when test='Wald'")
+        return None
+    if reduced is None:
+        raise ValueError("likelihood ratio test requires a 'reduced' design, see ?DESeq")
+    if betaPrior:
+        raise ValueError("test='LRT' does not support use of LFC shrinkage, use betaPrior=FALSE")
+    reduced = np.asarray(reduced, dtype=np.float64)
+    if reduced.ndim != 2 or reduced.shape[0] != x.shape[0] or reduced.shape[1] == 0:
+        raise ValueError(f"reduced must be a model matrix with one row per sample ({x.shape[0]}), got shape "
+                         f"{reduced.shape}")
+    for name, mm in (("full", x), ("reduced", reduced)):
+        if dqrdc2_rank(mm) < mm.shape[1]:
+            raise ValueError(f"the {name} model matrix is not full rank, so the model cannot be fit as specified")
+    if x.shape[1] <= reduced.shape[1]:
+        raise ValueError("the number of columns of 'full' should be more than the number of columns of 'reduced'")
+    return reduced
+
+
 def getAndCheckWeights(weights, x, weightThreshold=1e-2):
     """R/core.R:2697-2752 for a full-rank model matrix.  Returns (weights / row maximum, weightsFail).  Raises
     ValueError where the reference stops: a negative or NaN weight (stopifnot), a row without a positive weight or an
@@ -858,24 +883,35 @@ def _fit_intercept_only(counts, nf, alpha_hat, weights=None):
             "hat_diagonals": w / xtwx[:, None]}
 
 
+def fitReducedModel(counts, nf, reduced, dispersion, engine=None, betaTol=1e-8, maxit=100, useQR=True, minmu=0.5,
+                    useOptim=True, weights=None):
+    """nbinomLRT's reduced fit (R/core.R:1863-1873): the closed form for ~1 (_fit_intercept_only), else fitNbinomGLMs."""
+    if reduced.shape[1] == 1 and np.all(reduced == 1):
+        return _fit_intercept_only(counts, nf, dispersion, weights)
+    return fitNbinomGLMs(counts, nf, reduced, dispersion, engine=engine, betaTol=betaTol, maxit=maxit, useQR=useQR,
+                         minmu=minmu, useOptim=useOptim, weights=weights)
+
+
+def lrtStatistic(logLikeFull, logLikeReduced, df):
+    """LRTStatistic = 2 (logLike_full - logLike_reduced) and its pchisq upper tail (R/core.R:1877-1878)."""
+    from scipy import stats as _st
+    stat = 2.0 * (logLikeFull - logLikeReduced)
+    return stat, _st.chi2.sf(stat, df)
+
+
 def nbinomLRT(counts, nf, full, reduced, dispersion, engine=None, betaTol=1e-8, maxit=100, useQR=True, minmu=0.5,
               useOptim=True, weights=None):
     """R/core.R:1787-2012 with user-supplied model matrices, betaPrior=FALSE; Cook's distances are not restated.
     `full` / `reduced` are m x p model matrices (reduced nested in full); `weights`: normalised weights or None."""
-    from scipy import stats as _st
     counts = np.asarray(counts)
     if reduced.shape[1] >= full.shape[1]:
         raise ValueError("less than one degree of freedom, perhaps full and reduced models are not in the correct order")
     fullModel = fitNbinomGLMs(counts, nf, full, dispersion, engine=engine, betaTol=betaTol, maxit=maxit, useQR=useQR,
                               minmu=minmu, useOptim=useOptim, weights=weights)
-    if reduced.shape[1] == 1 and np.all(reduced == 1):
-        reducedModel = _fit_intercept_only(counts, nf, dispersion, weights)
-    else:
-        reducedModel = fitNbinomGLMs(counts, nf, reduced, dispersion, engine=engine, betaTol=betaTol, maxit=maxit,
-                                     useQR=useQR, minmu=minmu, useOptim=useOptim, weights=weights)
+    reducedModel = fitReducedModel(counts, nf, reduced, dispersion, engine=engine, betaTol=betaTol, maxit=maxit,
+                                   useQR=useQR, minmu=minmu, useOptim=useOptim, weights=weights)
     df = full.shape[1] - reduced.shape[1]
-    LRTStatistic = 2.0 * (fullModel["logLike"] - reducedModel["logLike"])
-    LRTPvalue = _st.chi2.sf(LRTStatistic, df)
+    LRTStatistic, LRTPvalue = lrtStatistic(fullModel["logLike"], reducedModel["logLike"], df)
     return {"LRTStatistic": LRTStatistic, "LRTPvalue": LRTPvalue, "deviance": -2.0 * fullModel["logLike"],
             "betaMatrix": fullModel["betaMatrix"], "betaSE": fullModel["betaSE"], "fullBetaConv": fullModel["betaConv"],
             "reducedBetaConv": reducedModel["betaConv"], "betaIter": fullModel["betaIter"], "mu": fullModel["mu"],
@@ -989,7 +1025,7 @@ def fitGLMsWithPrior(counts, nf, factors, dispersion, baseMean, dispFit, engine=
 
 def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.inf, useOptim=True, betaPrior=False,
           factors=None, weights=None, weightThreshold=1e-2, minmu=0.5, normalizationFactors=None, sfType="ratio",
-          fitType="parametric"):
+          fitType="parametric", test="Wald", reduced=None):
     """R/core.R:280-432 with test='Wald', fitType='parametric', betaPrior=FALSE by default.
     minReplicatesForReplace: the reference's default is 7 (outlier replacement + refit whenever a design cell has >= 7
     samples, R/core.R:419-426, refitWithoutOutliers :2484-2565); the default here is Inf = off, which is what the
@@ -1012,11 +1048,16 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     iteration and objective-call counts are returned under `sfIterate`.
     fitType: "parametric" (the default; `trendCoefs`) or "mean" (R/core.R:900-905; `meanDisp` instead of
     `trendCoefs`).  Both are reported under `fitType`.
+    test='LRT', reduced=<m x p_r model matrix>: nbinomLRT with the Wald path's full fit (the same fitNbinomGLMs call)
+    and fitReducedModel on the same rows; adds `LRTStatistic`, `LRTPvalue`, `df`, `fullBetaConv`, `reducedBetaConv`
+    and `reducedModelMatrix`, and the refitted rows of an outlier replacement get their LRT columns from the refit.
+    The test is reported under `test`.  R's stops raise ValueError (check_test_args).
     Returns per-gene vectors over ALL rows; all-zero rows carry NaN (buildDataFrameWithNARows, R/core.R:2232)."""
     engine = engine or _default_engine
     counts = np.asarray(counts)
     N, m = counts.shape
     p = x.shape[1]
+    reduced = check_test_args(np.asarray(x, dtype=np.float64), test, reduced, betaPrior)
     if sfType not in ("ratio", "poscounts", "iterate"):
         raise ValueError("sfType must be 'ratio', 'poscounts' or 'iterate'")
     if fitType not in ("parametric", "mean"):
@@ -1100,6 +1141,12 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
                 "dispIter": mp["dispIter"].astype(float), "maxCooks": recordMaxCooks(x, cooks)}
     if betaPrior:
         per_gene["mleBetaMatrix"] = gp["mleBetaMatrix"]
+    if test == "LRT":
+        red = fitReducedModel(cnz, nf, reduced, mp["dispersion"], engine=engine, minmu=minmu, useOptim=useOptim,
+                              weights=wnz)
+        df = p - reduced.shape[1]
+        per_gene["LRTStatistic"], per_gene["LRTPvalue"] = lrtStatistic(wt["logLike"], red["logLike"], df)
+        per_gene["reducedBetaConv"] = red["betaConv"].astype(float)
     extra = dict(prior)
     if np.isfinite(minReplicatesForReplace) and nOrMoreInCell(x, minReplicatesForReplace).any():
         # ---- refitWithoutOutliers (R/core.R:2484-2565) on the rows that had a count replaced
@@ -1125,10 +1172,17 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
                    "WaldPvalue": wt2["WaldPvalue"], "betaConv": wt2["betaConv"].astype(float),
                    "betaIter": wt2["betaIter"], "deviance": wt2["deviance"],
                    "dispGeneIter": ge2["dispGeneIter"].astype(float), "dispIter": mp2["dispIter"].astype(float)}
+            resultsCols = ["betaMatrix", "betaSE", "WaldStatistic", "WaldPvalue", "betaConv", "betaIter", "deviance"]
+            if test == "LRT":                                                    # nbinomLRT(objectSub) (:2530-2531)
+                red2 = fitReducedModel(sub, np.broadcast_to(_div(sfSub), sub.shape), reduced, mp2["dispersion"],
+                                       engine=engine, useOptim=useOptim)
+                upd["LRTStatistic"], upd["LRTPvalue"] = lrtStatistic(wt2["logLike"], red2["logLike"], df)
+                upd["reducedBetaConv"] = red2["betaConv"].astype(float)
+                resultsCols += ["LRTStatistic", "LRTPvalue", "reducedBetaConv"]
             for k, v in upd.items():
                 per_gene[k] = per_gene[k].copy()
                 per_gene[k][rr] = v
-            for k in ("betaMatrix", "betaSE", "WaldStatistic", "WaldPvalue", "betaConv", "betaIter", "deviance"):
+            for k in resultsCols:
                 per_gene[k][newAllZero] = np.nan                                 # "results" columns (:2534)
             if replaceable.all():
                 per_gene["maxCooks"] = np.full(len(cnz), np.nan)
@@ -1150,7 +1204,9 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     res = {k: full(np.asarray(v, dtype=np.float64)) for k, v in per_gene.items()}
     res.update({"sizeFactors": None if sfAll.ndim == 2 else sfAll, "allZero": mvAll["allZero"], "dispPriorVar": dispPriorVar,
                 "varLogDispEsts": tf["varLogDispEsts"], "n_refit_geneest": ge["n_refit"],
-                "n_refit_map": mp["n_refit"], "fitType": fitType})
+                "n_refit_map": mp["n_refit"], "fitType": fitType, "test": test})
+    if test == "LRT":
+        res.update(df=df, fullBetaConv=res["betaConv"], reducedModelMatrix=reduced)
     if fitType == "mean":
         res["meanDisp"] = tf["meanDisp"]
     else:

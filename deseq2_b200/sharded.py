@@ -146,7 +146,9 @@ def sharded_DESeq_device(y_local, x, sizeFactors=None, **kw):
     (m + 1 doubles), summed on every rank in rank order, so xim does not depend on the number of ranks (the reference's
     DESeqParallel uses each chunk's own xim instead, R/parallel.R:18-20).  Not supported with finite
     minReplicatesForReplace (the refitted rows' xim would need another collective) or avgTxLength (estimating the
-    factors needs a global median): estimate them on one device or pass them."""
+    factors needs a global median): estimate them on one device or pass them.
+    test="LRT", reduced=... (passed on to DESeq_device): the LRT columns are per gene, so no collective is added;
+    LRTStatistic and LRTPvalue travel in the result gather in place of WaldPvalue (1 + 2p + 2 doubles per gene)."""
     from . import device_pipeline as DP
     if kw.get("sfType") == "iterate":
         raise ValueError("sharded runs do not estimate iterate size factors (every perturbation needs a quantile over "
@@ -175,12 +177,17 @@ def sharded_DESeq_device(y_local, x, sizeFactors=None, **kw):
         kw["nfXim"] = DP.nf_xim(tot[:m], tot[m])
     res = DP.DESeq_device(y_local, x, sizeFactors, allgather=pg, **kw)
     p = res["betaMatrix"].shape[1]
+    lrt = res["test"] == "LRT"
+    tests = [res["LRTStatistic"], res["LRTPvalue"]] if lrt else [res["WaldPvalue"][:, k] for k in range(p)]
     cols = [res["dispersion"]] + [res["betaMatrix"][:, k] for k in range(p)] \
-        + [res["betaSE"][:, k] for k in range(p)] + [res["WaldPvalue"][:, k] for k in range(p)]
+        + [res["betaSE"][:, k] for k in range(p)] + tests
     g = pg(cols)
     res["gathered"] = {"dispersion": g[0], "betaMatrix": torch.stack(g[1:1 + p], dim=1),
-                       "betaSE": torch.stack(g[1 + p:1 + 2 * p], dim=1),
-                       "WaldPvalue": torch.stack(g[1 + 2 * p:1 + 3 * p], dim=1)}
+                       "betaSE": torch.stack(g[1 + p:1 + 2 * p], dim=1)}
+    if lrt:
+        res["gathered"]["LRTStatistic"], res["gathered"]["LRTPvalue"] = g[1 + 2 * p], g[2 + 2 * p]
+    else:
+        res["gathered"]["WaldPvalue"] = torch.stack(g[1 + 2 * p:1 + 3 * p], dim=1)
     res["collectives"] = pg.collectives
     return res
 
