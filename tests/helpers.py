@@ -1,4 +1,5 @@
 """Shared helpers for the parity tests: realistic fitDisp / fitBeta inputs built with the host glue."""
+import functools
 import os
 
 import numpy as np
@@ -25,6 +26,17 @@ def emu_dev(emu):
         yield emu
     finally:
         D._stream = saved
+
+
+def gm(a, dev, dtype=None):
+    """(n, m) numpy matrix -> gene-major (n, ld) tensor on `dev`: int32 for integer input, float64 otherwise, or
+    converted to `dtype` first."""
+    import torch
+    from deseq2_b200 import device as D
+    return D.to_gene_major(np.asarray(a, dtype=dtype), torch.device(dev))
+
+
+gm64 = functools.partial(gm, dtype=np.float64)          # counts as float64 too: the float64-count path of the kernels
 
 
 DISP_KEYS = ("log_alpha", "last_change", "initial_lp", "initial_dlp", "last_lp", "last_dlp", "last_d2lp")

@@ -4,17 +4,13 @@ on the expanded matrix against pipeline.DESeq(betaPrior=True) driving the same e
 The CPU tests run the engine's CUDA source on the SIMT emulator (`emu` fixture); the `-m gpu` tests run on a GPU, or on
 the emulator when B200NB_LIB points at it."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, emu_dev, rel_err
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from helpers import DEV, emu_dev, gm, rel_err
+from ranks import DEVICE, nccl_world, run_ranks
 
 
 def _factor(m, levels):
@@ -220,59 +216,42 @@ def test_beta_prior_argument_errors(emu_dev):
             fn(arg, x, d["sizeFactors"], betaPrior=True, factors=factors, minReplicatesForReplace=7)
 
 
-def _sharded_worker(rank, world, port, q, emu_lib):
-    sys.path.insert(0, ROOT)
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), OMP_NUM_THREADS="2", B200NB_LIB=emu_lib,
-                      B200NB_TEST_EMULATOR="1")
-    import torch.distributed as dist
-    from deseq2_b200 import _lib, device as D, device_pipeline as DP, pipeline, sharded, synth
-    _lib._SO, _lib._lib = emu_lib, None          # this module imported the package before B200NB_LIB was set
-    D._stream = lambda: C.c_void_p(0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    factors = [_factor(12, 3)]
+def _sharded_data(n, m, levels):
+    from deseq2_b200 import pipeline, synth
+    factors = [_factor(m, levels)]
     x = pipeline.factorDesign(factors)[0]
-    d = synth.make_example_counts(400, 12, x=x, seed=91)
-    lo, hi = sharded.shard_bounds(400, world, rank)
-    y = D.to_gene_major(d["counts"][lo:hi], torch.device("cpu"))
-    plain = sharded.sharded_DESeq_device(y, x, d["sizeFactors"])
-    r = sharded.sharded_DESeq_device(y, x, d["sizeFactors"], betaPrior=True, factors=factors)
-    if rank == 0:
-        q.put({"pv": r["betaPriorVar"], "beta": r["gathered"]["betaMatrix"].numpy(),
-               "se": r["gathered"]["betaSE"].numpy(), "pval": r["gathered"]["WaldPvalue"].numpy(),
-               "collectives": r["collectives"], "collectives_plain": plain["collectives"],
-               "n_local": int(r["idx"].numel())})
-    dist.barrier()
-    dist.destroy_process_group()
+    d = synth.make_example_counts(n, m, x=x, seed=91)
+    return d["counts"], x, d["sizeFactors"], factors
+
+
+def _sharded_rank(rank, world, dev, n, m, levels):
+    from deseq2_b200 import sharded
+    K, x, sf, factors = _sharded_data(n, m, levels)
+    lo, hi = sharded.shard_bounds(n, world, rank)
+    y = gm(K[lo:hi], dev)
+    plain = sharded.sharded_DESeq_device(y, x, sf)
+    r = sharded.sharded_DESeq_device(y, x, sf, betaPrior=True, factors=factors)
+    return {"betaPriorVar": r["betaPriorVar"], "gathered": r["gathered"],
+            "extra_collectives": r["collectives"] - plain["collectives"], "n_local": r["idx"].numel()}
+
+
+def _check_sharded(backend, n, m, levels, world=2):
+    """The prior variance is estimated from every gene's MLE coefficients (one extra packed all-gather), so
+    betaPriorVar and every gathered MAP result equal the single-process run bit for bit."""
+    from deseq2_b200 import device_pipeline as DP
+    got = run_ranks(_sharded_rank, n, m, levels, world=world, backend=backend)
+    K, x, sf, factors = _sharded_data(n, m, levels)
+    whole = DP.DESeq_device(gm(K, DEVICE[backend]), x, sf, betaPrior=True, factors=factors)
+    for g in got:
+        assert 0 < g["n_local"] < whole["idx"].numel()
+        assert g["extra_collectives"] == 1
+        assert np.array_equal(g["betaPriorVar"], whole["betaPriorVar"])
+        for k in ("betaMatrix", "betaSE", "WaldPvalue"):
+            assert np.array_equal(g["gathered"][k], whole[k].cpu().numpy(), equal_nan=True), k
 
 
 def test_sharded_beta_prior_equals_whole(emu_dev):
-    """Two gloo ranks: the prior variance is estimated from every gene's MLE coefficients (one extra packed
-    all-gather), so betaPriorVar and every gathered MAP result equal the single-process run bit for bit."""
-    import torch.multiprocessing as mp
-    sys.path.insert(0, os.path.join(ROOT, "tests", "simt_emu"))
-    import build_emu
-    from deseq2_b200 import device as D, device_pipeline as DP, pipeline, synth
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 35500 + (os.getpid() % 2000)
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, q, build_emu.build())) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = q.get(timeout=900)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    factors = [_factor(12, 3)]
-    x = pipeline.factorDesign(factors)[0]
-    d = synth.make_example_counts(400, 12, x=x, seed=91)
-    whole = DP.DESeq_device(D.to_gene_major(d["counts"], torch.device("cpu")), x, d["sizeFactors"], betaPrior=True,
-                            factors=factors)
-    assert 0 < got["n_local"] < whole["idx"].numel()
-    assert got["collectives"] == got["collectives_plain"] + 1
-    assert np.array_equal(got["pv"], whole["betaPriorVar"])
-    assert np.array_equal(got["beta"], whole["betaMatrix"].numpy(), equal_nan=True)
-    assert np.array_equal(got["se"], whole["betaSE"].numpy(), equal_nan=True)
-    assert np.array_equal(got["pval"], whole["WaldPvalue"].numpy(), equal_nan=True)
+    _check_sharded("gloo", 400, 12, 3)
 
 
 # ---------------------------------------------------------------- GPU (or the emulator with B200NB_LIB)
@@ -336,16 +315,5 @@ def test_config4_size(engine):
 
 
 @pytest.mark.gpu
-def test_sharded_beta_prior_over_nccl_equals_whole():
-    n_gpu = torch.cuda.device_count() if DEV == "cuda" else 0
-    if n_gpu < 2:
-        pytest.skip("needs at least 2 GPUs")
-    env = dict(os.environ)
-    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK", "MASTER_ADDR", "MASTER_PORT"):
-        env.pop(k, None)
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29643",
-                        os.path.join(ROOT, "scripts", "sharded_beta_prior_nccl.py")], env=env, capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0, (r.stdout[-2000:], r.stderr[-3000:])
-    assert "sharded == whole: True" in r.stdout and "extra collectives: 1" in r.stdout, r.stdout[-2000:]
+def test_sharded_beta_prior_over_nccl_equals_whole(engine):
+    _check_sharded("nccl", 20000, 60, 6, nccl_world())

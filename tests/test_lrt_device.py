@@ -4,26 +4,17 @@ R/fitNbinomGLMs.R:99-137, the device against the host mirror pipeline.DESeq(test
 refit of replaced genes, results_device on an LRT result (the applicable expectations of the reference's
 test_results.R and test_LRT.R) and the gene-sharded run.  The CPU tests run the engine's CUDA source on the SIMT
 emulator (`emu_dev`); the `-m gpu` tests run on a GPU, or on the emulator when B200NB_LIB points at it."""
-import ctypes as C
-import os
-import subprocess
-import sys
 import warnings
 
 import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, emu_dev, rel_err  # noqa: F401
+from helpers import DEV, emu_dev, gm, rel_err  # noqa: F401
 from deseq2_b200 import pipeline, synth
+from ranks import DEVICE, nccl_world, run_ranks
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LRT_KEYS = ("LRTStatistic", "LRTPvalue", "df", "fullBetaConv", "reducedBetaConv", "reducedModelMatrix", "test")
-
-
-def _gm(a, dev):
-    from deseq2_b200 import device as D
-    return D.to_gene_major(np.asarray(a), torch.device(dev))
 
 
 def _same(a, b):
@@ -57,10 +48,10 @@ def _weights(n, m, x, seed):
     return w
 
 
-def _case(kind, n=160, seed=11):
+def _case(kind, n=160, seed=11, m=12):
     """(counts, full, reduced, DESeq kwargs as numpy) of a named design."""
     if kind == "batch":                                       # C5-like: ~batch + condition vs ~batch
-        x = synth.design_batch_condition(12, 3)
+        x = synth.design_batch_condition(m, 3)
         xr = x[:, :3]
     elif kind == "intercept":                                 # ~condition vs ~1
         x = synth.design_condition(12)
@@ -79,7 +70,7 @@ def _device_kw(kw, K, x, dev):
     out = dict(kw)
     for k in ("weights", "normalizationFactors"):
         if out.get(k) is not None:
-            out[k] = _gm(out[k], dev)
+            out[k] = gm(out[k], dev)
     return out
 
 
@@ -98,7 +89,7 @@ def _check_composition(dev, K, x, xr, kw):
     """DESeq_device(test="LRT") == DESeq_device followed by nbinomLRT_device on its dispersions, bit for bit; every
     key the Wald run has is the same in the LRT run."""
     from deseq2_b200 import device_pipeline as DP
-    y = _gm(K, dev)
+    y = gm(K, dev)
     dkw = _device_kw(kw, K, x, dev)
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
@@ -133,7 +124,7 @@ def test_defaults_unchanged_emulated(emu_dev):
     """test="Wald" spelled out is the default call, and two calls give the same bits."""
     from deseq2_b200 import device_pipeline as DP
     K, x, _, kw = _case("batch")
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     a = _snapshot(DP.DESeq_device(y, x, **kw))
     b = _snapshot(DP.DESeq_device(y, x, test="Wald", **kw))
     assert all(_same(a[k], b[k]) for k in a if k != "stage_ms")
@@ -160,7 +151,7 @@ def test_intercept_closed_form_emulated(emu_dev, oracle, variant):
     from deseq2_b200 import device_pipeline as DP
     K, x, xr, kw = _case("intercept")
     kw = _variant(variant, K, x, kw)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
         res = DP.DESeq_device(y, x, test="LRT", reduced=xr, useOptim=False, **_device_kw(kw, K, x, "cpu"))
@@ -247,7 +238,7 @@ def _check_host(dev, engine, name, n=160):
     kw.update(extra)
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
-        dv = DP.DESeq_device(_gm(K, dev), x, test="LRT", reduced=xr, useOptim=False, **_device_kw(kw, K, x, dev))
+        dv = DP.DESeq_device(gm(K, dev), x, test="LRT", reduced=xr, useOptim=False, **_device_kw(kw, K, x, dev))
     rerun = _Rerun(engine, K, x, useOptim=False, test="LRT", reduced=xr, **kw)
     host = rerun()
     # with weights the GeneEst mean is an IRLS fit on both sides (no linear mu), stopped by betaTol = 1e-8: the
@@ -281,7 +272,7 @@ def _check_replacement(dev, engine, n=120):
     both sides, which differ there (L-BFGS-B vs Newton); the comparison is over the rows the IRLS fitted."""
     from deseq2_b200 import device_pipeline as DP
     K, x, xr, kw = _replace_case(n)
-    y = _gm(K, dev)
+    y = gm(K, dev)
     dv = _snapshot(DP.DESeq_device(y, x, test="LRT", reduced=xr, **kw))
     rerun = _Rerun(engine, K, x, test="LRT", reduced=xr, **kw)
     host = rerun()
@@ -324,7 +315,7 @@ def _results_case():
 def test_results_of_an_lrt_result_emulated(emu_dev):
     from deseq2_b200 import device_pipeline as DP
     K, x, xr, factors, sf = _results_case()
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     lrt = _snapshot(DP.DESeq_device(y, x, sf, test="LRT", reduced=xr))
     wald = _snapshot(DP.DESeq_device(y, x, sf))
     R = lambda res, **a: DP.results_device(res, y, x, factors=factors, **a)
@@ -364,7 +355,7 @@ def test_results_of_an_lrt_result_emulated(emu_dev):
 def test_errors_device_and_host(emu_dev):
     from deseq2_b200 import device_pipeline as DP
     K, x, xr, kw = _case("batch", n=40)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     factors = [np.array([0, 1, 2] * 4), np.repeat([0, 1], 6)]
     xb = pipeline.factorDesign(factors)[0]
     rank_def = np.c_[x, x[:, 1] + x[:, 3]]                     # a linear combination of the other columns
@@ -393,7 +384,7 @@ def test_small_sizes_emulated(emu_dev, N):
     for kind in ("batch", "intercept"):
         K, x, xr, kw = _case(kind, n=N + 6)
         K = K[K.sum(axis=1) > 0][:N]
-        y = _gm(K, "cpu")
+        y = gm(K, "cpu")
         kw["fitType"] = "mean" if N < 10 else "parametric"
         a = _snapshot(DP.DESeq_device(y, x, test="LRT", reduced=xr, **kw))
         b = _snapshot(DP.DESeq_device(y, x, test="LRT", reduced=xr, **kw))
@@ -404,69 +395,48 @@ def test_small_sizes_emulated(emu_dev, N):
             assert _same(a["LRTStatistic"], seq["LRTStatistic"])
 
 
-# ---------------------------------------------------------------- sharded (two gloo ranks, emulated engine)
+# ---------------------------------------------------------------- sharded
 
-def _sharded_case():
-    K, x, xr, kw = _case("batch", n=301, seed=93)
+def _sharded_case(n, m):
+    K, x, xr, kw = _case("batch", n=n, seed=93, m=m)
     K[250] = 0
     return K, x, xr, kw["sizeFactors"]
 
 
-def _sharded_worker(rank, world, port, q, emu_lib):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), OMP_NUM_THREADS="2", B200NB_LIB=emu_lib,
-                      B200NB_TEST_EMULATOR="1")
-    import torch.distributed as dist
-    from deseq2_b200 import _lib, device as D, sharded
-    _lib._SO, _lib._lib = emu_lib, None            # this module imported the package before B200NB_LIB was set
-    D._stream = lambda: C.c_void_p(0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    K, x, xr, sf = _sharded_case()
-    lo, hi = sharded.shard_bounds(K.shape[0], world, rank)
-    y = D.to_gene_major(K[lo:hi], torch.device("cpu"))
+def _sharded_rank(rank, world, dev, n, m):
+    from deseq2_b200 import sharded
+    K, x, xr, sf = _sharded_case(n, m)
+    lo, hi = sharded.shard_bounds(n, world, rank)
+    y = gm(K[lo:hi], dev)
     wald = sharded.sharded_DESeq_device(y, x, sf)
     r = sharded.sharded_DESeq_device(y, x, sf, test="LRT", reduced=xr)
     out = sharded.sharded_results_device(r, y, x)
-    if rank == 0:
-        q.put({"gathered": {k: v.numpy() for k, v in r["gathered"].items()}, "collectives": r["collectives"],
-               "collectives_wald": wald["collectives"], "results_collectives": out["collectives"]})
-    q.put((rank, out["stat"].numpy(), out["padj"].numpy()))
-    dist.barrier()
-    dist.destroy_process_group()
+    return {"gathered": r["gathered"], "extra_collectives": r["collectives"] - wald["collectives"],
+            "results_collectives": out["collectives"], "stat": out["stat"], "padj": out["padj"]}
+
+
+def _check_sharded(backend, n, m, world=2):
+    """The gathered LRT results equal the unsharded run bit for bit, through the Wald run's collectives; sharded
+    results() of the LRT result equals results_device of the whole."""
+    from deseq2_b200 import device_pipeline as DP
+    got = run_ranks(_sharded_rank, n, m, world=world, backend=backend)
+    K, x, xr, sf = _sharded_case(n, m)
+    y = gm(K, DEVICE[backend])
+    whole = DP.DESeq_device(y, x, sf, test="LRT", reduced=xr)
+    wr = DP.results_device(whole, y, x)
+    for g in got:
+        assert g["extra_collectives"] == 0
+        assert set(g["gathered"]) == {"dispersion", "betaMatrix", "betaSE", "LRTStatistic", "LRTPvalue"}
+        for k, v in g["gathered"].items():
+            assert np.array_equal(v, whole[k].cpu().numpy(), equal_nan=True), k
+        assert g["results_collectives"] == 2
+    for k in ("stat", "padj"):
+        cat = np.concatenate([g[k] for g in got])
+        assert np.array_equal(cat, wr[k].cpu().numpy(), equal_nan=True), k
 
 
 def test_sharded_lrt_equals_whole(emu_dev):
-    """Two gloo ranks: the gathered LRT results equal the unsharded run bit for bit, through the Wald run's
-    collectives; sharded results() of the LRT result equals results_device of the whole."""
-    import torch.multiprocessing as mp
-    sys.path.insert(0, os.path.join(ROOT, "tests", "simt_emu"))
-    import build_emu
-    from deseq2_b200 import device_pipeline as DP
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 39500 + (os.getpid() % 2000)
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, q, build_emu.build())) for r in range(2)]
-    for p in procs:
-        p.start()
-    items = [q.get(timeout=900) for _ in range(3)]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    got = next(i for i in items if isinstance(i, dict))
-    parts = dict((i[0], i[1:]) for i in items if isinstance(i, tuple))
-    K, x, xr, sf = _sharded_case()
-    y = _gm(K, "cpu")
-    whole = DP.DESeq_device(y, x, sf, test="LRT", reduced=xr)
-    assert got["collectives"] == got["collectives_wald"]
-    assert set(got["gathered"]) == {"dispersion", "betaMatrix", "betaSE", "LRTStatistic", "LRTPvalue"}
-    for k, v in got["gathered"].items():
-        assert np.array_equal(v, whole[k].numpy(), equal_nan=True), k
-    wr = DP.results_device(whole, y, x)
-    assert got["results_collectives"] == 2
-    for j, k in enumerate(("stat", "padj")):
-        cat = np.concatenate([parts[0][j], parts[1][j]])
-        assert np.array_equal(cat, wr[k].numpy(), equal_nan=True), k
+    _check_sharded("gloo", 301, 12)
 
 
 # ---------------------------------------------------------------- GPU (or the emulator with B200NB_LIB)
@@ -499,7 +469,7 @@ def test_c2_size_gpu(engine, reduced):
     x = synth.design_batch_condition(100, 2) if reduced == "condition" else synth.design_condition(100)
     xr = x[:, :2] if reduced == "condition" else np.ones((100, 1))
     d = synth.make_example_counts(n, 100, x=x, seed=3)
-    y = _gm(d["counts"], DEV)
+    y = gm(d["counts"], DEV)
     a = _snapshot(DP.DESeq_device(y, x, d["sizeFactors"], test="LRT", reduced=xr))
     b = _snapshot(DP.DESeq_device(y, x, d["sizeFactors"], test="LRT", reduced=xr))
     assert all(_same(a[k], b[k]) for k in a if k != "stage_ms")
@@ -512,16 +482,5 @@ def test_c2_size_gpu(engine, reduced):
 
 
 @pytest.mark.gpu
-def test_sharded_lrt_over_nccl_equals_whole():
-    n_gpu = torch.cuda.device_count() if DEV == "cuda" else 0
-    if n_gpu < 2:
-        pytest.skip("needs at least 2 GPUs")
-    env = dict(os.environ)
-    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK", "MASTER_ADDR", "MASTER_PORT"):
-        env.pop(k, None)
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29651",
-                        os.path.join(ROOT, "scripts", "sharded_lrt_nccl.py")], env=env, capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0, (r.stdout[-2000:], r.stderr[-3000:])
-    assert "sharded == whole: True" in r.stdout and "extra collectives: 0" in r.stdout, r.stdout[-2000:]
+def test_sharded_lrt_over_nccl_equals_whole(engine):
+    _check_sharded("nccl", 20000, 60, nccl_world())

@@ -10,8 +10,9 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, emu_dev
+from helpers import DEV, emu_dev, gm
 from deseq2_b200 import pipeline, synth
+from ranks import DEVICE, nccl_world, run_ranks
 
 NAN = np.nan
 
@@ -168,11 +169,6 @@ def test_results_checks():
 
 # ---------------------------------------------------------------- device vs host
 
-def _gm(a, dev):
-    from deseq2_b200 import device as D
-    return D.to_gene_major(np.asarray(a), torch.device(dev))
-
-
 def _host_inputs(res, y, K, x, dev, nf=None, weights=None):
     """pipeline.DESeq's layout (all N rows) from a DESeq_device result, and the first fit's Cook's matrix; weights: the
     raw weights (numpy), whose weightsFail rows keep pipeline.DESeq's weighted baseMean."""
@@ -262,12 +258,12 @@ def _run(dev, engine, kind, deseq_kw=None, lrt=False, **kw):
     from deseq2_b200 import device_pipeline as DP
     K, x, factors, base = _case(kind, dev)
     base.update(deseq_kw or {})
-    y = _gm(K, dev)
+    y = gm(K, dev)
     nf, w = base.get("normalizationFactors"), base.get("weights")
     if nf is not None:
-        base["normalizationFactors"] = _gm(nf, dev)
+        base["normalizationFactors"] = gm(nf, dev)
     if w is not None:
-        base["weights"] = _gm(w, dev)
+        base["weights"] = gm(w, dev)
         kw = dict(kw, weights=base["weights"])
     if base.get("betaPrior"):
         base["factors"] = factors
@@ -358,7 +354,7 @@ def test_weights_fail_rows_emulated(emu_dev):
     want = pipeline.getBaseMeansAndVariances(K, kw["sizeFactors"], w)["baseMean"][8]
     assert abs(dv["baseMean"][8].item() - want) <= 1e-12 * want and np.isnan(dv["pvalue"][8].item())
     with pytest.raises(ValueError, match="weights="):
-        DP.results_device(res, _gm(K, "cpu"), _case("factors", "cpu")[1])
+        DP.results_device(res, gm(K, "cpu"), _case("factors", "cpu")[1])
 
 
 def test_two_group_heuristic_emulated(emu_dev):
@@ -371,7 +367,7 @@ def test_two_group_heuristic_emulated(emu_dev):
     p = dv["pvalue"].numpy()
     assert np.isfinite(p[0]) and np.isnan(p[1])
     K, x, _, _ = _case("two_group", "cpu")
-    assert np.isnan(DP.results_device(res, _gm(K, "cpu"), x, cooksCutoff=2.0)["pvalue"].numpy()[0])
+    assert np.isnan(DP.results_device(res, gm(K, "cpu"), x, cooksCutoff=2.0)["pvalue"].numpy()[0])
 
 
 def test_reference_expectations_emulated(emu_dev):
@@ -379,7 +375,7 @@ def test_reference_expectations_emulated(emu_dev):
     gives the contrasts -3 / -1 / -2 and the list contrast 2; contrastAllZero sets LFC, stat 0 and p 1."""
     from deseq2_b200 import device_pipeline as DP
     K, x, factors, kw = _case("unit_sf", "cpu")
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     res = DP.DESeq_device(y, x, **kw)
     R = lambda **a: DP.results_device(res, y, x, factors=factors, **a)
     for c, want in (((1, 0, 2), -3), ((1, 0, 1), -1), ((1, 1, 2), -2)):
@@ -395,7 +391,7 @@ def test_reference_expectations_emulated(emu_dev):
 def test_results_device_errors_and_abi(emu_dev):
     from deseq2_b200 import _lib, device_pipeline as DP
     K, x, factors, kw = _case("factors", "cpu")
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     res = DP.DESeq_device(y, x, **kw)
     for bad in (dict(alpha=1.0), dict(lfcThreshold=-1), dict(altHypothesis="lessAbs"), dict(pAdjustMethod="hommel"),
                 dict(theta=[0.5]), dict(filter=np.ones(5)), dict(filter=lambda r: r), dict(contrast=np.zeros(4))):
@@ -444,10 +440,10 @@ def test_stale_workspace_is_refused(emu_dev):
     refuses the stale result instead of reading replaced memory."""
     from deseq2_b200 import device_pipeline as DP
     K, x, factors, kw = _case("two_group", "cpu")
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     res = DP.DESeq_device(y, x, **kw)
     DP.results_device(res, y, x, factors=factors)
-    DP.DESeq_device(_gm(K[:200], "cpu"), x, **kw)
+    DP.DESeq_device(gm(K[:200], "cpu"), x, **kw)
     with pytest.raises(ValueError, match="workspace"):
         DP.results_device(res, y, x, factors=factors)
     DP.results_device(res, y, x)                              # no heuristic: the views are not read
@@ -530,7 +526,7 @@ def test_results_device_c2_gpu(engine):
     x = pipeline.factorDesign(factors)[0]
     d = synth.make_example_counts(50000, 100, x=x, seed=3)
     K = d["counts"]
-    y = _gm(K, DEV)
+    y = gm(K, DEV)
     res = DP.DESeq_device(y, x, sizeFactors=d["sizeFactors"])
     dds, cooks = _host_inputs(res, y, K, x, DEV)
     dv = DP.results_device(res, y, x, factors=factors)
@@ -540,75 +536,59 @@ def test_results_device_c2_gpu(engine):
         assert torch.equal(torch.nan_to_num(dv[k], nan=-7.0), torch.nan_to_num(dv2[k], nan=-7.0))
 
 
-# ---------------------------------------------------------------- sharded (two gloo ranks, emulated engine)
+# ---------------------------------------------------------------- sharded
 
-def _sharded_case():
+_SHARDED_CALLS = (("default", {}), ("holm", dict(pAdjustMethod="holm", cooksCutoff=2.0)),
+                  ("no_filter", dict(independentFiltering=False)))
+
+
+def _sharded_case(n):
     factors = [np.repeat([0, 1], 6)]
     x = pipeline.factorDesign(factors)[0]
-    d = synth.make_example_counts(401, 12, x=x, seed=93)
+    d = synth.make_example_counts(n, 12, x=x, seed=93)
     K = d["counts"].copy()
     K[[5, 250]] = 0
     K[7] = [10, 12, 11, 9, 10, 11, 12, 13, 10, 12, 11, 900]
     return K, x, factors, d["sizeFactors"]
 
 
-def _sharded_worker(rank, world, port, q, emu_lib):
-    import os
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    sys.path.insert(0, root)
-    sys.path.insert(0, os.path.join(root, "tests"))
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), OMP_NUM_THREADS="2", B200NB_LIB=emu_lib,
-                      B200NB_TEST_EMULATOR="1")
-    import torch.distributed as dist
-    from deseq2_b200 import _lib, device as D, device_pipeline as DP, sharded
-    _lib._SO, _lib._lib = emu_lib, None            # this module imported the package before B200NB_LIB was set
-    D._stream = lambda: C.c_void_p(0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    K, x, factors, sf = _sharded_case()
-    lo, hi = sharded.shard_bounds(K.shape[0], world, rank)
-    y = D.to_gene_major(K[lo:hi], torch.device("cpu"))
+def _sharded_rank(rank, world, dev, n):
+    from deseq2_b200 import sharded
+    K, x, factors, sf = _sharded_case(n)
+    lo, hi = sharded.shard_bounds(n, world, rank)
+    y = gm(K[lo:hi], dev)
     res = sharded.sharded_DESeq_device(y, x, sf)
     out = {}
-    for name, kw in (("default", {}), ("holm", dict(pAdjustMethod="holm", cooksCutoff=2.0)),
-                     ("no_filter", dict(independentFiltering=False))):
+    for name, kw in _SHARDED_CALLS:
         r = sharded.sharded_results_device(res, y, x, factors=factors, **kw)
-        out[name] = {k: r[k].numpy() for k in ("baseMean", "log2FoldChange", "stat", "pvalue", "padj")}
+        out[name] = {k: r[k] for k in ("baseMean", "log2FoldChange", "stat", "pvalue", "padj")}
         out[name]["j"] = r["metadata"].get("j")
         out[name]["collectives"] = r["collectives"]
-    q.put((rank, out))
-    dist.barrier()
-    dist.destroy_process_group()
+    return out
+
+
+def _check_sharded(backend, n, world=2):
+    """results() over the ranks (one PackedGather of [filter, pvalue]) equals the unsharded results_device bit for
+    bit."""
+    from deseq2_b200 import device_pipeline as DP
+    got = run_ranks(_sharded_rank, n, world=world, backend=backend)
+    K, x, factors, sf = _sharded_case(n)
+    y = gm(K, DEVICE[backend])
+    res = DP.DESeq_device(y, x, sf)
+    for name, kw in _SHARDED_CALLS:
+        whole = DP.results_device(res, y, x, factors=factors, **kw)
+        for g in got:
+            assert g[name]["j"] == whole["metadata"].get("j")
+            assert g[name]["collectives"] == 2                    # the size agreement and the one gather
+        for k in ("baseMean", "log2FoldChange", "stat", "pvalue", "padj"):
+            cat = np.concatenate([g[name][k] for g in got])
+            assert np.array_equal(cat, whole[k].cpu().numpy(), equal_nan=True), (name, k)
 
 
 def test_sharded_results_equal_whole(emu_dev):
-    """results() over two gloo ranks (one PackedGather of [filter, pvalue]) equals the unsharded results_device bit
-    for bit."""
-    import os
-    import sys
-    import torch.multiprocessing as mp
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    sys.path.insert(0, os.path.join(root, "tests", "simt_emu"))
-    import build_emu
-    from deseq2_b200 import device_pipeline as DP
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 35500 + (os.getpid() % 2000)
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, q, build_emu.build())) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=600) for _ in range(2))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    K, x, factors, sf = _sharded_case()
-    y = _gm(K, "cpu")
-    res = DP.DESeq_device(y, x, sf)
-    for name, kw in (("default", {}), ("holm", dict(pAdjustMethod="holm", cooksCutoff=2.0)),
-                     ("no_filter", dict(independentFiltering=False))):
-        whole = DP.results_device(res, y, x, factors=factors, **kw)
-        assert got[0][name]["j"] == whole["metadata"].get("j")
-        assert got[0][name]["collectives"] == 2                   # the size agreement and the one gather
-        for k in ("baseMean", "log2FoldChange", "stat", "pvalue", "padj"):
-            cat = np.concatenate([got[0][name][k], got[1][name][k]])
-            assert np.array_equal(cat, whole[k].numpy(), equal_nan=True), (name, k)
+    _check_sharded("gloo", 401)
+
+
+@pytest.mark.gpu
+def test_sharded_results_over_nccl_equals_whole(engine):
+    _check_sharded("nccl", 20000, nccl_world())

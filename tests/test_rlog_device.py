@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, emu_dev
+from helpers import DEV, emu_dev, gm
 
 LN2 = np.log(2.0)
 
@@ -20,11 +20,6 @@ def ref():
     from oracle import ref as R
     R.lib()
     return R
-
-
-def _gm(a, dev):
-    from deseq2_b200 import device as D
-    return D.to_gene_major(np.asarray(a), torch.device(dev))
 
 
 def _stream(dev):
@@ -102,8 +97,8 @@ def _check_fit(ref, n, m, seed, f64, use_nf, frozen, dev="cpu", bpv=0.8):
         icpt[5 % n] = -np.inf                           # left out: 0
     if not f64:
         K = K.astype(np.int32)
-    y = _gm(K, dev)
-    kw = dict(nf=_gm(nfm, dev)) if use_nf else dict(sf=torch.as_tensor(sf, device=dev))
+    y = gm(K, dev)
+    kw = dict(nf=gm(nfm, dev)) if use_nf else dict(sf=torch.as_tensor(sf, device=dev))
     itd = None if icpt is None else torch.as_tensor(icpt, device=dev)
     got, gicpt, git = _call_fit(y, m, torch.as_tensor(disp, device=dev), bpv, intercept=itd, ld_out=m + 3, **kw)
     assert np.all(got[:, m:] == -7.0)
@@ -145,7 +140,7 @@ def test_fit_kernel_divergence(emu_dev, ref):
     m = 6
     K, sf, nf, disp = _fit_case(8, m, 21, f64=True)
     K[4] = 2e13 * np.arange(1, m + 1)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     sfd = torch.as_tensor(sf)
     nfm = np.broadcast_to(sf, K.shape).copy()
     got, gicpt, git = _call_fit(y, m, torch.as_tensor(disp), 0.8, sf=sfd)
@@ -154,7 +149,7 @@ def test_fit_kernel_divergence(emu_dev, ref):
     assert git[4] == 100 and np.array_equal(git[fitted], wit)
     assert _within(got[fitted], want) and abs(gicpt[4] * LN2) > 30
     K, sf, nf, disp = _fit_case(8, m, 22, f64=True)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     sfd = torch.as_tensor(sf)
     nfm = np.broadcast_to(sf, K.shape).copy()
     icpt = np.log2((K / nfm).mean(axis=1) + 0.5)
@@ -200,8 +195,8 @@ def test_prior_var_matches_host(emu_dev, use_nf, m):
     div = sf[None, :] * np.exp(np.random.default_rng(1).normal(0.0, 0.2, (n, m))) if use_nf else sf
     want, bm, x = _host_prior(K, div, disp)
     assert np.any(np.abs(x) >= 10)
-    y = _gm(K, "cpu")
-    sfd = _gm(div, "cpu") if use_nf else torch.as_tensor(sf)
+    y = gm(K, "cpu")
+    sfd = gm(div, "cpu") if use_nf else torch.as_tensor(sf)
     bmd, dd = torch.as_tensor(bm), torch.as_tensor(disp)
     got = DP.rlog_prior_var(y, m, sfd, bmd, dd)
     assert abs(got.item() - want) <= 1e-12 * want
@@ -211,7 +206,7 @@ def test_prior_var_matches_host(emu_dev, use_nf, m):
 
 def test_prior_var_nothing_kept(emu_dev):
     from deseq2_b200 import device_pipeline as DP
-    y = _gm(np.zeros((5, 3), dtype=np.int32), "cpu")
+    y = gm(np.zeros((5, 3), dtype=np.int32), "cpu")
     v = DP.rlog_prior_var(y, 3, torch.ones(3, dtype=torch.float64), torch.zeros(5, dtype=torch.float64),
                           torch.ones(5, dtype=torch.float64))
     assert torch.isnan(v)
@@ -251,7 +246,7 @@ def test_rlog_matches_host(emu_dev, oracle, blind, fitType):
     x = synth.design_batch_condition(12, 3)
     K, sf = _counts(200, 12, 41, x)
     host = pipeline.rlog(K, x=x, blind=blind, fitType=fitType, sizeFactors=sf, engine=oracle)
-    dv = DP.rlog_device(_gm(K, "cpu"), 12, x=x, blind=blind, fitType=fitType, sizeFactors=sf)
+    dv = DP.rlog_device(gm(K, "cpu"), 12, x=x, blind=blind, fitType=fitType, sizeFactors=sf)
     _compare(dv, host)
     assert dv["fitType"] == fitType and np.all(dv["rlog"].numpy()[[3, 17]] == 0.0)
     nz = K.sum(axis=1) > 0
@@ -262,15 +257,15 @@ def test_rlog_factors(emu_dev, oracle):
     """Estimated size factors, a gene-specific nf matrix, and the nf avgTxLength estimates."""
     from deseq2_b200 import device_pipeline as DP, pipeline
     K, sf = _counts(200, 8, 43)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     dv = DP.rlog_device(y, 8)
     host = pipeline.rlog(K, engine=oracle)
     assert np.max(np.abs(dv["sizeFactors"] - host["sizeFactors"]) / host["sizeFactors"]) < 1e-12
     _compare(dv, host)
     nf = sf[None, :] * np.exp(np.random.default_rng(2).normal(0.0, 0.25, K.shape))
-    dv = DP.rlog_device(y, 8, normalizationFactors=_gm(nf, "cpu"))
+    dv = DP.rlog_device(y, 8, normalizationFactors=gm(nf, "cpu"))
     _compare(dv, pipeline.rlog(K, sizeFactors=nf, engine=oracle))
-    tx = _gm(np.exp(np.random.default_rng(3).normal(7.0, 0.5, K.shape)), "cpu")
+    tx = gm(np.exp(np.random.default_rng(3).normal(7.0, 0.5, K.shape)), "cpu")
     dv = DP.rlog_device(y, 8, avgTxLength=tx)
     nfe = DP.normalization_factors(y, 8, avgTxLength=tx)["normalizationFactors"]
     assert torch.equal(dv["normalizationFactors"], nfe)
@@ -283,13 +278,13 @@ def test_frozen_rlog(emu_dev, oracle):
     prior is estimated on nf 2^intercept."""
     from deseq2_b200 import device_pipeline as DP, pipeline
     K, sf = _counts(200, 10, 45)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     res = DP.rlog_device(y, 10, sizeFactors=sf)
     icpt, disp = res["intercept"], res["dispFit"]
     for K2, sf2 in ((K, sf), _counts(200, 5, 46), (K[:, :1], np.array([1.0]))):
         m2 = K2.shape[1]
         kw = dict(intercept=icpt, dispFit=disp, blind=False, sizeFactors=sf2)
-        dv = DP.rlog_device(_gm(K2, "cpu"), m2, betaPriorVar=res["betaPriorVar"], **kw)
+        dv = DP.rlog_device(gm(K2, "cpu"), m2, betaPriorVar=res["betaPriorVar"], **kw)
         host = pipeline.rlog(K2, intercept=icpt.numpy(), betaPriorVar=res["betaPriorVar"], dispFit=disp.numpy(),
                              blind=False, sizeFactors=sf2, engine=oracle)
         _compare(dv, host, frozen=True)
@@ -304,7 +299,7 @@ def test_rlog_with_deseq_dispfit(emu_dev, oracle):
     from deseq2_b200 import device_pipeline as DP, pipeline, synth
     x = synth.design_condition(8)
     K, sf = _counts(200, 8, 47, x)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     ds = DP.DESeq_device(y, x, sizeFactors=sf)
     disp = torch.full((200,), float("nan"), dtype=torch.float64)
     disp[torch.as_tensor(ds["idx"])] = ds["dispFit"]
@@ -319,7 +314,7 @@ def test_rlog_with_deseq_dispfit(emu_dev, oracle):
 def test_rlog_errors(emu_dev, oracle):
     from deseq2_b200 import device_pipeline as DP, pipeline
     K, sf = _counts(100, 6, 49)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     with pytest.raises(ValueError, match="intercept should be as long"):
         DP.rlog_device(y, 6, intercept=np.zeros(99))
     with pytest.raises(ValueError, match="intercept should be as long"):
@@ -343,7 +338,7 @@ def test_rlog_errors(emu_dev, oracle):
     zero_heavy = np.zeros((300, 6), dtype=np.int64)
     zero_heavy[:, 0] = 1000
     zero_heavy[:, 1] = 1
-    for f in (lambda: DP.rlog_device(_gm(zero_heavy, "cpu"), 6, sizeFactors=np.ones(6), betaPriorVar=1.0,
+    for f in (lambda: DP.rlog_device(gm(zero_heavy, "cpu"), 6, sizeFactors=np.ones(6), betaPriorVar=1.0,
                                      blind=False, dispFit=np.full(300, 0.1)),
               lambda: pipeline.rlog(zero_heavy, sizeFactors=np.ones(6), betaPriorVar=1.0, blind=False,
                                     dispFit=np.full(300, 0.1), engine=oracle)):
@@ -356,9 +351,9 @@ def test_rlog_errors(emu_dev, oracle):
 def test_rlog_abi_rejects_bad_arguments(emu_dev):
     from deseq2_b200 import _lib
     L = _lib.lib()
-    y = _gm(np.ones((5, 3)), "cpu")
+    y = gm(np.ones((5, 3)), "cpu")
     sf = torch.ones(3, dtype=torch.float64)
-    nf = _gm(np.ones((5, 3)), "cpu")
+    nf = gm(np.ones((5, 3)), "cpu")
     disp = torch.full((5,), 0.1, dtype=torch.float64)
     icpt = torch.zeros(5, dtype=torch.float64)
     out = torch.empty((5, 3), dtype=torch.float64)
@@ -399,7 +394,7 @@ def test_rlog_abi_rejects_bad_arguments(emu_dev):
 
 def test_fit_kernel_bad_dispersion_gives_nan(emu_dev):
     """A fitted row whose dispersion is not finite and > 0 gets NaN (the entry point does not read device data)."""
-    y = _gm(np.full((3, 4), 10, dtype=np.int32), "cpu")
+    y = gm(np.full((3, 4), 10, dtype=np.int32), "cpu")
     disp = torch.tensor([0.1, -1.0, float("nan")], dtype=torch.float64)
     out, icpt, it = _call_fit(y, 4, disp, 0.5, sf=torch.ones(4, dtype=torch.float64))
     assert np.all(np.isfinite(out[0])) and np.all(np.isnan(out[1:])) and np.all(np.isnan(it[1:]))
@@ -419,7 +414,7 @@ def test_fit_kernel_against_general_fit_beta_gpu(engine, m):
     fitted = K.sum(axis=1) > 0
     K, disp = K[fitted], disp[fitted]
     n = K.shape[0]
-    y = _gm(K, DEV)
+    y = gm(K, DEV)
     sfd = torch.as_tensor(sf, device=DEV)
     dd = torch.as_tensor(disp, device=DEV)
     bpv = 0.7
@@ -460,7 +455,7 @@ def test_rlog_at_config_against_reference_gpu(engine, ref, config):
     from deseq2_b200 import device_pipeline as DP
     K = _config(config)
     n, m = K.shape
-    y = _gm(K, DEV)
+    y = gm(K, DEV)
     dv = DP.rlog_device(y, m)
     sf = dv["sizeFactors"]
     disp = dv["dispFit"].cpu().numpy()

@@ -5,22 +5,14 @@ the error cases, and DESeq_device(fitType = "mean") against pipeline.DESeq, incl
 The CPU tests run the engine's CUDA source on the SIMT emulator (`emu` fixture); the `-m gpu` tests run on a GPU, or on
 the emulator when B200NB_LIB points at it."""
 import ctypes as C
-import os
-import sys
 import warnings
 
 import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, emu_dev, rel_err
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _gm(a, dev):
-    from deseq2_b200 import device as D
-    return D.to_gene_major(np.asarray(a, dtype=np.float64), torch.device(dev))
+from helpers import DEV, emu_dev, gm, gm64, rel_err
+from ranks import DEVICE, nccl_world, run_ranks
 
 
 def _objective_case(n, m, seed, ties=False):
@@ -47,7 +39,7 @@ def _sorted_center_ll(K, q, alpha, par):
 def _device_objective(K, q, alpha, par, dev, f64=True, tile=0):
     from deseq2_b200 import device as D, device_pipeline as DP
     y = D.to_gene_major(np.asarray(K, dtype=np.float64 if f64 else np.int32), torch.device(dev))
-    return DP.sf_iterate_objective(y, _gm(q, dev), torch.as_tensor(alpha, device=dev),
+    return DP.sf_iterate_objective(y, gm64(q, dev), torch.as_tensor(alpha, device=dev),
                                    torch.as_tensor(np.asarray(par, dtype=np.float64), device=dev), len(par),
                                    max_tile_cols=tile).cpu().numpy()
 
@@ -102,7 +94,7 @@ def test_objective_abi_rejects_bad_arguments(emu_dev):
     from deseq2_b200 import _lib
     L = _lib.lib()
     K, q, alpha, par = _objective_case(10, 3, 1)
-    y, qd = _gm(K, "cpu"), _gm(q, "cpu")
+    y, qd = gm64(K, "cpu"), gm64(q, "cpu")
     a, pd = torch.as_tensor(alpha), torch.as_tensor(par)
     out = torch.empty(7, dtype=torch.float64)
     P = lambda t: C.c_void_p(t.data_ptr())
@@ -147,7 +139,7 @@ def test_reference_property_host_and_device(emu_dev, oracle):
     cts, true_sf = _reference_property_counts()
     host = pipeline.estimateSizeFactorsIterate(cts, engine=oracle)
     _check_lm(host["sizeFactors"], true_sf)
-    dv = DP.size_factors_iterate(_gm(cts, "cpu"), 12)
+    dv = DP.size_factors_iterate(gm64(cts, "cpu"), 12)
     _check_lm(dv["sizeFactors"], true_sf)
     assert dv["iterations"] == host["iterations"]
     assert np.max(rel_err(dv["sizeFactors"], host["sizeFactors"])) < 1e-4
@@ -160,7 +152,7 @@ def _compare_iterate(oracle, counts, dev, **kw):
     from deseq2_b200 import device_pipeline as DP, pipeline
     m = counts.shape[1]
     host = pipeline.estimateSizeFactorsIterate(counts, engine=oracle)
-    dv = DP.size_factors_iterate(_gm(counts, dev), m, **kw)
+    dv = DP.size_factors_iterate(gm64(counts, dev), m, **kw)
     assert dv["iterations"] == host["iterations"]
     assert np.max(rel_err(dv["sizeFactors"], host["sizeFactors"])) < 1e-4
     assert np.max(rel_err(dv["dispersion"].cpu().numpy(), host["last"]["dispersion"])) < 1e-6
@@ -204,13 +196,13 @@ def test_replay_host_optimizer_points(emu_dev, oracle, monkeypatch):
 def test_iterate_errors(emu_dev, oracle):
     from deseq2_b200 import device_pipeline as DP, pipeline, sharded
     cts, _ = _reference_property_counts()
-    y = _gm(cts, "cpu")
+    y = gm64(cts, "cpu")
     with pytest.raises(ValueError, match="did not converge"):
         DP.size_factors_iterate(y, 12, niter=1)
     with pytest.raises(ValueError, match="did not converge"):
         pipeline.estimateSizeFactorsIterate(cts, niter=1, engine=oracle)
     x = np.ones((12, 1))
-    ones = _gm(np.ones(cts.shape), "cpu")
+    ones = gm64(np.ones(cts.shape), "cpu")
     for kw in (dict(weights=ones), dict(normalizationFactors=ones), dict(avgTxLength=ones)):
         with pytest.raises(ValueError, match="iterate"):
             DP.DESeq_device(y, x, sfType="iterate", **kw)
@@ -225,7 +217,7 @@ def test_iterate_errors(emu_dev, oracle):
     # every gene-wise estimate below 100 minDisp: R's stop in estimateDispersionsFit
     pois = np.random.default_rng(3).poisson(np.repeat([[5.0, 20.0, 80.0]], 60, axis=0).repeat(4, axis=1))
     with pytest.raises(ValueError, match="within 2 orders of magnitude"):
-        DP.size_factors_iterate(_gm(pois, "cpu"), 12, minDisp=1.0)
+        DP.size_factors_iterate(gm64(pois, "cpu"), 12, minDisp=1.0)
     with pytest.raises(ValueError, match="within 2 orders of magnitude"):
         pipeline.estimateSizeFactorsIterate(pois, engine=oracle, minDisp=1.0)
 
@@ -245,7 +237,7 @@ def _compare_mean(oracle, counts, x, dev, tol=1e-6, fitType="mean", **kw):
     steps on both sides agree within tol; the others must be rare."""
     from deseq2_b200 import device_pipeline as DP, pipeline
     host = pipeline.DESeq(counts, x, engine=oracle, useOptim=False, fitType=fitType, **kw)
-    dv = DP.DESeq_device(_gm(counts, dev), x, useOptim=False, fitType=fitType, **kw)
+    dv = DP.DESeq_device(gm64(counts, dev), x, useOptim=False, fitType=fitType, **kw)
     idx = dv["idx"].cpu().numpy()
     assert dv["fitType"] == host["fitType"] == fitType
     if fitType == "mean":
@@ -300,7 +292,7 @@ def test_iterate_size_factors_ignore_the_fit_minmu(emu_dev, oracle):
     counts = d["counts"].copy()
     counts[np.arange(240), np.arange(240) % 12] = 0                  # every gene has a zero
     host, dv = _compare_mean(oracle, counts, x, "cpu", fitType="parametric", sfType="iterate", minmu=1e-6)
-    alone = DP.size_factors_iterate(_gm(counts, "cpu"), 12)["sizeFactors"]
+    alone = DP.size_factors_iterate(gm64(counts, "cpu"), 12)["sizeFactors"]
     assert np.array_equal(dv["sizeFactors"], alone)
     assert np.max(rel_err(dv["sizeFactors"], host["sizeFactors"])) < 1e-4
     assert dv["sfIterate"]["iterations"] == host["sfIterate"]["iterations"]
@@ -337,55 +329,41 @@ def test_mean_disp_trims(emu_dev):
     assert abs(got - want) < 1e-14 * want
 
 
-def _sharded_worker(rank, world, port, q, emu_lib):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), OMP_NUM_THREADS="2", B200NB_LIB=emu_lib,
-                      B200NB_TEST_EMULATOR="1")
-    import torch.distributed as dist
-    from deseq2_b200 import _lib, device as D, device_pipeline as DP, sharded, synth
-    _lib._SO, _lib._lib = emu_lib, None
-    D._stream = lambda: C.c_void_p(0)
+def _sharded_data(n, m):
+    from deseq2_b200 import synth
+    x = synth.design_batch_condition(m, 3)
+    d = synth.make_example_counts(n, m, x=x, seed=91)
+    return d["counts"], x, d["sizeFactors"]
+
+
+def _sharded_rank(rank, world, dev, n, m):
+    from deseq2_b200 import sharded
+    K, x, sf = _sharded_data(n, m)
+    lo, hi = sharded.shard_bounds(n, world, rank)
+    y = gm(K[lo:hi], dev)
     warnings.simplefilter("ignore")
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    x = synth.design_batch_condition(12, 3)
-    d = synth.make_example_counts(400, 12, x=x, seed=91)
-    lo, hi = sharded.shard_bounds(400, world, rank)
-    y = D.to_gene_major(d["counts"][lo:hi], torch.device("cpu"))
-    plain = sharded.sharded_DESeq_device(y, x, d["sizeFactors"])
-    r = sharded.sharded_DESeq_device(y, x, d["sizeFactors"], fitType="mean")
-    out = {k: r["gathered"][k].numpy() for k in ("dispersion", "betaMatrix", "betaSE", "WaldPvalue")}
-    out.update(collectives=r["collectives"], collectives_plain=plain["collectives"], meanDisp=r["meanDisp"])
-    q.put((rank, out))
-    dist.barrier()
-    dist.destroy_process_group()
+    plain = sharded.sharded_DESeq_device(y, x, sf)
+    r = sharded.sharded_DESeq_device(y, x, sf, fitType="mean")
+    return {"gathered": r["gathered"], "extra_collectives": r["collectives"] - plain["collectives"],
+            "meanDisp": r["meanDisp"]}
+
+
+def _check_sharded(backend, n, m, world=2):
+    """The same bits as one process (the trimmed mean is of the gathered estimates, in rank order = gene order) and
+    the same number of collectives as the parametric run."""
+    from deseq2_b200 import device_pipeline as DP
+    got = run_ranks(_sharded_rank, n, m, world=world, backend=backend)
+    K, x, sf = _sharded_data(n, m)
+    whole = DP.DESeq_device(gm64(K, DEVICE[backend]), x, sf, fitType="mean")
+    for g in got:
+        assert g["meanDisp"] == whole["meanDisp"]
+        assert g["extra_collectives"] == 0
+        for k in ("dispersion", "betaMatrix", "betaSE", "WaldPvalue"):
+            assert np.array_equal(g["gathered"][k], whole[k].cpu().numpy()), k
 
 
 def test_sharded_mean_equal_whole(emu_dev):
-    """Two gloo ranks: the same bits as one process (the trimmed mean is of the gathered estimates, in rank order =
-    gene order) and the same number of collectives as the parametric run."""
-    import torch.multiprocessing as mp
-    sys.path.insert(0, os.path.join(ROOT, "tests", "simt_emu"))
-    import build_emu
-    from deseq2_b200 import device_pipeline as DP, synth
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 41500 + (os.getpid() % 2000)
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, q, build_emu.build())) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=300) for _ in range(2))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    x = synth.design_batch_condition(12, 3)
-    d = synth.make_example_counts(400, 12, x=x, seed=91)
-    whole = DP.DESeq_device(_gm(d["counts"], "cpu"), x, d["sizeFactors"], fitType="mean")
-    g = got[0]
-    assert got[0]["meanDisp"] == got[1]["meanDisp"] == whole["meanDisp"]
-    assert g["collectives"] == g["collectives_plain"]
-    for k in ("dispersion", "betaMatrix", "betaSE", "WaldPvalue"):
-        assert np.array_equal(g[k], whole[k].numpy()), k
+    _check_sharded("gloo", 400, 12)
 
 
 # ---------------------------------------------------------------- GPU (or the emulator with B200NB_LIB)
@@ -418,7 +396,7 @@ def test_size_factors_iterate_matches_host_gpu(engine, oracle, n, m):
 def test_reference_property_gpu(engine):
     from deseq2_b200 import device_pipeline as DP
     cts, true_sf = _reference_property_counts()
-    _check_lm(DP.size_factors_iterate(_gm(cts, DEV), 12)["sizeFactors"], true_sf)
+    _check_lm(DP.size_factors_iterate(gm64(cts, DEV), 12)["sizeFactors"], true_sf)
 
 
 @pytest.mark.gpu
@@ -431,7 +409,7 @@ def test_iterate_at_scale(engine, shape):
     if DEV != "cuda":
         n, m = n // 100, m // 20                     # the emulator: 500 x 5, 200 x 100
     d = synth.make_example_counts(n, m, x=synth.design_condition(m), seed=17)
-    y = _gm(d["counts"], DEV)
+    y = gm64(d["counts"], DEV)
     dv = DP.DESeq_device(y, synth.design_condition(m), sfType="iterate", fitType="mean")
     assert dv["sfIterate"]["iterations"] >= 2
     for k in ("dispersion", "betaMatrix", "WaldPvalue"):
@@ -455,3 +433,8 @@ def test_iterate_at_scale(engine, shape):
         ll = pipeline.nbinomLogLike(K, qh * np.exp(p - np.mean(p))[None, :], dh)
         want[i] = ll[ll > np.quantile(ll, 0.05, method="linear")].sum()
     assert _objective_err(got[cols], want) < 1e-12
+
+
+@pytest.mark.gpu
+def test_sharded_mean_over_nccl_equals_whole(engine):
+    _check_sharded("nccl", 20000, 12, nccl_world())

@@ -10,15 +10,10 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, emu_dev, rel_err
+from helpers import DEV, emu_dev, gm, rel_err
 
 LN2 = np.log(2.0)
 MODES = {"parametric": (0, 0.05, 2.0), "mean": (1, 0.07, 0.0), "log2": (2, 1.0, 0.0)}
-
-
-def _gm(a, dev):
-    from deseq2_b200 import device as D
-    return D.to_gene_major(np.asarray(a), torch.device(dev))
 
 
 def _numpy_transform(K, div, mode, c0, c1):
@@ -64,9 +59,9 @@ def _call(y, m, mode, c0, c1, sf=None, nf=None, ld_out=None):
 def _check_kernel(n, m, mode, f64, use_nf, dev, seed=1, ld_out_pad=0):
     K, sf, nf = _kernel_case(n, m, seed, f64)
     code, c0, c1 = MODES[mode]
-    y = _gm(K, dev)
+    y = gm(K, dev)
     if use_nf:
-        got = _call(y, m, code, c0, c1, nf=_gm(nf, dev), ld_out=m + ld_out_pad)
+        got = _call(y, m, code, c0, c1, nf=gm(nf, dev), ld_out=m + ld_out_pad)
         want = _numpy_transform(K, nf, mode, c0, c1)
     else:
         got = _call(y, m, code, c0, c1, sf=torch.as_tensor(sf, device=dev), ld_out=m + ld_out_pad)
@@ -101,13 +96,13 @@ def test_vst_closed_form_property(emu_dev, mode):
     q = np.exp(np.linspace(0.0, np.log(1e5), 40))
     h = 1e-4 * q
     pts = np.stack([q - h, q + h], axis=1).reshape(1, -1)
-    out = _call(_gm(pts, "cpu"), pts.shape[1], code, c0, c1, sf=torch.ones(pts.shape[1], dtype=torch.float64))[0]
+    out = _call(gm(pts, "cpu"), pts.shape[1], code, c0, c1, sf=torch.ones(pts.shape[1], dtype=torch.float64))[0]
     deriv = (out[1::2] - out[0::2]) / (2 * h)
     disp = c0 + c1 / q if mode == "parametric" else c0
     const = deriv * np.sqrt(q + disp * q ** 2)
     assert np.max(np.abs(const / (np.sqrt(c0) / LN2) - 1.0)) < 1e-6
     big = np.array([[1e9, 1e11, 1e13]])
-    v = _call(_gm(big, "cpu"), 3, code, c0, c1, sf=torch.ones(3, dtype=torch.float64))[0]
+    v = _call(gm(big, "cpu"), 3, code, c0, c1, sf=torch.ones(3, dtype=torch.float64))[0]
     assert np.all(np.abs(v - np.log2(big[0])) < 1e-6)
     assert abs(v[-1] - np.log2(1e13)) < 1e-10
 
@@ -115,9 +110,9 @@ def test_vst_closed_form_property(emu_dev, mode):
 def test_transform_abi_rejects_bad_arguments(emu_dev):
     from deseq2_b200 import _lib
     L = _lib.lib()
-    y = _gm(np.ones((5, 3)), "cpu")
+    y = gm(np.ones((5, 3)), "cpu")
     sf = torch.ones(3, dtype=torch.float64)
-    nf = _gm(np.ones((5, 3)), "cpu")
+    nf = gm(np.ones((5, 3)), "cpu")
     out = torch.empty((5, 3), dtype=torch.float64)
     P = lambda t: C.c_void_p(t.data_ptr())
     good = dict(y=P(y), sf=P(sf), nf=None, n=5, m=3, ld=4, mode=0, c0=0.05, c1=2.0, out=P(out), ld_out=3)
@@ -176,7 +171,7 @@ def test_device_subset_equals_host(emu_dev, oracle):
     K, sf = _vst_counts(300, 6, 5)
     for given in (None, sf):
         host = pipeline.vst(K, nsub=120, sizeFactors=given, engine=oracle)
-        dv = DP.vst_device(_gm(K, "cpu"), 6, nsub=120, sizeFactors=given)
+        dv = DP.vst_device(gm(K, "cpu"), 6, nsub=120, sizeFactors=given)
         assert np.array_equal(dv["subset"].numpy(), host["subset"])
     tied = host["subset"][np.isin(host["subset"], np.arange(20, 31))]
     assert len(tied) >= 2 and np.all(np.diff(tied) > 0)
@@ -221,7 +216,7 @@ def test_vst_functions_match_host(emu_dev, oracle, design, blind, fitType):
     K = d["counts"].copy()
     K[[5, 77]] = 0
     sf = d["sizeFactors"]
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     host = pipeline.varianceStabilizingTransformation(K, x=x, blind=blind, fitType=fitType, sizeFactors=sf,
                                                       engine=oracle)
     dv = DP.varianceStabilizingTransformation_device(y, m, x=x, blind=blind, fitType=fitType, sizeFactors=sf)
@@ -243,7 +238,7 @@ def test_vst_functions_match_host_nf(emu_dev, oracle, fitType, blind):
     K = d["counts"].copy()
     K[9] = 0
     nf = _nf_for(K, d["sizeFactors"], 2)
-    y, nfd = _gm(K, "cpu"), _gm(nf, "cpu")
+    y, nfd = gm(K, "cpu"), gm(nf, "cpu")
     host = pipeline.varianceStabilizingTransformation(K, x=x, blind=blind, fitType=fitType, sizeFactors=nf,
                                                       engine=oracle)
     dv = DP.varianceStabilizingTransformation_device(y, 12, x=x, blind=blind, fitType=fitType,
@@ -260,13 +255,13 @@ def test_estimated_factors_and_avg_tx_length(emu_dev, oracle):
     """No factors given: the median-of-ratios size factors; avgTxLength: the nf DESeq_device estimates."""
     from deseq2_b200 import device_pipeline as DP, pipeline
     K, _ = _vst_counts(300, 8, 7, ties=False)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     dv = DP.varianceStabilizingTransformation_device(y, 8)
     host = pipeline.varianceStabilizingTransformation(K, engine=oracle)
     assert np.max(rel_err(dv["sizeFactors"], host["sizeFactors"])) < 1e-12
     _compare(dv, host, 300, "parametric")
     tx = np.exp(np.random.default_rng(3).normal(7.0, 0.5, K.shape))
-    txd = _gm(tx, "cpu")
+    txd = gm(tx, "cpu")
     nf = DP.normalization_factors(y, 8, avgTxLength=txd)["normalizationFactors"]
     dv = DP.vst_device(y, 8, nsub=120, avgTxLength=txd)
     assert torch.equal(dv["normalizationFactors"], nf)
@@ -279,10 +274,10 @@ def test_estimated_factors_and_avg_tx_length(emu_dev, oracle):
 def test_norm_transform_matches_host(emu_dev, use_nf):
     from deseq2_b200 import device_pipeline as DP, pipeline
     K, sf = _vst_counts(200, 7, 9, ties=False)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     if use_nf:
         nf = _nf_for(K, sf, 4)
-        got = DP.normTransform_device(y, 7, normalizationFactors=_gm(nf, "cpu"), pc=0.5).numpy()
+        got = DP.normTransform_device(y, 7, normalizationFactors=gm(nf, "cpu"), pc=0.5).numpy()
         want = pipeline.normTransform(K, nf, pc=0.5)
     else:
         got = DP.normTransform_device(y, 7).numpy()
@@ -299,7 +294,7 @@ def test_frozen_vst(emu_dev, oracle, fitType):
     from deseq2_b200 import device_pipeline as DP, pipeline, synth
     x = synth.design_condition(12)
     d = synth.make_example_counts(240, 12, x=x, seed=45, betaSD=0.3)
-    y = _gm(d["counts"], "cpu")
+    y = gm(d["counts"], "cpu")
     res = DP.DESeq_device(y, x, sizeFactors=d["sizeFactors"], fitType=fitType)
     got = DP.vst_transform(y, 12, res, sizeFactors=res["sizeFactors"])
     if fitType == "parametric":
@@ -311,7 +306,7 @@ def test_frozen_vst(emu_dev, oracle, fitType):
     d2 = synth.make_example_counts(150, 5, x=synth.design_condition(5), seed=46)
     K2 = d2["counts"].copy()
     K2[4] = 0
-    y2 = _gm(K2, "cpu")
+    y2 = gm(K2, "cpu")
     fn = {k: res[k] for k in ("fitType", "trendCoefs", "meanDisp") if k in res}
     frozen = DP.varianceStabilizingTransformation_device(y2, 5, blind=False, dispersionFunction=fn)
     host_fn = {k: (v.numpy() if isinstance(v, torch.Tensor) else v) for k, v in fn.items()}
@@ -325,14 +320,14 @@ def test_frozen_vst(emu_dev, oracle, fitType):
 def test_vst_errors(emu_dev, oracle):
     from deseq2_b200 import _lib, device_pipeline as DP, pipeline
     K, sf = _vst_counts(300, 6, 11, ties=False)
-    y = _gm(K, "cpu")
+    y = gm(K, "cpu")
     with pytest.raises(ValueError, match="less than 'nsub' rows,"):
         DP.vst_device(y, 6, nsub=301)
     with pytest.raises(ValueError, match="less than 'nsub' rows,"):
         pipeline.vst(K, nsub=301, engine=oracle)
     low = np.minimum(K, 3)
     with pytest.raises(ValueError, match="mean normalized count > 5"):
-        DP.vst_device(_gm(low, "cpu"), 6, nsub=100)
+        DP.vst_device(gm(low, "cpu"), 6, nsub=100)
     with pytest.raises(ValueError, match="mean normalized count > 5"):
         pipeline.vst(low, nsub=100, engine=oracle)
     for f in (lambda: DP.vst_device(y, 6, nsub=100, fitType="local"),
@@ -352,12 +347,12 @@ def test_vst_errors(emu_dev, oracle):
     bad = np.ones(K.shape)
     bad[2, 1] = 0.0
     with pytest.raises(ValueError, match="normalizationFactors"):
-        DP.varianceStabilizingTransformation_device(y, 6, normalizationFactors=_gm(bad, "cpu"))
+        DP.varianceStabilizingTransformation_device(y, 6, normalizationFactors=gm(bad, "cpu"))
     with pytest.raises(ValueError, match="normalizationFactors"):
         DP.normTransform_device(y, 6, normalizationFactors=torch.ones((300, 6), dtype=torch.float64))
     with pytest.raises(ValueError, match="not both"):
         DP.vst_transform(y, 6, {"fitType": "mean", "meanDisp": 0.1}, sizeFactors=sf,
-                         normalizationFactors=_gm(np.ones(K.shape), "cpu"))
+                         normalizationFactors=gm(np.ones(K.shape), "cpu"))
     with pytest.raises(ValueError, match="sizeFactors or normalizationFactors"):
         DP.vst_transform(y, 6, {"fitType": "mean", "meanDisp": 0.1})
     with pytest.raises(_lib.EngineError, match="pc"):
@@ -384,7 +379,7 @@ def _config(config):
 def test_transform_kernel_at_config_gpu(engine, config):
     K, sf = _config(config)
     n, m = K.shape
-    y = _gm(K, DEV)
+    y = gm(K, DEV)
     sfd = torch.as_tensor(sf, device=DEV)
     for mode, (code, c0, c1) in MODES.items():
         got = _call(y, m, code, c0, c1, sf=sfd)
@@ -398,7 +393,7 @@ def test_vst_end_to_end_at_config_gpu(engine, oracle, config):
     from deseq2_b200 import device_pipeline as DP, pipeline
     K, _ = _config(config)
     n, m = K.shape
-    y = _gm(K, DEV)
+    y = gm(K, DEV)
     nsub = 1000 if DEV == "cuda" else 200
     dv = DP.vst_device(y, m, nsub=nsub)
     host = pipeline.vst(K, nsub=nsub, engine=oracle)

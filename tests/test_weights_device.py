@@ -5,25 +5,14 @@ against pipeline.DESeq / nbinomLRT / getContrast driving the same engine, proper
 test_weights.R, and the gene-sharded run.
 The CPU tests run the engine's CUDA source on the SIMT emulator (`emu` fixture); the `-m gpu` tests run on a GPU, or on
 the emulator when B200NB_LIB points at it."""
-import ctypes as C
-import os
-import subprocess
-import sys
 import warnings
 
 import numpy as np
 import pytest
 import torch
 
-from helpers import DEV, emu_dev, rel_err
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _gm(a, dev):
-    """(n, m) float64 numpy -> gene-major (n, ld) float64 tensor."""
-    from deseq2_b200 import device as D
-    return D.to_gene_major(np.asarray(a, dtype=np.float64), torch.device(dev))
+from helpers import DEV, emu_dev, gm, gm64, rel_err
+from ranks import DEVICE, nccl_world, run_ranks
 
 
 def _continuous(m, seed=3):
@@ -56,8 +45,8 @@ def _host_prep(counts, x, sf, w, minDisp=1e-8, thr=1e-2):
 
 def _check_prep(counts, x, sf, w, dev="cpu", expect_fail=None):
     from deseq2_b200 import device_pipeline as DP
-    y = _gm(counts, dev)
-    pr = DP.prep(y, x, sf, want_mu=False, weights=_gm(w, dev))
+    y = gm64(counts, dev)
+    pr = DP.prep(y, x, sf, want_mu=False, weights=gm64(w, dev))
     m = x.shape[0]
     assert int(pr["status"].item()) == 0
     wn, fail, mv, a0 = _host_prep(counts, x, sf, w)
@@ -88,7 +77,7 @@ def test_prep_all_ones_equals_unweighted(emu_dev, design):
     from deseq2_b200 import device_pipeline as DP, synth
     x = _DESIGNS[design]()
     d = _make(60, x, 5)
-    y = _gm(d["counts"], "cpu")
+    y = gm64(d["counts"], "cpu")
     pw = DP.prep(y, x, d["sizeFactors"], want_mu=False, weights=torch.ones_like(y))
     pu = DP.prep(y, x, d["sizeFactors"], want_mu=False)
     for k in ("baseMean", "baseVar", "alpha0", "allZero", "beta0"):
@@ -198,7 +187,7 @@ def test_weight_errors_device_and_host(emu_dev):
     bad["all_zero_row"] = w
     for name, w in bad.items():
         with pytest.raises(ValueError):
-            DP.DESeq_device(y, x, d["sizeFactors"], weights=_gm(w, "cpu"))
+            DP.DESeq_device(y, x, d["sizeFactors"], weights=gm64(w, "cpu"))
         with pytest.raises(ValueError):
             pipeline.DESeq(d["counts"], x, sizeFactors=d["sizeFactors"], engine=emu_dev, weights=w)
     ok = np.ones((30, 12))
@@ -206,20 +195,20 @@ def test_weight_errors_device_and_host(emu_dev):
         with pytest.raises(ValueError):
             DP.DESeq_device(y, x, d["sizeFactors"], weights=torch.ones(shape, dtype=torch.float64))
     with pytest.raises(ValueError):
-        DP.DESeq_device(y, x, d["sizeFactors"], weights=_gm(ok, "cpu").to(torch.float32))
+        DP.DESeq_device(y, x, d["sizeFactors"], weights=gm64(ok, "cpu").to(torch.float32))
     with pytest.raises(ValueError):
         pipeline.DESeq(d["counts"], x, sizeFactors=d["sizeFactors"], engine=emu_dev, weights=np.ones((30, 11)))
     for kw in ({"betaPrior": True, "factors": [np.r_[np.zeros(6), np.ones(6)].astype(int)]},
                {"minReplicatesForReplace": 7}):
         with pytest.raises(ValueError):
-            DP.DESeq_device(y, x, d["sizeFactors"], weights=_gm(ok, "cpu"), **kw)
+            DP.DESeq_device(y, x, d["sizeFactors"], weights=gm64(ok, "cpu"), **kw)
         with pytest.raises(ValueError):
             pipeline.DESeq(d["counts"], x, sizeFactors=d["sizeFactors"], engine=emu_dev, weights=ok, **kw)
     w = np.ones((30, 12))
     w[2, 1] = -1.0
     with pytest.raises(ValueError):
         DP.getContrast_device(y, x, d["sizeFactors"], torch.full((30,), 0.1, dtype=torch.float64),
-                              torch.zeros((30, 2), dtype=torch.float64), [0.0, 1.0], weights=_gm(w, "cpu"))
+                              torch.zeros((30, 2), dtype=torch.float64), [0.0, 1.0], weights=gm64(w, "cpu"))
 
 
 # ---------------------------------------------------------------- DESeq_device(weights) against pipeline.DESeq(weights)
@@ -260,7 +249,7 @@ def _compare_weighted(engine, oracle, counts, x, sf, w, dev, minmu=0.5, tol=1e-6
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
         host = pipeline.DESeq(counts, x, sizeFactors=sf, engine=engine, useOptim=False, weights=w, minmu=minmu)
-        dv = DP.DESeq_device(_gm(counts, dev), x, sf, useOptim=False, weights=_gm(w, dev), minmu=minmu)
+        dv = DP.DESeq_device(gm64(counts, dev), x, sf, useOptim=False, weights=gm64(w, dev), minmu=minmu)
     idx = dv["idx"].cpu().numpy()
     assert np.array_equal(idx, host["idx"])
     assert np.array_equal(dv["weightsFail"].cpu().numpy(), host["weightsFail"])
@@ -334,8 +323,8 @@ def test_zero_weight_equals_dropping_the_sample_lrt(emu_dev, reduced):
     # both IRLS runs to a tight deviance tolerance: with the default 1e-8 the two starts (beta0 is unweighted and
     # sees the zero-weight sample) leave differences of order sqrt(1e-8) in beta
     kw = dict(useOptim=False, betaTol=1e-13, maxit=500)
-    a = DP.nbinomLRT_device(_gm(counts, "cpu"), x, xr, d["sizeFactors"], disp, weights=_gm(w, "cpu"), **kw)
-    yk = _gm(counts[:, keep], "cpu")
+    a = DP.nbinomLRT_device(gm64(counts, "cpu"), x, xr, d["sizeFactors"], disp, weights=gm64(w, "cpu"), **kw)
+    yk = gm64(counts[:, keep], "cpu")
     # an intercept-only reduced model takes R's closed form only with weights (the unweighted device LRT fits it by
     # IRLS): all-ones weights on the dropped-sample run give the unweighted closed form
     wk = torch.ones_like(yk) if reduced == "intercept" else None
@@ -357,8 +346,8 @@ def test_zero_weight_equals_dropping_the_sample_dispersion(emu_dev):
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
         # the weighted run's mu is an IRLS fit (no linear mu with weights): to a tight tolerance it is the group mean
-        a = DP.DESeq_device(_gm(counts, "cpu"), x, sf, weights=_gm(w, "cpu"), betaTol=1e-12, dispTol=1e-12)
-        b = DP.DESeq_device(_gm(counts[:, keep], "cpu"), x[keep], sf[keep], betaTol=1e-12, dispTol=1e-12)
+        a = DP.DESeq_device(gm64(counts, "cpu"), x, sf, weights=gm64(w, "cpu"), betaTol=1e-12, dispTol=1e-12)
+        b = DP.DESeq_device(gm64(counts[:, keep], "cpu"), x[keep], sf[keep], betaTol=1e-12, dispTol=1e-12)
     ia, ib = a["idx"].cpu().numpy(), b["idx"].cpu().numpy()
     common = np.intersect1d(ia, ib)
     ga = a["dispGeneEst"].cpu().numpy()[np.searchsorted(ia, common)]
@@ -366,8 +355,8 @@ def test_zero_weight_equals_dropping_the_sample_dispersion(emu_dev):
     # genes where either run fell back to its start value (the noIncrease rule, R/core.R:806-808: the log posterior
     # rose by less than 1e-6 relative) are left out: the starts differ by design, the weighted moments average over
     # all m samples
-    a0a = DP.prep(_gm(counts, "cpu"), x, sf, want_mu=False, weights=_gm(w, "cpu"))["alpha0"].cpu().numpy()[ia]
-    a0b = DP.prep(_gm(counts[:, keep], "cpu"), x[keep], sf[keep], want_mu=False)["alpha0"].cpu().numpy()
+    a0a = DP.prep(gm64(counts, "cpu"), x, sf, want_mu=False, weights=gm64(w, "cpu"))["alpha0"].cpu().numpy()[ia]
+    a0b = DP.prep(gm64(counts[:, keep], "cpu"), x[keep], sf[keep], want_mu=False)["alpha0"].cpu().numpy()
     fallback = (ga == a0a[np.searchsorted(ia, common)]) | (gb == a0b[ib][np.searchsorted(ib, common)])
     fallback |= (ga == 12.0) | (gb == 11.0)             # at the upper bound max(10, m), which differs by one sample
     assert np.mean(fallback) < 0.2
@@ -384,9 +373,9 @@ def test_downweighting_an_outlier_lowers_dispersion(emu_dev):
     counts[0, 0] = 100 * counts[0].max()
     w = np.ones(counts.shape)
     w[0, 0] = 0.0
-    y = _gm(counts, "cpu")
+    y = gm64(counts, "cpu")
     plain = DP.DESeq_device(y, x, np.ones(12))
-    weighted = DP.DESeq_device(y, x, np.ones(12), weights=_gm(w, "cpu"))
+    weighted = DP.DESeq_device(y, x, np.ones(12), weights=gm64(w, "cpu"))
     assert weighted["dispMAP"][0] < plain["dispMAP"][0]
     assert weighted["dispGeneEst"][0] < plain["dispGeneEst"][0]
 
@@ -398,14 +387,14 @@ def test_get_contrast_weights_matches_host(emu_dev):
     w = _fail_some_rows(_zi_weights(200, 36, 3, counts=d["counts"]), x)
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
-        dv = DP.DESeq_device(_gm(d["counts"], "cpu"), x, d["sizeFactors"], weights=_gm(w, "cpu"), useOptim=False)
+        dv = DP.DESeq_device(gm64(d["counts"], "cpu"), x, d["sizeFactors"], weights=gm64(w, "cpu"), useOptim=False)
     idx = dv["idx"].cpu().numpy()
     counts = d["counts"][idx]
-    ynz = _gm(counts, "cpu")
+    ynz = gm64(counts, "cpu")
     nf = np.broadcast_to(d["sizeFactors"][None, :], counts.shape)
     disp, beta = dv["dispersion"].cpu().numpy(), dv["betaMatrix"].cpu().numpy()
     for con in ([0, 1, -1, 0], [0, 0, 0, 1], [0, 0.5, 0.5, -1]):
-        for wd in (dv["weights"], _gm(w[idx], "cpu")):           # normalised or raw: the same normalisation
+        for wd in (dv["weights"], gm64(w[idx], "cpu")):           # normalised or raw: the same normalisation
             g = DP.getContrast_device(ynz, x, d["sizeFactors"], dv["dispersion"], dv["betaMatrix"], con, weights=wd)
             h = pipeline.getContrast(counts, nf, x, disp, beta, con, engine=emu_dev, weights=w[idx])
             for k in ("log2FoldChange", "lfcSE", "stat"):
@@ -415,60 +404,46 @@ def test_get_contrast_weights_matches_host(emu_dev):
 
 # ---------------------------------------------------------------- sharding
 
-def _sharded_worker(rank, world, port, q, emu_lib):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), OMP_NUM_THREADS="2", B200NB_LIB=emu_lib,
-                      B200NB_TEST_EMULATOR="1")
-    import torch.distributed as dist
-    from deseq2_b200 import _lib, device as D, device_pipeline as DP, sharded, synth
-    _lib._SO, _lib._lib = emu_lib, None          # this module imported the package before B200NB_LIB was set
-    D._stream = lambda: C.c_void_p(0)
-    warnings.simplefilter("ignore")
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    x = synth.design_batch_condition(12, 3)
-    d = synth.make_example_counts(400, 12, x=x, seed=91)
-    w = _fail_some_rows(_zi_weights(400, 12, 5), x)
-    lo, hi = sharded.shard_bounds(400, world, rank)
-    y = D.to_gene_major(d["counts"][lo:hi], torch.device("cpu"))
-    wl = D.to_gene_major(w[lo:hi], torch.device("cpu"))
-    plain = sharded.sharded_DESeq_device(y, x, d["sizeFactors"])
-    r = sharded.sharded_DESeq_device(y, x, d["sizeFactors"], weights=wl)
-    if rank == 0:
-        q.put({k: r["gathered"][k].numpy() for k in ("dispersion", "betaMatrix", "betaSE", "WaldPvalue")}
-              | {"collectives": r["collectives"], "collectives_plain": plain["collectives"],
-                 "n_local": int(r["idx"].numel())})
-    dist.barrier()
-    dist.destroy_process_group()
+def _sharded_data(n, m):
+    from deseq2_b200 import synth
+    x = synth.design_batch_condition(m, 3)
+    d = synth.make_example_counts(n, m, x=x, seed=91)
+    return d["counts"], x, d["sizeFactors"], _fail_some_rows(_zi_weights(n, m, 5), x)
+
+
+def _sharded_rank(rank, world, dev, n, m):
+    from deseq2_b200 import sharded
+    K, x, sf, w = _sharded_data(n, m)
+    lo, hi = sharded.shard_bounds(n, world, rank)
+    y = gm(K[lo:hi], dev)
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        plain = sharded.sharded_DESeq_device(y, x, sf)
+        r = sharded.sharded_DESeq_device(y, x, sf, weights=gm(w[lo:hi], dev))
+    return {"gathered": r["gathered"], "extra_collectives": r["collectives"] - plain["collectives"],
+            "n_local": r["idx"].numel()}
+
+
+def _check_sharded(backend, n, m, world=2):
+    """Weights sharded by rows: every gathered result equals the single-process run bit for bit, through the same
+    collectives as the unweighted run (the trend step's gather carries the weighted baseMean)."""
+    from deseq2_b200 import device_pipeline as DP
+    got = run_ranks(_sharded_rank, n, m, world=world, backend=backend)
+    K, x, sf, w = _sharded_data(n, m)
+    dev = DEVICE[backend]
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        whole = DP.DESeq_device(gm64(K, dev), x, sf, weights=gm64(w, dev))
+    assert bool(whole["weightsFail"].any())
+    for g in got:
+        assert 0 < g["n_local"] < whole["idx"].numel()
+        assert g["extra_collectives"] == 0
+        for k in ("dispersion", "betaMatrix", "betaSE", "WaldPvalue"):
+            assert np.array_equal(g["gathered"][k], whole[k].cpu().numpy(), equal_nan=True), k
 
 
 def test_sharded_weights_equal_whole(emu_dev):
-    """Two gloo ranks with weights sharded by rows: every gathered result equals the single-process run bit for bit,
-    through the same collectives as the unweighted run (the trend step's gather carries the weighted baseMean)."""
-    import torch.multiprocessing as mp
-    sys.path.insert(0, os.path.join(ROOT, "tests", "simt_emu"))
-    import build_emu
-    from deseq2_b200 import device_pipeline as DP, synth
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 37500 + (os.getpid() % 2000)
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, q, build_emu.build())) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = q.get(timeout=900)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    x = synth.design_batch_condition(12, 3)
-    d = synth.make_example_counts(400, 12, x=x, seed=91)
-    w = _fail_some_rows(_zi_weights(400, 12, 5), x)
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        whole = DP.DESeq_device(_gm(d["counts"], "cpu"), x, d["sizeFactors"], weights=_gm(w, "cpu"))
-    assert 0 < got["n_local"] < whole["idx"].numel()
-    assert got["collectives"] == got["collectives_plain"]
-    for k in ("dispersion", "betaMatrix", "betaSE", "WaldPvalue"):
-        assert np.array_equal(got[k], whole[k].numpy(), equal_nan=True), k
+    _check_sharded("gloo", 400, 12)
 
 
 # ---------------------------------------------------------------- GPU (or the emulator with B200NB_LIB)
@@ -491,7 +466,7 @@ def test_device_pipeline_weights_match_host_gpu(engine, oracle, design, n, m, po
     if poscounts:
         low = np.random.default_rng(2).random(counts.shape) < 0.3
         counts[low] = 0                                                # dropouts, down-weighted
-        sf = DP.size_factors(_gm(counts, DEV), m, type="poscounts")["sizeFactors"].cpu().numpy()
+        sf = DP.size_factors(gm64(counts, DEV), m, type="poscounts")["sizeFactors"].cpu().numpy()
         minmu = 1e-6
     w = _fail_some_rows(_zi_weights(n, m, 19, low=low, counts=counts), x)
     _compare_weighted(engine, oracle, counts, x, sf, w, DEV, minmu=minmu)
@@ -509,7 +484,7 @@ def test_config_sizes_with_weights(engine, config):
     w = _fail_some_rows(_zi_weights(n, m, 23, counts=d["counts"]), x)
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
-        dv = DP.DESeq_device(_gm(d["counts"], DEV), x, d["sizeFactors"], weights=_gm(w, DEV))
+        dv = DP.DESeq_device(gm64(d["counts"], DEV), x, d["sizeFactors"], weights=gm64(w, DEV))
     for k in ("dispersion", "betaMatrix", "betaSE", "WaldStatistic", "WaldPvalue", "deviance"):
         assert torch.isfinite(dv[k]).all(), k
     assert (dv["betaIter"] < 100).double().mean().item() >= 0.99
@@ -521,16 +496,5 @@ def test_config_sizes_with_weights(engine, config):
 
 
 @pytest.mark.gpu
-def test_sharded_weights_over_nccl_equals_whole():
-    n_gpu = torch.cuda.device_count() if DEV == "cuda" else 0
-    if n_gpu < 2:
-        pytest.skip("needs at least 2 GPUs")
-    env = dict(os.environ)
-    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK", "MASTER_ADDR", "MASTER_PORT"):
-        env.pop(k, None)
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29647",
-                        os.path.join(ROOT, "scripts", "sharded_weights_nccl.py")], env=env, capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0, (r.stdout[-2000:], r.stderr[-3000:])
-    assert "sharded == whole: True" in r.stdout and "extra collectives: 0" in r.stdout, r.stdout[-2000:]
+def test_sharded_weights_over_nccl_equals_whole(engine):
+    _check_sharded("nccl", 20000, 60, nccl_world())
