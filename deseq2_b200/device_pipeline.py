@@ -33,6 +33,9 @@ R/helper.R:421-435) fit the dispersion function with DESeq_device's GeneEst bloc
 matrix with one kernel (b200nb_transform_dev, csrc/transform.cuh).
 rlog_device (R/rlog.R) fits the dispersion function the same way, then runs rlogData's prior variance
 (b200nb_rlog_prior_var_dev) and its per-gene fit of the design [1 | I_m] (b200nb_rlog_fit_dev, csrc/rlog.cuh).
+lfcShrink_device (R/lfcShrink.R, type "normal") refits a DESeq_device result with a zero-centred normal prior: the
+standard (coef) or expanded (contrast) prior variance from the prior-variance kernel, the MAP fit shared with
+DESeq_device(betaPrior=True) (_map_fit), and results_device on it.
 """
 from __future__ import annotations
 
@@ -356,20 +359,29 @@ def beta_prior_columns(fidx):
     return np.asarray(a, np.int32), np.asarray(b, np.int32), np.asarray(owner)
 
 
-def estimate_beta_prior_var(betaMatrix, factors, baseMean, dispFit, upperQuantile=0.05):
-    """estimateBetaPriorVar (R/core.R:1601-1689, betaPriorMethod "weighted", expanded model matrix) on the device.
-    betaMatrix: (n, p) MLE log2 fold changes on the standard matrix factorDesign(factors)[0] (DESeq_device's
-    "betaMatrix"); baseMean / dispFit: (n,) device tensors.  The quantiles of all columns and contrasts are one kernel
-    launch; averagePriorsOverLevels (R/expanded.R:20-73) is a few torch ops.  Returns the prior variances of the
-    EXPANDED matrix's columns as a device tensor (1e6 for the intercept).  Raises ValueError like R when one of
-    them is NA or not positive (one host read)."""
+def estimate_beta_prior_var(betaMatrix, factors, baseMean, dispFit, upperQuantile=0.05, expandedType=True):
+    """estimateBetaPriorVar (R/core.R:1601-1689, betaPriorMethod "weighted") on the device.
+    betaMatrix: (n, p) MLE log2 fold changes (DESeq_device's "betaMatrix"); baseMean / dispFit: (n,) device tensors.
+    expandedType=True (modelMatrixType "expanded", DESeq(betaPrior=TRUE) and lfcShrink(contrast=)): betaMatrix is on
+    the standard matrix factorDesign(factors)[0]; the quantiles of all columns and addAllContrasts' level differences
+    are one kernel launch, averagePriorsOverLevels (R/expanded.R:20-73) a few torch ops, and the result holds the
+    prior variances of the EXPANDED matrix's columns.  expandedType=False (modelMatrixType "standard",
+    lfcShrink(coef=)): betaMatrix is on any design whose column 0 is the intercept (factors is not used); one quantile
+    per other column, in one launch, and the result holds the prior variances of those p columns.  Either way the
+    intercept gets 1e6, a column with no |beta| < 10 gets 1e6, and a single gene gets beta^2 (R/core.R:1648-1666).
+    Returns a device tensor.  Raises ValueError like R when one of them is NA or not positive (one host read)."""
     from scipy import stats as _st
     from .pipeline import factorDesign
-    _, _, fidx, _ = factorDesign(factors, expanded=False)
-    _, enames, efidx, _ = factorDesign(factors, expanded=True)
     bt = betaMatrix.T.contiguous()                                      # (p, n): a view's base when it is one
     dev = bt.device
-    col_a, col_b, owner = beta_prior_columns(fidx)
+    if expandedType:
+        _, _, fidx, _ = factorDesign(factors, expanded=False)
+        _, enames, efidx, _ = factorDesign(factors, expanded=True)
+        col_a, col_b, owner = beta_prior_columns(fidx)
+    else:
+        p = bt.shape[0]
+        col_a, col_b = np.arange(1, p, dtype=np.int32), np.full(p - 1, -1, np.int32)
+        enames = ["Intercept"] + [f"column {k}" for k in range(1, p)]
     if bt.shape[1] > 1:
         q = beta_prior_quantile(bt, baseMean, dispFit, col_a, col_b, 1.0 - upperQuantile)
         z = float(_st.norm.ppf(1.0 - upperQuantile / 2.0))
@@ -379,10 +391,13 @@ def estimate_beta_prior_var(betaMatrix, factors, baseMean, dispFit, upperQuantil
         b = torch.as_tensor(col_b.astype(np.int64), device=dev)
         x = bt[a, 0] - torch.where(b >= 0, bt[b.clamp(min=0), 0], torch.zeros_like(bt[a, 0]))
         pv = x ** 2
-    out = torch.full((len(efidx),), 1e6, dtype=F64, device=dev)
-    owner_d = torch.as_tensor(owner, device=dev)
-    for f in sorted({int(v) for v in efidx if v >= 0}):
-        out[torch.as_tensor(efidx == f, device=dev)] = pv[owner_d == f].mean()
+    if expandedType:
+        out = torch.full((len(efidx),), 1e6, dtype=F64, device=dev)
+        owner_d = torch.as_tensor(owner, device=dev)
+        for f in sorted({int(v) for v in efidx if v >= 0}):
+            out[torch.as_tensor(efidx == f, device=dev)] = pv[owner_d == f].mean()
+    else:
+        out = torch.cat([torch.full((1,), 1e6, dtype=F64, device=dev), pv])
     bad = (torch.isnan(out) | (out <= 0)).cpu().numpy()
     if bad.any():
         raise ValueError("beta prior for " + ",".join(np.asarray(enames)[bad]) + " is NA or not greater than 0")
@@ -1008,7 +1023,6 @@ def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, dispFit_all,
     over all genes, then the MAP fit on the expanded matrix, its log-likelihood and the optim fallback with the same
     lambda.  Returns (fit, loglik, betaConv, extra result entries)."""
     from .pipeline import factorDesign
-    dev = ynz.device
     p = mle["beta_mat"].shape[0]
     mleBeta = mle["beta_mat"] / LN2                                     # (p, n), log2 scale
     if allgather is not None:
@@ -1019,18 +1033,31 @@ def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, dispFit_all,
         beta_all = mleBeta
     pv = estimate_beta_prior_var(beta_all.T, factors, bm_all, dispFit_all)
     x_exp = factorDesign(factors, expanded=True)[0]
-    pe = x_exp.shape[1]
-    xe = D.x_to_device(x_exp, dev)
-    lam = 1.0 / (LN2 ** 2 * pv)
-    contrast = torch.zeros(pe, dtype=F64, device=dev)
-    contrast[0] = 1.0
-    # the expanded matrix is rank deficient: start at (log baseMean, 0, ..., 0) (R/fitNbinomGLMs.R:146-151)
-    beta0 = torch.zeros((pe, ynz.shape[0]), dtype=F64, device=dev)
-    beta0[0] = torch.log(bm)
-    fit, ll, betaConv, n_optim = _glm_fit(ynz, xe, sfd, dispersion, contrast, beta0, lam, betaTol=betaTol, maxit=maxit,
-                                          minmu=minmu, useOptim=useOptim, want_hat=False, want_mu=False)
+    fit, ll, betaConv, n_optim = _map_fit(ynz, x_exp, sfd, dispersion, pv, _expanded_start(bm, x_exp.shape[1]),
+                                          betaTol, maxit, minmu, useOptim)
     return fit, ll, betaConv, {"mleBetaMatrix": mleBeta.T, "betaPriorVar": pv.cpu().numpy(), "modelMatrix": x_exp,
                                "n_optim_map": n_optim}
+
+
+def _expanded_start(bm, pe):
+    """The start values of a fit on the rank-deficient expanded matrix: (log baseMean, 0, ..., 0) per gene
+    (R/fitNbinomGLMs.R:146-151), as a (pe, n) device tensor."""
+    beta0 = torch.zeros((pe, bm.numel()), dtype=F64, device=bm.device)
+    beta0[0] = torch.log(bm)
+    return beta0
+
+
+def _map_fit(ynz, x, sfd, dispersion, betaPriorVar, beta0, betaTol, maxit, minmu, useOptim, weights=None):
+    """fitGLMsWithPrior's refit (R/fitNbinomGLMs.R:311-330): fitNbinomGLMs on the model matrix x (numpy) with
+    lambda = 1 / betaPriorVar ((p,) device tensor, log2 scale) from the start values beta0 ((p, n), natural log): the
+    IRLS fit, the log-likelihood at the unclamped mean and the optim fallback with the same lambda.  weights: the
+    normalised observation weights of the rows.  Returns _glm_fit's (fit, loglik, betaConv, number of optim rows)."""
+    p = x.shape[1]
+    lam = 1.0 / (LN2 ** 2 * betaPriorVar)
+    contrast = torch.zeros(p, dtype=F64, device=ynz.device)
+    contrast[0] = 1.0
+    return _glm_fit(ynz, D.x_to_device(x, ynz.device), sfd, dispersion, contrast, beta0, lam, betaTol=betaTol,
+                    maxit=maxit, minmu=minmu, useOptim=useOptim, weights=weights, want_hat=False, want_mu=False)
 
 
 def _replacement_counts(ys, nfm, over, replaceable, m, trim=0.2):
@@ -1548,15 +1575,21 @@ def results_heuristic(ynz, m, rows, cooks_rows, keep):
                "results_heuristic_dev")
 
 
-def _first_fit_cooks(res, ynz, rows, x, sfd):
-    """The Cook's rows of `rows` from the first fit's mu / H (res["mu"] / res["H"], DESeq_device's workspace views: R
-    restores the first fit's Cook's distances after a refit, R/core.R:2556).  Raises ValueError when a later
-    DESeq_device call has since replaced the workspace."""
+def _check_first_fit_views(res, ynz):
+    """Raises ValueError when res["mu"] / res["H"], views of DESeq_device's workspace, have been replaced by a later
+    DESeq_device call."""
     mu_ws, h_ws = _WS.get(("mu_cooks", str(ynz.device))), _WS.get(("H", str(ynz.device)))
     if (mu_ws is None or h_ws is None or res["mu"].data_ptr() != mu_ws.data_ptr()
             or res["H"].data_ptr() != h_ws.data_ptr() or tuple(res["mu"].shape) != tuple(ynz.shape)):
         raise ValueError("res['mu'] / res['H'] are views of DESeq_device's workspace and a later DESeq_device call has "
                          "replaced it: run results_device before the next DESeq_device call")
+
+
+def _first_fit_cooks(res, ynz, rows, x, sfd):
+    """The Cook's rows of `rows` from the first fit's mu / H (res["mu"] / res["H"], DESeq_device's workspace views: R
+    restores the first fit's Cook's distances after a refit, R/core.R:2556).  Raises ValueError when a later
+    DESeq_device call has since replaced the workspace."""
+    _check_first_fit_views(res, ynz)
     nf = sfd[rows].contiguous() if sfd.dim() == 2 else None
     return cooks(ynz[rows].contiguous(), res["mu"][rows].contiguous(), res["H"][rows].contiguous(), x,
                  res.get("sizeFactors"), normalizationFactors=nf)["cooks"]
@@ -1686,4 +1719,128 @@ def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcT
         out["padj"] = padj[lo:hi]
     meta["lfcThreshold"] = lfcThreshold
     out["metadata"] = meta
+    return out
+
+
+# ---------------------------------------------------------------- lfcShrink(type = "normal") (R/lfcShrink.R:145-327)
+
+def _scatter_rows(v, rows, n):
+    """v's rows at `rows` of a fresh (n, ...) tensor, NaN (False for bool) elsewhere."""
+    fill = False if v.dtype == torch.bool else float("nan")
+    out = torch.full((n,) + tuple(v.shape[1:]), fill, dtype=v.dtype, device=v.device)
+    out[rows] = v
+    return out
+
+
+def lfcShrink_device(res, y, x, coef=None, contrast=None, results=None, lfcThreshold=0, factors=None, weights=None,
+                     allgather=None, betaTol=1e-8, maxit=100, useOptim=True, minmu=0.5, type="normal"):
+    """lfcShrink(type = "normal") (R/lfcShrink.R:145-327) on a DESeq_device result `res` (betaPrior=False, any
+    test) for the gene-major (N, ld) counts y it was run on and its design x.  Only type "normal" exists in DESeq2;
+    "apeglm" and "ashr" call other packages and raise ValueError, as do R's other stops (pipeline.lfcShrink_checks).
+    coef (a column index or factorDesign name of x; x may be any full-rank design whose first column is the
+    intercept, numeric covariates included -- R's user-supplied-matrix path): estimateBetaPriorVar with
+    modelMatrixType "standard" (R/core.R:1601-1689: one weighted quantile per non-intercept MLE column, one launch of
+    b200nb_beta_prior_quantile_dev), then fitNbinomGLMs(lambda = 1 / betaPriorVar) on x from the pre-step kernel's
+    linear-model start values (R/fitNbinomGLMs.R:242-337; the MLE is skipped because mu and H exist).
+    contrast (as results_device takes it with factors, over the expanded matrix's columns; x must be
+    factorDesign(factors)[0]): the expanded prior (estimate_beta_prior_var) and the MAP fit on
+    factorDesign(factors, expanded=True)[0] from (log baseMean, 0, ..., 0) -- what DESeq_device(betaPrior=True)
+    computes.  Both fits are _map_fit: the IRLS kernel, the log-likelihood at the unclamped mean and the optim
+    fallback with the same lambda, with nbinomWaldTest's betaTol / maxit / useOptim / minmu (R's lfcShrink passes
+    none of DESeq's on).  The prior's weights are 1 / (1 / baseMean + dispFit) of res's rows (the weighted baseMean
+    for a weights result, whose normalised weights also go to the MAP fit; weights: the raw weights, as for
+    results_device, coef only).
+    Outlier-refit results (R/core.R:2484-2564): the MAP fit runs on the ORIGINAL counts with the refitted
+    dispersions, and the prior uses the replaced baseMean / dispFit and the refitted MLE betas; rows whose replaced
+    counts are all zero are allZero in R and are neither in the prior nor fitted (the shrunk table's nowZero rule
+    gives them log2FoldChange and lfcSE 0).  For a contrast the shrunk table's getContrast reads the replaced counts
+    (R/results.R:779-781), rebuilt by results_device from res's "replace" / "replaceable" / "n_replaced"; with
+    lfcThreshold > 0 its Cook's cutoff uses the first fit's maxCooks, recomputed from res["mu"] / res["H"] on the
+    original counts without the replaceable-sample zeroing, as nbinomWaldTest recomputes it (R/core.R:1452-1460).
+    res["mu"] / res["H"] are DESeq_device's workspace views: where they are read, a stale result raises ValueError
+    as in results_device.
+    results: the table to modify (a results_device dict over the N rows); by default results_device(res, y, x,
+    name=coef) or (..., contrast=contrast) with its defaults.  The shrunk table is results_device on the MAP fit with
+    the same selection, lfcThreshold and minmu; its log2FoldChange and lfcSE replace the table's, and with
+    lfcThreshold > 0 its stat, pvalue and padj too (the other columns stay the table's tensors).
+    allgather (sharded.sharded_lfcShrink_device): ONE packed collective carries baseMean, dispFit and the non-intercept
+    MLE columns of every rank's rows for the prior; the default table and the thresholded table take one each.
+    Returns the table's dict with those columns replaced, metadata["priorInfo"] = {"type": "normal", "package":
+    "DESeq2", "betaPriorVar": numpy}, and "shrinkFit": the MAP fit over res's rows ("betaMatrix", "betaSE",
+    "betaConv", "betaIter", "modelMatrix", "n_optim")."""
+    from .pipeline import factorDesign, lfcShrink_checks
+    x = np.asarray(x, dtype=np.float64)
+    m, p = x.shape
+    expanded, k = lfcShrink_checks(x, coef, contrast, results is not None, lfcThreshold, factors,
+                                   res.get("weightsFail") is not None or weights is not None,
+                                   res.get("modelMatrix") is not None, type)
+    sel = dict(contrast=contrast) if expanded else dict(name=k)
+    if results is None:
+        results = results_device(res, y, x, factors=factors, weights=weights, allgather=allgather, **sel)
+    dev = y.device
+    idx = res["idx"]
+    n = idx.numel()
+    ynz = y if n == y.shape[0] else y[idx].contiguous()
+    nf = res.get("normalizationFactors")
+    sfd = nf if nf is not None else torch.as_tensor(res["sizeFactors"], device=dev)
+    n_rep = res.get("n_replaced", 0)
+    bm = res["baseMean"]
+    rows = None                                       # the rows fitted: all of res's, or those not all zero once replaced
+    if n_rep > 0:
+        rows = torch.nonzero(~(res["replace"] & (bm == 0))).squeeze(1)
+        if rows.numel() == n:
+            rows = None
+    sub = (lambda v: v) if rows is None else (lambda v: v[rows].contiguous())
+    # ---- the prior over every fitted row of every rank
+    B = sub(res["betaMatrix"])
+    bmp, dfp = sub(bm), sub(res["dispFit"])
+    if allgather is not None:
+        g = allgather([bmp, dfp] + [B[:, j] for j in range(1, p)])
+        bmp, dfp = g[0], g[1]
+        B = torch.stack([torch.zeros_like(g[0])] + list(g[2:]), dim=1)   # the intercept's column is not read
+    pv = estimate_beta_prior_var(B, factors, bmp, dfp, expandedType=expanded)
+    # ---- the MAP fit on the original counts
+    fy = sub(ynz)
+    fsfd = sfd if rows is None else _rows(sfd, rows)
+    if expanded:
+        xf = factorDesign(factors, expanded=True)[0]
+        bm0 = bm
+        if n_rep > 0:           # the start is the mean of the ORIGINAL normalised counts; baseMean is the replaced one
+            rr = torch.nonzero_static(res["replace"], size=n_rep).squeeze(1)
+            nfm = sfd[rr][:, :m] if sfd.dim() == 2 else sfd[None, :]
+            bm0 = bm.clone()
+            bm0[rr] = (ynz[rr][:, :m].to(F64) / nfm).mean(dim=1)
+        beta0 = _expanded_start(sub(bm0), xf.shape[1])
+    else:
+        xf = x
+        beta0 = prep(fy, x, None if nf is not None else res["sizeFactors"], minmu=minmu, want_mu=False,
+                     normalizationFactors=fsfd if nf is not None else None, xim=1.0)["beta0"]
+    wn = res.get("weights")
+    fit, _, betaConv, n_optim = _map_fit(fy, xf, fsfd, sub(res["dispersion"]), pv, beta0, betaTol, maxit, minmu,
+                                         useOptim, weights=None if wn is None else sub(wn))
+    st = _wald_stats(fit)
+    st["betaConv"], st["betaIter"] = betaConv, fit["iter"]
+    if rows is not None:
+        st = {key: _scatter_rows(v, rows, n) for key, v in st.items()}
+    # ---- the shrunk table: results() of the MAP fit
+    shr = {key: res.get(key) for key in ("idx", "baseMean", "dispersion", "sizeFactors", "mu", "H", "maxCooks")}
+    shr.update(st, test="Wald")
+    for key in ("normalizationFactors", "weights", "weightsFail", "replace", "replaceable", "n_replaced"):
+        if key in res:
+            shr[key] = res[key]
+    if expanded:
+        shr["modelMatrix"], shr["betaPriorVar"] = xf, pv.cpu().numpy()
+    if lfcThreshold > 0 and n_rep > 0:
+        _check_first_fit_views(res, ynz)
+        shr["maxCooks"] = cooks(ynz, res["mu"], res["H"], x, res.get("sizeFactors"), want_matrix=False,
+                                normalizationFactors=nf)["maxCooks"]
+    tab = results_device(shr, y, x, factors=factors, lfcThreshold=lfcThreshold, minmu=minmu, weights=weights,
+                         allgather=allgather if lfcThreshold > 0 else None, **sel)
+    out = dict(results)
+    for key in ["log2FoldChange", "lfcSE"] + (["stat", "pvalue", "padj"] if lfcThreshold > 0 else []):
+        out[key] = tab[key]
+    out["metadata"] = dict(results.get("metadata", {}))
+    out["metadata"]["priorInfo"] = {"type": "normal", "package": "DESeq2", "betaPriorVar": pv.cpu().numpy()}
+    out["shrinkFit"] = {"betaMatrix": st["betaMatrix"], "betaSE": st["betaSE"], "betaConv": st["betaConv"],
+                        "betaIter": st["betaIter"], "modelMatrix": xf, "n_optim": n_optim}
     return out

@@ -1005,20 +1005,36 @@ def estimateBetaPriorVar(betaMatrix, names, fidx, baseMean, dispFit, expandedTyp
 
 
 def fitGLMsWithPrior(counts, nf, factors, dispersion, baseMean, dispFit, engine=None, betaTol=1e-8, maxit=100,
-                     useQR=True, minmu=0.5, useOptim=True):
+                     useQR=True, minmu=0.5, useOptim=True, betaPriorVar=None, modelMatrix=None, weights=None):
     """R/fitNbinomGLMs.R:242-337 for an additive factor design with the expanded model matrix (the default when
     betaPrior=TRUE): MLE fit on the standard matrix -> estimateBetaPriorVar -> MAP fit on the expanded matrix with
-    lambda = 1 / betaPriorVar.  useOptim goes to both fits (fitNbinomGLMs)."""
-    x_std, names, fidx, _ = factorDesign(factors, expanded=False)
-    mle = fitNbinomGLMs(counts, nf, x_std, dispersion, engine=engine, betaTol=betaTol, maxit=maxit, useQR=useQR,
-                        minmu=minmu, useOptim=useOptim)
-    _, mean_by_factor = estimateBetaPriorVar(mle["betaMatrix"], names, fidx, baseMean, dispFit, expandedType=True)
-    x_exp, enames, efidx, _ = factorDesign(factors, expanded=True)
-    betaPriorVar = np.array([1e6 if f < 0 else mean_by_factor[int(f)] for f in efidx])
+    lambda = 1 / betaPriorVar.  useOptim goes to both fits (fitNbinomGLMs).
+    betaPriorVar given (lfcShrink): the MLE fit and the prior are skipped, as R skips them when the first fit's mu
+    and H exist (:250, :289-305); the MAP fit is on modelMatrix (modelMatrixType "standard" or "user-supplied") or,
+    when it is None, on the expanded matrix of the factors, and "H", "mu", "mleBetaMatrix" and "mle" are None.
+    weights: normalised observation weights of the rows, for the MAP fit."""
+    mle = None
+    if betaPriorVar is None:
+        x_std, names, fidx, _ = factorDesign(factors, expanded=False)
+        mle = fitNbinomGLMs(counts, nf, x_std, dispersion, engine=engine, betaTol=betaTol, maxit=maxit, useQR=useQR,
+                            minmu=minmu, useOptim=useOptim)
+        _, mean_by_factor = estimateBetaPriorVar(mle["betaMatrix"], names, fidx, baseMean, dispFit, expandedType=True)
+        x_exp, enames, efidx, _ = factorDesign(factors, expanded=True)
+        betaPriorVar = np.array([1e6 if f < 0 else mean_by_factor[int(f)] for f in efidx])
+    elif modelMatrix is None:
+        x_exp, enames = factorDesign(factors, expanded=True)[:2]
+    else:
+        x_exp, enames = np.asarray(modelMatrix, dtype=np.float64), None
+    betaPriorVar = np.asarray(betaPriorVar, dtype=np.float64)
+    if betaPriorVar.shape != (x_exp.shape[1],):
+        raise ValueError(f"betaPriorVar should have length {x_exp.shape[1]} to match the model matrix")
     if np.any(betaPriorVar == 0):
         raise ValueError("beta prior variances are equal to zero for some variables")
     fit = fitNbinomGLMs(counts, nf, x_exp, dispersion, lambda_=1.0 / betaPriorVar, engine=engine, betaTol=betaTol,
-                        maxit=maxit, useQR=useQR, minmu=minmu, useOptim=useOptim)
+                        maxit=maxit, useQR=useQR, minmu=minmu, useOptim=useOptim, weights=weights)
+    if mle is None:
+        return {"fit": fit, "H": None, "mu": None, "betaPriorVar": betaPriorVar, "modelMatrix": x_exp,
+                "mleBetaMatrix": None, "names": enames, "mle": None}
     return {"fit": fit, "H": mle["hat_diagonals"], "mu": mle["mu"], "betaPriorVar": betaPriorVar,
             "modelMatrix": x_exp, "mleBetaMatrix": mle["betaMatrix"], "names": enames, "mle": mle}
 
@@ -1914,3 +1930,128 @@ def results(dds, counts, x, name=None, contrast=None, listValues=(1, -1), lfcThr
     meta["lfcThreshold"] = lfcThreshold
     return {"baseMean": np.asarray(dds["baseMean"], dtype=np.float64), "log2FoldChange": lfc, "lfcSE": se,
             "stat": stat, "pvalue": pv, "padj": padj, "metadata": meta}
+
+
+# ---------------------------------------------------------------- lfcShrink(type = "normal") (R/lfcShrink.R:145-327)
+
+SHRINK_TYPES = ("normal", "apeglm", "ashr")
+
+
+def lfcShrink_checks(x, coef, contrast, res_given, lfcThreshold, factors, weighted, betaPrior, type="normal"):
+    """lfcShrink()'s stops (R/lfcShrink.R:145-327) and this restatement's limits, shared by lfcShrink and
+    device_pipeline.lfcShrink_device.  x: the design DESeq ran on; res_given: whether a results table was passed;
+    weighted: whether the DESeq run had observation weights; betaPrior: whether it ran with betaPrior=TRUE.
+    Returns (expanded, k): whether the prior is on the expanded model matrix (a contrast) or on x (a coefficient),
+    and the coefficient's column of x (None for a contrast)."""
+    if type not in SHRINK_TYPES:
+        raise ValueError(f"type must be one of {', '.join(SHRINK_TYPES)}")
+    if type != "normal":
+        raise ValueError(f"type={type!r} calls the {type} package, which is not part of DESeq2: only type='normal' is "
+                         "implemented")
+    if betaPrior:
+        raise ValueError("lfcShrink() should be used downstream of DESeq() with betaPrior=FALSE (the default)")
+    if coef is None and contrast is None:
+        raise ValueError("type='normal' requires either 'coef' or 'contrast' be specified.")
+    if coef is not None and contrast is not None:
+        raise ValueError("give either 'coef' or 'contrast', not both")
+    if not (np.isfinite(lfcThreshold) and lfcThreshold >= 0):
+        raise ValueError("lfcThreshold must be finite and >= 0")
+    x = np.asarray(x, dtype=np.float64)
+    if not np.all(x[:, 0] == 1):
+        raise ValueError("lfcShrink needs a design with an intercept: the first column of x must be all ones")
+    if contrast is None:
+        names = factorDesign(factors)[1] if factors is not None else None
+        return False, _col_index(coef, names, x.shape[1])
+    if not isinstance(contrast, (tuple, list)) and not res_given:
+        raise ValueError("for type='normal' and numeric contrast, user must provide 'res' object (results=)")
+    if factors is None:
+        raise ValueError("a contrast is shrunk on the expanded model matrix, which needs the design factors "
+                         "(factors=...)")
+    if not np.array_equal(x, factorDesign(factors)[0]):
+        raise ValueError("user-supplied design matrix supports shrinkage only with 'coef': for a contrast x must be "
+                         "the standard model matrix of the factors, factorDesign(factors)[0]")
+    if weighted:
+        raise ValueError("observation weights are not supported with a contrast (the expanded model matrix is rank "
+                         "deficient): shrink a coefficient (coef=) instead")
+    return True, None
+
+
+def lfcShrink(dds, counts, x, coef=None, contrast=None, res=None, lfcThreshold=0, factors=None, engine=None,
+              betaTol=1e-8, maxit=100, useOptim=True, minmu=0.5, type="normal", cooks=None):
+    """lfcShrink(type = "normal") (R/lfcShrink.R:145-327) on a pipeline.DESeq result dds (betaPrior=False) for the
+    (N, m) counts it was run on and its design x.  coef: a column index or factorDesign name of x (the prior is
+    estimateBetaPriorVar's "standard" one over x's MLE columns, the MAP fit is on x); contrast: as results() takes it
+    with factors, over the expanded matrix's columns (the prior is the expanded one, the MAP fit on
+    factorDesign(factors, expanded=True)[0]).  The prior is over the rows that are neither all zero, weightsFail nor
+    all zero after an outlier replacement; the MAP fit (fitGLMsWithPrior with the given betaPriorVar) is on their
+    ORIGINAL counts, with dds's dispersions and normalised weights.  res: the results table to modify, by default
+    results(dds, name=coef) or results(dds, contrast=contrast) (with dds's LRT columns after test="LRT").  The shrunk
+    table is results() of the MAP fit with lfcThreshold, minmu and defaults otherwise; its log2FoldChange and lfcSE
+    replace res's, and with lfcThreshold > 0 its stat, pvalue and padj too.  Its Cook's cutoff uses the first fit's
+    maxCooks without the replaceable-sample zeroing (nbinomWaldTest recomputes it, R/core.R:1452-1460), from cooks:
+    the (N, m) Cook's distances of the first fit, needed then and by the two-group heuristic.  Returns res's dict
+    with those columns replaced and metadata["priorInfo"] = {"type", "package", "betaPriorVar"}."""
+    engine = engine or _default_engine
+    counts = np.asarray(counts)
+    N, m = counts.shape
+    x = np.asarray(x, dtype=np.float64)
+    p = x.shape[1]
+    expanded, k = lfcShrink_checks(x, coef, contrast, res is not None, lfcThreshold, factors,
+                                   dds.get("weights") is not None, dds.get("modelMatrix") is not None, type)
+    nz = ~np.asarray(dds["allZero"], bool)
+    if "weightsFail" in dds:
+        nz = nz & ~np.asarray(dds["weightsFail"], bool)
+    fit = nz.copy()
+    replaced = "replace" in dds and np.nansum(dds["replace"]) > 0
+    if replaced:                                    # all zero once replaced: allZero in R (R/core.R:2491-2492)
+        fit &= ~(np.asarray(dds["replace"], bool) & (dds["baseMean"] == 0))
+    betaMatrix, baseMean, dispFit = dds["betaMatrix"][fit], dds["baseMean"][fit], dds["dispFit"][fit]
+    if expanded:
+        _, names, fidx, _ = factorDesign(factors)
+        _, mean_by_factor = estimateBetaPriorVar(betaMatrix, names, fidx, baseMean, dispFit, expandedType=True)
+        betaPriorVar = np.array([1e6 if f < 0 else mean_by_factor[int(f)]
+                                 for f in factorDesign(factors, expanded=True)[2]])
+    else:
+        names = ["Intercept"] + [f"column {j}" for j in range(1, p)]
+        betaPriorVar, _ = estimateBetaPriorVar(betaMatrix, names, np.r_[-1, np.zeros(p - 1, int)], baseMean,
+                                               dispFit, expandedType=False)
+    if dds.get("normalizationFactors") is not None:
+        nf = np.asarray(dds["normalizationFactors"])[fit]
+    else:
+        nf = np.broadcast_to(dds["sizeFactors"], (int(fit.sum()), m))
+    w = dds.get("weights")
+    if w is not None:
+        w = np.asarray(w)[fit[nz]]
+    gp = fitGLMsWithPrior(counts[fit], nf, factors, dds["dispersion"][fit], None, None, engine=engine,
+                          betaTol=betaTol, maxit=maxit, minmu=minmu, useOptim=useOptim, betaPriorVar=betaPriorVar,
+                          modelMatrix=None if expanded else x, weights=w)
+    f = gp["fit"]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        stat = f["betaMatrix"] / f["betaSE"]
+    shr = dict(dds)
+    shr["test"] = "Wald"
+    for key, v in (("betaMatrix", f["betaMatrix"]), ("betaSE", f["betaSE"]), ("WaldStatistic", stat),
+                   ("WaldPvalue", 2.0 * _sp.ndtr(-np.abs(stat)))):
+        shr[key] = np.full((N, v.shape[1]), np.nan)
+        shr[key][fit] = v
+    if expanded:
+        shr["betaPriorVar"], shr["modelMatrix"] = betaPriorVar, gp["modelMatrix"]
+    if replaced and lfcThreshold > 0:
+        if cooks is None:
+            raise ValueError("after an outlier refit a thresholded shrunk table needs the first fit's Cook's "
+                             "distances (cooks=...)")
+        shr["maxCooks"] = np.full(N, np.nan)
+        shr["maxCooks"][nz] = recordMaxCooks(x, np.asarray(cooks, dtype=np.float64)[nz])
+    sel = dict(contrast=contrast) if expanded else dict(name=k)
+    if res is None:
+        lrt = ({"LRTStatistic": dds["LRTStatistic"], "LRTPvalue": dds["LRTPvalue"]} if dds.get("test") == "LRT"
+               else None)
+        res = results(dds, counts, x, factors=factors, lrt=lrt, cooks=cooks, engine=engine, **sel)
+    tab = results(shr, counts, x, lfcThreshold=lfcThreshold, factors=factors, minmu=minmu, cooks=cooks,
+                  engine=engine, **sel)
+    out = dict(res)
+    for key in ["log2FoldChange", "lfcSE"] + (["stat", "pvalue", "padj"] if lfcThreshold > 0 else []):
+        out[key] = tab[key]
+    out["metadata"] = dict(res.get("metadata", {}))
+    out["metadata"]["priorInfo"] = {"type": "normal", "package": "DESeq2", "betaPriorVar": betaPriorVar}
+    return out

@@ -216,3 +216,18 @@ def sharded_results_device(res_local, y_local, x, **kw):
     out = DP.results_device(res_local, y_local, x, allgather=pg, **kw)
     out["collectives"] = pg.collectives
     return out
+
+
+def sharded_lfcShrink_device(res_local, y_local, x, **kw):
+    """lfcShrink(type = "normal") on this rank's shard of a sharded_DESeq_device run (y_local: the shard's rows as
+    shard_bounds splits them; res_local: its result).  The prior needs every gene: ONE packed all-gather carries
+    baseMean, dispFit and the p - 1 non-intercept MLE columns of every rank's rows (2 + p - 1 doubles per gene), and
+    every rank estimates the same prior from them; the MAP fit stays local.  The default results table (when
+    results= is not given) and, with lfcThreshold > 0, the shrunk table each take sharded_results_device's one gather
+    of [filter, pvalue].  Keyword arguments as device_pipeline.lfcShrink_device; returns its dict for the shard plus
+    "collectives" (the size agreement included)."""
+    from . import device_pipeline as DP
+    pg = PackedGather(y_local.shape[0], y_local.device)
+    out = DP.lfcShrink_device(res_local, y_local, x, allgather=pg, **kw)
+    out["collectives"] = pg.collectives
+    return out
