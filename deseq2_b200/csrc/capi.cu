@@ -1152,10 +1152,12 @@ int b200nb_fit_disp_dev(const void* y, int y_type, const double* x, const double
   a.last_d2lp = out_last_d2lp; a.grid = nullptr; a.grid_n = 0;
   if (n == 0) return 0;
   if (check_device() || next_scratch(nb::disp_scratch_bytes(n), &a.scratch)) return 1;
-  if (use_generic(p) || long_rows(m, use_weights)) {
+  const bool smallp_fits = nb::fit_disp_smallp_fits(m, p, use_weights);
+  if (use_generic(p) || long_rows(m, use_weights) || !smallp_fits) {
     DesignDev dd;
     if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
-    if (use_generic(p) || dd.seg.pos != nullptr) {   // long rows: only designs the segmented kernels take
+    // long rows: only designs the segmented kernels take, unless the small-p kernels cannot hold the rows at all
+    if (use_generic(p) || dd.seg.pos != nullptr || !smallp_fits) {
       apply_design(dd, use_weights, &a);
       CU(nb::launch_fit_disp_generic(a, (cudaStream_t)stream));
       g_launches += 1;
@@ -1184,7 +1186,7 @@ int b200nb_fit_disp_grid_dev(const void* y, int y_type, const double* x, const d
   a.n = n; a.m = m; a.p = p; a.ld = ld; a.log_alpha = out_log_alpha; a.grid = disp_grid; a.grid_n = disp_grid_n;
   if (n == 0) return 0;
   if (check_device() || next_scratch(nb::disp_scratch_bytes(n), &a.scratch)) return 1;
-  if (use_generic(p)) {
+  if (use_generic(p) || !nb::fit_disp_smallp_fits(m, p, use_weights)) {
     DesignDev dd;
     if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
     apply_design(dd, use_weights, &a);
@@ -1219,11 +1221,12 @@ int b200nb_fit_beta_dev(const void* y, int y_type, const double* x, const double
   a.n = n; a.m = m; a.p = p; a.ld = ld; a.beta_out = out_beta_mat; a.beta_var = out_beta_var_mat; a.iter = out_iter;
   a.hat_diag = out_hat_diagonals; a.mu_out = out_mu; a.contrast_num = out_contrast_num;
   a.contrast_denom = out_contrast_denom; a.deviance = out_deviance; a.counter = ctr;
-  if (use_generic(p) || long_rows(m, use_weights)) {
+  const bool smallp_fits = nb::fit_beta_smallp_fits(m, p, use_weights, nf_is_vector);
+  if (use_generic(p) || long_rows(m, use_weights) || !smallp_fits) {
     if (n == 0) return 0;
     DesignDev dd;
     if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
-    if (use_generic(p) || dd.seg.pos != nullptr) {
+    if (use_generic(p) || dd.seg.pos != nullptr || !smallp_fits) {
       apply_design(dd, &a);
       CU(nb::launch_fit_beta_generic(a, (cudaStream_t)stream));
       g_launches++;

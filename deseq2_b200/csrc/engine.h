@@ -59,6 +59,7 @@ struct DispArgs {
   const int* gid;     // m
   int G, grouped;
   double* row_scratch;   // general-p path, long rows: per-warp global scratch for the sample rows (set by the launcher)
+  int rows_global;       // 0: rows in shared memory; 1: sample rows in row_scratch; 2: every array of length m global
   // saturated design (G == p, distinct rows X_g invertible): X'WX = X_g' diag(W_g) X_g, so
   // log det = 2 log|det X_g| + sum_g log W_g and tr(B^-1 dB) = sum_g dW_g / W_g -- no p x p algebra at all
   int saturated;
@@ -114,6 +115,7 @@ struct BetaArgs {
   const int* gid;
   int G, grouped;
   double* row_scratch;   // long rows: per-warp global scratch for the sample rows (set by the launcher)
+  int rows_global;       // as DispArgs::rows_global
   SegLayout seg;
 };
 
@@ -154,6 +156,7 @@ struct OptimArgs {
   double* beta_out;       // n x p column-major
   int32_t* converged;     // n: 1 = stationary point reached (optim's convergence == 0)
   int32_t* iter;          // n: Newton iterations used
+  double* row_scratch;    // set by the launcher: per-gene global rows when two rows of m do not fit in shared memory
 };
 cudaError_t launch_beta_optim(const OptimArgs& a, cudaStream_t stream);
 
@@ -190,6 +193,7 @@ struct PrepArgs {
   // gene-specific normalization factors (b200nb_prep_nf_dev; nullptr: size_factors): gene-major n x ld, read in place
   // of size_factors; xim is then mean(1 / colMeans(nf)) over the non-all-zero rows
   const double* nf;
+  double* row_scratch;         // set by the launcher: per-warp global rows when one warp's rows do not fit in shared memory
 };
 cudaError_t launch_prep(const PrepArgs& a, cudaStream_t stream);
 
@@ -369,6 +373,7 @@ struct CooksArgs {
   double* max_cooks;           // n
   double* robust_disp;         // n
   const double* nf;            // gene-major n x ld normalization factors, read in place of size_factors; or nullptr
+  double* row_scratch;         // set by the launcher: per-warp global rows when one warp's rows do not fit in shared memory
 };
 cudaError_t launch_cooks(const CooksArgs& a, cudaStream_t stream);
 cudaError_t launch_trend_fit(const double* means, const double* disps, int n, double min_disp, double* out4,
@@ -377,6 +382,13 @@ cudaError_t launch_trend_fit(const double* means, const double* disps, int n, do
 // returns cudaSuccess or the launch error; kernels are enqueued on `stream`
 cudaError_t launch_fit_disp(const DispArgs& a, cudaStream_t stream);
 cudaError_t launch_fit_beta(const BetaArgs& a, cudaStream_t stream);
+// Whether one warp of the small-p kernels above fits in shared memory (its sample rows are staged there in full).
+// When it does not, the entry points fit the gene on the general-p kernels, which move long rows to global memory.
+bool fit_disp_smallp_fits(int m, int p, int use_weights);
+// A grow-only device buffer of at least `bytes` from a ring of four (one per launch in flight on a stream): the global
+// rows of the kernels whose per-warp rows do not fit in shared memory (fit_generic.cu)
+cudaError_t row_scratch(size_t bytes, double** out);
+bool fit_beta_smallp_fits(int m, int p, int use_weights, int nf_is_vector);
 // any p <= kMaxP (shared-memory normal equations, grouped design); used for p > kMaxSmallP
 cudaError_t launch_fit_disp_generic(const DispArgs& a, cudaStream_t stream);
 cudaError_t launch_fit_beta_generic(const BetaArgs& a, cudaStream_t stream);

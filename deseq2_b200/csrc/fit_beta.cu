@@ -336,16 +336,31 @@ cudaError_t launch_beta_grp(const BetaArgs& a, int mpad, size_t fixed, size_t ro
   return cudaGetLastError();
 }
 
+// shared memory of the small-p IRLS kernels: the staged design and the log size-factor row (P + 1 rows of mpad) once
+// per CTA, and per warp (or lane group) the y and mu rows, the log nf row of an nf matrix and the weights
+struct BetaSmem {
+  int mpad;
+  size_t fixed, rowbytes;
+};
+BetaSmem beta_smem(int m, int p, bool use_w, bool nf_is_vector) {
+  const int mpad = (m + 3) & ~3;
+  const int nrow = 2 + (nf_is_vector ? 0 : 1) + (use_w ? 1 : 0);
+  return {mpad, (size_t)(p + 1) * mpad * sizeof(double), (size_t)nrow * mpad * sizeof(double)};
+}
+constexpr size_t kBetaSmemCap = 227 * 1024;
+// a one-warp plan must also leave room for the kernels' static shared memory, which counts against the same 227 KB per
+// block: the log and log y! tables, 5152 bytes (ptxas -v)
+constexpr size_t kBetaSmemCapOneWarp = kBetaSmemCap - 5152;
+
 template <int P, bool USE_W>
 cudaError_t launch_beta_t(const BetaArgs& a, cudaStream_t stream) {
-  const int mpad = (a.m + 3) & ~3;
-  const int nrow = 2 + (a.nf_is_vector ? 0 : 1) + (USE_W ? 1 : 0);
-  const size_t fixed = (size_t)(P + 1) * mpad * sizeof(double);
-  const size_t rowbytes = (size_t)nrow * mpad * sizeof(double);
-  const size_t smem_cap = 227 * 1024;
+  const BetaSmem S = beta_smem(a.m, P, USE_W, a.nf_is_vector != 0);
+  const int mpad = S.mpad;
+  const size_t fixed = S.fixed, rowbytes = S.rowbytes;
+  const size_t smem_cap = kBetaSmemCap;
   int warps = NB_LB_THREADS / 32;
   while (warps > 1 && fixed + warps * rowbytes > smem_cap / 2) warps >>= 1;
-  if (fixed + warps * rowbytes > smem_cap) return cudaErrorInvalidValue;
+  if (fixed + warps * rowbytes > kBetaSmemCapOneWarp) return cudaErrorInvalidValue;   // callers check fit_beta_smallp_fits
   const size_t smem = fixed + warps * rowbytes;
   auto kern = fit_beta_kernel<P, USE_W>;
   cudaError_t e = cudaMemsetAsync(a.counter, 0, sizeof(unsigned int), stream);
@@ -426,6 +441,11 @@ cudaError_t launch_nb_loglik(const LogLikArgs& a, cudaStream_t stream) {
   if (a.n == 0) return cudaSuccess;
   nb_loglik_kernel<<<(a.n + 7) / 8, 256, 0, stream>>>(a);
   return cudaGetLastError();
+}
+
+bool fit_beta_smallp_fits(int m, int p, int use_weights, int nf_is_vector) {
+  const BetaSmem S = beta_smem(m, p, use_weights != 0, nf_is_vector != 0);
+  return S.fixed + S.rowbytes <= kBetaSmemCapOneWarp;
 }
 
 cudaError_t launch_fit_beta(const BetaArgs& a, cudaStream_t stream) {

@@ -550,17 +550,32 @@ cudaError_t launch_disp_grp(const DispArgs& a, int mpad, size_t xbytes, size_t r
   return cudaGetLastError();
 }
 
+// shared memory of the small-p kernels: the staged design (P rows of mpad) once per CTA, and per warp (or lane group)
+// the NROW sample rows and the factor table
+struct DispSmem {
+  int mpad;
+  size_t xbytes, rowbytes;
+};
+DispSmem disp_smem(int m, int p, bool use_w) {
+  const int mpad = (m + 3) & ~3;
+  const int nrow = use_w ? 3 : 2;
+  return {mpad, (size_t)p * mpad * sizeof(double), ((size_t)nrow * mpad + kTabMax) * sizeof(double)};
+}
+constexpr size_t kDispSmemCap = 227 * 1024;
+// a one-warp plan must also leave room for the kernels' static shared memory, which counts against the same 227 KB per
+// block: the log tables, 3104 bytes (ptxas -v)
+constexpr size_t kDispSmemCapOneWarp = kDispSmemCap - 3104;
+
 template <int P, bool USE_W>
 cudaError_t launch_disp_t(const DispArgs& a0, cudaStream_t stream) {
   DispArgs a = a0;
-  const int mpad = (a.m + 3) & ~3;
-  constexpr int NROW = USE_W ? 3 : 2;
-  const size_t xbytes = (size_t)P * mpad * sizeof(double);
-  const size_t rowbytes = ((size_t)NROW * mpad + kTabMax) * sizeof(double);
-  const size_t smem_cap = 227 * 1024;
+  const DispSmem L = disp_smem(a.m, P, USE_W);
+  const int mpad = L.mpad;
+  const size_t xbytes = L.xbytes, rowbytes = L.rowbytes;
+  const size_t smem_cap = kDispSmemCap;
   int warps = NB_LB_THREADS / 32;
   while (warps > 1 && xbytes + warps * rowbytes > smem_cap / 2) warps >>= 1;   // aim for >= 2 CTAs/SM
-  if (xbytes + warps * rowbytes > smem_cap) return cudaErrorInvalidValue;
+  if (xbytes + warps * rowbytes > kDispSmemCapOneWarp) return cudaErrorInvalidValue;   // callers check fit_disp_smallp_fits
   const size_t smem = xbytes + warps * rowbytes;
   // scratch: [queue counter | 3 mode counters | 3 n gene lists]
   cudaError_t e = cudaMemsetAsync(a.scratch, 0, kDispScratchHead * sizeof(unsigned int), stream);
@@ -618,6 +633,11 @@ cudaError_t launch_disp_p(const DispArgs& a, cudaStream_t stream) {
 }
 
 }  // namespace
+
+bool fit_disp_smallp_fits(int m, int p, int use_weights) {
+  const DispSmem L = disp_smem(m, p, use_weights != 0);
+  return L.xbytes + L.rowbytes <= kDispSmemCapOneWarp;
+}
 
 cudaError_t launch_fit_disp(const DispArgs& a, cudaStream_t stream) {
   if (a.n == 0) return cudaSuccess;

@@ -142,15 +142,25 @@ struct GenWarp {
 // factor table (optional); `nacc` accumulator sets (3 for the dispersion kernel, 2 for IRLS).
 struct GenShape {
   int has_r1, has_r2, use_w, has_tab, nacc;
-  int rows_global;   // the sample rows live in a per-warp slice of a GLOBAL scratch buffer (L2-resident), not in shared memory
+  // 0: everything in shared memory.  1: the sample rows live in a per-warp slice of a GLOBAL scratch buffer
+  // (L2-resident).  2: so do the samplewise accumulators and quad forms, and the kernel reads the design rows and the
+  // row ids from global memory: no array of length m is left in shared memory, so any m fits.
+  int rows_global;
 };
 __host__ __device__ inline int gen_rows(GenShape sh) { return 1 + sh.has_r1 + sh.has_r2 + sh.use_w; }
+// the samplewise per-sample sums and quad forms are global (rows_global == 2)
+__host__ __device__ inline bool gen_acc_global(int grouped, GenShape sh) { return sh.rows_global == 2 && !grouped; }
 __host__ __device__ inline size_t gen_warp_doubles(int mpad, int p, int ps, int G, int grouped, GenShape sh) {
   const size_t terms = grouped ? (size_t)G : (size_t)mpad;
   const size_t acc = grouped ? (size_t)G * 32 : (size_t)mpad;
   const size_t rows = sh.rows_global ? 0 : (size_t)gen_rows(sh);
-  return rows * mpad + (sh.has_tab ? kTabMaxG : 0) + sh.nacc * acc + (grouped ? sh.nacc * terms : 0) + terms +
-         4 * (size_t)p * ps + 4 * 32;
+  const size_t sums = gen_acc_global(grouped, sh) ? 0 : sh.nacc * acc + (grouped ? sh.nacc * terms : 0) + terms;
+  return rows * mpad + (sh.has_tab ? kTabMaxG : 0) + sums + 4 * (size_t)p * ps + 4 * 32;
+}
+// a warp's slice of the global scratch: its sample rows, then (rows_global == 2, samplewise) the nacc sums and q
+__host__ __device__ inline size_t gen_global_doubles(int mpad, int grouped, GenShape sh) {
+  if (!sh.rows_global) return 0;
+  return ((size_t)gen_rows(sh) + (gen_acc_global(grouped, sh) ? sh.nacc + 1 : 0)) * mpad;
 }
 
 // `rowbase`: the warp's slice of the global row scratch when sh.rows_global, else ignored (rows come first in `base`)
@@ -167,17 +177,20 @@ __device__ __forceinline__ GenWarp carve(double* base, double* rowbase, int mpad
   S.wsm = sh.use_w ? rq : nullptr; rq += sh.use_w ? mpad : 0;
   if (!sh.rows_global) q = rq;
   S.tab = sh.has_tab ? q : nullptr; q += sh.has_tab ? kTabMaxG : 0;
-  S.accA = q; q += acc;
-  S.accB = q; q += acc;
-  S.accC = (sh.nacc > 2) ? q : nullptr; q += (sh.nacc > 2) ? acc : 0;
+  const bool acc_global = gen_acc_global(grouped, sh);
+  double* t = acc_global ? rq : q;   // the sums and quad forms: in shared memory after the table, or after the rows
+  S.accA = t; t += acc;
+  S.accB = t; t += acc;
+  S.accC = (sh.nacc > 2) ? t : nullptr; t += (sh.nacc > 2) ? acc : 0;
   if (grouped) {
-    S.WA = q; q += terms;
-    S.WB = q; q += terms;
-    S.WC = (sh.nacc > 2) ? q : nullptr; q += (sh.nacc > 2) ? terms : 0;
+    S.WA = t; t += terms;
+    S.WB = t; t += terms;
+    S.WC = (sh.nacc > 2) ? t : nullptr; t += (sh.nacc > 2) ? terms : 0;
   } else {
     S.WA = S.accA; S.WB = S.accB; S.WC = S.accC;
   }
-  S.q = q; q += terms;
+  S.q = t; t += terms;
+  if (!acc_global) q = t;
   S.M0 = q; q += (size_t)p * ps;
   S.M1 = q; q += (size_t)p * ps;
   S.M2 = q; q += (size_t)p * ps;
@@ -446,19 +459,22 @@ __global__ void __launch_bounds__(256, 1) fit_disp_generic_kernel(const DispArgs
   init_log_table();
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
-  const int xrows = A.grouped ? A.G : A.m;
+  // rows_global == 2: the samplewise design and the row ids stay in global memory
+  const bool all_global = A.rows_global == 2;
+  const int xrows = A.grouped ? A.G : (all_global ? 0 : A.m);
+  const int gids = all_global ? 0 : A.m;
   double* xg = smem;                                         // xrows * ps
-  int* gid = reinterpret_cast<int*>(xg + (size_t)xrows * ps);  // m ints (padded to doubles)
-  double* wbase = xg + (size_t)xrows * ps + (A.m + 1) / 2 + (size_t)warp * warp_doubles;
+  int* gid = reinterpret_cast<int*>(xg + (size_t)xrows * ps);  // gids ints (padded to doubles)
+  double* wbase = xg + (size_t)xrows * ps + (gids + 1) / 2 + (size_t)warp * warp_doubles;
   for (int i = threadIdx.x; i < xrows * ps; i += blockDim.x) xg[i] = A.xg[i];
-  for (int i = threadIdx.x; i < A.m; i += blockDim.x) gid[i] = A.gid[i];
+  for (int i = threadIdx.x; i < gids; i += blockDim.x) gid[i] = A.gid[i];
   __syncthreads();
   GDispCtx C;
-  C.D = Design{xg, gid, A.p, ps, A.G, A.grouped, A.m};
-  const GenShape shp{1, 0, A.use_weights != 0, 1, 3, A.row_scratch != nullptr};
+  C.D = Design{xrows ? xg : A.xg, gids ? gid : A.gid, A.p, ps, A.G, A.grouped, A.m};
+  const GenShape shp{1, 0, A.use_weights != 0, 1, 3, A.rows_global};
   const size_t gwarp = (size_t)blockIdx.x * (blockDim.x >> 5) + warp;
-  C.S = carve(wbase, A.row_scratch ? A.row_scratch + gwarp * gen_rows(shp) * mpad : nullptr, mpad, A.p, ps, A.G, A.grouped,
-              shp);
+  C.S = carve(wbase, A.row_scratch ? A.row_scratch + gwarp * gen_global_doubles(mpad, A.grouped, shp) : nullptr, mpad, A.p,
+              ps, A.G, A.grouped, shp);
   C.prior_sigmasq = A.prior_sigmasq;
   C.inv_sigmasq = 1.0 / A.prior_sigmasq;
   C.weight_threshold = A.weight_threshold;
@@ -595,16 +611,21 @@ __global__ void __launch_bounds__(256, 1) fit_beta_generic_kernel(const BetaArgs
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int p = A.p;
-  const int xrows = A.grouped ? A.G : A.m;
+  // rows_global == 2: the samplewise design and the row ids stay in global memory, and each warp keeps the log size
+  // factors in its own global row, as it does for an nf matrix
+  const bool all_global = A.rows_global == 2;
+  const int xrows = A.grouped ? A.G : (all_global ? 0 : A.m);
+  const int gids = all_global ? 0 : A.m;
+  const bool lnf_in_smem = A.nf_is_vector && !all_global;
   double* xg = smem;
   int* gid = reinterpret_cast<int*>(xg + (size_t)xrows * ps);
-  double* lnf_shared = xg + (size_t)xrows * ps + (A.m + 1) / 2;     // mpad
-  double* lam = lnf_shared + mpad;                                  // 32
+  double* lnf_shared = xg + (size_t)xrows * ps + (gids + 1) / 2;    // mpad (unused when the log nf are per warp)
+  double* lam = lnf_shared + (all_global ? 0 : mpad);               // 32
   double* contrast = lam + 32;                                      // 32
   double* wbase = contrast + 32 + (size_t)warp * warp_doubles;
   for (int i = threadIdx.x; i < xrows * ps; i += blockDim.x) xg[i] = A.xg[i];
-  for (int i = threadIdx.x; i < A.m; i += blockDim.x) gid[i] = A.gid[i];
-  if (A.nf_is_vector)
+  for (int i = threadIdx.x; i < gids; i += blockDim.x) gid[i] = A.gid[i];
+  if (lnf_in_smem)
     for (int j = threadIdx.x; j < A.m; j += blockDim.x) lnf_shared[j] = log(A.nf[j]);
   for (int k = threadIdx.x; k < p; k += blockDim.x) {
     lam[k] = A.lambda[k];
@@ -612,15 +633,15 @@ __global__ void __launch_bounds__(256, 1) fit_beta_generic_kernel(const BetaArgs
   }
   __syncthreads();
   GBetaCtx C;
-  C.D = Design{xg, gid, p, ps, A.G, A.grouped, A.m};
-  const GenShape shp{A.nf_is_vector ? 0 : 1, 1, A.use_weights != 0, 0, 2, A.row_scratch != nullptr};
+  C.D = Design{xrows ? xg : A.xg, gids ? gid : A.gid, p, ps, A.G, A.grouped, A.m};
+  const GenShape shp{lnf_in_smem ? 0 : 1, 1, A.use_weights != 0, 0, 2, A.rows_global};
   const size_t gwarp = (size_t)blockIdx.x * (blockDim.x >> 5) + warp;
-  C.S = carve(wbase, A.row_scratch ? A.row_scratch + gwarp * gen_rows(shp) * mpad : nullptr, mpad, p, ps, A.G, A.grouped,
-              shp);
+  C.S = carve(wbase, A.row_scratch ? A.row_scratch + gwarp * gen_global_doubles(mpad, A.grouped, shp) : nullptr, mpad, p,
+              ps, A.G, A.grouped, shp);
   C.use_w = A.use_weights;
   C.minmu = A.minmu;
   C.log_minmu = log(A.minmu);
-  C.lnf = A.nf_is_vector ? lnf_shared : C.S.r1;
+  C.lnf = lnf_in_smem ? lnf_shared : C.S.r1;
   const GenWarp& S = C.S;
   double* B = S.M0;      // X'WX
   double* L = S.M1;      // equilibrated, factored X'WX + Lambda
@@ -642,7 +663,7 @@ __global__ void __launch_bounds__(256, 1) fit_beta_generic_kernel(const BetaArgs
       if (j < A.m)
         y = A.y_is_f64 ? static_cast<const double*>(A.y)[off + j] : (double)static_cast<const int32_t*>(A.y)[off + j];
       S.ys[j] = y;
-      if (!A.nf_is_vector) S.r1[j] = (j < A.m) ? log(A.nf[off + j]) : 0.0;
+      if (!lnf_in_smem) S.r1[j] = (j < A.m) ? log(A.nf_is_vector ? A.nf[j] : A.nf[off + j]) : 0.0;
       if (A.use_weights) S.wsm[j] = (j < A.m) ? A.w[off + j] : 0.0;
     }
     if (lane < p) beta[lane] = A.beta_in[(size_t)g + (size_t)A.n * lane];
@@ -727,7 +748,7 @@ __global__ void __launch_bounds__(256, 1) fit_beta_generic_kernel(const BetaArgs
         if (A.hat_diag != nullptr) {
           double w = mu * rcp_fast(fma(alpha, mu, 1.0));
           if (A.use_weights) w *= S.wsm[j];
-          A.hat_diag[off + j] = w * S.q[C.D.grouped ? gid[j] : j];
+          A.hat_diag[off + j] = w * S.q[C.D.grouped ? C.D.gid[j] : j];
         }
       }
     }
@@ -775,18 +796,24 @@ struct GenLaunch {
   int rows_global;
 };
 
-bool plan_one(int m, int p, int G, int grouped, GenShape sh, size_t extra_doubles, GenLaunch& out) {
+// extra_doubles: the kernel's own part of the CTA's shared memory; extra_row: the part of it that has length m, which
+// rows_global == 2 moves out of shared memory
+bool plan_one(int m, int p, int G, int grouped, GenShape sh, size_t extra_doubles, size_t extra_row, GenLaunch& out) {
   out.mpad = (m + 3) & ~3;
   out.ps = p | 1;
   out.rows_global = sh.rows_global;
   out.warp_doubles = gen_warp_doubles(out.mpad, p, out.ps, G, grouped, sh);
-  const size_t fixed = ((size_t)(grouped ? G : m) * out.ps + (m + 1) / 2 + extra_doubles) * sizeof(double);
-  const size_t cap = 227 * 1024;
+  const size_t fixed =
+      sh.rows_global == 2 ? ((size_t)(grouped ? G : 0) * out.ps + extra_doubles) * sizeof(double)
+                          : ((size_t)(grouped ? G : m) * out.ps + (m + 1) / 2 + extra_doubles + extra_row) * sizeof(double);
+  // the kernels' static shared memory (the log tables, 3104 bytes per ptxas -v) counts against the 227 KB per block
+  const size_t cap = 227 * 1024 - 3104;
   int warps = 8;
   while (warps > 1 && fixed + warps * out.warp_doubles * sizeof(double) > cap) warps--;
-  // several CTAs per SM need room for each: prefer 8-warp CTAs that fit at least twice
-  while (warps > 4 && 2 * (fixed + warps * out.warp_doubles * sizeof(double)) > cap &&
-         fixed + (warps - 1) * out.warp_doubles * sizeof(double) <= cap / 2)
+  // several CTAs per SM need room for each: prefer 8-warp CTAs that fit at least twice (227 KB per SM)
+  const size_t sm_cap = 227 * 1024;
+  while (warps > 4 && 2 * (fixed + warps * out.warp_doubles * sizeof(double)) > sm_cap &&
+         fixed + (warps - 1) * out.warp_doubles * sizeof(double) <= sm_cap / 2)
     warps--;
   out.warps = warps;
   out.smem = fixed + warps * out.warp_doubles * sizeof(double);
@@ -795,43 +822,21 @@ bool plan_one(int m, int p, int G, int grouped, GenShape sh, size_t extra_double
 
 // Rows in shared memory whenever they fit.  Config 4 (m = 1000, two rows = 16 KB per warp) leaves 7 warps per SM; moving
 // the rows to a per-warp slice of an L2-resident global scratch buffer (rows_global) doubles the resident warps, but
-// the per-pass row reads turn from shared-memory into L2 latency and the kernel is not occupancy-bound.  The global path remains for rows that do not fit in shared memory at all (m > ~6000) and as the
-// A/B switch B200NB_GENERIC_ROWS=global.
-bool plan(int m, int p, int G, int grouped, GenShape sh, size_t extra_doubles, GenLaunch& out) {
+// the per-pass row reads turn from shared-memory into L2 latency and the kernel is not occupancy-bound.  The global
+// rows remain for rows that do not fit in shared memory (and as the A/B switch B200NB_GENERIC_ROWS=global); when even
+// one warp's m-long sums, the samplewise design or the row ids do not fit beside them, rows_global == 2 moves those
+// too, so that every m has a plan.
+bool plan(int m, int p, int G, int grouped, GenShape sh, size_t extra_doubles, size_t extra_row, GenLaunch& out) {
   const char* force = getenv("B200NB_GENERIC_ROWS");   // "smem" | "global": A/B switch
   if (force && (force[0] == 's' || force[0] == 'g')) {
     sh.rows_global = force[0] == 'g';
-    if (plan_one(m, p, G, grouped, sh, extra_doubles, out)) return true;
+    if (plan_one(m, p, G, grouped, sh, extra_doubles, extra_row, out)) return true;
   }
-  sh.rows_global = 0;
-  if (plan_one(m, p, G, grouped, sh, extra_doubles, out)) return true;
-  sh.rows_global = 1;
-  return plan_one(m, p, G, grouped, sh, extra_doubles, out);
-}
-
-// global row scratch: a small ring of grow-only device buffers (one per launch in flight)
-constexpr int kRowRing = 4;
-void* g_rowbuf[kRowRing] = {};
-size_t g_rowcap[kRowRing] = {};
-unsigned int g_rownext = 0;
-std::mutex g_rowmu;
-cudaError_t row_scratch(size_t bytes, double** out) {
-  std::lock_guard<std::mutex> lk(g_rowmu);
-  const int s = (int)(g_rownext++ % kRowRing);
-  if (g_rowcap[s] < bytes) {
-    if (g_rowbuf[s]) {
-      cudaError_t e = cudaDeviceSynchronize();
-      if (e != cudaSuccess) return e;
-      cudaFree(g_rowbuf[s]);
-      g_rowbuf[s] = nullptr;
-      g_rowcap[s] = 0;
-    }
-    cudaError_t e = cudaMalloc(&g_rowbuf[s], bytes + bytes / 8);
-    if (e != cudaSuccess) return e;
-    g_rowcap[s] = bytes + bytes / 8;
+  for (int level = 0; level <= 2; level++) {
+    sh.rows_global = level;
+    if (plan_one(m, p, G, grouped, sh, extra_doubles, extra_row, out)) return true;
   }
-  *out = static_cast<double*>(g_rowbuf[s]);
-  return cudaSuccess;
+  return false;
 }
 
 // ---- segmented kernels: launch plan.  One CTA per SM of up to 16 warps; the kernels are compiled for 256 / 384 / 512
@@ -879,6 +884,33 @@ cudaError_t launch_beta_seg_t(const BetaArgs& a, const SegPlan& P, cudaStream_t 
 
 }  // namespace
 
+// global row scratch: a small ring of grow-only device buffers (one per launch in flight)
+namespace {
+constexpr int kRowRing = 4;
+void* g_rowbuf[kRowRing] = {};
+size_t g_rowcap[kRowRing] = {};
+unsigned int g_rownext = 0;
+std::mutex g_rowmu;
+}  // namespace
+cudaError_t row_scratch(size_t bytes, double** out) {
+  std::lock_guard<std::mutex> lk(g_rowmu);
+  const int s = (int)(g_rownext++ % kRowRing);
+  if (g_rowcap[s] < bytes) {
+    if (g_rowbuf[s]) {
+      cudaError_t e = cudaDeviceSynchronize();
+      if (e != cudaSuccess) return e;
+      cudaFree(g_rowbuf[s]);
+      g_rowbuf[s] = nullptr;
+      g_rowcap[s] = 0;
+    }
+    cudaError_t e = cudaMalloc(&g_rowbuf[s], bytes + bytes / 8);
+    if (e != cudaSuccess) return e;
+    g_rowcap[s] = bytes + bytes / 8;
+  }
+  *out = static_cast<double*>(g_rowbuf[s]);
+  return cudaSuccess;
+}
+
 cudaError_t launch_fit_disp_generic(const DispArgs& a0, cudaStream_t stream) {
   DispArgs a = a0;
   if (a.grouped && !a.use_weights && a.grid == nullptr && seg_enabled(a.seg)) {
@@ -898,14 +930,15 @@ cudaError_t launch_fit_disp_generic(const DispArgs& a0, cudaStream_t stream) {
     }
   }
   GenLaunch L;
-  const GenShape sh{1, 0, a.use_weights != 0, 1, 3, 0};
-  if (!plan(a.m, a.p, a.G, a.grouped, sh, 0, L)) return cudaErrorInvalidValue;
+  GenShape sh{1, 0, a.use_weights != 0, 1, 3, 0};
+  if (!plan(a.m, a.p, a.G, a.grouped, sh, 0, 0, L)) return cudaErrorInvalidValue;
   unsigned grid = 0;
   cudaError_t e = persistent_grid(reinterpret_cast<const void*>(fit_disp_generic_kernel), L.warps * 32, L.smem, L.warps, a.n, &grid);
   if (e != cudaSuccess) return e;
   a.row_scratch = nullptr;
+  a.rows_global = sh.rows_global = L.rows_global;
   if (L.rows_global) {
-    e = row_scratch((size_t)grid * L.warps * gen_rows(sh) * L.mpad * sizeof(double), &a.row_scratch);
+    e = row_scratch((size_t)grid * L.warps * gen_global_doubles(L.mpad, a.grouped, sh) * sizeof(double), &a.row_scratch);
     if (e != cudaSuccess) return e;
   }
   e = cudaMemsetAsync(a.scratch, 0, 4 * sizeof(unsigned int), stream);
@@ -934,14 +967,16 @@ cudaError_t launch_fit_beta_generic(const BetaArgs& a0, cudaStream_t stream) {
   }
   GenLaunch L;
   const int mpad = (a.m + 3) & ~3;
-  const GenShape sh{a.nf_is_vector ? 0 : 1, 1, a.use_weights != 0, 0, 2, 0};
-  if (!plan(a.m, a.p, a.G, a.grouped, sh, (size_t)mpad + 64, L)) return cudaErrorInvalidValue;
+  GenShape sh{a.nf_is_vector ? 0 : 1, 1, a.use_weights != 0, 0, 2, 0};
+  if (!plan(a.m, a.p, a.G, a.grouped, sh, 64, (size_t)mpad, L)) return cudaErrorInvalidValue;
   unsigned grid = 0;
   cudaError_t e = persistent_grid(reinterpret_cast<const void*>(fit_beta_generic_kernel), L.warps * 32, L.smem, L.warps, a.n, &grid);
   if (e != cudaSuccess) return e;
   a.row_scratch = nullptr;
+  a.rows_global = sh.rows_global = L.rows_global;
+  if (L.rows_global == 2) sh.has_r1 = 1;   // the log size factors move to a per-warp row with the other m-long arrays
   if (L.rows_global) {
-    e = row_scratch((size_t)grid * L.warps * gen_rows(sh) * L.mpad * sizeof(double), &a.row_scratch);
+    e = row_scratch((size_t)grid * L.warps * gen_global_doubles(L.mpad, a.grouped, sh) * sizeof(double), &a.row_scratch);
     if (e != cudaSuccess) return e;
   }
   e = cudaMemsetAsync(a.counter, 0, sizeof(unsigned int), stream);

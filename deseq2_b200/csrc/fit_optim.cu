@@ -53,18 +53,20 @@ __device__ double objective(const OptimArgs& A, size_t off, int lane, double alp
 __global__ void __launch_bounds__(32) beta_optim_kernel(const OptimArgs A) {
   extern __shared__ __align__(16) double sm[];
   const int lane = threadIdx.x;
-  const int g = blockIdx.x;
-  if (g >= A.n) return;
   const int p = A.p, mpad = (A.m + 3) & ~3;
-  double* ge = sm;                   // mpad: d f / d eta_j
+  // A.row_scratch: the two rows of length m live in the CTA's slice of a global buffer, the rest in shared memory
+  double* ge = A.row_scratch ? A.row_scratch + (size_t)blockIdx.x * 2 * mpad : sm;   // mpad: d f / d eta_j
   double* he = ge + mpad;            // mpad: -d2 f / d eta_j^2  (> 0)
-  double* H = he + mpad;             // p x p: -Hessian (positive definite) of the reduced problem
+  double* H = A.row_scratch ? sm : he + mpad;   // p x p: -Hessian (positive definite) of the reduced problem
   double* grad = H + (size_t)p * p;  // p
   double* beta = grad + p;           // p
   double* trial = beta + p;          // p
   double* step = trial + p;          // p
   double* Lm = step + p;             // p x p: Cholesky factor
   int* active = reinterpret_cast<int*>(Lm + (size_t)p * p);   // p
+  // genes strided over the grid: one per CTA when the grid covers every gene (shared-memory rows)
+  for (int g = blockIdx.x; g < A.n; g += gridDim.x) {
+  __syncwarp();
   const size_t off = (size_t)g * A.ld;
   const double alpha = A.alpha[g], r = 1.0 / alpha;
   const double U = A.bound;
@@ -204,6 +206,7 @@ __global__ void __launch_bounds__(32) beta_optim_kernel(const OptimArgs A) {
     A.converged[g] = converged;
     A.iter[g] = it;
   }
+  }
 }
 
 }  // namespace
@@ -211,11 +214,21 @@ __global__ void __launch_bounds__(32) beta_optim_kernel(const OptimArgs A) {
 cudaError_t launch_beta_optim(const OptimArgs& a, cudaStream_t stream) {
   if (a.n == 0) return cudaSuccess;
   const int mpad = (a.m + 3) & ~3;
-  const size_t smem = ((size_t)2 * mpad + 2 * (size_t)a.p * a.p + 5 * (size_t)a.p + 2) * sizeof(double);
-  if (smem > 200 * 1024) return cudaErrorInvalidValue;
+  size_t smem = ((size_t)2 * mpad + 2 * (size_t)a.p * a.p + 5 * (size_t)a.p + 2) * sizeof(double);
+  OptimArgs b = a;
+  b.row_scratch = nullptr;
+  unsigned grid = (unsigned)a.n;
+  if (smem > 200 * 1024) {
+    // the two rows do not fit: they go to a global buffer, one slice per CTA, genes strided over at most 8 CTAs per SM
+    smem -= (size_t)2 * mpad * sizeof(double);
+    const unsigned cap = 8u * (unsigned)device_sm_count();
+    if (grid > cap) grid = cap;
+    cudaError_t e = row_scratch((size_t)grid * 2 * mpad * sizeof(double), &b.row_scratch);
+    if (e != cudaSuccess) return e;
+  }
   cudaError_t e = cudaFuncSetAttribute(beta_optim_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  beta_optim_kernel<<<a.n, 32, smem, stream>>>(a);
+  beta_optim_kernel<<<grid, 32, smem, stream>>>(b);
   return cudaGetLastError();
 }
 

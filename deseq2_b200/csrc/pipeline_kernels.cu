@@ -80,6 +80,12 @@ __device__ __forceinline__ void store_weight_flags(const PrepArgs& A, int g, boo
   if (invalid) atomicAdd(A.status, 1);
 }
 
+// per-warp shared-memory doubles of prep_kernel with global rows: the two coefficient vectors, the Gram matrices (W)
+template <bool W>
+__host__ __device__ __forceinline__ size_t prep_global_warp_doubles(int mpad, int p) {
+  return 64 + (W ? prep_weighted_extra<W>(mpad, p, false) - mpad : 0);
+}
+
 template <bool W, bool NF>
 __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
   static_assert(!(W && NF), "observation weights together with normalization factors are not supported");
@@ -87,19 +93,26 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int mpad = (A.m + 3) & ~3;
-  double* sf = smem;                                   // mpad
-  double* wrow = smem + mpad + (size_t)warp * (2 * mpad + 64 + prep_weighted_extra<W>(mpad, A.p, false));
-  double* vn = wrow;                                   // normalised counts
-  double* vl = wrow + mpad;                            // log(norm + 0.1)
-  double* coef = wrow + 2 * mpad;                      // 32: P * norm
+  // A.row_scratch: the rows of length m (size factors, normalised counts, their logs, the weights) are read from and
+  // kept in global memory, 3 rows per warp; shared memory holds only the coefficients and the Gram matrices
+  const bool rows_global = A.row_scratch != nullptr;
+  double* sf = rows_global ? const_cast<double*>(A.size_factors) : smem;                  // mpad
+  double* wrow = rows_global ? smem + (size_t)warp * prep_global_warp_doubles<W>(mpad, A.p)
+                             : smem + mpad + (size_t)warp * (2 * mpad + 64 + prep_weighted_extra<W>(mpad, A.p, false));
+  double* grow = rows_global ? A.row_scratch + ((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * 3 * mpad : wrow;
+  double* vn = grow;                                   // normalised counts
+  double* vl = grow + mpad;                            // log(norm + 0.1)
+  double* coef = rows_global ? wrow : wrow + 2 * mpad; // 32: P * norm
   double* coefl = coef + 32;                           // 32: P * log(norm + .1)
-  double* wn = coefl + 32;                             // W: mpad, the weights (raw, then normalised)
-  double* gram = wn + mpad;                            // W: 2 p x p Gram matrices
+  double* wn = rows_global ? grow + 2 * mpad : coefl + 32;   // W: mpad, the weights (raw, then normalised)
+  double* gram = rows_global ? coefl + 32 : wn + mpad;      // W: 2 p x p Gram matrices
   if constexpr (!NF)
-    for (int j = threadIdx.x; j < A.m; j += blockDim.x) sf[j] = A.size_factors[j];
+    if (!rows_global)
+      for (int j = threadIdx.x; j < A.m; j += blockDim.x) sf[j] = A.size_factors[j];
   __syncthreads();
-  const int g = blockIdx.x * (blockDim.x >> 5) + warp;
-  if (g >= A.n) return;
+  // genes strided over the grid: one pass when the grid covers every gene (shared-memory rows), several with global rows
+  for (int g = blockIdx.x * (blockDim.x >> 5) + warp; g < A.n; g += gridDim.x * (blockDim.x >> 5)) {
+  __syncwarp();
   const size_t off = (size_t)g * A.ld;
   double s = 0.0, s2 = 0.0, raw = 0.0;
   double wmax = 0.0;
@@ -211,6 +224,7 @@ __global__ void __launch_bounds__(256) prep_kernel(const PrepArgs A) {
     A.alpha0[g] = a0;
     A.all_zero[g] = (raw == 0.0) ? 1 : 0;
     if constexpr (W) store_weight_flags(A, g, invalid, ok);
+  }
   }
 }
 
@@ -571,10 +585,24 @@ cudaError_t launch_prep(const PrepArgs& a, cudaStream_t stream) {
     warps >>= 1;
     smem = ((size_t)mpad + (size_t)warps * per_warp) * sizeof(double);
   }
+  PrepArgs b = a;
+  b.row_scratch = nullptr;
+  unsigned grid = (unsigned)((a.n + warps - 1) / warps);
+  if (smem > 200 * 1024) {
+    // one warp's rows do not fit: 8-warp CTAs, one per SM, genes strided over them, the rows of length m in global
+    // memory (3 rows per warp)
+    warps = 8;
+    smem = (size_t)warps * (weighted ? prep_global_warp_doubles<true>(mpad, a.p) : prep_global_warp_doubles<false>(mpad, a.p)) *
+           sizeof(double);
+    grid = (unsigned)((a.n + warps - 1) / warps);
+    if (grid > (unsigned)device_sm_count()) grid = (unsigned)device_sm_count();
+    cudaError_t e = row_scratch((size_t)grid * warps * 3 * mpad * sizeof(double), &b.row_scratch);
+    if (e != cudaSuccess) return e;
+  }
   const auto kern = weighted ? prep_kernel<true, false> : (nf ? prep_kernel<false, true> : prep_kernel<false, false>);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  kern<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a);
+  kern<<<grid, warps * 32, smem, stream>>>(b);
   return cudaGetLastError();
 }
 
@@ -731,23 +759,34 @@ __global__ void __launch_bounds__(256) cooks_kernel(const CooksArgs A) {
   const int warp = threadIdx.x >> 5;
   const int mpad = (A.m + 3) & ~3;
   const int sqlen = cooks_sqlen(A.m, mpad, A.max_cell);
-  int* cell_ptr = reinterpret_cast<int*>(smem);                 // ncell + 1
-  int* cell_samples = cell_ptr + A.ncell + 1;                   // m
-  double* sf = smem + ((A.ncell + 1 + A.m + 1) / 2 + 1);        // mpad
-  double* wbase = sf + mpad + (size_t)warp * cooks_warp_doubles(A.m, mpad, A.max_cell);
+  // A.row_scratch: nothing of length m in shared memory; the cell lists and size factors are read from global memory
+  // and each warp keeps its rows in its slice of the global scratch
+  const bool rows_global = A.row_scratch != nullptr;
+  const int* cell_ptr = rows_global ? A.cell_ptr : reinterpret_cast<int*>(smem);             // ncell + 1
+  const int* cell_samples = rows_global ? A.cell_samples : cell_ptr + A.ncell + 1;            // m
+  const double* sf = rows_global ? A.size_factors : smem + ((A.ncell + 1 + A.m + 1) / 2 + 1); // mpad
+  double* wbase = rows_global ? A.row_scratch + ((size_t)blockIdx.x * (blockDim.x >> 5) + warp) *
+                                                    cooks_warp_doubles(A.m, mpad, A.max_cell)
+                              : smem + ((A.ncell + 1 + A.m + 1) / 2 + 1) + mpad +
+                                    (size_t)warp * cooks_warp_doubles(A.m, mpad, A.max_cell);
   double* vn = wbase;                                           // normalised counts
   double* sq = wbase + mpad;                                    // one cell's values, then its squared errors
   unsigned char* taken = reinterpret_cast<unsigned char*>(wbase + mpad + sqlen);   // extraction path only
-  for (int i = threadIdx.x; i <= A.ncell; i += blockDim.x) cell_ptr[i] = A.cell_ptr[i];
-  for (int i = threadIdx.x; i < A.m; i += blockDim.x) {
-    cell_samples[i] = A.cell_samples[i];
-    if constexpr (!NF) sf[i] = A.size_factors[i];
+  if (!rows_global) {
+    int* cp = reinterpret_cast<int*>(smem);
+    double* sfs = smem + ((A.ncell + 1 + A.m + 1) / 2 + 1);
+    for (int i = threadIdx.x; i <= A.ncell; i += blockDim.x) cp[i] = A.cell_ptr[i];
+    for (int i = threadIdx.x; i < A.m; i += blockDim.x) {
+      cp[A.ncell + 1 + i] = A.cell_samples[i];
+      if constexpr (!NF) sfs[i] = A.size_factors[i];
+    }
   }
   __syncthreads();
   const double trimratio[3] = {1.0 / 3.0, 1.0 / 4.0, 1.0 / 8.0};
   const double scale_c[3] = {2.04, 1.86, 1.51};
-  const int g = blockIdx.x * (blockDim.x >> 5) + warp;
-  if (g >= A.n) return;
+  // genes strided over the grid: one pass when the grid covers every gene (shared-memory rows), several with global rows
+  for (int g = blockIdx.x * (blockDim.x >> 5) + warp; g < A.n; g += gridDim.x * (blockDim.x >> 5)) {
+  __syncwarp();
   const size_t off = (size_t)g * A.ld;
   double s = 0.0;
   if constexpr (NF)                                             // staged in vn and divided in place (as in prep)
@@ -826,6 +865,7 @@ __global__ void __launch_bounds__(256) cooks_kernel(const CooksArgs A) {
     A.robust_disp[g] = alpha_r;
     A.max_cooks[g] = (any3 && A.m > A.p) ? mx : nan("");
   }
+  }
 }
 
 }  // namespace
@@ -840,11 +880,24 @@ cudaError_t launch_cooks(const CooksArgs& a, cudaStream_t stream) {
   // several CTAs per SM: 4 warps each, 8 when the per-warp scratch is small enough for two such CTAs
   int warps = (2 * bytes(8) <= 220 * 1024) ? 8 : 4;
   while (warps > 1 && bytes(warps) > 200 * 1024) warps >>= 1;
-  const size_t smem = bytes(warps);
+  size_t smem = bytes(warps);
+  CooksArgs b = a;
+  b.row_scratch = nullptr;
+  unsigned grid = (unsigned)((a.n + warps - 1) / warps);
+  if (smem > 200 * 1024) {
+    // one warp's rows do not fit: 8-warp CTAs, one per SM, genes strided over them, every row of length m global
+    warps = 8;
+    smem = 0;
+    grid = (unsigned)((a.n + warps - 1) / warps);
+    if (grid > (unsigned)device_sm_count()) grid = (unsigned)device_sm_count();
+    cudaError_t e = row_scratch((size_t)grid * warps * cooks_warp_doubles(a.m, mpad, a.max_cell) * sizeof(double),
+                                &b.row_scratch);
+    if (e != cudaSuccess) return e;
+  }
   const auto kern = a.nf != nullptr ? cooks_kernel<true> : cooks_kernel<false>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  kern<<<(a.n + warps - 1) / warps, warps * 32, smem, stream>>>(a);
+  kern<<<grid, warps * 32, smem, stream>>>(b);
   return cudaGetLastError();
 }
 

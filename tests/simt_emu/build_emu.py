@@ -2,7 +2,9 @@
 against the SIMT emulator in this directory.  TEST INFRASTRUCTURE ONLY (see cuda_runtime.h here).
 
 The sources are copied into the build directory with three mechanical rewrites, nothing else:
-  1. `kernel<<<grid, block, smem, stream>>>(args);` -> `simt_emu::launch(dim3(grid), dim3(block), smem, [=]() { kernel(args); });`
+  1. `kernel<<<grid, block, smem, stream>>>(args);` -> `simt_emu::launch(kernel, dim3(grid), dim3(block), smem, [=]() { kernel(args); });`
+     (the kernel's address keys the shared-memory limit that cudaFuncSetAttribute set for it; the kernel expression
+     and the launching function name the launch in the log that simt_emu_launch_log returns)
   2. `extern __shared__ ... T name[];`              -> `T* name = reinterpret_cast<T*>(simt_emu::dyn_smem_ptr());`
   3. the one inline-PTX statement (`rcp.approx.ftz.f64`) -> `simt_emu::rcp_approx_f64`
 Every rewrite is counted and the build fails if a count differs from what the sources are known to contain, so a
@@ -81,8 +83,8 @@ def rewrite_launches(src: str) -> tuple[str, int]:
         a0 = src.index("(", j)
         a1 = _match_paren(src, a0)
         assert src[a1 + 1] == ";", src[a1:a1 + 20]
-        call = (f"simt_emu::launch(dim3({cfg[0]}), dim3({cfg[1]}), (size_t)({smem}), "
-                f"[=]() {{ {kern}{src[a0:a1 + 1]}; }});")
+        call = (f"simt_emu::launch(reinterpret_cast<const void*>({kern}), dim3({cfg[0]}), dim3({cfg[1]}), (size_t)({smem}), "
+                f"[=]() {{ {kern}{src[a0:a1 + 1]}; }}, \"{kern}\", __PRETTY_FUNCTION__);")
         src = src[:k] + call + src[a1 + 2:]
         n += 1
 

@@ -12,7 +12,11 @@
  *     NOT advance in lock step), and a collective that not all named lanes reach is reported as a deadlock: both
  *     are bugs on the GPU too, so the emulator doubles as a synchronisation checker;
  *   - "device memory" is host memory, streams are no-ops, launches are synchronous; fresh device and dynamic
- *     shared memory is poisoned with 0xFF bytes (NaNs) so reads of uninitialised memory surface in the results.
+ *     shared memory is poisoned with 0xFF bytes (NaNs) so reads of uninitialised memory surface in the results;
+ *   - a launch whose DYNAMIC shared memory exceeds what sm_90 grants that kernel fails as on the GPU (see
+ *     kDynSmemOptinMax below).  `__shared__` becomes `static`, so a kernel's STATIC shared memory is invisible here:
+ *     the launch plans subtract it themselves (e.g. fit_generic.cu::plan_seg's 4 KB), and only a run on the GPU
+ *     checks that the sum of both fits.
  * Purpose: the CPU test-suite (tests/test_emulated_kernels.py) runs the kernels' own source against the oracle
  * without a GPU.  Arithmetic is IEEE fp64 with FMA contraction like nvcc's default, but it is not bit-identical
  * to the GPU (MUFU.RCP64H seed, contraction choices), so the tests use the same tolerances as the -m gpu tests.
@@ -70,7 +74,15 @@ static const int warpSize = 32;
 
 /* ------------------------------------------------------------------ scheduler interface (emu.cpp) */
 namespace simt_emu {
-void launch(dim3 grid, dim3 block, size_t dyn_smem_bytes, const std::function<void()>& body);
+/* Per-block dynamic shared-memory limits of sm_90, enforced as the runtime does: a launch above the opt-in maximum,
+ * or above 48 KB without a cudaFuncSetAttribute(MaxDynamicSharedMemorySize) for that kernel that allows it, fails
+ * (cudaErrorInvalidValue from cudaGetLastError) and its kernel does not run. */
+constexpr size_t kDynSmemDefault = 48 * 1024;
+constexpr size_t kDynSmemOptinMax = 232448;
+void launch(const void* kernel, dim3 grid, dim3 block, size_t dyn_smem_bytes, const std::function<void()>& body,
+            const char* what = "", const char* where = "");
+int set_max_dyn_smem(const void* kernel, int bytes);   /* cudaFuncSetAttribute(MaxDynamicSharedMemorySize) */
+int last_error(bool reset);                             /* cudaGetLastError / cudaPeekAtLastError */
 void* dyn_smem_ptr();
 void barrier_warp(unsigned mask);
 void barrier_cta();
@@ -238,8 +250,8 @@ inline cudaError_t cudaMemset(void* d, int v, size_t n) {
   if (n) memset(d, v, n);
   return cudaSuccess;
 }
-inline cudaError_t cudaGetLastError() { return cudaSuccess; }
-inline cudaError_t cudaPeekAtLastError() { return cudaSuccess; }
+inline cudaError_t cudaGetLastError() { return simt_emu::last_error(true); }
+inline cudaError_t cudaPeekAtLastError() { return simt_emu::last_error(false); }
 inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "simt_emu error"; }
 inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
 inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
@@ -262,8 +274,12 @@ inline cudaError_t cudaDeviceGetPCIBusId(char* s, int len, int) {   // no such d
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 /* two "SMs", one resident CTA each: persistent kernels get a grid of 2, the second CTA finds the queue drained */
 inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int) { *v = 2; return cudaSuccess; }
+/* keyed by the kernel's address, as layout.cu::persistent_grid and the launch rewrite of build_emu.py both pass it */
 template <typename K>
-inline cudaError_t cudaFuncSetAttribute(K, cudaFuncAttribute, int) { return cudaSuccess; }
+inline cudaError_t cudaFuncSetAttribute(K kernel, cudaFuncAttribute attr, int value) {
+  if (attr != cudaFuncAttributeMaxDynamicSharedMemorySize) return cudaErrorInvalidValue;
+  return simt_emu::set_max_dyn_smem(reinterpret_cast<const void*>(kernel), value);
+}
 template <typename K>
 inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int* n, K, int, size_t) { *n = 1; return cudaSuccess; }
 

@@ -7,6 +7,7 @@
 
 #include <algorithm>
 #include <mutex>
+#include <string>
 #include <vector>
 
 #include "cuda_runtime.h"
@@ -293,7 +294,53 @@ double rcp_approx_f64(double x) {
   return r;
 }
 
-void launch(dim3 grid, dim3 block, size_t dyn_smem_bytes, const std::function<void()>& kernel_body) {
+// the runtime's per-host-thread last error, and the dynamic shared-memory limit set per kernel
+thread_local int t_last_error = 0;
+std::mutex smem_attr_mu;
+std::vector<std::pair<const void*, size_t>> smem_attr;
+
+int last_error(bool reset) {
+  const int e = t_last_error;
+  if (reset) t_last_error = 0;
+  return e;
+}
+
+int set_max_dyn_smem(const void* kernel, int bytes) {
+  if (bytes < 0 || (size_t)bytes > kDynSmemOptinMax) return cudaErrorInvalidValue;
+  std::lock_guard<std::mutex> lk(smem_attr_mu);
+  for (auto& a : smem_attr)
+    if (a.first == kernel) { a.second = (size_t)bytes; return cudaSuccess; }
+  smem_attr.emplace_back(kernel, (size_t)bytes);
+  return cudaSuccess;
+}
+
+size_t max_dyn_smem(const void* kernel) {
+  std::lock_guard<std::mutex> lk(smem_attr_mu);
+  for (const auto& a : smem_attr)
+    if (a.first == kernel) return a.second;
+  return kDynSmemDefault;
+}
+
+// one line per launch, "<kernel expression> | <launching function> | <threads> | <dynamic shared bytes>": tests read it to
+// see which kernel a launch plan chose (simt_emu_launch_log)
+std::mutex log_mu;
+std::string launch_log;
+
+void launch(const void* kernel, dim3 grid, dim3 block, size_t dyn_smem_bytes, const std::function<void()>& kernel_body,
+            const char* what, const char* where) {
+  {
+    std::lock_guard<std::mutex> lk(log_mu);
+    char tail[64];
+    snprintf(tail, sizeof tail, " | %u | %zu\n", block.x * block.y * block.z, dyn_smem_bytes);
+    if (launch_log.size() > (1u << 22)) launch_log.clear();   // nobody reads it: keep it bounded
+    launch_log += std::string(what) + " | " + where + tail;
+  }
+  if (dyn_smem_bytes > max_dyn_smem(kernel)) {   // refused before it runs, as the runtime refuses it
+    fprintf(stderr, "simt_emu: launch refused: %zu bytes of dynamic shared memory, the kernel may use %zu\n",
+            dyn_smem_bytes, max_dyn_smem(kernel));
+    t_last_error = cudaErrorInvalidValue;
+    return;
+  }
   // one grid at a time: host threads that launch concurrently (the chunk workers of capi.cu) are serialised here
   static std::mutex launch_mu;
   std::lock_guard<std::mutex> lk(launch_mu);
@@ -355,3 +402,15 @@ cudaError_t cudaHostAlloc(void** p, size_t bytes, unsigned) {
 cudaError_t cudaFreeHost(void* p) { free(p); return cudaSuccess; }
 
 extern "C" long long simt_emu_launches() { return simt_emu::launches(); }
+// returns the launch log's length; with a buffer, copies the log into it (NUL-terminated, truncated to len) and clears it
+extern "C" long long simt_emu_launch_log(char* buf, long long len) {
+  std::lock_guard<std::mutex> lk(simt_emu::log_mu);
+  const long long n = (long long)simt_emu::launch_log.size();
+  if (buf && len > 0) {
+    const long long k = n < len - 1 ? n : len - 1;
+    memcpy(buf, simt_emu::launch_log.data(), (size_t)k);
+    buf[k] = 0;
+    simt_emu::launch_log.clear();
+  }
+  return n;
+}

@@ -78,6 +78,20 @@ __global__ void k_uninitialised_smem(double* out) {
   out[threadIdx.x] = smem[threadIdx.x];
 }
 
+// touches the last double of its dynamic shared memory, so that a launch that runs is visible in `ran`
+__global__ void k_smem_limit(int* ran, size_t doubles) {
+  extern __shared__ __align__(16) double smem[];
+  smem[doubles - 1] = 1.0;
+  *ran = (int)smem[doubles - 1];
+}
+
+// the same, for the launches that never set the attribute (its limit stays the 48 KB default whatever ran before)
+__global__ void k_smem_default(int* ran, size_t doubles) {
+  extern __shared__ __align__(16) double smem[];
+  smem[doubles - 1] = 1.0;
+  *ran = (int)smem[doubles - 1];
+}
+
 extern "C" {
 int st_warp_collectives(double* out_sum, int* out_misc, int blocks, int threads) {
   k_warp_collectives<<<blocks, threads, 0, 0>>>(out_sum, out_misc);
@@ -97,6 +111,20 @@ int st_missing_syncwarp(int* out, int with_sync) {
 }
 int st_divergent_collective(int* out) {
   k_divergent_collective<<<1, 32, 0, 0>>>(out);
+  return (int)cudaGetLastError();
+}
+// attr > 0: cudaFuncSetAttribute(MaxDynamicSharedMemorySize, attr) first (attr == 0: a kernel that never sets it);
+// returns the first error
+int st_smem_limit(int* ran, int bytes, int attr) {
+  if (attr == 0) {
+    k_smem_default<<<1, 32, (size_t)bytes, 0>>>(ran, (size_t)bytes / sizeof(double));
+    return (int)cudaGetLastError();
+  }
+  {
+    const cudaError_t e = cudaFuncSetAttribute(k_smem_limit, cudaFuncAttributeMaxDynamicSharedMemorySize, attr);
+    if (e != cudaSuccess) return (int)e;
+  }
+  k_smem_limit<<<1, 32, (size_t)bytes, 0>>>(ran, (size_t)bytes / sizeof(double));
   return (int)cudaGetLastError();
 }
 int st_uninitialised_smem(double* out) {

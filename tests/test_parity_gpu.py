@@ -45,14 +45,14 @@ def _compare_disp(g, o, name, min_robust=0.9):
                            f"margin {o['margin'][bad[:5]]}")
     assert robust.mean() >= min_robust, f"{name}: only {robust.mean():.3f} of genes have robust decisions"
     sel = robust & same
-    for k in DISP_KEYS:
+    for k in DISP_KEYS if sel.any() else ():
         if k in ("last_dlp", "last_change", "last_d2lp", "initial_dlp"):
             # derivatives / differences of nearly equal numbers: absolute error on the scale of the posterior
             err = np.abs(g[k][sel] - o[k][sel]) / (np.abs(o["last_lp"][sel]) * 1e-3 + np.abs(o[k][sel]) + 1e-12)
         else:
             err = rel_err(g[k][sel], o[k][sel])
         assert np.nanmax(err) < TOL, f"{name}: {k} max rel err {np.nanmax(err):.3e}"
-    assert np.max(rel_err(np.exp(g["log_alpha"][sel]), np.exp(o["log_alpha"][sel]))) < TOL
+    assert not sel.any() or np.max(rel_err(np.exp(g["log_alpha"][sel]), np.exp(o["log_alpha"][sel]))) < TOL
     # knife-edge genes (either side may take the other branch): both must still end at the same posterior value
     rest = ~sel
     if rest.any():

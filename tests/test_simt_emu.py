@@ -91,6 +91,28 @@ def test_divergent_collective_is_reported_as_deadlock(st):
     assert "deadlock" in r.stderr and "warp collective" in r.stderr and "__syncthreads" in r.stderr
 
 
+# sm_90: 48 KB of dynamic shared memory without an opt-in, 232448 bytes (227 KB) at most with one
+@pytest.mark.parametrize("bytes_, attr, ok", [
+    (48 * 1024, 0, True),              # the default limit, no attribute
+    (48 * 1024 + 8, 0, False),         # above it without cudaFuncSetAttribute
+    (100 * 1024, 99 * 1024, False),    # above the limit the attribute set
+    (232448, 232448, True),            # at the opt-in maximum
+    (232448 + 8, 232448, False),       # above it
+])
+def test_dynamic_shared_memory_limits(st, bytes_, attr, ok):
+    """The emulator refuses a launch the H100 refuses, so that a launch plan that only fits on the emulator fails on
+    the CPU too; the refused kernel does not run."""
+    ran = np.zeros(1, dtype=np.int32)
+    rc = st.st_smem_limit(_p(ran), bytes_, attr)
+    assert (rc == 0) == ok and ran[0] == int(ok)
+    assert st.st_smem_limit(_p(ran), 1024, 0) == 0     # a refusal is not sticky: the next launch runs
+
+
+def test_shared_memory_attribute_above_the_maximum_is_refused(st):
+    ran = np.zeros(1, dtype=np.int32)
+    assert st.st_smem_limit(_p(ran), 1024, 232448 + 8) != 0 and ran[0] == 0
+
+
 @pytest.mark.parametrize("order", ["reverse", "random:7"])
 def test_lane_order_is_configurable(st, order):
     """SIMT_EMU_ORDER changes which lane runs first between barriers: correct kernels do not care, the kernel with the
