@@ -69,25 +69,45 @@ def _ws(name, shape, dtype, dev):
     return t
 
 
+def size_factor_ratios(y, m, poscounts=False, divisor=None):
+    """One launch of b200nb_size_factors_dev (b200nb_size_factors_norm_dev with a gene-major (n, ld) divisor matrix):
+    returns {"sizeFactors": (m,), "loggeomeans": (n,), "ratios": the (m, n) log ratios of the median, one sample per
+    row, +Inf where an entry does not take part (a view of a workspace: valid until the next call), "n_finite": the
+    number of genes with a finite log geometric mean as a 1-element device tensor}.  Does not raise when it is 0."""
+    L = _lib.lib()
+    dev = y.device
+    n, ld = y.shape
+    out = {"sizeFactors": torch.empty(m, dtype=F64, device=dev), "loggeomeans": torch.empty(n, dtype=F64, device=dev),
+           "n_finite": torch.zeros(1, dtype=torch.int32, device=dev)}
+    gm = _ws("sf_ratios", (n, ld), F64, dev)
+    cm = _ws("sf_ratios_cm", (n * m,), F64, dev)
+    if divisor is None:
+        _lib.check(L.b200nb_size_factors_dev(D._p(y), D._ytype(y), int(poscounts), n, m, ld, D._p(out["loggeomeans"]),
+                                             D._p(gm), D._p(cm), D._p(out["sizeFactors"]), D._p(out["n_finite"]),
+                                             D._stream()), "size_factors")
+    else:
+        _lib.check(L.b200nb_size_factors_norm_dev(D._p(y), D._ytype(y), D._p(divisor), int(poscounts), n, m, ld,
+                                                  D._p(out["loggeomeans"]), D._p(gm), D._p(cm),
+                                                  D._p(out["sizeFactors"]), D._p(out["n_finite"]), D._stream()),
+                   "size_factors_norm")
+    out["ratios"] = cm.view(m, n)
+    return out
+
+
+def _no_finite_loggeomean():
+    return ValueError("every gene contains at least one zero, cannot compute log geometric means")
+
+
 def size_factors(y, m, type="ratio"):
     """b200nb_size_factors_dev: estimateSizeFactorsForMatrix (R/core.R:535-578, locfunc = median) on the device.
     y: gene-major (n, ld) device tensor, m samples.  Returns {"sizeFactors": (m,) device tensor, "loggeomeans": (n,)}.
     Raises like the reference when every gene contains a zero (the only host read: one int)."""
     if type not in ("ratio", "poscounts"):
         raise ValueError("type must be 'ratio' or 'poscounts'")
-    L = _lib.lib()
-    dev = y.device
-    n, ld = y.shape
-    out = {"sizeFactors": torch.empty(m, dtype=F64, device=dev), "loggeomeans": torch.empty(n, dtype=F64, device=dev)}
-    nfin = torch.zeros(1, dtype=torch.int32, device=dev)
-    gm = _ws("sf_ratios", (n, ld), F64, dev)
-    cm = _ws("sf_ratios_cm", (n * m,), F64, dev)
-    _lib.check(L.b200nb_size_factors_dev(D._p(y), D._ytype(y), int(type == "poscounts"), n, m, ld,
-                                         D._p(out["loggeomeans"]), D._p(gm), D._p(cm), D._p(out["sizeFactors"]),
-                                         D._p(nfin), D._stream()), "size_factors")
-    if int(nfin.item()) == 0:
-        raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
-    return out
+    r = size_factor_ratios(y, m, poscounts=type == "poscounts")
+    if int(r["n_finite"].item()) == 0:
+        raise _no_finite_loggeomean()
+    return {"sizeFactors": r["sizeFactors"], "loggeomeans": r["loggeomeans"]}
 
 
 def sf_iterate_objective(y, q, alpha, par, m, h=1e-3, Q=0.05, max_tile_cols=0, out=None):
@@ -142,6 +162,16 @@ def normalization_factors(y, m, normMatrix=None, avgTxLength=None, type="ratio")
     rescaled to geometric mean 1, R/core.R:573-576), then nf = normMatrix * sf divided by its row geometric mean.
     Returns {"normalizationFactors": (n, ld) device tensor (padding columns 1), "sizeFactors": (m,)}.
     Raises ValueError for a non-positive / non-finite matrix and when every gene contains a zero."""
+    nm, d = norm_divisor(y, m, normMatrix, avgTxLength, type)
+    r = size_factor_ratios(y, m, poscounts=type == "poscounts", divisor=d)
+    if int(r["n_finite"].item()) == 0:
+        raise _no_finite_loggeomean()
+    return norm_factors_from(nm, d, r["sizeFactors"], m, type)
+
+
+def norm_divisor(y, m, normMatrix, avgTxLength, type):
+    """The checks of normalization_factors and its divisor: (normMatrix, or avgTxLength over its row geometric mean, as
+    an (n, m) tensor; the same in a gene-major (n, ld) matrix whose padding columns are 1)."""
     if type not in ("ratio", "poscounts"):
         raise ValueError("type must be 'ratio' or 'poscounts'")
     if (normMatrix is None) == (avgTxLength is None):
@@ -149,24 +179,18 @@ def normalization_factors(y, m, normMatrix=None, avgTxLength=None, type="ratio")
     name = "normMatrix" if normMatrix is not None else "avgTxLength"
     src = normMatrix if normMatrix is not None else avgTxLength
     _check_positive_matrix(src, y, m, name)
-    L = _lib.lib()
-    dev = y.device
     n, ld = y.shape
     nm = src[:, :m]
     if avgTxLength is not None:
         nm = nm / torch.exp(torch.log(nm).mean(dim=1, keepdim=True))
-    d = torch.ones((n, ld), dtype=F64, device=dev)
+    d = torch.ones((n, ld), dtype=F64, device=y.device)
     d[:, :m] = nm
-    sf = torch.empty(m, dtype=F64, device=dev)
-    lg = torch.empty(n, dtype=F64, device=dev)
-    nfin = torch.zeros(1, dtype=torch.int32, device=dev)
-    gm = _ws("sf_ratios", (n, ld), F64, dev)
-    cm = _ws("sf_ratios_cm", (n * m,), F64, dev)
-    _lib.check(L.b200nb_size_factors_norm_dev(D._p(y), D._ytype(y), D._p(d), int(type == "poscounts"), n,
-                                              m, ld, D._p(lg), D._p(gm), D._p(cm), D._p(sf), D._p(nfin), D._stream()),
-               "size_factors_norm")
-    if int(nfin.item()) == 0:
-        raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
+    return nm, d
+
+
+def norm_factors_from(nm, d, sf, m, type):
+    """normalization_factors' last step from the size factors of K / normMatrix: the poscounts rescaling, nf =
+    normMatrix * sf over its row geometric mean, written into d's first m columns."""
     if type == "poscounts":
         sf = sf / torch.exp(torch.log(sf).mean())
     nf = nm * sf[None, :]
@@ -781,8 +805,8 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
                  nfXim=None, sfType="ratio", fitType="parametric", test="Wald", reduced=None):
     """y: gene-major (N, ld) device tensor of counts (int32 or float64).  Returns a dict of device tensors over the
     rows with a non-zero sum (`idx` maps them back to the N input rows) plus the trend / prior scalars.
-    sizeFactors=None estimates them on the device first (median of ratios, R/core.R:535-578; returned under
-    "sizeFactors").  minReplicatesForReplace: the reference's default is 7 (replace count outliers by the trimmed mean
+    sizeFactors: (m,) numpy or a device tensor (read to the host once); None estimates them on the device first
+    (median of ratios, R/core.R:535-578; returned under "sizeFactors").  minReplicatesForReplace: the reference's default is 7 (replace count outliers by the trimmed mean
     and refit those genes, R/core.R:419-426, 2069-2115, 2484-2565); the default here is Inf = off (what bench.py's
     full_pipeline times).  With a finite value the per-gene results of the refitted rows are overwritten in place
     and "replace" / "replaceable" / "n_replaced" are added.
@@ -834,6 +858,8 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     dev = y.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
+    if isinstance(sizeFactors, torch.Tensor):       # e.g. size_factors' or sharded_size_factors_device's device tensor
+        sizeFactors = sizeFactors.cpu().numpy()
     reduced = check_test_args(x, test, reduced, betaPrior)
     if sfType not in ("ratio", "poscounts", "iterate"):
         raise ValueError("sfType must be 'ratio', 'poscounts' or 'iterate'")
@@ -1220,23 +1246,36 @@ def _vst_design(x, m, blind):
     return x
 
 
-def _dispersion_function(ynz, x, sizeFactors, nfz, fitType, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100,
-                         betaTol=1e-8, minmu=0.5):
-    """estimateDispersionsGeneEst + estimateDispersionsFit with their defaults on the rows of ynz (none of them
-    all-zero; nfz: their nf rows, xim is taken over them): the pre-step kernel, _gene_est and _dispersion_trend, as in
-    DESeq_device.  Returns {"fitType", "trendCoefs" (device (2,)) or "meanDisp" (float)}.  A failed parametric fit
-    raises FloatingPointError (R would fall back to the local fit)."""
+def gene_wise_dispersions(ynz, x, sizeFactors, nfz, xim=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100,
+                          betaTol=1e-8, minmu=0.5):
+    """estimateDispersionsGeneEst with its defaults on the rows of ynz (none of them all-zero; nfz: their nf rows, xim
+    over them unless given): the pre-step kernel and _gene_est, as in DESeq_device.  Returns (baseMean, dispGeneEst)."""
     m, p = x.shape
     linearMu = modelMatrixGroups(x) == p
-    pr = prep(ynz, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu, normalizationFactors=nfz)
+    pr = prep(ynz, x, sizeFactors, minDisp=minDisp, minmu=minmu, want_mu=linearMu, normalizationFactors=nfz, xim=xim)
     mu_glm = None if linearMu else _ws("mu_glm", tuple(ynz.shape), F64, ynz.device)
     _, _, dge, _ = _gene_est(ynz, pr["xd"], pr["sfd"], pr["alpha0"], pr["beta0"], pr["mu_lin"], m, minDisp=minDisp,
                              kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, betaTol=betaTol, minmu=minmu,
                              mu_out=mu_glm)
-    tr = _dispersion_trend(pr["baseMean"], dge, fitType, minDisp)
+    return pr["baseMean"], dge
+
+
+def dispersion_function_of(baseMean, dge, fitType, minDisp=1e-8):
+    """estimateDispersionsFit (_dispersion_trend) as a dispersion function: {"fitType", "trendCoefs" (device (2,)) or
+    "meanDisp" (float)}.  A failed parametric fit raises FloatingPointError (R would fall back to the local fit)."""
+    tr = _dispersion_trend(baseMean, dge, fitType, minDisp)
     if fitType == "mean":
         return {"fitType": "mean", "meanDisp": float(tr[0].item())}
     return {"fitType": "parametric", "trendCoefs": tr[:2].clone()}
+
+
+def _dispersion_function(ynz, x, sizeFactors, nfz, fitType, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100,
+                         betaTol=1e-8, minmu=0.5):
+    """estimateDispersionsGeneEst + estimateDispersionsFit with their defaults on the rows of ynz (none of them
+    all-zero; nfz: their nf rows, xim is taken over them): gene_wise_dispersions and dispersion_function_of."""
+    bm, dge = gene_wise_dispersions(ynz, x, sizeFactors, nfz, minDisp=minDisp, kappa_0=kappa_0, dispTol=dispTol,
+                                    maxit=maxit, betaTol=betaTol, minmu=minmu)
+    return dispersion_function_of(bm, dge, fitType, minDisp)
 
 
 def _vst_result(y, m, fn, sizeFactors, nf, sfd):

@@ -9,6 +9,8 @@ Backend: "nccl" on GPUs (tensors on the rank's device), "gloo" for the CPU tests
 """
 from __future__ import annotations
 
+import math
+
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -96,14 +98,18 @@ class PackedGather:
     """ONE collective per exchange: several per-gene 1-D vectors of this rank (all of the same, rank-dependent length)
     travel as one (1 + ncols) x cap buffer -- row 0 carries the shard's length -- through a single
     all_gather_into_tensor, and come back concatenated over the ranks in rank order (R/parallel.R:54-66's rbind).
-    `cap` (rows of the largest shard) is agreed once per run with one 8-byte all-reduce."""
+    `cap` (rows of the largest shard) is agreed once per run with one 8-byte all-reduce, or given by a caller to whom
+    every rank's row count is already known (no collective then)."""
 
-    def __init__(self, n_local_rows: int, device):
+    def __init__(self, n_local_rows: int, device, cap=None):
         self.world = dist.get_world_size()
-        c = torch.tensor([int(n_local_rows)], dtype=torch.int64, device=device)
-        dist.all_reduce(c, op=dist.ReduceOp.MAX)
-        self.cap = max(int(c.item()), 1)
-        self.collectives = 1
+        if cap is None:
+            c = torch.tensor([int(n_local_rows)], dtype=torch.int64, device=device)
+            dist.all_reduce(c, op=dist.ReduceOp.MAX)
+            cap, self.collectives = int(c.item()), 1
+        else:
+            self.collectives = 0
+        self.cap = max(int(cap), 1)
 
     def __call__(self, cols):
         single = isinstance(cols, torch.Tensor)
@@ -119,6 +125,7 @@ class PackedGather:
         out = out.view(self.world, buf.shape[0], self.cap)
         self.collectives += 1
         sizes = [int(v) for v in out[:, 0, 0].tolist()]
+        self.sizes = sizes
         res = [torch.cat([out[r, k + 1, :sizes[r]] for r in range(self.world)]) for k in range(len(cols))]
         return res[0] if single else res
 
@@ -126,6 +133,24 @@ class PackedGather:
 def allgather_1d(t: torch.Tensor) -> torch.Tensor:
     """Concatenate a 1-D tensor of rank-dependent length over the ranks (rank order): a PackedGather of one column."""
     return PackedGather(t.numel(), t.device)(t)
+
+
+def gathered_xim(nf_rows, m, pg):
+    """momentsDispEstimate's xim = mean(1 / colMeans(nf)) over the rows nf_rows of EVERY rank: ONE all-gather carries
+    each rank's m column sums and its row count (m + 1 doubles), summed on every rank in rank order, so every rank gets
+    the same bits.  Counted in pg.collectives.  The partial sums make the last bit depend on where the shards split,
+    so xim can differ in the last bit from the single-device sum over the same rows."""
+    from . import device_pipeline as DP
+    colsum, count = DP.nf_column_sums(nf_rows, m)
+    mine = torch.cat([colsum, torch.tensor([float(count)], dtype=torch.float64, device=colsum.device)])
+    allr = torch.empty(pg.world * (m + 1), dtype=torch.float64, device=mine.device)
+    dist.all_gather_into_tensor(allr, mine.contiguous())
+    allr = allr.view(pg.world, m + 1)
+    pg.collectives += 1
+    tot = allr[0].clone()
+    for r in range(1, pg.world):                    # rank order: the same bits on every rank
+        tot = tot + allr[r]
+    return DP.nf_xim(tot[:m], tot[m])
 
 
 def sharded_DESeq_device(y_local, x, sizeFactors=None, **kw):
@@ -145,8 +170,10 @@ def sharded_DESeq_device(y_local, x, sizeFactors=None, **kw):
     ALL ranks, as a serial DESeq() computes it: ONE more all-gather carries each rank's m column sums and its row count
     (m + 1 doubles), summed on every rank in rank order, so xim does not depend on the number of ranks (the reference's
     DESeqParallel uses each chunk's own xim instead, R/parallel.R:18-20).  Not supported with finite
-    minReplicatesForReplace (the refitted rows' xim would need another collective) or avgTxLength (estimating the
-    factors needs a global median): estimate them on one device or pass them.
+    minReplicatesForReplace (the refitted rows' xim would need another collective) or avgTxLength: estimate the
+    factors with sharded_normalization_factors and pass them.
+    sizeFactors=None estimates median-of-ratios size factors from this rank's shard only (unchanged: the ranks then
+    differ); pass sharded_size_factors_device(y_local, m)["sizeFactors"] for the size factors of all genes.
     test="LRT", reduced=... (passed on to DESeq_device): the LRT columns are per gene, so no collective is added;
     LRTStatistic and LRTPvalue travel in the result gather in place of WaldPvalue (1 + 2p + 2 doubles per gene)."""
     from . import device_pipeline as DP
@@ -165,16 +192,7 @@ def sharded_DESeq_device(y_local, x, sizeFactors=None, **kw):
         m = np.asarray(x).shape[0]
         DP._check_positive_matrix(nf, y_local, m, "normalizationFactors")
         nz = y_local[:, :m].sum(dim=1) != 0
-        colsum, count = DP.nf_column_sums(nf[nz], m)
-        mine = torch.cat([colsum, torch.tensor([float(count)], dtype=torch.float64, device=colsum.device)])
-        allr = torch.empty(pg.world * (m + 1), dtype=torch.float64, device=mine.device)
-        dist.all_gather_into_tensor(allr, mine.contiguous())
-        allr = allr.view(pg.world, m + 1)
-        pg.collectives += 1
-        tot = allr[0].clone()
-        for r in range(1, pg.world):                # rank order: the same bits on every rank
-            tot = tot + allr[r]
-        kw["nfXim"] = DP.nf_xim(tot[:m], tot[m])
+        kw["nfXim"] = gathered_xim(nf[nz], m, pg)
     res = DP.DESeq_device(y_local, x, sizeFactors, allgather=pg, **kw)
     p = res["betaMatrix"].shape[1]
     lrt = res["test"] == "LRT"
@@ -230,4 +248,326 @@ def sharded_lfcShrink_device(res_local, y_local, x, **kw):
     pg = PackedGather(y_local.shape[0], y_local.device)
     out = DP.lfcShrink_device(res_local, y_local, x, allgather=pg, **kw)
     out["collectives"] = pg.collectives
+    return out
+
+
+# ---------------------------------------------------------------- size factors, normalization factors and the
+# transforms on gene shards (R/core.R:535-578, 2159-2163; R/vst.R; R/helper.R:421-435)
+
+_SIGN = -(1 << 63)                                  # int64 with only the sign bit set
+_LOW63 = (1 << 63) - 1
+
+
+def _order_keys(v):
+    """sf_median_kernel's key_of (csrc/size_factors.cu): the order-preserving unsigned 64-bit image of float64 values,
+    its bits held in an int64 tensor (compare two keys as unsigned with _below)."""
+    b = v.view(torch.int64)
+    return torch.where(b < 0, ~b, b | _SIGN)
+
+
+def _key_values(k):
+    """value_of: the float64 values of _order_keys keys."""
+    return torch.where(k < 0, k & _LOW63, ~k).view(torch.float64)
+
+
+def _below(a, b):
+    """a < b for unsigned keys held in int64."""
+    return (a ^ _SIGN) < (b ^ _SIGN)
+
+
+_KEY_INF = (0x7ff0000000000000 | (1 << 63)) - (1 << 64)     # _order_keys(+Inf): entries that do not take part
+
+
+def _exp_as_kernel(v):
+    """exp(v) with the bits of sf_median_kernel's exp: CUDA's exp on the GPU (torch's CUDA exp is the same libdevice
+    function); where the engine's CUDA source runs on the host (the SIMT emulator), the C library's exp, which
+    math.exp calls, as torch's vectorised CPU exp can differ from it in the last bit."""
+    if v.device.type == "cuda":
+        return torch.exp(v)
+
+    def one(e):
+        try:
+            return math.exp(e)
+        except OverflowError:
+            return math.inf
+    return torch.tensor([one(e) for e in v.tolist()], dtype=torch.float64, device=v.device)
+
+
+def _local_ratios(y_local, m, poscounts, divisor=None):
+    """The size-factor kernel on this shard (device_pipeline.size_factor_ratios); an empty shard launches nothing."""
+    from . import device_pipeline as DP
+    if y_local.shape[0] == 0:
+        dev = y_local.device
+        return {"ratios": torch.empty((m, 0), dtype=torch.float64, device=dev),
+                "loggeomeans": torch.empty(0, dtype=torch.float64, device=dev),
+                "n_finite": torch.zeros(1, dtype=torch.int32, device=dev)}
+    return DP.size_factor_ratios(y_local, m, poscounts=poscounts, divisor=divisor)
+
+
+def _agree(r, failed=False):
+    """ONE integer all-reduce (SUM) of m + 2 int64: the number of ratios that take part in each sample's median, the
+    number of genes with a finite log geometric mean and the number of ranks whose arguments failed their checks.
+    Returns (per-sample counts as a device tensor, n_finite, failed ranks) -- the same on every rank -- and this
+    rank's entries that take part as (keys, sample of each key) for _global_median."""
+    ratios = r["ratios"]
+    m = ratios.shape[0]
+    dev = ratios.device
+    keys = _order_keys(ratios)
+    use = _below(keys, torch.tensor(_KEY_INF, dtype=torch.int64, device=dev))
+    head = torch.cat([use.sum(dim=1), r["n_finite"].to(torch.int64),
+                      torch.tensor([int(failed)], dtype=torch.int64, device=dev)])
+    dist.all_reduce(head)
+    tail = head[-2:].tolist()
+    entries = (keys[use], torch.arange(m, dtype=torch.int64, device=dev).view(m, 1).expand_as(keys)[use])
+    return head[:-2], int(tail[0]), int(tail[1]), entries
+
+
+def _global_median(entries, nv):
+    """The median of each sample's log ratios over the entries of EVERY rank that take part (not +Inf), as
+    sf_median_kernel takes it over one device's: the key of the lower middle element (0-based rank (nv - 1) / 2) and,
+    for an even count nv, of the upper middle element are found together by an MSB-first radix select on the
+    order-preserving 64-bit keys, 8 bits per round.  entries: this rank's (keys, sample of each key) from _agree.  Each
+    round every rank builds the digit histograms of its matching entries (2 targets x m samples x 256 digits, int64;
+    in the first round both targets share one) and ONE integer all-reduce (SUM) adds them, so the selected keys
+    depend neither on the number of ranks nor on the reduction order; then every rank keeps only the entries under one
+    of the two new prefixes.  8 collectives of 2 x m x 256 x 8 bytes; no ratio leaves its rank.  Returns (m,) medians
+    0.5 * (lower + upper) (the lower middle for an odd count, NaN for nv = 0) and the number of collectives."""
+    kk, jj = entries
+    m = nv.numel()
+    dev = nv.device
+    r0 = torch.clamp(nv - 1, min=0) // 2
+    rk = torch.stack([r0, r0 + (nv % 2 == 0).to(torch.int64)])     # residual ranks of the (lower, upper) targets
+    prefix = torch.zeros((2, m), dtype=torch.int64, device=dev)
+    for rnd in range(7, -1, -1):
+        s = 8 * rnd
+        idx = jj * 256 + ((kk >> s) & 255)
+        hist = torch.empty((2, m * 256), dtype=torch.int64, device=dev)
+        if rnd == 7:                                                 # no prefix yet: one histogram for both targets
+            hist[0] = torch.bincount(idx, minlength=m * 256)
+            hist[1] = hist[0]
+        else:
+            for t in range(2):
+                hist[t] = torch.bincount(idx[(kk >> (s + 8)) == (prefix[t][jj] >> (s + 8))], minlength=m * 256)
+        dist.all_reduce(hist)
+        cum = hist.view(2, m, 256).cumsum(dim=2)
+        b = (cum <= rk.unsqueeze(2)).sum(dim=2).clamp(max=255)       # the first digit whose cumulative count > rank
+        rk = rk - torch.where(b > 0, cum.gather(2, (b - 1).clamp(min=0).unsqueeze(2)).squeeze(2), 0)
+        prefix = prefix | (b << s)
+        top = kk >> s
+        keep = (top == (prefix[0][jj] >> s)) | (top == (prefix[1][jj] >> s))
+        kk, jj = kk[keep], jj[keep]
+    lo, hi = _key_values(prefix[0]), _key_values(prefix[1])
+    med = torch.where(nv % 2 == 1, lo, 0.5 * (lo + hi))
+    return torch.where(nv == 0, torch.nan, med), 8
+
+
+def _sizes_of(med, nv):
+    sf = _exp_as_kernel(med)
+    return torch.where(nv == 0, torch.nan, sf)
+
+
+def sharded_size_factors_device(y_local, m, type="ratio"):
+    """estimateSizeFactorsForMatrix (R/core.R:535-578, locfunc = median) over the genes of ALL ranks, y_local being this
+    rank's rows (gene-major, split as shard_bounds splits them).  The log geometric means are per gene and the log
+    ratios are the size-factor kernel's own (b200nb_size_factors_dev, whose column-major ratio scratch it reads); the
+    per-sample median over every rank's ratios is _global_median.  Every rank gets the sizeFactors that
+    device_pipeline.size_factors gives for the whole matrix, bit for bit; for "poscounts" they are then rescaled to
+    geometric mean 1 (the incoming-geoMeans step, R/core.R:573-576) exactly as DESeq_device does.  A sample with no
+    usable ratio gets NaN.  "Every gene contains at least one zero" is decided on the count of finite log geometric
+    means of all ranks and raises ValueError on every rank.  Returns {"sizeFactors": (m,) device tensor, "loggeomeans":
+    this shard's (n_local,), "collectives": 9 (one agreement all-reduce and 8 histogram rounds)}."""
+    from . import device_pipeline as DP
+    if type not in ("ratio", "poscounts"):
+        raise ValueError("type must be 'ratio' or 'poscounts'")
+    r = _local_ratios(y_local, m, type == "poscounts")
+    nv, n_finite, _, entries = _agree(r)
+    if n_finite == 0:
+        raise DP._no_finite_loggeomean()
+    med, c = _global_median(entries, nv)
+    sf = _sizes_of(med, nv)
+    if type == "poscounts":
+        sf = sf / torch.exp(torch.log(sf).mean())
+    return {"sizeFactors": sf, "loggeomeans": r["loggeomeans"], "collectives": 1 + c}
+
+
+def sharded_normalization_factors(y_local, m, normMatrix_local=None, avgTxLength_local=None, type="ratio"):
+    """device_pipeline.normalization_factors over the genes of ALL ranks (estimateNormFactors, R/core.R:2159-2163, and
+    the avgTxLength path): normMatrix_local / avgTxLength_local are this shard's rows, gene-major like y_local.  The size
+    factors of K / normMatrix come from the global median of sharded_size_factors_device; everything else is per gene.
+    A matrix that fails its checks on any rank raises ValueError on every rank (the failure travels in the agreement
+    all-reduce).  Returns {"normalizationFactors": this shard's (n_local, ld), "sizeFactors": (m,), "collectives": 9},
+    which sharded_DESeq_device(normalizationFactors=...) and the sharded transforms take."""
+    from . import device_pipeline as DP
+    err = None
+    try:
+        nm, d = DP.norm_divisor(y_local, m, normMatrix_local, avgTxLength_local, type)
+        r = _local_ratios(y_local, m, type == "poscounts", divisor=d)
+    except ValueError as e:
+        err = e
+        r = _local_ratios(y_local[:0], m, False)
+    nv, n_finite, failed, entries = _agree(r, failed=err is not None)
+    if err is not None:
+        raise err
+    if failed:
+        raise ValueError(f"normalization_factors: the arguments of {failed} other rank(s) failed their checks")
+    if n_finite == 0:
+        raise DP._no_finite_loggeomean()
+    med, c = _global_median(entries, nv)
+    out = DP.norm_factors_from(nm, d, _sizes_of(med, nv), m, type)
+    out["collectives"] = 1 + c
+    return out
+
+
+def _sharded_factors(y_local, m, sizeFactors, normalizationFactors, avgTxLength):
+    """device_pipeline._factors with the estimates of every rank: returns (size factors or None, nf rows or None, sfd,
+    the collectives of the estimate)."""
+    from . import device_pipeline as DP
+    n = 0
+    if avgTxLength is not None:
+        if normalizationFactors is not None:
+            raise ValueError("give normalizationFactors or avgTxLength, not both")
+        if sizeFactors is not None:
+            raise ValueError("avgTxLength estimates normalization factors: sizeFactors must be None")
+        r = sharded_normalization_factors(y_local, m, avgTxLength_local=avgTxLength)
+        normalizationFactors, n = r["normalizationFactors"], r["collectives"]
+    elif normalizationFactors is not None:
+        err = None
+        try:
+            DP._check_positive_matrix(normalizationFactors, y_local, m, "normalizationFactors")
+        except ValueError as e:
+            err = e
+        _fail_together(err, y_local.device, "normalizationFactors")
+        n = 1
+    elif sizeFactors is None:
+        r = sharded_size_factors_device(y_local, m)
+        sizeFactors, n = r["sizeFactors"], r["collectives"]
+    return DP._factors(y_local, m, sizeFactors, normalizationFactors) + (n,)
+
+
+def _fail_together(err, dev, what):
+    """ONE 8-byte all-reduce (SUM) of the ranks whose arguments failed their checks, so that a check that fails on one
+    rank raises ValueError on every rank instead of leaving the others blocked in the next collective."""
+    f = torch.tensor([int(err is not None)], dtype=torch.int64, device=dev)
+    dist.all_reduce(f)
+    if err is not None:
+        raise err
+    failed = int(f.item())
+    if failed:
+        raise ValueError(f"{what}: the arguments of {failed} other rank(s) failed their checks")
+
+
+def _gene_wise(ynz, x, sizeFactors, nfz, xim):
+    """device_pipeline.gene_wise_dispersions on this rank's rows; none on a rank without rows."""
+    from . import device_pipeline as DP
+    if ynz.shape[0] == 0:
+        e = torch.empty(0, dtype=torch.float64, device=ynz.device)
+        return e, e
+    return DP.gene_wise_dispersions(ynz, x, sizeFactors, nfz, xim=xim)
+
+
+def sharded_varianceStabilizingTransformation_device(y_local, m, x=None, blind=True, fitType="parametric",
+                                                     sizeFactors=None, normalizationFactors=None, avgTxLength=None,
+                                                     dispersionFunction=None):
+    """device_pipeline.varianceStabilizingTransformation_device over the genes of ALL ranks, for this rank's rows
+    y_local (gene-major, split as shard_bounds splits them; normalizationFactors / avgTxLength: this shard's rows).
+    Factors not given are estimated over all ranks (sharded_size_factors_device, sharded_normalization_factors).  When
+    the dispersion function is fitted, GeneEst runs on this shard's non-zero rows, ONE packed all-gather (after the
+    8-byte size agreement) brings (baseMean, dispGeneEst) of every rank, and every rank fits the same trend or mean;
+    with normalization factors xim is over the non-zero rows of all ranks (gathered_xim, one more all-gather).  The
+    transform is local.  Returns the single-device dict for this shard's rows ("vst" is (n_local, m)) plus
+    "collectives": 2 with given size factors, 4 with given normalization factors (+ their check and the xim sums),
+    11 with estimated size factors, 12 with avgTxLength (the estimate and the xim sums); with a frozen
+    dispersionFunction and blind=False 0, 1 or 9 (given size factors, given normalization factors, an estimate).  Given
+    normalization factors that fail their check on one rank raise ValueError on every rank."""
+    from . import device_pipeline as DP
+    refit = blind or dispersionFunction is None
+    if refit:
+        if not blind and x is None:
+            raise ValueError("blind=False needs the design x or a dispersionFunction")
+        DP._check_vst_fit_type(fitType)
+        x = DP._vst_design(x, m, blind)
+    sizeFactors, nf, sfd, n = _sharded_factors(y_local, m, sizeFactors, normalizationFactors, avgTxLength)
+    if refit:
+        pg = PackedGather(y_local.shape[0], y_local.device)
+        idx = torch.nonzero(y_local[:, :m].sum(dim=1) != 0).squeeze(1)
+        whole = idx.numel() == y_local.shape[0]
+        ynz = y_local if whole else y_local[idx].contiguous()
+        nfz = None if nf is None else (nf if whole else nf[idx].contiguous())
+        xim = None if nf is None else gathered_xim(nfz, m, pg)
+        bm, dge = pg(list(_gene_wise(ynz, x, sizeFactors, nfz, xim)))
+        dispersionFunction = DP.dispersion_function_of(bm, dge, fitType)
+        n += pg.collectives
+    res = DP._vst_result(y_local, m, dispersionFunction, sizeFactors, nf, sfd)
+    res["collectives"] = n
+    return res
+
+
+def sharded_vst_device(y_local, m, x=None, blind=True, nsub=1000, fitType="parametric", sizeFactors=None,
+                       normalizationFactors=None, avgTxLength=None):
+    """device_pipeline.vst_device (R/vst.R:219-267) over the genes of ALL ranks, for this rank's rows y_local
+    (gene-major, split as shard_bounds splits them).  Factors as in sharded_varianceStabilizingTransformation_device.
+    ONE packed all-gather brings every row's baseMean (1 double per gene); every rank then picks the same subset as
+    vst_device: the rows with baseMean > 5 in a stable sort of baseMean (ties in global row order) at
+    pipeline.vstSubsetPositions.  Each rank runs GeneEst on its rows of the subset, ONE more packed all-gather brings
+    (baseMean, dispGeneEst) of all of them, and they are put back into vst_device's fit order before the trend fit (with
+    normalization factors xim is over the subset rows of all ranks: one more all-gather).  R's two stops (fewer than
+    nsub rows; fewer than nsub rows with mean > 5) are decided from the gathered baseMean and raise ValueError on every
+    rank.  Returns the single-device dict for this shard's rows plus "subset" (global row indices, in fit order) and
+    "collectives": 3 with given size factors, 5 with given normalization factors (+ their check and the xim sums),
+    12 with estimated size factors, 13 with avgTxLength (the estimate and the xim sums)."""
+    from . import device_pipeline as DP
+    from .pipeline import vstSubsetPositions
+    if not blind and x is None:
+        raise ValueError("blind=False needs the design x")
+    DP._check_vst_fit_type(fitType)
+    x = DP._vst_design(x, m, blind)
+    sizeFactors, nf, sfd, n = _sharded_factors(y_local, m, sizeFactors, normalizationFactors, avgTxLength)
+    dev = y_local.device
+    pg = PackedGather(y_local.shape[0], dev)
+    bm_local = DP.prep(y_local, np.ones((m, 1)), sizeFactors, want_mu=False, want_beta0=False,
+                       normalizationFactors=nf, xim=1.0)["baseMean"] if y_local.shape[0] else \
+        torch.empty(0, dtype=torch.float64, device=dev)
+    bm = pg(bm_local)
+    if bm.numel() < nsub:
+        raise ValueError("less than 'nsub' rows, it is recommended to use varianceStabilizingTransformation directly")
+    cand = torch.nonzero(bm > 5).squeeze(1)
+    L = cand.numel()
+    if L < nsub:
+        raise ValueError("less than 'nsub' rows with mean normalized count > 5, it is recommended to use "
+                         "varianceStabilizingTransformation directly")
+    _, o = torch.sort(bm[cand], stable=True)
+    subset = cand[o[torch.as_tensor(vstSubsetPositions(L, nsub), device=dev)]]
+    ends = torch.as_tensor(np.cumsum(pg.sizes), device=dev)
+    owner = torch.searchsorted(ends, subset, right=True)             # the rank of each subset row, in fit order
+    lo = int(ends[dist.get_rank()] - pg.sizes[dist.get_rank()])
+    mine = torch.nonzero(owner == dist.get_rank()).squeeze(1)        # this rank's fit positions, ascending
+    rows = subset[mine] - lo
+    ysub = y_local[rows].contiguous()
+    nfsub = None if nf is None else nf[rows].contiguous()
+    # every rank knows every rank's subset count: the GeneEst gather is sized for the subset, not the shard
+    pg_sub = PackedGather(rows.numel(), dev, cap=int(torch.bincount(owner, minlength=pg.world).max()))
+    xim = None if nf is None else gathered_xim(nfsub, m, pg_sub)
+    g_bm, g_dge = pg_sub(list(_gene_wise(ysub, x, sizeFactors, nfsub, xim)))
+    fit_order = torch.sort(owner, stable=True)[1]                   # the fit position of each gathered entry
+    bm_fit, dge_fit = torch.empty_like(g_bm), torch.empty_like(g_dge)
+    bm_fit[fit_order], dge_fit[fit_order] = g_bm, g_dge
+    res = DP._vst_result(y_local, m, DP.dispersion_function_of(bm_fit, dge_fit, fitType), sizeFactors, nf, sfd)
+    res["subset"] = subset
+    res["collectives"] = n + pg.collectives + pg_sub.collectives
+    return res
+
+
+def sharded_normTransform_device(y_local, m, sizeFactors=None, normalizationFactors=None, pc=1.0):
+    """device_pipeline.normTransform_device (R/helper.R:421-435) for this rank's rows y_local: size factors, when neither
+    they nor normalizationFactors (this shard's rows) are given, from sharded_size_factors_device; the transform is
+    local.  Returns {"normTransform": (n_local, m) device tensor, "sizeFactors" or "normalizationFactors",
+    "collectives": 0, 1 with given normalizationFactors (their check), or 9 for an estimate}.  Given
+    normalizationFactors that fail their check on one rank raise ValueError on every rank (in the transforms too)."""
+    from . import device_pipeline as DP
+    sizeFactors, nf, sfd, n = _sharded_factors(y_local, m, sizeFactors, normalizationFactors, None)
+    out = {"normTransform": DP.transform(y_local, m, "log2", pc, 0.0, sfd), "collectives": n}
+    if nf is not None:
+        out["normalizationFactors"] = nf
+    else:
+        out["sizeFactors"] = sizeFactors
     return out

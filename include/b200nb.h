@@ -200,7 +200,10 @@ int b200nb_cooks_nf_dev(const void* y, int y_type, const double* mu, const doubl
  * size_factors[m] are outputs; scratch_gm (n x ld doubles) and scratch_cm (n x m doubles) are caller-provided device
  * scratch; n_finite (device int) receives the number of genes with a finite log geometric mean -- R stops with
  * "every gene contains at least one zero" when it is 0, the caller must do the same.  A sample with no usable
- * ratio gets NaN (median of an empty set is NA in R). */
+ * ratio gets NaN (median of an empty set is NA in R).  scratch_cm is also an output: on return it holds the log
+ * ratios log K_ij - loggeomean_i the median is taken over, column-major (sample j at scratch_cm + j n), +Inf where an
+ * entry does not take part; the gene-sharded estimator takes the median over every rank's ratios from it.  The same
+ * holds for b200nb_size_factors_norm_dev below. */
 int b200nb_size_factors_dev(const void* y, int y_type, int poscounts, int n, int m, long long ld,
                             double* loggeomeans, double* scratch_gm, double* scratch_cm, double* size_factors,
                             int32_t* n_finite, void* stream);
