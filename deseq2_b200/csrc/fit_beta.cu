@@ -40,7 +40,9 @@ constexpr int pow2_ceil_b(int n) { int p = 1; while (p < n) p <<= 1; return p; }
 // Four samples per lane per trip (clamped index + validity factor) for instruction-level parallelism.
 // GL = lanes per gene: 32 (one warp per gene) or 16 / 8 (fit_beta_grp.cuh; `lane` is then the lane index
 // inside the group and the reduction stays inside the group).
-template <int P, bool USE_W, int GL = 32>
+// IND: indicator design (smallp.cuh): x_0 b_0 leaves the sample loop, no w x_0 product, and the (a, a) X'WX sums come
+// from the (a, 0) sums.
+template <int P, bool USE_W, int GL = 32, bool IND = false>
 __device__ __forceinline__ void beta_pass(const BetaRow& rv, const double (&beta)[P], double alpha, double r,
                                           double log_alpha, double minmu, double log_minmu, int lane, double& dev_var,
                                           SymP<P>& XtWX, double (&XtWz)[P]) {
@@ -50,6 +52,7 @@ __device__ __forceinline__ void beta_pass(const BetaRow& rv, const double (&beta
 #pragma unroll
   for (int i = 0; i < NA; i++) acc[i] = 0.0;
   const int mlast = rv.m - 1;
+  const double eta0 = fma(1.0, beta[0], 0.0);   // IND: the first term of every sample's eta
   for (int j0 = lane; j0 < rv.m; j0 += 4 * GL) {
 #pragma unroll
     for (int u = 0; u < 4; u++) {
@@ -58,12 +61,10 @@ __device__ __forceinline__ void beta_pass(const BetaRow& rv, const double (&beta
       const int j = min(jr, mlast);
       double vw = (jr < rv.m) ? 1.0 : 0.0;
       double xv[P];
-      double eta = 0.0;
+      load_design_row<P, IND>(rv.x, rv.mpad, j, xv);
+      double eta = IND ? eta0 : 0.0;
 #pragma unroll
-      for (int k = 0; k < P; k++) {
-        xv[k] = rv.x[k * rv.mpad + j];
-        eta = fma(xv[k], beta[k], eta);
-      }
+      for (int k = IND ? 1 : 0; k < P; k++) eta = fma(xv[k], beta[k], eta);
       const double lnf = rv.lnf[j];
       const double le = eta + lnf;
       // fmax(NaN, minmu) = minmu, as in the reference (:326); huge |eta| takes libm's exp for inf / 0
@@ -88,12 +89,16 @@ __device__ __forceinline__ void beta_pass(const BetaRow& rv, const double (&beta
 #pragma unroll
       for (int a = 0; a < P; a++) {
         acc[1 + NS + a] = fma(wz, xv[a], acc[1 + NS + a]);
-        const double wx = w * xv[a];
+        const double wx = (IND && a == 0) ? w : w * xv[a];
 #pragma unroll
-        for (int b = 0; b <= a; b++) acc[1 + a * (a + 1) / 2 + b] = fma(wx, xv[b], acc[1 + a * (a + 1) / 2 + b]);
+        for (int b = 0; b <= a; b++) {
+          if (IND && b == a && a > 0) continue;
+          acc[1 + a * (a + 1) / 2 + b] = fma(wx, xv[b], acc[1 + a * (a + 1) / 2 + b]);
+        }
       }
     }
   }
+  fill_diag_from_col0<P, IND>(acc + 1);
   if constexpr (GL == 32) {
     warp_allreduce_sum_rs<NA>(acc, lane);
   } else if constexpr (NA <= GL) {
@@ -158,7 +163,7 @@ __device__ __forceinline__ double deviance_const(const BetaArgs& A, const BetaRo
 
 // post-loop block (src/DESeq2.cpp:429-455): hat diagonal, sandwich variance, contrast and the stores of gene g.  XtWX
 // belongs to the mu currently in shared memory.  Every lane of the group computes; `valid` false stores nothing.
-template <int P, bool USE_W, int GL>
+template <int P, bool USE_W, int GL, bool IND>
 __device__ __forceinline__ void beta_finish(const BetaArgs& A, unsigned int g, bool valid, int lg, const BetaRow& rv,
                                             const SymP<P>& XtWX, const double (&lam)[P], const double (&contrast)[P],
                                             const double (&beta)[P], double alpha, const IrlsProgress& ir) {
@@ -189,14 +194,14 @@ __device__ __forceinline__ void beta_finish(const BetaArgs& A, unsigned int g, b
         double w = mu * rcp_fast(fma(alpha, mu, 1.0));
         if (USE_W) w *= rv.w[j];
         double xv[P];
-#pragma unroll
-        for (int k = 0; k < P; k++) xv[k] = rv.x[k * rv.mpad + j];
+        load_design_row<P, IND>(rv.x, rv.mpad, j, xv);
         double q = 0.0;
 #pragma unroll
         for (int a = 0; a < P; a++) {
-          q = fma(xv[a] * xv[a], Ainv.get(a, a), q);
+          q = fma(design_prod<P, IND>(xv, a, a), Ainv.get(a, a), q);
 #pragma unroll
-          for (int b = 0; b < a; b++) q = fma(2.0 * xv[a] * xv[b], Ainv.get(a, b), q);
+          for (int b = 0; b < a; b++)
+            q = fma(IND ? 2.0 * design_prod<P, IND>(xv, a, b) : 2.0 * xv[a] * xv[b], Ainv.get(a, b), q);
         }
         A.hat_diag[off + j] = w * q;
       }
@@ -241,9 +246,10 @@ __device__ __forceinline__ void beta_finish(const BetaArgs& A, unsigned int g, b
 #define NB_LB_THREADS 256
 #define NB_LB_CTAS 2
 #endif
-template <int P, bool USE_W>
+template <int P, bool USE_W, bool IND>
 __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_beta_kernel(const BetaArgs A, int warps_per_cta, int mpad) {
   extern __shared__ __align__(16) double smem[];
+  if (indicator_design<P>(A.x, A.m) != IND) return;   // the other variant of the launch fits this design
   init_log_table();
   init_lfact_table();
   const int lane = threadIdx.x & 31;
@@ -310,10 +316,10 @@ __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_beta_kernel(con
         for (int k = 0; k < P; k++) big = big || (fabs(beta[k]) > kBetaLarge);
         if (big) { ir.diverged(A.maxit); break; }
       }
-      beta_pass<P, USE_W>(rv, beta, alpha, r, log_alpha, minmu, log_minmu, lane, dv, XtWX, XtWz);
+      beta_pass<P, USE_W, 32, IND>(rv, beta, alpha, r, log_alpha, minmu, log_minmu, lane, dv, XtWX, XtWz);
       if (t >= 0 && ir.stop_after_pass(dv, devc, A)) break;
     }
-    beta_finish<P, USE_W, 32>(A, g, true, lane, rv, XtWX, lam, contrast, beta, alpha, ir);
+    beta_finish<P, USE_W, 32, IND>(A, g, true, lane, rv, XtWX, lam, contrast, beta, alpha, ir);
     __syncwarp();
   }
 }
@@ -327,13 +333,17 @@ cudaError_t launch_beta_grp(const BetaArgs& a, int mpad, size_t fixed, size_t ro
   const size_t gsmem = fixed + (size_t)GW * NG * rowbytes;
   launched = false;
   if (gsmem > (size_t)227 * 1024 / GrpShape<GL>::ctas) return cudaSuccess;
-  auto kg = fit_beta_grp_kernel<P, USE_W, GL>;
-  unsigned grid = 0;
-  const cudaError_t e = persistent_grid(reinterpret_cast<const void*>(kg), GrpShape<GL>::threads, gsmem, GW * NG, a.n, &grid);
-  if (e != cudaSuccess) return e;
-  kg<<<grid, GrpShape<GL>::threads, gsmem, stream>>>(a, mpad);
+  for (int ind = 0; ind < 2; ind++) {   // both design variants: the one that does not fit the design returns at once
+    auto kg = ind ? fit_beta_grp_kernel<P, USE_W, GL, true> : fit_beta_grp_kernel<P, USE_W, GL, false>;
+    unsigned grid = 0;
+    cudaError_t e = persistent_grid(reinterpret_cast<const void*>(kg), GrpShape<GL>::threads, gsmem, GW * NG, a.n, &grid);
+    if (e != cudaSuccess) return e;
+    kg<<<grid, GrpShape<GL>::threads, gsmem, stream>>>(a, mpad);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
   launched = true;
-  return cudaGetLastError();
+  return cudaSuccess;
 }
 
 // shared memory of the small-p IRLS kernels: the staged design and the log size-factor row (P + 1 rows of mpad) once
@@ -362,7 +372,6 @@ cudaError_t launch_beta_t(const BetaArgs& a, cudaStream_t stream) {
   while (warps > 1 && fixed + warps * rowbytes > smem_cap / 2) warps >>= 1;
   if (fixed + warps * rowbytes > kBetaSmemCapOneWarp) return cudaErrorInvalidValue;   // callers check fit_beta_smallp_fits
   const size_t smem = fixed + warps * rowbytes;
-  auto kern = fit_beta_kernel<P, USE_W>;
   cudaError_t e = cudaMemsetAsync(a.counter, 0, sizeof(unsigned int), stream);
   if (e != cudaSuccess) return e;
   {
@@ -372,11 +381,16 @@ cudaError_t launch_beta_t(const BetaArgs& a, cudaStream_t stream) {
     else if (gl == 16) e = launch_beta_grp<P, USE_W, 16>(a, mpad, fixed, rowbytes, stream, launched);
     if (e != cudaSuccess || launched) return e;
   }
-  unsigned grid = 0;
-  e = persistent_grid(reinterpret_cast<const void*>(kern), warps * 32, smem, warps, a.n, &grid);
-  if (e != cudaSuccess) return e;
-  kern<<<grid, warps * 32, smem, stream>>>(a, warps, mpad);
-  return cudaGetLastError();
+  for (int ind = 0; ind < 2; ind++) {   // both design variants, as in launch_beta_grp
+    auto kern = ind ? fit_beta_kernel<P, USE_W, true> : fit_beta_kernel<P, USE_W, false>;
+    unsigned grid = 0;
+    e = persistent_grid(reinterpret_cast<const void*>(kern), warps * 32, smem, warps, a.n, &grid);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, warps * 32, smem, stream>>>(a, warps, mpad);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 template <bool USE_W>

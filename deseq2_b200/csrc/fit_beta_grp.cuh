@@ -41,9 +41,12 @@ inline int group_lanes_beta(int m) {
   return m <= 40 ? 8 : 16;
 }
 
-template <int P, bool USE_W, int GL>
+// IND: the variant for indicator designs (smallp.cuh); both variants are launched, and the one that does not fit the
+// design returns at once.
+template <int P, bool USE_W, int GL, bool IND>
 __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit_beta_grp_kernel(const BetaArgs A, int mpad) {
   extern __shared__ __align__(16) double smem[];
+  if (indicator_design<P>(A.x, A.m) != IND) return;
   init_log_table();
   init_lfact_table();
   constexpr int NG = 32 / GL;
@@ -137,7 +140,7 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
       SymP<P> XtWX_new;
       double XtWz_new[P];
       double dv;
-      beta_pass<P, USE_W, GL>(rv, bev, alpha, r, log_alpha, minmu, log_minmu, lg, dv, XtWX_new, XtWz_new);
+      beta_pass<P, USE_W, GL, IND>(rv, bev, alpha, r, log_alpha, minmu, log_minmu, lg, dv, XtWX_new, XtWz_new);
       if (active) {
         XtWX = XtWX_new;
 #pragma unroll
@@ -151,7 +154,7 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
       }
     }
 
-    beta_finish<P, USE_W, GL>(A, g, valid, lg, rv, XtWX, lam, contrast, beta, alpha, ir);
+    beta_finish<P, USE_W, GL, IND>(A, g, valid, lg, rv, XtWX, lam, contrast, beta, alpha, ir);
     __syncwarp();
   }
 }

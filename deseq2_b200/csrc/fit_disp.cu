@@ -54,7 +54,8 @@ constexpr int pow2_ceil(int n) { int p = 1; while (p < n) p <<= 1; return p; }
 // One fused pass: lp (and dlp when WANT_D) at log-alpha `a`.
 // GL = lanes per gene: 32 (one warp per gene) or 16 / 8 (two / four genes per warp, fit_disp_grp.cuh) with
 // `lane` the lane index inside the group; reductions then stay inside the group.
-template <int P, bool USE_W, bool WANT_D, int MODE, int GL = 32>
+// IND: indicator design (smallp.cuh): no design products, the (a, a) Cox-Reid sums come from the (a, 0) sums.
+template <int P, bool USE_W, bool WANT_D, int MODE, int GL = 32, bool IND = false>
 __device__ __forceinline__ void disp_eval_mode(const DispRow& rv, const DispScal& sc, double a, double pm,
                                                double sum_wy, int lane, double& lp, double& dlp) {
   constexpr int NS = SymP<P>::N;
@@ -116,13 +117,13 @@ __device__ __forceinline__ void disp_eval_mode(const DispRow& rv, const DispScal
       if (sc.use_cr) {
         const double dwd = -wdm * wd;
         double xv[P];
-#pragma unroll
-        for (int k = 0; k < P; k++) xv[k] = rv.x[k * rv.mpad + j];
+        load_design_row<P, IND>(rv.x, rv.mpad, j, xv);
 #pragma unroll
         for (int aa = 0; aa < P; aa++)
 #pragma unroll
           for (int bb = 0; bb <= aa; bb++) {
-            const double xx = xv[aa] * xv[bb];
+            if (IND && bb == aa && aa > 0) continue;
+            const double xx = design_prod<P, IND>(xv, aa, bb);
             const int q = aa * (aa + 1) / 2 + bb;
             acc[2 + q] = fma(wdm, xx, acc[2 + q]);
             if (WANT_D) acc[2 + NS + q] = fma(dwd, xx, acc[2 + NS + q]);
@@ -130,6 +131,8 @@ __device__ __forceinline__ void disp_eval_mode(const DispRow& rv, const DispScal
       }
     }
   }
+  fill_diag_from_col0<P, IND>(acc + 2);
+  if (WANT_D) fill_diag_from_col0<P, IND>(acc + 2 + NS);
   if constexpr (GL == 32) warp_allreduce_sum_rs<NA>(acc, lane);
   else if constexpr (NA <= GL) group_allreduce_sum_rs<NA, GL>(acc, lane);
   else group_allreduce_sum_n<NA, GL>(acc);
@@ -166,7 +169,7 @@ __device__ __forceinline__ void disp_eval_mode(const DispRow& rv, const DispScal
 
 // second derivative at `a` (once per gene): src/DESeq2.cpp:111-158.  In TAB mode the digamma / trigamma
 // differences come from the factor table: psi(y+r)-psi(r) = sum_{k<y} 1/(r+k), psi'(y+r)-psi'(r) = -sum 1/(r+k)^2.
-template <int P, bool USE_W, int GL = 32>
+template <int P, bool USE_W, int GL = 32, bool IND = false>
 __device__ __forceinline__ double disp_d2(const DispRow& rv, const DispScal& sc, int mode, double a, int lane) {
   constexpr int NS = SymP<P>::N;
   const double alpha = exp_fast(a);   // a is confined to [-30, 10] by the line search / grid
@@ -216,13 +219,13 @@ __device__ __forceinline__ double disp_d2(const DispRow& rv, const DispScal& sc,
       const double dwd = -wdm * wd;
       const double d2wd = 2.0 * wdm * wd * wd;
       double xv[P];
-#pragma unroll
-      for (int k = 0; k < P; k++) xv[k] = rv.x[k * rv.mpad + j];
+      load_design_row<P, IND>(rv.x, rv.mpad, j, xv);
 #pragma unroll
       for (int aa = 0; aa < P; aa++)
 #pragma unroll
         for (int bb = 0; bb <= aa; bb++) {
-          const double xx = xv[aa] * xv[bb];
+          if (IND && bb == aa && aa > 0) continue;
+          const double xx = design_prod<P, IND>(xv, aa, bb);
           const int q = aa * (aa + 1) / 2 + bb;
           acc[2 + q] = fma(wdm, xx, acc[2 + q]);
           acc[2 + NS + q] = fma(dwd, xx, acc[2 + NS + q]);
@@ -230,6 +233,8 @@ __device__ __forceinline__ double disp_d2(const DispRow& rv, const DispScal& sc,
         }
     }
   }
+#pragma unroll
+  for (int i = 0; i < 3; i++) fill_diag_from_col0<P, IND>(acc + 2 + i * NS);
   group_allreduce_sum_n<2 + 3 * NS, GL>(acc);
   double cr2 = 0.0, dcr = 0.0;
   if (sc.use_cr) {
@@ -425,7 +430,7 @@ __device__ __forceinline__ void build_table(const DispWarpSmem& S, int m, int lg
 
 // the line search of one gene (deseq_rules.cuh::DispLineSearch) with a single evaluation site; t = -1 is the
 // evaluation at the starting point, t >= 0 are the proposals
-template <int P, bool USE_W, int MODE>
+template <int P, bool USE_W, int MODE, bool IND>
 __device__ __forceinline__ void line_search_gene(const DispArgs& A, const DispRow& rv, const DispScal& sc,
                                                  unsigned int g, double sum_wy, int lane) {
   const double pm = A.prior_mean[g];
@@ -433,10 +438,10 @@ __device__ __forceinline__ void line_search_gene(const DispArgs& A, const DispRo
   for (int t = -1; t < A.maxit; t++) {
     const double a_new = ls.propose();
     double lp_new, dlp_new;
-    disp_eval_mode<P, USE_W, true, MODE>(rv, sc, a_new, pm, sum_wy, lane, lp_new, dlp_new);
+    disp_eval_mode<P, USE_W, true, MODE, 32, IND>(rv, sc, a_new, pm, sum_wy, lane, lp_new, dlp_new);
     if (ls.take(lp_new, dlp_new, A)) break;
   }
-  const double d2 = disp_d2<P, USE_W>(rv, sc, MODE, ls.a, lane);
+  const double d2 = disp_d2<P, USE_W, 32, IND>(rv, sc, MODE, ls.a, lane);
   if (lane == 0) ls.store(A, g, d2);
 }
 
@@ -444,9 +449,10 @@ __device__ __forceinline__ void line_search_gene(const DispArgs& A, const DispRo
 #define NB_LB_THREADS 256
 #define NB_LB_CTAS 2
 #endif
-template <int P, bool USE_W>
+template <int P, bool USE_W, bool IND>
 __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_disp_kernel(const DispArgs A, int warps_per_cta, int mpad) {
   extern __shared__ __align__(16) double smem[];
+  if (indicator_design<P>(A.x, A.m) != IND) return;   // the other variant of the launch fits this design
   init_log_table();
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -483,11 +489,11 @@ __global__ void __launch_bounds__(NB_LB_THREADS, NB_LB_CTAS) fit_disp_kernel(con
     if (mode == MODE_TAB) {
       build_table<USE_W, 32>(S, A.m, lane);
       rv.ntab = (int)ymax;
-      line_search_gene<P, USE_W, MODE_TAB>(A, rv, sc, g, sum_wy, lane);
+      line_search_gene<P, USE_W, MODE_TAB, IND>(A, rv, sc, g, sum_wy, lane);
     } else if (mode == MODE_BIG) {
-      line_search_gene<P, USE_W, MODE_BIG>(A, rv, sc, g, sum_wy, lane);
+      line_search_gene<P, USE_W, MODE_BIG, IND>(A, rv, sc, g, sum_wy, lane);
     } else {
-      line_search_gene<P, USE_W, MODE_GEN>(A, rv, sc, g, sum_wy, lane);
+      line_search_gene<P, USE_W, MODE_GEN, IND>(A, rv, sc, g, sum_wy, lane);
     }
     __syncwarp();
   }
@@ -533,7 +539,8 @@ __global__ void __launch_bounds__(256, 2) fit_disp_grid_kernel(const DispArgs A,
   }
 }
 
-// launch the GL-lanes-per-gene experiment kernel if its shared-memory slices fit; `launched` tells
+// launch the GL-lanes-per-gene kernel if its shared-memory slices fit; `launched` tells.  Both design variants are
+// launched (the design lives on the device): the general one returns at once on an indicator design, and vice versa.
 template <int P, bool USE_W, int GL>
 cudaError_t launch_disp_grp(const DispArgs& a, int mpad, size_t xbytes, size_t rowbytes, cudaStream_t stream,
                             bool& launched) {
@@ -541,13 +548,17 @@ cudaError_t launch_disp_grp(const DispArgs& a, int mpad, size_t xbytes, size_t r
   const size_t gsmem = xbytes + (size_t)GW * NG * rowbytes;
   launched = false;
   if (gsmem > (size_t)227 * 1024 / GrpShape<GL>::ctas) return cudaSuccess;
-  auto kg = fit_disp_grp_kernel<P, USE_W, GL>;
-  unsigned grid = 0;
-  const cudaError_t e = persistent_grid(reinterpret_cast<const void*>(kg), GrpShape<GL>::threads, gsmem, GW * NG, a.n, &grid);
-  if (e != cudaSuccess) return e;
-  kg<<<grid, GrpShape<GL>::threads, gsmem, stream>>>(a, mpad);
+  for (int ind = 0; ind < 2; ind++) {
+    auto kg = ind ? fit_disp_grp_kernel<P, USE_W, GL, true> : fit_disp_grp_kernel<P, USE_W, GL, false>;
+    unsigned grid = 0;
+    cudaError_t e = persistent_grid(reinterpret_cast<const void*>(kg), GrpShape<GL>::threads, gsmem, GW * NG, a.n, &grid);
+    if (e != cudaSuccess) return e;
+    kg<<<grid, GrpShape<GL>::threads, gsmem, stream>>>(a, mpad);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
   launched = true;
-  return cudaGetLastError();
+  return cudaSuccess;
 }
 
 // shared memory of the small-p kernels: the staged design (P rows of mpad) once per CTA, and per warp (or lane group)
@@ -614,11 +625,15 @@ cudaError_t launch_disp_t(const DispArgs& a0, cudaStream_t stream) {
   if (gl == 8) e = launch_disp_grp<P, USE_W, 8>(a, mpad, xbytes, rowbytes, stream, launched);
   else if (gl == 16) e = launch_disp_grp<P, USE_W, 16>(a, mpad, xbytes, rowbytes, stream, launched);
   if (e != cudaSuccess || launched) return e;
-  auto kern = fit_disp_kernel<P, USE_W>;
-  e = persistent_grid(reinterpret_cast<const void*>(kern), warps * 32, smem, warps, a.n, &grid);
-  if (e != cudaSuccess) return e;
-  kern<<<grid, warps * 32, smem, stream>>>(a, warps, mpad);
-  return cudaGetLastError();
+  for (int ind = 0; ind < 2; ind++) {   // both design variants, as in launch_disp_grp
+    auto kern = ind ? fit_disp_kernel<P, USE_W, true> : fit_disp_kernel<P, USE_W, false>;
+    e = persistent_grid(reinterpret_cast<const void*>(kern), warps * 32, smem, warps, a.n, &grid);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, warps * 32, smem, stream>>>(a, warps, mpad);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 template <bool USE_W>

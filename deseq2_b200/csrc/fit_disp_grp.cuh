@@ -49,7 +49,7 @@ inline int group_lanes_disp(int m) {
 
 // One round of the line search for the NG genes a warp holds (deseq_rules.cuh::DispLineSearch), warp-uniform control
 // flow: a group whose gene has stopped, or that got no gene, evaluates at its frozen a until every group is done.
-template <int P, bool USE_W, int MODE, int GL>
+template <int P, bool USE_W, int MODE, int GL, bool IND>
 __device__ __forceinline__ void line_search_round(const DispArgs& A, const DispRow& rv, const DispScal& sc,
                                                   unsigned int g, bool valid, double sum_wy, int lg) {
   const double pm = valid ? A.prior_mean[g] : 0.0;
@@ -58,19 +58,21 @@ __device__ __forceinline__ void line_search_round(const DispArgs& A, const DispR
   while (__any_sync(0xffffffffu, active)) {
     const double a_new = active ? ls.propose() : ls.a;
     double lp_new, dlp_new;
-    disp_eval_mode<P, USE_W, true, MODE, GL>(rv, sc, a_new, pm, sum_wy, lg, lp_new, dlp_new);
+    disp_eval_mode<P, USE_W, true, MODE, GL, IND>(rv, sc, a_new, pm, sum_wy, lg, lp_new, dlp_new);
     // the reference's `for (t = 0; t < maxit; t++)` bounds the proposals
     if (active) active = !ls.take(lp_new, dlp_new, A) && ls.it < A.maxit;
   }
-  const double d2 = disp_d2<P, USE_W, GL>(rv, sc, MODE, ls.a, lg);
+  const double d2 = disp_d2<P, USE_W, GL, IND>(rv, sc, MODE, ls.a, lg);
   if (valid && lg == 0) ls.store(A, g, d2);
 }
 
 // One kernel for the three evaluation-mode families, one family after the other, each with its own queue counter
-// (scratch[0], [4], [5]) so that all groups of a warp always run the same MODE code.
-template <int P, bool USE_W, int GL>
+// (scratch[0], [4], [5]) so that all groups of a warp always run the same MODE code.  IND: the variant for indicator
+// designs (smallp.cuh); both variants are launched, and the one that does not fit the design returns at once.
+template <int P, bool USE_W, int GL, bool IND>
 __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit_disp_grp_kernel(const DispArgs A, int mpad) {
   extern __shared__ __align__(16) double smem[];
+  if (indicator_design<P>(A.x, A.m) != IND) return;
   init_log_table();
   constexpr int NG = 32 / GL;
   const int lane = threadIdx.x & 31;
@@ -112,11 +114,11 @@ __global__ void __launch_bounds__(GrpShape<GL>::threads, GrpShape<GL>::ctas) fit
       if (mode == MODE_TAB) {
         build_table<USE_W, GL>(S, A.m, lg);
         rv.ntab = valid ? (int)ymax : 0;
-        line_search_round<P, USE_W, MODE_TAB, GL>(A, rv, sc, g, valid, sum_wy, lg);
+        line_search_round<P, USE_W, MODE_TAB, GL, IND>(A, rv, sc, g, valid, sum_wy, lg);
       } else if (mode == MODE_BIG) {
-        line_search_round<P, USE_W, MODE_BIG, GL>(A, rv, sc, g, valid, sum_wy, lg);
+        line_search_round<P, USE_W, MODE_BIG, GL, IND>(A, rv, sc, g, valid, sum_wy, lg);
       } else {
-        line_search_round<P, USE_W, MODE_GEN, GL>(A, rv, sc, g, valid, sum_wy, lg);
+        line_search_round<P, USE_W, MODE_GEN, GL, IND>(A, rv, sc, g, valid, sum_wy, lg);
       }
       __syncwarp();
     }

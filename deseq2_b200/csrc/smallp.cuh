@@ -20,6 +20,50 @@ struct SymP {
   }
 };
 
+// ---------------------------------------------------------------- indicator designs
+// A design whose column 0 is all 1.0 and whose other entries are all +0.0 or 1.0 (a factor design with an intercept:
+// ~condition, ~batch + condition) makes every design product exact and predictable: x_a x_0 = x_a, x_a x_a = x_a,
+// and x_a x_b is the AND of the two high words (1.0 = 0x3FF00000'00000000).  Each small-p kernel comes in two
+// variants, both launched; each tests the design as it starts, and only the one that fits it runs.  The indicator
+// variant forms the products without FP64 multiplies and takes the (a, a) sums of X'WX-type accumulators from the
+// (a, 0) sums, which receive the same operations in the same order.  Every value is the general path's bit for bit.
+
+// the warp reads the whole m x P design (column-major) from global memory; warp-uniform result.  The kernels call it
+// first thing, so the variant of a launch that does not fit the design returns before any set-up.
+template <int P>
+__device__ __forceinline__ bool indicator_design(const double* x, int m) {
+  bool ok = true;
+  for (int idx = threadIdx.x & 31; idx < P * m; idx += 32) {
+    const long long b = __double_as_longlong(x[idx]);
+    ok = ok && (b == 0x3FF0000000000000LL || (idx >= m && b == 0));
+  }
+  return __all_sync(0xffffffffu, ok);
+}
+
+// design row of sample j; IND: x_0 = 1.0 is not loaded
+template <int P, bool IND>
+__device__ __forceinline__ void load_design_row(const double* xs, int mpad, int j, double (&xv)[P]) {
+  xv[0] = IND ? 1.0 : xs[j];
+#pragma unroll
+  for (int k = 1; k < P; k++) xv[k] = xs[k * mpad + j];
+}
+
+// x_a x_b (b <= a) of a design row; IND: without an FP64 multiply
+template <int P, bool IND>
+__device__ __forceinline__ double design_prod(const double (&xv)[P], int a, int b) {
+  if (!IND) return xv[a] * xv[b];
+  if (b == 0 || b == a) return xv[a];
+  return __hiloint2double(__double2hiint(xv[a]) & __double2hiint(xv[b]), 0);
+}
+
+// IND: the (a, a) entries of a packed accumulator, which the sample loop skips, are the (a, 0) entries
+template <int P, bool IND>
+__device__ __forceinline__ void fill_diag_from_col0(double* acc) {
+  if (!IND) return;
+#pragma unroll
+  for (int a = 1; a < P; a++) acc[a * (a + 1) / 2 + a] = acc[a * (a + 1) / 2];
+}
+
 // in-place Cholesky A = L L' (lower, packed).  Returns false if a pivot is not positive (or NaN).
 template <int P>
 __device__ __forceinline__ bool chol_factor(SymP<P>& A) {
