@@ -1165,7 +1165,7 @@ int b200nb_fit_disp_dev(const void* y, int y_type, const double* x, const double
     }
   }
   CU(nb::launch_fit_disp(a, (cudaStream_t)stream));
-  g_launches += 2;   // classify + line search
+  g_launches += nb::fit_disp_smallp_launches(m);   // classify [+ bucket sort] + both design variants of the line search
   return 0;
 }
 
@@ -1234,7 +1234,7 @@ int b200nb_fit_beta_dev(const void* y, int y_type, const double* x, const double
     }
   }
   CU(nb::launch_fit_beta(a, (cudaStream_t)stream));
-  if (n > 0) g_launches++;
+  if (n > 0) g_launches += 2;   // both design variants
   return 0;
 }
 

@@ -385,6 +385,8 @@ cudaError_t launch_fit_beta(const BetaArgs& a, cudaStream_t stream);
 // Whether one warp of the small-p kernels above fits in shared memory (its sample rows are staged there in full).
 // When it does not, the entry points fit the gene on the general-p kernels, which move long rows to global memory.
 bool fit_disp_smallp_fits(int m, int p, int use_weights);
+// kernels launch_fit_disp launches for a fitDisp call (not fitDispGrid) with m samples; launch_fit_beta launches two
+int fit_disp_smallp_launches(int m);
 // A grow-only device buffer of at least `bytes` from a ring of four (one per launch in flight on a stream): the global
 // rows of the kernels whose per-warp rows do not fit in shared memory (fit_generic.cu)
 cudaError_t row_scratch(size_t bytes, double** out);

@@ -654,6 +654,11 @@ bool fit_disp_smallp_fits(int m, int p, int use_weights) {
   return L.xbytes + L.rowbytes <= kDispSmemCapOneWarp;
 }
 
+int fit_disp_smallp_launches(int m) {
+  // launch_disp_t without a grid: classify_kernel, bucket_sort_kernel at 8 lanes per gene, both design variants
+  return 1 + (group_lanes_disp(m) == 8 ? 1 : 0) + 2;
+}
+
 cudaError_t launch_fit_disp(const DispArgs& a, cudaStream_t stream) {
   if (a.n == 0) return cudaSuccess;
   return a.use_weights ? launch_disp_p<true>(a, stream) : launch_disp_p<false>(a, stream);

@@ -65,6 +65,7 @@ struct Fiber {
   State state;
   unsigned wait_mask;
   unsigned parity;  // number of exchanges done: selects the exchange slot
+  long long ncoll;  // warp collectives (shuffles, votes, __syncwarp) this thread executed
   uint3 tid;
 };
 
@@ -80,6 +81,7 @@ std::vector<unsigned> xtag_store;
 void* dyn_smem = nullptr;
 size_t dyn_smem_cap = 0;
 long long n_launches = 0;
+long long max_coll = 0;   // the most warp collectives any thread of the running launch executed
 
 char* stack_for(size_t i) {
   while (stacks.size() <= i) {
@@ -247,6 +249,7 @@ long long launches() { return n_launches; }
 void barrier_warp(unsigned mask) {
   if (cur < 0) die("warp collective outside a kernel");
   if (!((mask >> lane_id()) & 1u)) die("a thread executes a *_sync collective whose mask does not name it");
+  if (++fibers[cur].ncoll > max_coll) max_coll = fibers[cur].ncoll;
   fibers[cur].state = WAIT_WARP;
   fibers[cur].wait_mask = mask;
   yield_to_scheduler();
@@ -321,21 +324,25 @@ size_t max_dyn_smem(const void* kernel) {
   return kDynSmemDefault;
 }
 
-// one line per launch, "<kernel expression> | <launching function> | <threads> | <dynamic shared bytes>": tests read it to
-// see which kernel a launch plan chose (simt_emu_launch_log)
+// one line per launch, "<kernel expression> | <launching function> | <threads> | <dynamic shared bytes> | <collectives>",
+// where <collectives> is the most warp collectives (shuffles, votes, __syncwarp) any thread of the launch executed (0
+// for a refused launch): tests read it to see which kernel a launch plan chose, and whether a kernel did any work
+// after its entry test (simt_emu_launch_log)
 std::mutex log_mu;
 std::string launch_log;
 
+void log_launch(const char* what, const char* where, dim3 block, size_t dyn_smem_bytes, long long collectives) {
+  std::lock_guard<std::mutex> lk(log_mu);
+  char tail[96];
+  snprintf(tail, sizeof tail, " | %u | %zu | %lld\n", block.x * block.y * block.z, dyn_smem_bytes, collectives);
+  if (launch_log.size() > (1u << 22)) launch_log.clear();   // nobody reads it: keep it bounded
+  launch_log += std::string(what) + " | " + where + tail;
+}
+
 void launch(const void* kernel, dim3 grid, dim3 block, size_t dyn_smem_bytes, const std::function<void()>& kernel_body,
             const char* what, const char* where) {
-  {
-    std::lock_guard<std::mutex> lk(log_mu);
-    char tail[64];
-    snprintf(tail, sizeof tail, " | %u | %zu\n", block.x * block.y * block.z, dyn_smem_bytes);
-    if (launch_log.size() > (1u << 22)) launch_log.clear();   // nobody reads it: keep it bounded
-    launch_log += std::string(what) + " | " + where + tail;
-  }
   if (dyn_smem_bytes > max_dyn_smem(kernel)) {   // refused before it runs, as the runtime refuses it
+    log_launch(what, where, block, dyn_smem_bytes, 0);
     fprintf(stderr, "simt_emu: launch refused: %zu bytes of dynamic shared memory, the kernel may use %zu\n",
             dyn_smem_bytes, max_dyn_smem(kernel));
     t_last_error = cudaErrorInvalidValue;
@@ -348,6 +355,7 @@ void launch(const void* kernel, dim3 grid, dim3 block, size_t dyn_smem_bytes, co
   const int nthreads = (int)(block.x * block.y * block.z);
   if (nthreads <= 0 || nthreads > 1024) die("bad block size");
   n_launches++;
+  max_coll = 0;
   if (dyn_smem_bytes + 64 > dyn_smem_cap) {
     free(dyn_smem);
     dyn_smem_cap = dyn_smem_bytes + 64;
@@ -374,12 +382,14 @@ void launch(const void* kernel, dim3 grid, dim3 block, size_t dyn_smem_bytes, co
           f.state = RUNNABLE;
           f.wait_mask = 0;
           f.parity = 0;
+          f.ncoll = 0;
           f.tid = uint3{(unsigned)i % block.x, ((unsigned)i / block.x) % block.y, (unsigned)i / (block.x * block.y)};
         }
         run_cta(nthreads);
       }
   cur = -1;
   body = nullptr;
+  log_launch(what, where, block, dyn_smem_bytes, max_coll);
 }
 
 }  // namespace simt_emu

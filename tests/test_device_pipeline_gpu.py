@@ -82,10 +82,11 @@ class _MarginOracle:
         return r
 
 
-def test_long_rows_take_the_segmented_kernels(engine, oracle):
+def test_long_rows_take_the_segmented_kernels_in_one_launch(engine, oracle):
     """From m = 400 samples on, the DEVICE entry points run designs with p <= 4 on the segmented general-p kernels
-    (capi.cu::long_rows; the host entry points keep the small-p kernels): one launch instead of classify + line search,
-    switched off by B200NB_LONG_ROWS=0 (read per call), results equal to the small-p kernels' and the oracle's."""
+    (capi.cu::long_rows; the host entry points keep the small-p kernels): one launch instead of classify and the two
+    design variants of the line search, switched off by B200NB_LONG_ROWS=0 (read per call), results equal to the
+    small-p kernels' and the oracle's."""
     import os
     import torch
     from deseq2_b200 import _lib, device as D, synth
@@ -112,7 +113,7 @@ def test_long_rows_take_the_segmented_kernels(engine, oracle):
         small, n_small = disp()
     finally:
         os.environ.pop("B200NB_LONG_ROWS")
-    assert (n_seg, n_small) == (1, 2)
+    assert (n_seg, n_small) == (1, 3)
     od = oracle.fitDisp(**disp_args(c, mu, np.log(c["alpha0"])), with_margin=True)
     same = (seg["iter"] == od["iter"]) & (seg["iter_accept"] == od["iter_accept"])
     assert np.all(same | (od["margin"] <= 64.0))

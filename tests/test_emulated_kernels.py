@@ -133,7 +133,8 @@ DEVICE_CASES = [
     ("DESeq on device ~condition", lambda T, e, o: T.test_device_pipeline_matches_host_pipeline(e, o, "condition", 240, 40)),
     ("DESeq on device ~condition m=6", lambda T, e, o: T.test_device_pipeline_matches_host_pipeline(e, o, "condition", 300, 6)),
     ("DESeq on device ~batch+condition", lambda T, e, o: T.test_device_pipeline_matches_host_pipeline(e, o, "batch", 160, 36)),
-    ("long rows (m >= 400) on the segmented kernels", lambda T, e, o: T.test_long_rows_take_the_segmented_kernels(e, o)),
+    ("long rows (m >= 400) on the segmented kernels in one launch",
+     lambda T, e, o: T.test_long_rows_take_the_segmented_kernels_in_one_launch(e, o)),
     ("LRT on device", lambda T, e: T.test_lrt_device_matches_host(e, n=250)),
     ("optim fallback on device", lambda T, e: T.test_optim_fallback_device_vs_host(e, n=120)),
     ("size factors 700x12", lambda T, e: T.TS.test_size_factors_match_numpy(e, 700, 12, 1, False)),

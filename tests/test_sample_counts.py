@@ -416,7 +416,7 @@ def _route(log):
             "launch_fit_beta_generic", "launch_disp_seg_t", "launch_beta_seg_t")
     out = set()
     for line in log.splitlines():
-        what, where, threads, smem = [s.strip() for s in line.split(" | ")]
+        what, where, threads, smem = [s.strip() for s in line.split(" | ")][:4]   # the fifth field: collectives
         if any(k in where for k in keep) and what != "classify_kernel" and what != "bucket_sort_kernel":
             out.add((what, where, threads, "generic" in where and int(smem) > SMEM - 16 * 1024))
     return out
