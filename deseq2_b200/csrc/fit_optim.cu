@@ -11,8 +11,9 @@
 // objective): exact gradient X'[w (y - mu)/(1 + alpha mu)] - Lambda beta and Hessian
 // -X' diag(w mu (1 + alpha y)/(1 + alpha mu)^2) X - Lambda from one pass over the samples, coordinates sitting on a bound
 // with an outward gradient frozen (active set), the reduced system solved by Cholesky (diagonal damping if it fails),
-// projected back-tracking until the objective increases.  Rows are few (a handful per 50 000 genes), so nothing here is
-// tuned: any p <= kMaxP, the p x p algebra by lane 0 in shared memory.
+// projected back-tracking until the objective increases (the full step when fp64 cannot resolve the gain), stopped
+// when every free gradient entry is below 1e-10 of the size of its terms.  Rows are few (a handful per 50 000 genes),
+// so nothing here is tuned: any p <= kMaxP, the p x p algebra by lane 0 in shared memory.
 #include <math.h>
 
 #include "engine.h"
@@ -32,6 +33,11 @@ __device__ __forceinline__ double sample_y(const OptimArgs& A, size_t off, int j
 
 // objective only (beta-dependent part): sum w (y (eta + log nf) - (y + r) log1p(alpha mu)) - 1/2 sum lambda beta^2
 __device__ double objective(const OptimArgs& A, size_t off, int lane, double alpha, double r, const double* beta) {
+  // every read of beta comes before the warp_sum: once its shuffles are through, lane 0 may already be writing the
+  // next trial point, and a lane reading it after that would return a different f than the others and leave the
+  // back-tracking on its own branch (the warp's later shuffles then mix lanes of different calls)
+  double pen = 0.0;
+  for (int k = 0; k < A.p; k++) pen = fma(A.lambda[k] * beta[k], beta[k], pen);
   double acc = 0.0;
   for (int j = lane; j < A.m; j += 32) {
     double eta = 0.0;
@@ -45,8 +51,6 @@ __device__ double objective(const OptimArgs& A, size_t off, int lane, double alp
     acc += t;
   }
   acc = warp_sum(acc);
-  double pen = 0.0;
-  for (int k = 0; k < A.p; k++) pen = fma(A.lambda[k] * beta[k], beta[k], pen);
   return acc - 0.5 * pen;
 }
 
@@ -61,6 +65,7 @@ __global__ void __launch_bounds__(32) beta_optim_kernel(const OptimArgs A) {
   double* grad = H + (size_t)p * p;  // p
   double* beta = grad + p;           // p
   double* trial = beta + p;          // p
+  double* gscale = trial;            // p: the stop rule's scale of each gradient entry (used before trial is)
   double* step = trial + p;          // p
   double* Lm = step + p;             // p x p: Cholesky factor
   int* active = reinterpret_cast<int*>(Lm + (size_t)p * p);   // p
@@ -105,10 +110,20 @@ __global__ void __launch_bounds__(32) beta_optim_kernel(const OptimArgs A) {
     }
     __syncwarp();
     for (int a = 0; a < p; a++) {
-      double s = 0.0;
-      for (int j = lane; j < A.m; j += 32) s = fma(__ldg(A.x + (size_t)a * A.m + j), ge[j], s);
+      // gradient, and the size of its terms for the stop rule: |g1| + h1 >= w (y + mu) / (2 (1 + alpha mu)), the
+      // magnitude the rounding of y - mu and of the sum is relative to
+      double s = 0.0, sa = 0.0;
+      for (int j = lane; j < A.m; j += 32) {
+        const double xa = __ldg(A.x + (size_t)a * A.m + j);
+        s = fma(xa, ge[j], s);
+        sa = fma(fabs(xa), fabs(ge[j]) + he[j], sa);
+      }
       s = warp_sum(s);
-      if (lane == 0) grad[a] = s - A.lambda[a] * beta[a];
+      sa = warp_sum(sa);
+      if (lane == 0) {
+        grad[a] = s - A.lambda[a] * beta[a];
+        gscale[a] = 1.0 + sa + A.lambda[a] * fabs(beta[a]);
+      }
       for (int b = 0; b <= a; b++) {
         double t = 0.0;
         for (int j = lane; j < A.m; j += 32)
@@ -129,7 +144,7 @@ __global__ void __launch_bounds__(32) beta_optim_kernel(const OptimArgs A) {
       for (int k = 0; k < p; k++) {
         const int act = (beta[k] >= U && grad[k] > 0.0) || (beta[k] <= -U && grad[k] < 0.0);
         active[k] = act;
-        if (!act) pg = fmax(pg, fabs(grad[k]));
+        if (!act) pg = fmax(pg, fabs(grad[k]) / gscale[k]);
       }
       for (int k = 0; k < p; k++)
         if (active[k]) {
@@ -179,7 +194,10 @@ __global__ void __launch_bounds__(32) beta_optim_kernel(const OptimArgs A) {
     pg = __shfl_sync(0xffffffffu, pg, 0);
     __syncwarp();
     if (!ok || !(gdot == gdot)) break;                 // not even the damped system factors: give up (conv = 0)
-    if (pg <= 1e-10 * (1.0 + fabs(f))) { converged = 1; break; }   // projected gradient vanishes
+    // projected gradient vanishes: every free entry below 1e-10 of the size of its own terms.  Relative to the terms,
+    // not to |f|: f is dominated by y (eta + log nf) whatever the fit, so 1e-10 |f| can stop a row of large counts with
+    // its coefficients units away from the maximiser
+    if (pg <= 1e-10) { converged = 1; break; }
     // ---- projected back-tracking
     double t = 1.0, fnew = f;
     bool moved = false;
@@ -188,18 +206,23 @@ __global__ void __launch_bounds__(32) beta_optim_kernel(const OptimArgs A) {
       __syncwarp();
       fnew = objective(A, off, lane, alpha, r, trial);
       if (fnew == fnew && !isinf(fnew) && fnew > f) { moved = true; break; }
-      if (fnew == f) break;                            // flat to rounding: stationary within fp64
+      if (fnew == f && !isinf(f)) break;               // flat to rounding (not two -inf: a start whose means
+                                                       // overflow has f = -inf, and shorter steps reach finite f)
       t *= 0.5;
     }
-    if (!moved) { converged = 1; break; }              // no ascent possible from here within fp64: stationary
-    double dmax = 0.0;
-    for (int k = 0; k < p; k++) dmax = fmax(dmax, fabs(trial[k] - beta[k]));
-    const double df = fnew - f;
+    if (!moved) {
+      // No step length shows an increase: the gain of the Newton step (gdot / 2) is below what the fp64 objective
+      // resolves, yet the gradient test above has not passed.  Near the maximiser the quadratic model is exact to
+      // rounding, so take the full projected step unverified and let the gradient decide (maxit bounds the loop).
+      for (int k = lane; k < p; k += 32) trial[k] = fmin(fmax(beta[k] + step[k], -U), U);
+      __syncwarp();
+      fnew = objective(A, off, lane, alpha, r, trial);
+      if (!(fnew == fnew) || isinf(fnew)) break;       // not even that: give up (conv = 0)
+    }
     __syncwarp();
     for (int k = lane; k < p; k += 32) beta[k] = trial[k];
     __syncwarp();
     f = fnew;
-    if (dmax <= 1e-10 && df <= 1e-13 * (1.0 + fabs(f))) { converged = 1; it++; break; }
   }
   for (int k = lane; k < p; k += 32) A.beta_out[(size_t)g + (size_t)A.n * k] = beta[k];
   if (lane == 0) {
