@@ -39,6 +39,8 @@ DESeq_device(betaPrior=True) (_map_fit), and results_device on it.
 """
 from __future__ import annotations
 
+import math
+
 import numpy as np
 import torch
 
@@ -471,7 +473,15 @@ def getContrast_device(ynz, x, sizeFactors, dispersion, betaMatrix, contrast, be
                    1e-8, 0, useQR=False, minmu=minmu, weights=wn, want_hat=False, want_mu=False)
     est, se = r["contrast_num"] / LN2, r["contrast_denom"] / LN2
     stat = est / se
-    return {"log2FoldChange": est, "lfcSE": se, "stat": stat, "pvalue": 2.0 * torch.special.ndtr(-stat.abs())}
+    return {"log2FoldChange": est, "lfcSE": se, "stat": stat, "pvalue": wald_pvalue(stat)}
+
+
+def wald_pvalue(stat):
+    """R's two-sided normal p-value 2 * pnorm(abs(stat), lower.tail = FALSE) (R/core.R:1507, R/results.R:822) as
+    erfc(|stat| / sqrt 2): relative accuracy of a few ulps plus stat^2 ulps (the rounding of the argument) down to
+    DBL_MIN, subnormal beyond |stat| = 37.5, 1 at 0, 0 at +-inf, NaN at NaN.  torch's ndtr is (1 + erf(x / sqrt 2)) / 2,
+    which cancels: its p-values are multiples of about 1.1e-16 and reach 0 from |stat| = 8.3 on."""
+    return torch.erfc(stat.abs() * 0.7071067811865476)
 
 
 def _size_or_norm_factors(y, m, sizeFactors, normalizationFactors, weights):
@@ -585,11 +595,27 @@ def _lrt_model_fit(ynz, x, sizeFactors, sfd, dispersion, wn, closed_form, betaTo
 
 def _lrt_stats(ll_full, ll_reduced, df):
     """nbinomLRT's LRTStatistic = 2 (logLike_full - logLike_reduced) (R/core.R:1877) and its chi-square upper tail with
-    df degrees of freedom."""
+    df degrees of freedom, pchisq(stat, df, lower.tail = FALSE) (:1878): 1 for a statistic <= 0."""
     stat = 2.0 * (ll_full - ll_reduced)
-    pval = torch.special.gammaincc(torch.tensor(df / 2.0, dtype=F64, device=stat.device),
-                                   torch.clamp(stat, min=0.0) / 2.0)
-    return stat, pval
+    return stat, chisq_upper(stat, df)
+
+
+def chisq_upper(stat, df):
+    """pchisq(stat, df, lower.tail = FALSE) for an integer df >= 1 as Q(df / 2, x), x = max(stat, 0) / 2, by its
+    finite sums of positive terms: Q(k, x) = e^-x sum_{j < k} x^j / j! for even df, and Q(k + 1/2, x) = erfc(sqrt x)
+    + sum_{j = 1..k} e^-x x^(j - 1/2) / Gamma(j + 1/2) for odd df, each term as exp(j log x - x - lgamma).  Nothing
+    cancels, so the relative error is a few ulps plus the rounding of the exponent, about x ulps.  torch's igammac
+    forms Q as 1 - P for small x and loses up to 30 ulps there (DESIGN.md, p-value accuracy).  1 at stat <= 0, 0 at
+    +inf, NaN at NaN."""
+    x = torch.clamp(stat, min=0.0) / 2.0
+    lx = torch.log(x)
+    odd = df % 2 == 1
+    p = torch.erfc(torch.sqrt(x)) if odd else torch.exp(-x)
+    for j in range(1, (df + 1) // 2):
+        a = j - 0.5 if odd else float(j)
+        term = torch.exp(a * lx - x - math.lgamma(a + 1.0))
+        p = p + torch.where(torch.isinf(x), 0.0, term)               # e^-x x^a at x = inf: inf - inf
+    return p
 
 
 def _intercept_only(ynz, sfd, dispersion, wn, m):
@@ -796,7 +822,7 @@ def _wald_stats(fit):
     betaSE = torch.sqrt(torch.clamp(fit["beta_var_mat"], min=0.0)) / LN2
     stat = betaMatrix / betaSE
     return {"betaMatrix": betaMatrix.T, "betaSE": betaSE.T, "WaldStatistic": stat.T,
-            "WaldPvalue": (2.0 * torch.special.ndtr(-stat.abs())).T}
+            "WaldPvalue": wald_pvalue(stat).T}
 
 
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
@@ -1709,10 +1735,7 @@ def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcT
         g = getContrast_device(ycnt, xf, None if nf is not None else res["sizeFactors"], res["dispersion"],
                                res["betaMatrix"], sel["vec"], betaPriorVar=res.get("betaPriorVar"), minmu=minmu,
                                weights=res.get("weights"), normalizationFactors=nf)
-        cols = [g[key].contiguous() for key in ("log2FoldChange", "lfcSE", "stat")]
-        # getContrast's 2 pnorm(|stat|, lower.tail = FALSE) (R/results.R:822) as erfc(|stat| / sqrt 2): torch's ndtr
-        # loses relative accuracy in the far tail on the CPU
-        cols.append(torch.erfc(cols[2].abs() * 0.7071067811865476))
+        cols = [g[key].contiguous() for key in ("log2FoldChange", "lfcSE", "stat", "pvalue")]
     if lrt is not None:
         cols[2], cols[3] = lrt["LRTStatistic"].contiguous(), lrt["LRTPvalue"].contiguous()
     mask = None if sel["mask"] is None else torch.as_tensor(sel["mask"].astype(np.int32), device=dev)

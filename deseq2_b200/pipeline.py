@@ -893,9 +893,16 @@ def fitReducedModel(counts, nf, reduced, dispersion, engine=None, betaTol=1e-8, 
 
 
 def lrtStatistic(logLikeFull, logLikeReduced, df):
-    """LRTStatistic = 2 (logLike_full - logLike_reduced) and its pchisq upper tail (R/core.R:1877-1878)."""
+    """LRTStatistic = 2 (logLike_full - logLike_reduced) and its pchisq upper tail (R/core.R:1877-1878); df = 1 and 2
+    by the closed forms erfc(sqrt(s / 2)) and exp(-s / 2) (the first terms of device_pipeline.chisq_upper's sums):
+    scipy's chi2.sf loses up to 130 ulps at df = 1 for s below about 5."""
     from scipy import stats as _st
     stat = 2.0 * (logLikeFull - logLikeReduced)
+    half = np.maximum(stat, 0.0) / 2.0
+    if df == 1:
+        return stat, _sp.erfc(np.sqrt(half))
+    if df == 2:
+        return stat, np.exp(-half)
     return stat, _st.chi2.sf(stat, df)
 
 
