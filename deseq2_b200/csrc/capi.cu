@@ -564,13 +564,6 @@ int mat_layout_rows(MatIn& M, size_t g0, size_t gc, const void* d_raw, cudaStrea
   g_launches++;
   return 0;
 }
-int mat_fill_rows(MatIn& M, size_t g0, size_t gc, cudaStream_t st) {   // both halves on one stream
-  if (M.resident || gc == 0) return 0;
-  void* d_raw;
-  if (ws_get(S_RAW, gc * M.m * M.elem, &d_raw)) return 1;
-  if (mat_h2d_rows(M, g0, gc, d_raw, st)) return 1;
-  return mat_layout_rows(M, g0, gc, d_raw, st);
-}
 
 // after the last rows: the device computes the content hash of the complete copy and the entry becomes valid
 int mat_finish(MatIn& M, cudaStream_t st) {
@@ -588,17 +581,6 @@ int mat_finish(MatIn& M, cudaStream_t st) {
   dst->upload_call = g_call_seq;
   dst->fprint = M.fp;
   dst->last_use = ++g_cache_clock;
-  return 0;
-}
-
-// Column-major host matrix (n x m, elem 4 or 8) -> gene-major device matrix, through the cache, in one piece.
-int upload_matrix(const void* host, int n, int m, int elem, cudaStream_t st, CallInputs& ci, void** out) {
-  MatIn M;
-  M.host = host; M.n = n; M.m = m; M.elem = elem;
-  if (mat_acquire(M, ci)) return 1;
-  if (mat_fill_rows(M, 0, (size_t)n, st)) return 1;
-  if (mat_finish(M, st)) return 1;
-  *out = M.dev;
   return 0;
 }
 
@@ -687,33 +669,36 @@ int next_counter(unsigned int** out) {
 }
 
 
-// scratch buffers for fit_disp launches (work queue + per-mode gene lists): ONE device arena cut into a ring of
-// equal slots, one slot per launch in flight (slot reuse after kScratchRing further launches; launches on one stream
-// are ordered).  The arena is (re)allocated only when a call needs a larger slot than any before -- a per-slot
-// cudaFree/cudaMalloc was measured to stall the pipeline by up to 80 ms whenever the gene count changed, and a
-// lazily allocated ring stalled the first 8 steps of every run.
-constexpr int kScratchRing = 16;
-void* g_scratch_arena = nullptr;
-size_t g_scratch_slot = 0;
-std::atomic<unsigned int> g_scratch_next{0};
-int next_scratch(size_t bytes, unsigned int** out) {
-  std::lock_guard<std::mutex> lk(g_arena_mu);
-  bytes = (bytes + 255) & ~(size_t)255;
-  if (g_scratch_slot < bytes) {
-    if (g_scratch_arena) {
-      CU(cudaDeviceSynchronize());
-      CU(cudaFree(g_scratch_arena));
+// ONE device arena cut into a ring of equal slots, one slot per launch in flight (slot reuse after kSlots further
+// launches; launches on one stream are ordered).  The arena is (re)allocated only when a call needs a larger slot than
+// any before -- a per-slot cudaFree/cudaMalloc was measured to stall the pipeline by up to 80 ms whenever the gene
+// count changed, and a lazily allocated ring stalled the first 8 steps of every run.
+struct ArenaRing {
+  static constexpr int kSlots = 16;
+  void* arena = nullptr;
+  size_t slot = 0;
+  std::atomic<unsigned int> next{0};
+  template <class T>
+  int take(size_t bytes, T** out) {
+    std::lock_guard<std::mutex> lk(g_arena_mu);
+    bytes = (bytes + 255) & ~(size_t)255;
+    if (slot < bytes) {
+      if (arena) {
+        CU(cudaDeviceSynchronize());
+        CU(cudaFree(arena));
+      }
+      arena = nullptr;
+      slot = 0;
+      const size_t want = (bytes + bytes / 2 + 4095) & ~(size_t)4095;
+      CU(cudaMalloc(&arena, want * kSlots));
+      slot = want;
     }
-    g_scratch_arena = nullptr;
-    g_scratch_slot = 0;
-    const size_t slot = (bytes + bytes / 2 + 4095) & ~(size_t)4095;
-    CU(cudaMalloc(&g_scratch_arena, slot * kScratchRing));
-    g_scratch_slot = slot;
+    *out = reinterpret_cast<T*>(static_cast<char*>(arena) + (size_t)(next.fetch_add(1) % kSlots) * slot);
+    return 0;
   }
-  const unsigned int s = g_scratch_next.fetch_add(1) % kScratchRing;
-  *out = reinterpret_cast<unsigned int*>(static_cast<char*>(g_scratch_arena) + (size_t)s * g_scratch_slot);
-  return 0;
-}
+};
+ArenaRing g_scratch_ring;   // fit_disp launches: work queue + per-mode gene lists
+ArenaRing g_design_ring;    // analysed designs of the general-p launches (prepare_design)
 
 // ---------------------------------------------------------------- design analysis for the general-p kernels
 // Distinct rows of the design matrix (what R/core.R:2450 modelMatrixGroups computes) and a row id per sample.
@@ -726,16 +711,11 @@ bool use_generic(int p) {
 // Long rows on the small-p designs too: from m = 400 samples on the segmented general-p kernels (fit_generic_seg.cuh:
 // one gene per warp, per-segment sums, 1024-entry factor table) beat the register-resident small-p kernels, whose
 // per-sample X'WX accumulation and 256-entry table are sized for short rows (at m = 300 and below the small-p kernels
-// win).  Only the device entry points called
-// directly take this route (it fetches the design matrix: one stream sync per call); the host entry points keep the
-// small-p kernels, whose launches per row chunk overlap the uploads.  B200NB_LONG_ROWS=<m> moves the threshold, 0 = off.
-thread_local int t_in_host_call = 0;
-struct HostCallScope {
-  HostCallScope() { t_in_host_call++; }
-  ~HostCallScope() { t_in_host_call--; }
-};
+// win).  Only the device entry points take this route (it fetches the design matrix: one stream sync per call; see
+// route_fit); the host entry points keep the small-p kernels, whose launches per row chunk overlap the uploads.
+// B200NB_LONG_ROWS=<m> moves the threshold, 0 = off.
 bool long_rows(int m, int use_weights) {
-  if (t_in_host_call || use_weights) return false;
+  if (use_weights) return false;
   int thr = 400;
   const char* e = getenv("B200NB_LONG_ROWS");
   if (e) thr = atoi(e);
@@ -800,29 +780,6 @@ void build_seg_layout(const std::vector<int>& gid, int m, int G, SegHost* h) {
   for (int l = 0; l < 32; l++)
     for (size_t r = 0; r < ends[l].size(); r++) h->seg_end[r * 32 + l] = (unsigned short)ends[l][r];
 }
-constexpr int kDesignRing = 16;
-void* g_design_arena = nullptr;
-size_t g_design_slot = 0;
-std::atomic<unsigned int> g_design_next{0};
-int next_design_slot(size_t need, char** out) {
-  std::lock_guard<std::mutex> lk(g_arena_mu);
-  need = (need + 255) & ~(size_t)255;
-  if (g_design_slot < need) {
-    if (g_design_arena) {
-      CU(cudaDeviceSynchronize());
-      CU(cudaFree(g_design_arena));
-    }
-    g_design_arena = nullptr;
-    g_design_slot = 0;
-    const size_t slot = (need + need / 2 + 4095) & ~(size_t)4095;
-    CU(cudaMalloc(&g_design_arena, slot * kDesignRing));
-    g_design_slot = slot;
-  }
-  const unsigned int s = g_design_next.fetch_add(1) % kDesignRing;
-  *out = static_cast<char*>(g_design_arena) + (size_t)s * g_design_slot;
-  return 0;
-}
-
 // x_host: m x p column-major.  Uploads xg / gid on `st`.
 int prepare_design(const double* x_host, int m, int p, cudaStream_t st, DesignDev* out) {
   const int ps = p | 1;
@@ -872,7 +829,7 @@ int prepare_design(const double* x_host, int m, int p, cudaStream_t st, DesignDe
     memcpy(pack.data() + o_hi, sh.ghi.data(), sh.ghi.size());
   }
   char* base = nullptr;
-  if (next_design_slot(need, &base)) return 1;
+  if (g_design_ring.take(need, &base)) return 1;
   // pageable H2D copies are staged before cudaMemcpyAsync returns, so the vector may die at scope exit
   CU(cudaMemcpyAsync(base, pack.data(), need, cudaMemcpyHostToDevice, st));
   CU(cudaStreamSynchronize(st));
@@ -927,6 +884,31 @@ int prepare_design_from_device(const double* x_dev, int m, int p, cudaStream_t s
   CU(cudaMemcpyAsync(xh.data(), x_dev, xh.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return prepare_design(xh.data(), m, p, st, out);
+}
+
+// Which launcher fits a fitDisp, fitDispGrid or fitBeta call with n > 0 genes.  The general-p kernels (generic, with
+// the analysed design in dd) take p > kMaxSmallP and rows the small-p kernels cannot hold; with allow_long_rows,
+// fitDisp and fitBeta also send long unweighted rows there when the design gets a segment layout.  Everything else
+// runs on the small-p kernels.  launches: the kernels the chosen launcher starts (b200nb_kernel_launches).
+enum FitKind { FIT_DISP, FIT_DISP_GRID, FIT_BETA };
+struct FitRoute {
+  bool generic = false;
+  DesignDev dd;
+  int launches = 0;
+};
+int route_fit(FitKind kind, const double* x_dev, int m, int p, int use_weights, int nf_is_vector, bool allow_long_rows,
+              cudaStream_t st, FitRoute* r) {
+  const bool fits = kind == FIT_BETA ? nb::fit_beta_smallp_fits(m, p, use_weights, nf_is_vector)
+                                     : nb::fit_disp_smallp_fits(m, p, use_weights);
+  r->generic = use_generic(p) || !fits;
+  if (r->generic || (kind != FIT_DISP_GRID && allow_long_rows && long_rows(m, use_weights))) {
+    if (prepare_design_from_device(x_dev, m, p, st, &r->dd)) return 1;
+    r->generic = r->generic || r->dd.seg.pos != nullptr;
+  }
+  // small-p fitDisp: classify [+ bucket sort] + both design variants of the line search; fitDispGrid: one kernel;
+  // fitBeta: both design variants
+  r->launches = r->generic ? 1 : kind == FIT_DISP ? nb::fit_disp_smallp_launches(m) : kind == FIT_DISP_GRID ? 1 : 2;
+  return 0;
 }
 
 // The library keeps per-process device state (work-queue arenas, workspace, pinned staging): one process drives one
@@ -1008,7 +990,8 @@ struct PhaseClock {
     ms[phase++] = std::chrono::duration<double, std::milli>(t1 - t0).count();
     t0 = t1;
   }
-  void report(const char* what, int n) {
+  void report(const char* what, int n) {   // closes the last phase
+    next();
     if (on)
       fprintf(stderr, "b200nb timing %s %d genes: hash+upload %.3f ms, kernels %.3f ms, download %.3f ms | H2D %.1f MB, "
                       "D2H %.1f MB, hashed %.1f MB, served from the device cache %.1f MB; upload staging: %.3f ms copying "
@@ -1017,6 +1000,94 @@ struct PhaseClock {
               (g_cache_hit_bytes - hit0) / 1e6, (g_stage_copy_us - copy0) / 1e3, (g_stage_wait_us - wait0) / 1e3);
   }
 };
+
+// The input matrices of a host call: acquires them (mat_acquire), fills the device copies of those that are not
+// resident and runs launch_rows(g0, gc, stream) on rows [g0, g0 + gc) of them -- in one piece, or, when a matrix has
+// to be uploaded, in `chunks` row chunks whose layout conversion and kernels run on the compute stream while the next
+// chunk crosses PCIe.  Then the device hashes the fresh copies (mat_finish).
+template <class F>
+int upload_and_launch(const std::vector<MatIn*>& mats, CallInputs& ci, int n, int chunks, cudaStream_t st,
+                      PhaseClock& clk, F&& launch_rows) {
+  bool any_miss = false;
+  for (MatIn* M : mats) {
+    if (mat_acquire(*M, ci)) return 1;
+    any_miss = any_miss || !M->resident;
+  }
+  const int C = any_miss ? chunks : 1;
+  if (C == 1) {
+    for (MatIn* M : mats) {
+      void* d_raw;
+      if (M->resident) continue;
+      if (ws_get(S_RAW, (size_t)n * M->m * M->elem, &d_raw) || mat_h2d_rows(*M, 0, n, d_raw, st) ||
+          mat_layout_rows(*M, 0, n, d_raw, st))
+        return 1;
+    }
+    clk.next();
+    if (launch_rows((size_t)0, n, st)) return 1;
+  } else {
+    cudaStream_t ks;
+    if (ws_compute_stream(&ks)) return 1;
+    const size_t gc = (((size_t)n + C - 1) / C + 63) & ~(size_t)63;
+    // two sets of raw (column-major) chunk buffers: chunk c + 1 crosses PCIe into one while chunk c is converted
+    // from the other
+    std::vector<size_t> roff;
+    size_t rset = 0;
+    for (MatIn* M : mats) {
+      roff.push_back(rset);
+      rset += (gc * M->m * M->elem + 255) & ~(size_t)255;
+    }
+    void* rawbase;
+    if (ws_get(S_RAW, 2 * rset, &rawbase)) return 1;
+    int c = 0;
+    for (size_t g0 = 0; g0 < (size_t)n; g0 += gc, c++) {
+      const size_t cnt = (g0 + gc <= (size_t)n) ? gc : (size_t)n - g0;
+      char* raw = static_cast<char*>(rawbase) + (size_t)(c & 1) * rset;
+      if (c >= 2) CU(cudaStreamWaitEvent(st, g_ws.layout_ev[c - 2], 0));   // this buffer set has been consumed
+      for (size_t i = 0; i < mats.size(); i++)
+        if (mat_h2d_rows(*mats[i], g0, cnt, raw + roff[i], st)) return 1;
+      CU(cudaEventRecord(g_ws.up_ev[c], st));
+      CU(cudaStreamWaitEvent(ks, g_ws.up_ev[c], 0));
+      for (size_t i = 0; i < mats.size(); i++)
+        if (mat_layout_rows(*mats[i], g0, cnt, raw + roff[i], ks)) return 1;
+      CU(cudaEventRecord(g_ws.layout_ev[c], ks));
+      if (launch_rows(g0, (int)cnt, ks)) return 1;
+    }
+    CU(cudaEventRecord(g_ws.done_ev, ks));
+    CU(cudaStreamWaitEvent(st, g_ws.done_ev, 0));   // hashing and the download below follow the last kernel
+    clk.next();
+  }
+  for (MatIn* M : mats)
+    if (mat_finish(*M, st)) return 1;
+  return 0;
+}
+
+bool speculation_on() {
+  static const bool on = hostrt::env_int("B200NB_SPECULATE", 1, 0, 1) != 0;
+  return on;
+}
+
+// The protocol of the host entry points.  Calls are serialised and numbered (g_call_seq).  Each runs at most twice:
+// attempt 0 may launch on resident copies of its input matrices before their content has been verified
+// (CallInputs::validate, overlapped with the kernels); if a verification fails the attempt returns kRetry, its launch
+// is discarded and attempt 1 repeats the call with verified inputs only.  B200NB_SPECULATE=0 skips attempt 0's mode.
+constexpr int kRetry = 2;
+template <class F>
+int host_call(const char* name, int n, F&& attempt) {
+  std::lock_guard<std::mutex> lk(g_call_mu);
+  g_call_seq++;
+  cudaStream_t st;
+  if (ws_stream(&st)) return 1;
+  for (int k = 0; k < 2; k++) {
+    PhaseClock clk(st);
+    CallInputs ci;
+    ci.speculate = (k == 0) && speculation_on();
+    const int rc = attempt(ci, clk, st);
+    if (rc == 0) clk.report(name, n);
+    if (rc != kRetry) return rc;
+    CU(cudaStreamSynchronize(st));
+  }
+  return fail("%s: input verification failed twice", name);
+}
 
 }  // namespace
 
@@ -1128,6 +1199,65 @@ void b200nb_release_workspace(void) {
 
 /* ------------------------------------------------------------------ device entry points */
 
+// fitDisp or fitDispGrid (a.grid) on the kernels route_fit picks; allow_long_rows: see route_fit
+static int launch_disp(nb::DispArgs& a, bool allow_long_rows, cudaStream_t st) {
+  if (a.n == 0) return 0;
+  FitRoute r;
+  if (check_device() || g_scratch_ring.take(nb::disp_scratch_bytes(a.n), &a.scratch) ||
+      route_fit(a.grid ? FIT_DISP_GRID : FIT_DISP, a.x, a.m, a.p, a.use_weights, 0, allow_long_rows, st, &r))
+    return 1;
+  if (r.generic) apply_design(r.dd, a.use_weights, &a);
+  CU(r.generic ? nb::launch_fit_disp_generic(a, st) : nb::launch_fit_disp(a, st));
+  g_launches += r.launches;
+  return 0;
+}
+
+// b200nb_fit_disp_dev and b200nb_fit_beta_dev after their argument checks
+static int fit_disp_dev(const void* y, int y_type, const double* x, const double* mu_hat, const double* log_alpha,
+                        const double* log_alpha_prior_mean, double log_alpha_prior_sigmasq, double min_log_alpha,
+                        double kappa_0, double tol, int maxit, int use_prior, const double* weights,
+                        int use_weights, double weight_threshold, int use_cr, int n, int m, int p, long long ld,
+                        double* out_log_alpha, int32_t* out_iter, int32_t* out_iter_accept,
+                        double* out_last_change, double* out_initial_lp, double* out_initial_dlp,
+                        double* out_last_lp, double* out_last_dlp, double* out_last_d2lp, cudaStream_t st,
+                        bool allow_long_rows) {
+  nb::DispArgs a{};
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.mu = mu_hat; a.w = use_weights ? weights : nullptr; a.x = x;
+  a.log_alpha_in = log_alpha; a.prior_mean = log_alpha_prior_mean;
+  a.prior_sigmasq = log_alpha_prior_sigmasq; a.min_log_alpha = min_log_alpha; a.kappa_0 = kappa_0; a.tol = tol;
+  a.maxit = maxit; a.use_prior = use_prior; a.use_weights = use_weights; a.use_cr = use_cr;
+  a.weight_threshold = weight_threshold; a.n = n; a.m = m; a.p = p; a.ld = ld;
+  a.log_alpha = out_log_alpha; a.iter = out_iter; a.iter_accept = out_iter_accept; a.last_change = out_last_change;
+  a.initial_lp = out_initial_lp; a.initial_dlp = out_initial_dlp; a.last_lp = out_last_lp; a.last_dlp = out_last_dlp;
+  a.last_d2lp = out_last_d2lp; a.grid = nullptr; a.grid_n = 0;
+  return launch_disp(a, allow_long_rows, st);
+}
+
+static int fit_beta_dev(const void* y, int y_type, const double* x, const double* nf, int nf_is_vector,
+                        const double* alpha_hat, const double* contrast, const double* beta_mat,
+                        const double* lambda, const double* weights, int use_weights, double tol, int maxit,
+                        int use_qr, double minmu, int n, int m, int p, long long ld, double* out_beta_mat,
+                        double* out_beta_var_mat, double* out_iter, double* out_hat_diagonals,
+                        double* out_contrast_num, double* out_contrast_denom, double* out_deviance, double* out_mu,
+                        cudaStream_t st, bool allow_long_rows) {
+  unsigned int* ctr;
+  if ((n > 0 && check_device()) || next_counter(&ctr)) return 1;
+  nb::BetaArgs a{};
+  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.nf = nf; a.nf_is_vector = nf_is_vector;
+  a.w = use_weights ? weights : nullptr; a.x = x; a.alpha_hat = alpha_hat; a.contrast = contrast; a.beta_in = beta_mat;
+  a.lambda = lambda; a.use_weights = use_weights; a.tol = tol; a.maxit = maxit; a.use_qr = use_qr; a.minmu = minmu;
+  a.n = n; a.m = m; a.p = p; a.ld = ld; a.beta_out = out_beta_mat; a.beta_var = out_beta_var_mat; a.iter = out_iter;
+  a.hat_diag = out_hat_diagonals; a.mu_out = out_mu; a.contrast_num = out_contrast_num;
+  a.contrast_denom = out_contrast_denom; a.deviance = out_deviance; a.counter = ctr;
+  if (n == 0) return 0;
+  FitRoute r;
+  if (route_fit(FIT_BETA, x, m, p, use_weights, nf_is_vector, allow_long_rows, st, &r)) return 1;
+  if (r.generic) apply_design(r.dd, &a);
+  CU(r.generic ? nb::launch_fit_beta_generic(a, st) : nb::launch_fit_beta(a, st));
+  g_launches += r.launches;
+  return 0;
+}
+
 int b200nb_fit_disp_dev(const void* y, int y_type, const double* x, const double* mu_hat, const double* log_alpha,
                         const double* log_alpha_prior_mean, double log_alpha_prior_sigmasq, double min_log_alpha,
                         double kappa_0, double tol, int maxit, int use_prior, const double* weights,
@@ -1141,32 +1271,10 @@ int b200nb_fit_disp_dev(const void* y, int y_type, const double* x, const double
                                  out_last_change, out_initial_lp, out_initial_dlp, out_last_lp, out_last_dlp,
                                  out_last_d2lp}))
     return 1;
-  nb::DispArgs a{};
-  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.mu = mu_hat; a.w = use_weights ? weights : nullptr; a.x = x;
-  a.log_alpha_in = log_alpha; a.prior_mean = log_alpha_prior_mean;
-  a.prior_sigmasq = log_alpha_prior_sigmasq; a.min_log_alpha = min_log_alpha; a.kappa_0 = kappa_0; a.tol = tol;
-  a.maxit = maxit; a.use_prior = use_prior; a.use_weights = use_weights; a.use_cr = use_cr;
-  a.weight_threshold = weight_threshold; a.n = n; a.m = m; a.p = p; a.ld = ld;
-  a.log_alpha = out_log_alpha; a.iter = out_iter; a.iter_accept = out_iter_accept; a.last_change = out_last_change;
-  a.initial_lp = out_initial_lp; a.initial_dlp = out_initial_dlp; a.last_lp = out_last_lp; a.last_dlp = out_last_dlp;
-  a.last_d2lp = out_last_d2lp; a.grid = nullptr; a.grid_n = 0;
-  if (n == 0) return 0;
-  if (check_device() || next_scratch(nb::disp_scratch_bytes(n), &a.scratch)) return 1;
-  const bool smallp_fits = nb::fit_disp_smallp_fits(m, p, use_weights);
-  if (use_generic(p) || long_rows(m, use_weights) || !smallp_fits) {
-    DesignDev dd;
-    if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
-    // long rows: only designs the segmented kernels take, unless the small-p kernels cannot hold the rows at all
-    if (use_generic(p) || dd.seg.pos != nullptr || !smallp_fits) {
-      apply_design(dd, use_weights, &a);
-      CU(nb::launch_fit_disp_generic(a, (cudaStream_t)stream));
-      g_launches += 1;
-      return 0;
-    }
-  }
-  CU(nb::launch_fit_disp(a, (cudaStream_t)stream));
-  g_launches += nb::fit_disp_smallp_launches(m);   // classify [+ bucket sort] + both design variants of the line search
-  return 0;
+  return fit_disp_dev(y, y_type, x, mu_hat, log_alpha, log_alpha_prior_mean, log_alpha_prior_sigmasq, min_log_alpha,
+                      kappa_0, tol, maxit, use_prior, weights, use_weights, weight_threshold, use_cr, n, m, p, ld,
+                      out_log_alpha, out_iter, out_iter_accept, out_last_change, out_initial_lp, out_initial_dlp,
+                      out_last_lp, out_last_dlp, out_last_d2lp, (cudaStream_t)stream, true);
 }
 
 int b200nb_fit_disp_grid_dev(const void* y, int y_type, const double* x, const double* mu_hat,
@@ -1184,19 +1292,7 @@ int b200nb_fit_disp_grid_dev(const void* y, int y_type, const double* x, const d
   a.log_alpha_in = nullptr; a.prior_mean = log_alpha_prior_mean; a.prior_sigmasq = log_alpha_prior_sigmasq;
   a.use_prior = use_prior; a.use_weights = use_weights; a.use_cr = use_cr; a.weight_threshold = weight_threshold;
   a.n = n; a.m = m; a.p = p; a.ld = ld; a.log_alpha = out_log_alpha; a.grid = disp_grid; a.grid_n = disp_grid_n;
-  if (n == 0) return 0;
-  if (check_device() || next_scratch(nb::disp_scratch_bytes(n), &a.scratch)) return 1;
-  if (use_generic(p) || !nb::fit_disp_smallp_fits(m, p, use_weights)) {
-    DesignDev dd;
-    if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
-    apply_design(dd, use_weights, &a);
-    CU(nb::launch_fit_disp_generic(a, (cudaStream_t)stream));
-    g_launches++;
-    return 0;
-  }
-  CU(nb::launch_fit_disp(a, (cudaStream_t)stream));
-  g_launches++;
-  return 0;
+  return launch_disp(a, false, (cudaStream_t)stream);
 }
 
 int b200nb_fit_beta_dev(const void* y, int y_type, const double* x, const double* nf, int nf_is_vector,
@@ -1209,33 +1305,12 @@ int b200nb_fit_beta_dev(const void* y, int y_type, const double* x, const double
   if (check_dims(n, m, p) || check_y("fit_beta", y, y_type, n) || check_ld("fit_beta", "ld", ld, m, true)) return 1;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   if (maxit < 0) return fail("maxit must be >= 0");
-  unsigned int* ctr;
   if (check_ptrs("fit_beta", n, {x, nf, alpha_hat, contrast, beta_mat, lambda, out_beta_mat, out_beta_var_mat, out_iter,
-                                 out_contrast_num, out_contrast_denom, out_deviance}) ||
-      (n > 0 && check_device()) || next_counter(&ctr))
+                                 out_contrast_num, out_contrast_denom, out_deviance}))
     return 1;
-  nb::BetaArgs a{};
-  a.y = y; a.y_is_f64 = (y_type == B200NB_Y_F64); a.nf = nf; a.nf_is_vector = nf_is_vector;
-  a.w = use_weights ? weights : nullptr; a.x = x; a.alpha_hat = alpha_hat; a.contrast = contrast; a.beta_in = beta_mat;
-  a.lambda = lambda; a.use_weights = use_weights; a.tol = tol; a.maxit = maxit; a.use_qr = use_qr; a.minmu = minmu;
-  a.n = n; a.m = m; a.p = p; a.ld = ld; a.beta_out = out_beta_mat; a.beta_var = out_beta_var_mat; a.iter = out_iter;
-  a.hat_diag = out_hat_diagonals; a.mu_out = out_mu; a.contrast_num = out_contrast_num;
-  a.contrast_denom = out_contrast_denom; a.deviance = out_deviance; a.counter = ctr;
-  const bool smallp_fits = nb::fit_beta_smallp_fits(m, p, use_weights, nf_is_vector);
-  if (use_generic(p) || long_rows(m, use_weights) || !smallp_fits) {
-    if (n == 0) return 0;
-    DesignDev dd;
-    if (prepare_design_from_device(x, m, p, (cudaStream_t)stream, &dd)) return 1;
-    if (use_generic(p) || dd.seg.pos != nullptr || !smallp_fits) {
-      apply_design(dd, &a);
-      CU(nb::launch_fit_beta_generic(a, (cudaStream_t)stream));
-      g_launches++;
-      return 0;
-    }
-  }
-  CU(nb::launch_fit_beta(a, (cudaStream_t)stream));
-  if (n > 0) g_launches += 2;   // both design variants
-  return 0;
+  return fit_beta_dev(y, y_type, x, nf, nf_is_vector, alpha_hat, contrast, beta_mat, lambda, weights, use_weights, tol,
+                      maxit, use_qr, minmu, n, m, p, ld, out_beta_mat, out_beta_var_mat, out_iter, out_hat_diagonals,
+                      out_contrast_num, out_contrast_denom, out_deviance, out_mu, (cudaStream_t)stream, true);
 }
 
 int b200nb_nb_loglik_dev(const void* y, int y_type, const double* x, const double* nf, int nf_is_vector,
@@ -1688,14 +1763,7 @@ int b200nb_padj_dev(const double* p_sorted, const double* filter_sorted, const i
 }
 
 /* ------------------------------------------------------------------ host entry points */
-/* Each entry point runs at most twice: attempt 0 may launch on resident copies of its input matrices before their
- * content has been verified (CallInputs::validate, overlapped with the kernels); if a verification fails the launch
- * is discarded and attempt 1 repeats the call with verified inputs only.  B200NB_SPECULATE=0 skips attempt 0's mode. */
-
-static bool speculation_on() {
-  static const bool on = hostrt::env_int("B200NB_SPECULATE", 1, 0, 1) != 0;
-  return on;
-}
+/* Each runs through host_call (the speculation protocol) and upload_and_launch (its input matrices). */
 
 int b200nb_fit_disp(const void* y, int y_type, const double* x, const double* mu_hat, const double* log_alpha,
                     const double* log_alpha_prior_mean, double log_alpha_prior_sigmasq, double min_log_alpha,
@@ -1708,23 +1776,12 @@ int b200nb_fit_disp(const void* y, int y_type, const double* x, const double* mu
   if (n == 0) return 0;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   if (check_ptrs("fitDisp", n, {x, mu_hat, log_alpha, log_alpha_prior_mean}) || check_device()) return 1;
-  std::lock_guard<std::mutex> lk(g_call_mu);
-  HostCallScope host_scope;   // the row-chunked path keeps the small-p kernels (see long_rows)
-  g_call_seq++;
-  cudaStream_t st;
-  if (ws_stream(&st)) return 1;
   const int ye = (y_type == B200NB_Y_F64) ? 8 : 4;
   const long long ld = ld_for(m);
-  for (int attempt = 0; attempt < 2; attempt++) {
-    PhaseClock clk(st);
-    CallInputs ci;
-    ci.speculate = (attempt == 0) && speculation_on();
-    MatIn My, Mmu, Mw;
-    My.host = y; My.n = n; My.m = m; My.elem = ye;
-    Mmu.host = mu_hat; Mmu.n = n; Mmu.m = m; Mmu.elem = 8;
-    Mw.host = weights; Mw.n = n; Mw.m = m; Mw.elem = 8;
-    if (mat_acquire(My, ci) || mat_acquire(Mmu, ci)) return 1;
-    if (use_weights && mat_acquire(Mw, ci)) return 1;
+  return host_call("fitDisp", n, [&](CallInputs& ci, PhaseClock& clk, cudaStream_t st) -> int {
+    MatIn My{y, n, m, ye}, Mmu{mu_hat, n, m, 8}, Mw{weights, n, m, 8};
+    std::vector<MatIn*> mats{&My, &Mmu};
+    if (use_weights) mats.push_back(&Mw);
     SmallIn in;
     const size_t o_x = in.add(x, sizeof(double) * m * p), o_la = in.add(log_alpha, sizeof(double) * n),
                  o_pm = in.add(log_alpha_prior_mean, sizeof(double) * n);
@@ -1744,64 +1801,21 @@ int b200nb_fit_disp(const void* y, int y_type, const double* x, const double* mu
       const char* yb = static_cast<const char*>(My.dev) + g0 * (size_t)ld * ye;
       const double* mub = static_cast<const double*>(Mmu.dev) + g0 * (size_t)ld;
       const double* wb = use_weights ? static_cast<const double*>(Mw.dev) + g0 * (size_t)ld : nullptr;
-      return b200nb_fit_disp_dev(yb, y_type, reinterpret_cast<const double*>(din + o_x), mub,
-                                 reinterpret_cast<const double*>(din + o_la) + g0,
-                                 reinterpret_cast<const double*>(din + o_pm) + g0, log_alpha_prior_sigmasq, min_log_alpha,
-                                 kappa_0, tol, maxit, use_prior, wb, use_weights, weight_threshold, use_cr, gc, m, p, ld,
-                                 D(od[0]) + g0, reinterpret_cast<int32_t*>(dout + oi) + g0,
-                                 reinterpret_cast<int32_t*>(dout + oia) + g0, D(od[1]) + g0, D(od[2]) + g0, D(od[3]) + g0,
-                                 D(od[4]) + g0, D(od[5]) + g0, D(od[6]) + g0, ks);
+      return fit_disp_dev(yb, y_type, reinterpret_cast<const double*>(din + o_x), mub,
+                          reinterpret_cast<const double*>(din + o_la) + g0,
+                          reinterpret_cast<const double*>(din + o_pm) + g0, log_alpha_prior_sigmasq, min_log_alpha,
+                          kappa_0, tol, maxit, use_prior, wb, use_weights, weight_threshold, use_cr, gc, m, p, ld,
+                          D(od[0]) + g0, reinterpret_cast<int32_t*>(dout + oi) + g0,
+                          reinterpret_cast<int32_t*>(dout + oia) + g0, D(od[1]) + g0, D(od[2]) + g0, D(od[3]) + g0,
+                          D(od[4]) + g0, D(od[5]) + g0, D(od[6]) + g0, ks, false);
     };
-    const bool any_miss = !My.resident || !Mmu.resident || (use_weights && !Mw.resident);
-    const int C = (any_miss && !use_generic(p)) ? plan_chunks(n) : 1;
-    if (C == 1) {
-      if (mat_fill_rows(My, 0, (size_t)n, st) || mat_fill_rows(Mmu, 0, (size_t)n, st)) return 1;
-      if (use_weights && mat_fill_rows(Mw, 0, (size_t)n, st)) return 1;
-      clk.next();
-      if (launch_rows(0, n, st)) return 1;
-    } else {
-      cudaStream_t ks;
-      if (ws_compute_stream(&ks)) return 1;
-      const size_t gc = (((size_t)n + C - 1) / C + 63) & ~(size_t)63;
-      // two sets of raw (column-major) chunk buffers: chunk c + 1 crosses PCIe into one while chunk c is converted
-      // from the other
-      const size_t ry = (gc * m * ye + 255) & ~(size_t)255, r8 = (gc * m * 8 + 255) & ~(size_t)255;
-      const size_t rset = ry + r8 + (use_weights ? r8 : 0);
-      void* rawbase;
-      if (ws_get(S_RAW, 2 * rset, &rawbase)) return 1;
-      int c = 0;
-      for (size_t g0 = 0; g0 < (size_t)n; g0 += gc, c++) {
-        const size_t cnt = (g0 + gc <= (size_t)n) ? gc : (size_t)n - g0;
-        char* raw = static_cast<char*>(rawbase) + (size_t)(c & 1) * rset;
-        if (c >= 2) CU(cudaStreamWaitEvent(st, g_ws.layout_ev[c - 2], 0));   // this buffer set has been consumed
-        if (mat_h2d_rows(My, g0, cnt, raw, st) || mat_h2d_rows(Mmu, g0, cnt, raw + ry, st)) return 1;
-        if (use_weights && mat_h2d_rows(Mw, g0, cnt, raw + ry + r8, st)) return 1;
-        CU(cudaEventRecord(g_ws.up_ev[c], st));
-        CU(cudaStreamWaitEvent(ks, g_ws.up_ev[c], 0));
-        if (mat_layout_rows(My, g0, cnt, raw, ks) || mat_layout_rows(Mmu, g0, cnt, raw + ry, ks)) return 1;
-        if (use_weights && mat_layout_rows(Mw, g0, cnt, raw + ry + r8, ks)) return 1;
-        CU(cudaEventRecord(g_ws.layout_ev[c], ks));
-        if (launch_rows(g0, (int)cnt, ks)) return 1;
-      }
-      CU(cudaEventRecord(g_ws.done_ev, ks));
-      CU(cudaStreamWaitEvent(st, g_ws.done_ev, 0));   // hashing and the download below follow the last kernel
-      clk.next();
-    }
-    if (mat_finish(My, st) || mat_finish(Mmu, st)) return 1;
-    if (use_weights && mat_finish(Mw, st)) return 1;
+    if (upload_and_launch(mats, ci, n, use_generic(p) ? 1 : plan_chunks(n), st, clk, launch_rows)) return 1;
     if (out.begin(dout, st)) return 1;     // the result DMA queues behind the kernels ...
     const bool verified = ci.validate();   // ... while the host hashes the inputs of a speculative hit
     clk.next();
-    if (!verified) {
-      CU(cudaStreamSynchronize(st));
-      continue;
-    }
-    if (out.finish(st)) return 1;
-    clk.next();
-    clk.report("fitDisp", n);
-    return 0;
-  }
-  return fail("fitDisp: input verification failed twice");
+    if (!verified) return kRetry;
+    return out.finish(st);
+  });
 }
 
 int b200nb_fit_disp_grid(const void* y, int y_type, const double* x, const double* mu_hat, const double* disp_grid,
@@ -1813,20 +1827,12 @@ int b200nb_fit_disp_grid(const void* y, int y_type, const double* x, const doubl
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   if (disp_grid_n < 2) return fail("disp_grid needs at least 2 points");
   if (check_ptrs("fitDispGrid", n, {x, mu_hat, disp_grid, log_alpha_prior_mean}) || check_device()) return 1;
-  std::lock_guard<std::mutex> lk(g_call_mu);
-  HostCallScope host_scope;   // the row-chunked path keeps the small-p kernels (see long_rows)
-  g_call_seq++;
-  cudaStream_t st;
-  if (ws_stream(&st)) return 1;
   const int ye = (y_type == B200NB_Y_F64) ? 8 : 4;
   const long long ld = ld_for(m);
-  for (int attempt = 0; attempt < 2; attempt++) {
-    CallInputs ci;
-    ci.speculate = (attempt == 0) && speculation_on();
-    void *d_y, *d_mu, *d_w = nullptr;
-    if (upload_matrix(y, n, m, ye, st, ci, &d_y)) return 1;
-    if (upload_matrix(mu_hat, n, m, 8, st, ci, &d_mu)) return 1;
-    if (use_weights && upload_matrix(weights, n, m, 8, st, ci, &d_w)) return 1;
+  return host_call("fitDispGrid", n, [&](CallInputs& ci, PhaseClock& clk, cudaStream_t st) -> int {
+    MatIn My{y, n, m, ye}, Mmu{mu_hat, n, m, 8}, Mw{weights, n, m, 8};
+    std::vector<MatIn*> mats{&My, &Mmu};
+    if (use_weights) mats.push_back(&Mw);
     SmallIn in;
     const size_t o_x = in.add(x, sizeof(double) * m * p), o_grid = in.add(disp_grid, sizeof(double) * disp_grid_n),
                  o_pm = in.add(log_alpha_prior_mean, sizeof(double) * n);
@@ -1836,20 +1842,20 @@ int b200nb_fit_disp_grid(const void* y, int y_type, const double* x, const doubl
     const size_t o_la = out.add(out_log_alpha, sizeof(double) * n);
     char* dout;
     if (out.device(&dout)) return 1;
-    if (b200nb_fit_disp_grid_dev(d_y, y_type, reinterpret_cast<const double*>(din + o_x), (const double*)d_mu,
-                                 reinterpret_cast<const double*>(din + o_grid), disp_grid_n,
-                                 reinterpret_cast<const double*>(din + o_pm), log_alpha_prior_sigmasq, use_prior,
-                                 (const double*)d_w, use_weights, weight_threshold, use_cr, n, m, p, ld,
-                                 reinterpret_cast<double*>(dout + o_la), st))
-      return 1;
+    auto launch_all = [&](size_t, int, cudaStream_t ks) -> int {   // one piece: every row
+      return b200nb_fit_disp_grid_dev(My.dev, y_type, reinterpret_cast<const double*>(din + o_x),
+                                      (const double*)Mmu.dev, reinterpret_cast<const double*>(din + o_grid),
+                                      disp_grid_n, reinterpret_cast<const double*>(din + o_pm),
+                                      log_alpha_prior_sigmasq, use_prior, (const double*)Mw.dev, use_weights,
+                                      weight_threshold, use_cr, n, m, p, ld, reinterpret_cast<double*>(dout + o_la), ks);
+    };
+    if (upload_and_launch(mats, ci, n, 1, st, clk, launch_all)) return 1;
     if (out.begin(dout, st)) return 1;
-    if (!ci.validate()) {
-      CU(cudaStreamSynchronize(st));
-      continue;
-    }
+    const bool verified = ci.validate();
+    clk.next();
+    if (!verified) return kRetry;
     return out.finish(st);
-  }
-  return fail("fitDispGrid: input verification failed twice");
+  });
 }
 
 // R always hands fitBeta an n x m matrix of normalisation factors, which for the usual size-factor analysis is the same
@@ -1892,19 +1898,11 @@ int b200nb_fit_beta(const void* y, int y_type, const double* x, const double* nf
   if (n == 0) return 0;
   if (use_weights && !weights) return fail("use_weights set but weights == NULL");
   if (check_ptrs("fitBeta", n, {x, nf, alpha_hat, contrast, beta_mat, lambda}) || check_device()) return 1;
-  std::lock_guard<std::mutex> lk(g_call_mu);
-  HostCallScope host_scope;   // the row-chunked path keeps the small-p kernels (see long_rows)
-  g_call_seq++;
-  cudaStream_t st;
-  if (ws_stream(&st)) return 1;
+  if (maxit < 0) return fail("maxit must be >= 0");
   const int ye = (y_type == B200NB_Y_F64) ? 8 : 4;
   const long long ld = ld_for(m);
   const bool sf_detect = hostrt::env_int("B200NB_SF_DETECT", 1, 0, 1) != 0;
-  for (int attempt = 0; attempt < 2; attempt++) {
-    PhaseClock clk(st);
-    CallInputs ci;
-    ci.speculate = (attempt == 0) && speculation_on();
-    void *d_y, *d_nf = nullptr, *d_w = nullptr;
+  return host_call("fitBeta", n, [&](CallInputs& ci, PhaseClock& clk, cudaStream_t st) -> int {
     // normalisation factors: a replicated size-factor vector?  With speculation the full scan of the matrix is
     // deferred until the kernels are running (the three probed rows decide what to launch with)
     std::vector<double> sfv;
@@ -1917,9 +1915,10 @@ int b200nb_fit_beta(const void* y, int y_type, const double* x, const double* nf
         if (!ci.speculate) g_hashed_bytes += (long long)sizeof(double) * n * m;   // scanned before the launch
       }
     }
-    if (upload_matrix(y, n, m, ye, st, ci, &d_y)) return 1;
-    if (sfv.empty() && upload_matrix(nf, n, m, 8, st, ci, &d_nf)) return 1;
-    if (use_weights && upload_matrix(weights, n, m, 8, st, ci, &d_w)) return 1;
+    MatIn My{y, n, m, ye}, Mnf{nf, n, m, 8}, Mw{weights, n, m, 8};
+    std::vector<MatIn*> mats{&My};
+    if (sfv.empty()) mats.push_back(&Mnf);
+    if (use_weights) mats.push_back(&Mw);
     SmallIn in;
     const size_t o_x = in.add(x, sizeof(double) * m * p), o_alpha = in.add(alpha_hat, sizeof(double) * n),
                  o_c = in.add(contrast, sizeof(double) * p), o_lam = in.add(lambda, sizeof(double) * p),
@@ -1939,14 +1938,15 @@ int b200nb_fit_beta(const void* y, int y_type, const double* x, const double* nf
     if (out_hat_diagonals && ws_get(S_H, sizeof(double) * n * ld, &d_h)) return 1;
     if (out_mu && ws_get(S_MUO, sizeof(double) * n * ld, &d_mu)) return 1;
     if ((out_hat_diagonals || out_mu) && ws_get(S_HC, sizeof(double) * n * m, &d_hc)) return 1;
-    clk.next();
     auto Din = [&](size_t off) { return reinterpret_cast<const double*>(din + off); };
     auto Dout = [&](size_t off) { return reinterpret_cast<double*>(dout + off); };
-    if (b200nb_fit_beta_dev(d_y, y_type, Din(o_x), sfv.empty() ? (const double*)d_nf : Din(o_sf), sfv.empty() ? 0 : 1,
-                            Din(o_alpha), Din(o_c), Din(o_b), Din(o_lam), (const double*)d_w, use_weights, tol, maxit,
-                            use_qr, minmu, n, m, p, ld, Dout(o_bo), Dout(o_bv), Dout(o_it), (double*)d_h, Dout(o_cn),
-                            Dout(o_cd), Dout(o_dev), (double*)d_mu, st))
-      return 1;
+    auto launch_all = [&](size_t, int, cudaStream_t ks) -> int {   // one piece: every row
+      return fit_beta_dev(My.dev, y_type, Din(o_x), sfv.empty() ? (const double*)Mnf.dev : Din(o_sf),
+                          sfv.empty() ? 0 : 1, Din(o_alpha), Din(o_c), Din(o_b), Din(o_lam), (const double*)Mw.dev,
+                          use_weights, tol, maxit, use_qr, minmu, n, m, p, ld, Dout(o_bo), Dout(o_bv), Dout(o_it),
+                          (double*)d_h, Dout(o_cn), Dout(o_cd), Dout(o_dev), (double*)d_mu, ks, false);
+    };
+    if (upload_and_launch(mats, ci, n, 1, st, clk, launch_all)) return 1;
     if (out_hat_diagonals && b200nb_to_col_major_dev((const double*)d_h, (double*)d_hc, n, m, ld, st)) return 1;
     // Results in page-locked memory (b200nb_host_alloc) leave by DMA right behind the kernels, overlapping the host-side
     // verification below; a failed verification repeats the call and overwrites them.
@@ -1965,10 +1965,7 @@ int b200nb_fit_beta(const void* y, int y_type, const double* x, const double* nf
       verified = verified && same;
     }
     clk.next();
-    if (!verified) {
-      CU(cudaStreamSynchronize(st));
-      continue;
-    }
+    if (!verified) return kRetry;
     if (out_hat_diagonals && !h_sent) {
       if (d2h_staged(out_hat_diagonals, d_hc, sizeof(double) * (size_t)n * m, st)) return 1;
     }
@@ -1977,33 +1974,27 @@ int b200nb_fit_beta(const void* y, int y_type, const double* x, const double* nf
       if (d2h_staged(out_mu, d_hc, sizeof(double) * (size_t)n * m, st)) return 1;
     }
     if (!small_early && out.begin(dout, st)) return 1;
-    if (out.finish(st)) return 1;
-    clk.next();
-    clk.report("fitBeta", n);
-    return 0;
-  }
-  return fail("fitBeta: input verification failed twice");
+    return out.finish(st);
+  });
 }
 
 int b200nb_test_special(const double* x, int n, double* out_lgamma, double* out_digamma, double* out_trigamma) {
   if (n <= 0) return 0;
-  std::lock_guard<std::mutex> lk(g_call_mu);
-  g_call_seq++;
-  cudaStream_t st;
-  if (ws_stream(&st)) return 1;
-  SmallIn in;
-  const size_t o_x = in.add(x, sizeof(double) * n);
-  char* din;
-  if (in.upload(st, &din)) return 1;
-  SmallOut out;
-  const size_t o_l = out.add(out_lgamma, sizeof(double) * n), o_d = out.add(out_digamma, sizeof(double) * n),
-               o_t = out.add(out_trigamma, sizeof(double) * n);
-  char* dout;
-  if (out.device(&dout)) return 1;
-  CU(nb::launch_special_test(reinterpret_cast<const double*>(din + o_x), n, reinterpret_cast<double*>(dout + o_l),
-                             reinterpret_cast<double*>(dout + o_d), reinterpret_cast<double*>(dout + o_t), st));
-  g_launches++;
-  return out.download(dout, st);
+  return host_call("special", n, [&](CallInputs&, PhaseClock&, cudaStream_t st) -> int {
+    SmallIn in;
+    const size_t o_x = in.add(x, sizeof(double) * n);
+    char* din;
+    if (in.upload(st, &din)) return 1;
+    SmallOut out;
+    const size_t o_l = out.add(out_lgamma, sizeof(double) * n), o_d = out.add(out_digamma, sizeof(double) * n),
+                 o_t = out.add(out_trigamma, sizeof(double) * n);
+    char* dout;
+    if (out.device(&dout)) return 1;
+    CU(nb::launch_special_test(reinterpret_cast<const double*>(din + o_x), n, reinterpret_cast<double*>(dout + o_l),
+                               reinterpret_cast<double*>(dout + o_d), reinterpret_cast<double*>(dout + o_t), st));
+    g_launches++;
+    return out.download(dout, st);
+  });
 }
 
 }  // extern "C"
