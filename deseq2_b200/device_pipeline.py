@@ -71,18 +71,19 @@ def _ws(name, shape, dtype, dev):
     return t
 
 
-def size_factor_ratios(y, m, poscounts=False, divisor=None):
+def size_factor_ratios(y, m, poscounts=False, divisor=None, ws="sf_ratios"):
     """One launch of b200nb_size_factors_dev (b200nb_size_factors_norm_dev with a gene-major (n, ld) divisor matrix):
     returns {"sizeFactors": (m,), "loggeomeans": (n,), "ratios": the (m, n) log ratios of the median, one sample per
-    row, +Inf where an entry does not take part (a view of a workspace: valid until the next call), "n_finite": the
-    number of genes with a finite log geometric mean as a 1-element device tensor}.  Does not raise when it is 0."""
+    row, +Inf where an entry does not take part (a view of the workspace named `ws`: valid until the next call that
+    uses it), "n_finite": the number of genes with a finite log geometric mean as a 1-element device tensor}.  Does
+    not raise when it is 0."""
     L = _lib.lib()
     dev = y.device
     n, ld = y.shape
     out = {"sizeFactors": torch.empty(m, dtype=F64, device=dev), "loggeomeans": torch.empty(n, dtype=F64, device=dev),
            "n_finite": torch.zeros(1, dtype=torch.int32, device=dev)}
-    gm = _ws("sf_ratios", (n, ld), F64, dev)
-    cm = _ws("sf_ratios_cm", (n * m,), F64, dev)
+    gm = _ws(ws, (n, ld), F64, dev)
+    cm = _ws(ws + "_cm", (n * m,), F64, dev)
     if divisor is None:
         _lib.check(L.b200nb_size_factors_dev(D._p(y), D._ytype(y), int(poscounts), n, m, ld, D._p(out["loggeomeans"]),
                                              D._p(gm), D._p(cm), D._p(out["sizeFactors"]), D._p(out["n_finite"]),
@@ -100,16 +101,114 @@ def _no_finite_loggeomean():
     return ValueError("every gene contains at least one zero, cannot compute log geometric means")
 
 
-def size_factors(y, m, type="ratio"):
+def size_factors(y, m, type="ratio", controlGenes=None, geoMeans=None):
     """b200nb_size_factors_dev: estimateSizeFactorsForMatrix (R/core.R:535-578, locfunc = median) on the device.
     y: gene-major (n, ld) device tensor, m samples.  Returns {"sizeFactors": (m,) device tensor, "loggeomeans": (n,)}.
-    Raises like the reference when every gene contains a zero (the only host read: one int)."""
-    if type not in ("ratio", "poscounts"):
-        raise ValueError("type must be 'ratio' or 'poscounts'")
-    r = size_factor_ratios(y, m, poscounts=type == "poscounts")
+    Raises like the reference when every gene contains a zero (the only host read: one int).
+    controlGenes (a boolean mask with one entry per row, or 0-based row indices; pipeline.controlGeneRows) and
+    geoMeans (one value per row, numpy or a device tensor) as in R, through control_ratios: the median is over the
+    control rows, the stop looks at every row, and with geoMeans the factors are rescaled to geometric mean 1 (type
+    "ratio" only: "poscounts" with geoMeans raises ValueError).  As without them, "poscounts" factors are returned
+    unscaled."""
+    if controlGenes is None and geoMeans is None:
+        if type not in ("ratio", "poscounts"):
+            raise ValueError("type must be 'ratio' or 'poscounts'")
+        r = size_factor_ratios(y, m, poscounts=type == "poscounts")
+        if int(r["n_finite"].item()) == 0:
+            raise _no_finite_loggeomean()
+        return {"sizeFactors": r["sizeFactors"], "loggeomeans": r["loggeomeans"]}
+    r = control_ratios(y, m, type, None, controlGenes, geoMeans)
     if int(r["n_finite"].item()) == 0:
         raise _no_finite_loggeomean()
-    return {"sizeFactors": r["sizeFactors"], "loggeomeans": r["loggeomeans"]}
+    return {"sizeFactors": control_sizes(r), "loggeomeans": r["loggeomeans"]}
+
+
+def _kernel_ratios(y, m, poscounts, divisor, ws):
+    """size_factor_ratios, or for no rows what the median of no rows gives: NaN factors, no ratio, n_finite 0."""
+    if y.shape[0] == 0:
+        dev = y.device
+        return {"sizeFactors": torch.full((m,), math.nan, dtype=F64, device=dev),
+                "ratios": torch.empty((m, 0), dtype=F64, device=dev),
+                "loggeomeans": torch.empty(0, dtype=F64, device=dev),
+                "n_finite": torch.zeros(1, dtype=torch.int32, device=dev)}
+    return size_factor_ratios(y, m, poscounts=poscounts, divisor=divisor, ws=ws)
+
+
+def given_geo_mean_ratios(y, m, loggeomeans, divisor=None):
+    """The (m, n) log ratios of the median against given log geometric means, laid out as the size-factor kernel's
+    ratio scratch: log K_ij - loggeomeans_i (log(K_ij / d_ij) with a gene-major divisor), +Inf where the entry does not
+    take part (loggeomeans_i not finite, or K_ij = 0).  One elementwise pass in torch; the log is torch's."""
+    k = y[:, :m].to(F64)
+    if divisor is not None:
+        k = k / divisor[:, :m]
+    use = torch.isfinite(loggeomeans)[:, None] & (k > 0)
+    return torch.where(use, torch.log(k) - loggeomeans[:, None], math.inf).t().contiguous()
+
+
+def column_medians(ratios):
+    """(m,) exact medians of the rows of an (m, k) ratio matrix over their entries below +Inf, as sf_median_kernel takes
+    them: the lower middle element for an odd count, the mean of the two middle elements for an even one (R's median),
+    NaN for none; and the (m,) counts.  One segmented sort."""
+    m, k = ratios.shape
+    nv = (ratios < math.inf).sum(dim=1)
+    if k == 0:
+        return torch.full((m,), math.nan, dtype=F64, device=ratios.device), nv
+    s = torch.sort(ratios, dim=1)[0]
+    lo = s.gather(1, (torch.clamp(nv - 1, min=0) // 2)[:, None]).squeeze(1)
+    hi = s.gather(1, torch.clamp(nv // 2, max=k - 1)[:, None]).squeeze(1)
+    med = torch.where(nv % 2 == 1, lo, 0.5 * (lo + hi))
+    return torch.where(nv == 0, math.nan, med), nv
+
+
+def control_ratios(y, m, type, divisor, controlGenes, geoMeans):
+    """The ratios estimateSizeFactorsForMatrix takes the median of when controlGenes and / or geoMeans are given
+    (R/core.R:539-572), for size_factors, normalization_factors and their gene-sharded forms.  Checks the arguments
+    (ValueError) and returns {"ratios": (m, k) ratios of the k control rows (+Inf where an entry does not take part),
+    "loggeomeans": (n,) of every row, "n_finite": 1-element device count of the rows whose loggeomeans is not infinite
+    (R stops when it is 0), "sizeFactors": the kernel's medians of "ratios", or None with geoMeans,
+    "incoming": whether geoMeans were given}.
+      * controlGenes only: the size-factor kernel on all rows (loggeomeans and the stop count, exactly as without
+        controlGenes), then on the gathered control rows for the ratios and their medians (its own workspace).  The
+        log geometric means are per row, so the second launch's equal the first's.
+      * geoMeans: loggeomeans = torch.log(geoMeans) (0 gives -Inf, a negative value or NaN gives NaN), the ratios of
+        the control rows (every row without controlGenes) by given_geo_mean_ratios."""
+    from .pipeline import checkGeoMeansType, controlGeneRows
+    checkGeoMeansType(type, geoMeans)
+    n = y.shape[0]
+    dev = y.device
+    rows = None
+    if controlGenes is not None:
+        rows = torch.as_tensor(controlGeneRows(controlGenes, n), device=dev)
+
+    def sub(t):
+        return t if rows is None or t is None else t[rows].contiguous()
+
+    if geoMeans is None:
+        full = _kernel_ratios(y, m, type == "poscounts", divisor, "sf_ratios")
+        part = _kernel_ratios(sub(y), m, type == "poscounts", sub(divisor), "sf_ratios_ctl")
+        return {"ratios": part["ratios"], "loggeomeans": full["loggeomeans"], "n_finite": full["n_finite"],
+                "sizeFactors": part["sizeFactors"], "incoming": False}
+    g = geoMeans if isinstance(geoMeans, torch.Tensor) else torch.as_tensor(np.asarray(geoMeans, dtype=np.float64))
+    if g.dim() != 1 or g.shape[0] != n:
+        raise ValueError("geoMeans should be as long as the number of rows of counts")
+    lg = torch.log(g.to(device=dev, dtype=F64))
+    return {"ratios": given_geo_mean_ratios(sub(y), m, sub(lg), sub(divisor)), "loggeomeans": lg,
+            "n_finite": (~torch.isinf(lg)).sum().reshape(1), "sizeFactors": None, "incoming": True}
+
+
+def rescaled_to_geo_mean_one(sf):
+    """The incoming-geoMeans rescaling sf / exp(mean(log sf)) (R/core.R:573-576): one NaN factor makes all NaN."""
+    return sf / torch.exp(torch.log(sf).mean())
+
+
+def control_sizes(r):
+    """The size factors of control_ratios' result on one device: the kernel's medians, or with geoMeans the exact
+    column medians through the kernel's exp (sharded._sizes_of), rescaled to geometric mean 1."""
+    if r["sizeFactors"] is not None:
+        return r["sizeFactors"]
+    from .sharded import _sizes_of
+    med, nv = column_medians(r["ratios"])
+    return rescaled_to_geo_mean_one(_sizes_of(med, nv))
 
 
 def sf_iterate_objective(y, q, alpha, par, m, h=1e-3, Q=0.05, max_tile_cols=0, out=None):
@@ -156,15 +255,22 @@ def _check_positive_matrix(t, y, m, name):
         raise ValueError(f"{name} must be finite and positive")
 
 
-def normalization_factors(y, m, normMatrix=None, avgTxLength=None, type="ratio"):
+def normalization_factors(y, m, normMatrix=None, avgTxLength=None, type="ratio", controlGenes=None, geoMeans=None):
     """estimateSizeFactors with a normMatrix or an avgTxLength assay (R/methods.R:363-406) on the device: exactly one of
     the two, a gene-major (n, ld) float64 tensor aligned with y.  avgTxLength is first divided by its row geometric
     mean.  estimateNormFactors (R/core.R:2159-2163): the median-of-ratios size factors of K / normMatrix
     (b200nb_size_factors_norm_dev; for "poscounts" the log geometric means come from the raw counts and the factors are
     rescaled to geometric mean 1, R/core.R:573-576), then nf = normMatrix * sf divided by its row geometric mean.
+    controlGenes and geoMeans as in size_factors: the median is over the control rows, given geoMeans are compared with
+    K / normMatrix (and the factors rescaled), and nf is formed for every row.
     Returns {"normalizationFactors": (n, ld) device tensor (padding columns 1), "sizeFactors": (m,)}.
     Raises ValueError for a non-positive / non-finite matrix and when every gene contains a zero."""
     nm, d = norm_divisor(y, m, normMatrix, avgTxLength, type)
+    if controlGenes is not None or geoMeans is not None:
+        r = control_ratios(y, m, type, d, controlGenes, geoMeans)
+        if int(r["n_finite"].item()) == 0:
+            raise _no_finite_loggeomean()
+        return norm_factors_from(nm, d, control_sizes(r), m, type)
     r = size_factor_ratios(y, m, poscounts=type == "poscounts", divisor=d)
     if int(r["n_finite"].item()) == 0:
         raise _no_finite_loggeomean()

@@ -50,16 +50,74 @@ from .wrappers import fitBetaWrapper, fitDispGridWrapper, fitDispWrapper
 LN2 = np.log(2.0)
 
 
-def estimateSizeFactorsForMatrix(counts, type="ratio"):
-    """R/core.R:535-578, locfunc=median.  type "ratio": loggeomeans = rowMeans(log K).  type "poscounts" (as
-    estimateSizeFactors calls it, R/methods.R:377-390): geoMeans = geoMeanNZ per row, log(exp(sum(log K[K > 0]) / m))
-    (0 for an all-zero row), passed as incoming geoMeans, so the factors are rescaled to geometric mean 1 (:573-576)."""
+def controlGeneRows(controlGenes, n):
+    """estimateSizeFactorsForMatrix's `controlGenes` (R/core.R:564-571) as 0-based row indices: a boolean mask with one
+    entry per row, or non-negative integer row indices (numpy, a list or a torch tensor), a duplicated index counting
+    once per occurrence as counts[controlGenes, ] does.  R recycles a short mask, drops negative indices and turns an
+    index past the end into an NA row; those are refused here (ValueError), as is any other type."""
+    if hasattr(controlGenes, "detach"):
+        controlGenes = controlGenes.detach().cpu().numpy()
+    c = np.asarray(controlGenes)
+    if c.ndim != 1:
+        raise ValueError("controlGenes should be a 1-d boolean mask or integer row indices")
+    if c.dtype == np.bool_:
+        if c.shape[0] != n:
+            raise ValueError(f"a controlGenes mask needs one entry per row ({n}), got {c.shape[0]}")
+        return np.flatnonzero(c)
+    if c.size == 0:
+        return np.zeros(0, dtype=np.int64)
+    if not np.issubdtype(c.dtype, np.integer):
+        raise ValueError("controlGenes should be either a boolean mask or integer row indices")
+    if c.min() < 0 or c.max() >= n:
+        raise ValueError(f"controlGenes indices must lie in [0, {n})")
+    return c.astype(np.int64)
+
+
+def logGeoMeans(geoMeans, n):
+    """log(geoMeans) with R's length check (R/core.R:551-556): a zero gives -Inf, a negative value or NaN gives NaN."""
+    g = np.asarray(geoMeans, dtype=np.float64)
+    if g.ndim != 1 or g.shape[0] != n:
+        raise ValueError("geoMeans should be as long as the number of rows of counts")
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.log(g)
+
+
+def checkGeoMeansType(type, geoMeans):
+    """R's estimateSizeFactors replaces given geoMeans by geoMeanNZ for type "poscounts" while
+    estimateSizeFactorsForMatrix uses them: the combination is refused rather than resolved one way."""
     if type not in ("ratio", "poscounts"):
         raise ValueError("type must be 'ratio' or 'poscounts'")
+    if type == "poscounts" and geoMeans is not None:
+        raise ValueError("type 'poscounts' computes its own geoMeans: give geoMeans with type 'ratio'")
+
+
+def _selectedMedianSizes(logc, counts, loggeomeans, controlGenes):
+    """R/core.R:560-572: per sample, exp(median(log K - loggeomeans)) over the (control) rows with a finite loggeomeans
+    and K > 0; NaN for a sample without such a row."""
+    rows = np.arange(counts.shape[0]) if controlGenes is None else controlGeneRows(controlGenes, counts.shape[0])
+    lg, lc, cn = loggeomeans[rows], logc[rows], counts[rows]
+    sf = np.empty(counts.shape[1])
+    for j in range(counts.shape[1]):
+        sel = np.isfinite(lg) & (cn[:, j] > 0)
+        sf[j] = np.exp(np.median(lc[sel, j] - lg[sel])) if sel.any() else np.nan
+    return sf
+
+
+def estimateSizeFactorsForMatrix(counts, type="ratio", geoMeans=None, controlGenes=None):
+    """R/core.R:535-578, locfunc=median.  type "ratio": loggeomeans = rowMeans(log K).  type "poscounts" (as
+    estimateSizeFactors calls it, R/methods.R:377-390): geoMeans = geoMeanNZ per row, log(exp(sum(log K[K > 0]) / m))
+    (0 for an all-zero row), passed as incoming geoMeans, so the factors are rescaled to geometric mean 1 (:573-576).
+    geoMeans: one value per row; loggeomeans = log(geoMeans) and the factors are rescaled the same way (not together
+    with "poscounts", checkGeoMeansType).  controlGenes (controlGeneRows): the median is over these rows only.  The
+    stop "every gene contains at least one zero" looks at the loggeomeans of all rows, so control rows that all
+    contain a zero (or all-negative geoMeans, whose log is NaN, not infinite) give NaN factors instead."""
+    checkGeoMeansType(type, geoMeans)
     counts = np.asarray(counts, dtype=np.float64)
     with np.errstate(divide="ignore"):
         logc = np.log(counts)
-    if type == "poscounts":
+    if geoMeans is not None:
+        loggeomeans = logGeoMeans(geoMeans, counts.shape[0])
+    elif type == "poscounts":
         pos = counts > 0
         s = np.where(pos, logc, 0.0).sum(axis=1)
         with np.errstate(divide="ignore"):
@@ -68,12 +126,8 @@ def estimateSizeFactorsForMatrix(counts, type="ratio"):
         loggeomeans = logc.mean(axis=1)
     if np.all(np.isinf(loggeomeans)):
         raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
-    ok = np.isfinite(loggeomeans)
-    sf = np.empty(counts.shape[1])
-    for j in range(counts.shape[1]):
-        sel = ok & (counts[:, j] > 0)
-        sf[j] = np.exp(np.median(logc[sel, j] - loggeomeans[sel]))
-    if type == "poscounts":
+    sf = _selectedMedianSizes(logc, counts, loggeomeans, controlGenes)
+    if type == "poscounts" or geoMeans is not None:
         sf = sf / np.exp(np.mean(np.log(sf)))
     return sf
 
@@ -175,13 +229,14 @@ def _div(sizeFactors):
     return sf if sf.ndim == 2 else sf[None, :]
 
 
-def estimateNormFactors(counts, normMatrix, type="ratio"):
+def estimateNormFactors(counts, normMatrix, type="ratio", geoMeans=None, controlGenes=None):
     """R/core.R:2159-2163 as estimateSizeFactors calls it (R/methods.R:377-402), in the reference's formula order:
     the median-of-ratios size factors of counts / normMatrix -- for type "poscounts" with the geoMeans of the raw
     counts, log(exp(sum(log K[K > 0]) / m)), and the incoming-geoMeans rescaling sf / exp(mean(log sf))
-    (R/core.R:573-576) -- then nf = normMatrix * sf divided by its row geometric mean."""
-    if type not in ("ratio", "poscounts"):
-        raise ValueError("type must be 'ratio' or 'poscounts'")
+    (R/core.R:573-576) -- then nf = normMatrix * sf divided by its row geometric mean.  geoMeans and controlGenes as
+    in estimateSizeFactorsForMatrix: the given geoMeans are compared with counts / normMatrix, the median is over the
+    control rows, and nf is formed for every row."""
+    checkGeoMeansType(type, geoMeans)
     counts = np.asarray(counts, dtype=np.float64)
     nm = np.asarray(normMatrix, dtype=np.float64)
     if nm.shape != counts.shape or not np.all(np.isfinite(nm) & (nm > 0)):
@@ -189,21 +244,19 @@ def estimateNormFactors(counts, normMatrix, type="ratio"):
     cnts = counts / nm
     m = counts.shape[1]
     with np.errstate(divide="ignore"):
-        if type == "poscounts":
+        logc = np.log(cnts)
+        if geoMeans is not None:
+            loggeomeans = logGeoMeans(geoMeans, counts.shape[0])
+        elif type == "poscounts":
             pos = counts > 0
             s = np.where(pos, np.log(np.where(pos, counts, 1.0)), 0.0).sum(axis=1)
-            geoMeans = np.where(pos.any(axis=1), np.exp(s / m), 0.0)
-            loggeomeans = np.log(geoMeans)
+            loggeomeans = np.log(np.where(pos.any(axis=1), np.exp(s / m), 0.0))
         else:
-            loggeomeans = np.log(cnts).mean(axis=1)
-        if np.all(np.isinf(loggeomeans)):
-            raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
-        ok = np.isfinite(loggeomeans)
-        sf = np.empty(m)
-        for j in range(m):
-            sel = ok & (cnts[:, j] > 0)
-            sf[j] = np.exp(np.median(np.log(cnts[sel, j]) - loggeomeans[sel]))
-    if type == "poscounts":
+            loggeomeans = logc.mean(axis=1)
+    if np.all(np.isinf(loggeomeans)):
+        raise ValueError("every gene contains at least one zero, cannot compute log geometric means")
+    sf = _selectedMedianSizes(logc, cnts, loggeomeans, controlGenes)
+    if type == "poscounts" or geoMeans is not None:
         sf = sf / np.exp(np.mean(np.log(sf)))
     nf = nm * sf[None, :]
     return nf / np.exp(np.log(nf).mean(axis=1))[:, None]

@@ -366,7 +366,24 @@ def _sizes_of(med, nv):
     return torch.where(nv == 0, torch.nan, sf)
 
 
-def sharded_size_factors_device(y_local, m, type="ratio"):
+def _control_local(y_local, m, type, divisor, controlGenes_local, geoMeans_local):
+    """device_pipeline.control_ratios on this shard, with its ValueError held rather than raised, so that the rank
+    still joins the agreement all-reduce (which carries the failure to every rank): returns (ratios dict, error)."""
+    from . import device_pipeline as DP
+    try:
+        return DP.control_ratios(y_local, m, type, divisor, controlGenes_local, geoMeans_local), None
+    except ValueError as e:
+        return _local_ratios(y_local[:0], m, False), e
+
+
+def _raise_failed(err, failed, what):
+    if err is not None:
+        raise err
+    if failed:
+        raise ValueError(f"{what}: the arguments of {failed} other rank(s) failed their checks")
+
+
+def sharded_size_factors_device(y_local, m, type="ratio", controlGenes_local=None, geoMeans_local=None):
     """estimateSizeFactorsForMatrix (R/core.R:535-578, locfunc = median) over the genes of ALL ranks, y_local being this
     rank's rows (gene-major, split as shard_bounds splits them).  The log geometric means are per gene and the log
     ratios are the size-factor kernel's own (b200nb_size_factors_dev, whose column-major ratio scratch it reads); the
@@ -375,8 +392,26 @@ def sharded_size_factors_device(y_local, m, type="ratio"):
     geometric mean 1 (the incoming-geoMeans step, R/core.R:573-576) exactly as DESeq_device does.  A sample with no
     usable ratio gets NaN.  "Every gene contains at least one zero" is decided on the count of finite log geometric
     means of all ranks and raises ValueError on every rank.  Returns {"sizeFactors": (m,) device tensor, "loggeomeans":
-    this shard's (n_local,), "collectives": 9 (one agreement all-reduce and 8 histogram rounds)}."""
+    this shard's (n_local,), "collectives": 9 (one agreement all-reduce and 8 histogram rounds)}.
+    controlGenes_local (a mask or 0-based indices into this rank's rows) and geoMeans_local (this rank's rows; when
+    geoMeans are used every rank passes its part, an empty one for an empty shard) as in device_pipeline.size_factors:
+    the ratios are control_ratios' (the kernel's on the gathered control rows, or given_geo_mean_ratios), the median is
+    _global_median over the control entries of every rank, the stop count is over every row of every rank, and with
+    geoMeans the factors are rescaled to geometric mean 1.  Every rank then gets the single-device size_factors of the
+    whole matrix and its control rows, bit for bit (rescaled for "poscounts" as above).  Arguments that fail their
+    checks on one rank raise ValueError on every rank; the count of collectives stays 9."""
     from . import device_pipeline as DP
+    if controlGenes_local is not None or geoMeans_local is not None:
+        r, err = _control_local(y_local, m, type, None, controlGenes_local, geoMeans_local)
+        nv, n_finite, failed, entries = _agree(r, failed=err is not None)
+        _raise_failed(err, failed, "size_factors")
+        if n_finite == 0:
+            raise DP._no_finite_loggeomean()
+        med, c = _global_median(entries, nv)
+        sf = _sizes_of(med, nv)
+        if type == "poscounts" or r["incoming"]:
+            sf = DP.rescaled_to_geo_mean_one(sf)
+        return {"sizeFactors": sf, "loggeomeans": r["loggeomeans"], "collectives": 1 + c}
     if type not in ("ratio", "poscounts"):
         raise ValueError("type must be 'ratio' or 'poscounts'")
     r = _local_ratios(y_local, m, type == "poscounts")
@@ -390,30 +425,36 @@ def sharded_size_factors_device(y_local, m, type="ratio"):
     return {"sizeFactors": sf, "loggeomeans": r["loggeomeans"], "collectives": 1 + c}
 
 
-def sharded_normalization_factors(y_local, m, normMatrix_local=None, avgTxLength_local=None, type="ratio"):
+def sharded_normalization_factors(y_local, m, normMatrix_local=None, avgTxLength_local=None, type="ratio",
+                                  controlGenes_local=None, geoMeans_local=None):
     """device_pipeline.normalization_factors over the genes of ALL ranks (estimateNormFactors, R/core.R:2159-2163, and
     the avgTxLength path): normMatrix_local / avgTxLength_local are this shard's rows, gene-major like y_local.  The size
     factors of K / normMatrix come from the global median of sharded_size_factors_device; everything else is per gene.
+    controlGenes_local / geoMeans_local as in sharded_size_factors_device.
     A matrix that fails its checks on any rank raises ValueError on every rank (the failure travels in the agreement
     all-reduce).  Returns {"normalizationFactors": this shard's (n_local, ld), "sizeFactors": (m,), "collectives": 9},
     which sharded_DESeq_device(normalizationFactors=...) and the sharded transforms take."""
     from . import device_pipeline as DP
     err = None
+    chosen = controlGenes_local is not None or geoMeans_local is not None
     try:
         nm, d = DP.norm_divisor(y_local, m, normMatrix_local, avgTxLength_local, type)
-        r = _local_ratios(y_local, m, type == "poscounts", divisor=d)
+        if chosen:
+            r, err = _control_local(y_local, m, type, d, controlGenes_local, geoMeans_local)
+        else:
+            r = _local_ratios(y_local, m, type == "poscounts", divisor=d)
     except ValueError as e:
         err = e
         r = _local_ratios(y_local[:0], m, False)
     nv, n_finite, failed, entries = _agree(r, failed=err is not None)
-    if err is not None:
-        raise err
-    if failed:
-        raise ValueError(f"normalization_factors: the arguments of {failed} other rank(s) failed their checks")
+    _raise_failed(err, failed, "normalization_factors")
     if n_finite == 0:
         raise DP._no_finite_loggeomean()
     med, c = _global_median(entries, nv)
-    out = DP.norm_factors_from(nm, d, _sizes_of(med, nv), m, type)
+    sf = _sizes_of(med, nv)
+    if chosen and r["incoming"]:
+        sf = DP.rescaled_to_geo_mean_one(sf)
+    out = DP.norm_factors_from(nm, d, sf, m, type)
     out["collectives"] = 1 + c
     return out
 
