@@ -557,13 +557,17 @@ def _grid_refit(y, xd, mu, sel, m, prior_mean, prior_sigmasq, usePrior, weights=
 
 
 def getContrast_device(ynz, x, sizeFactors, dispersion, betaMatrix, contrast, betaPriorVar=None, minmu=0.5,
-                       weights=None, normalizationFactors=None):
+                       weights=None, normalizationFactors=None, useT=False, df=None):
     """getContrast (R/results.R:760-827) on device tensors: fitBeta's maxit = 0 mode (covariance at the given betas).
     ynz: gene-major counts the model was fitted to; betaMatrix: (n, p) log2-scale coefficients (DESeq_device's
     "betaMatrix").  weights: gene-major (n, ld) float64 observation weights of the same rows (raw, or DESeq_device's
     normalised "weights"), normalised by the row maximum and passed to fitBeta without the rank tests, as in the
     reference.  normalizationFactors: gene-major (n, ld) float64 factors of the same rows, in place of sizeFactors
-    (None then).  Returns log2FoldChange, lfcSE, stat, pvalue as device tensors."""
+    (None then).  useT: the p-value is 2 pt(|stat|, df, lower.tail = FALSE) (t_wald_pvalue, R/results.R:812-816) with
+    df the rows' t degrees of freedom (a DESeq_device(useT=True) result's "tDegreesFreedom"); useT without df raises
+    ValueError, as R's stopifnot.  Returns log2FoldChange, lfcSE, stat, pvalue as device tensors."""
+    if useT and df is None:
+        raise ValueError("useT=True needs the t degrees of freedom (tDegreesFreedom) of the rows")
     dev = ynz.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
@@ -579,7 +583,8 @@ def getContrast_device(ynz, x, sizeFactors, dispersion, betaMatrix, contrast, be
                    1e-8, 0, useQR=False, minmu=minmu, weights=wn, want_hat=False, want_mu=False)
     est, se = r["contrast_num"] / LN2, r["contrast_denom"] / LN2
     stat = est / se
-    return {"log2FoldChange": est, "lfcSE": se, "stat": stat, "pvalue": wald_pvalue(stat)}
+    return {"log2FoldChange": est, "lfcSE": se, "stat": stat,
+            "pvalue": t_wald_pvalue(stat, df) if useT else wald_pvalue(stat)}
 
 
 def wald_pvalue(stat):
@@ -588,6 +593,193 @@ def wald_pvalue(stat):
     DBL_MIN, subnormal beyond |stat| = 37.5, 1 at 0, 0 at +-inf, NaN at NaN.  torch's ndtr is (1 + erf(x / sqrt 2)) / 2,
     which cancels: its p-values are multiples of about 1.1e-16 and reach 0 from |stat| = 8.3 on."""
     return torch.erfc(stat.abs() * 0.7071067811865476)
+
+
+# lgamma(z) - ((z - 1/2) log z - z + log(2 pi) / 2) = sum_k B_2k / (2k (2k - 1) z^(2k - 1)): the first eight terms,
+# whose truncation error is below 1e-17 for z >= 10
+_STIRLING = (1.0 / 12.0, -1.0 / 360.0, 1.0 / 1260.0, -1.0 / 1680.0, 1.0 / 1188.0, -691.0 / 360360.0, 1.0 / 156.0,
+             -3617.0 / 122400.0)
+_SQRT_PI = 1.7724538509055160
+_T_CHUNK = 8            # continued-fraction steps between two checks of which genes are still iterating
+_T_MAXIT = 20000
+
+
+def _stirling_delta(z):
+    r = 1.0 / z
+    r2 = r * r
+    s = torch.full_like(z, _STIRLING[-1])
+    for c in _STIRLING[-2::-1]:
+        s = s * r2 + c
+    return s * r
+
+
+def _gamma_ratio_half(a):
+    """Gamma(a + 1/2) / Gamma(a) for a > 0 to a few ulps, without lgamma (whose absolute error, relative to the ratio,
+    is ~lgamma(a) ulps): for b = a + k >= 10 it is sqrt(b) exp(b log1p(1 / (2b)) - 1/2 + delta(b + 1/2) - delta(b))
+    (Stirling's series; the exponent is O(1/b), so its rounding costs nothing), and below 10 the recurrence
+    Gamma(a + 1/2) / Gamma(a) = Gamma(b + 1/2) / Gamma(b) prod_{j < k} (a + j) / (a + j + 1/2)."""
+    k = torch.clamp(torch.ceil(10.0 - a), min=0.0)
+    b = a + k
+    r = torch.sqrt(b) * torch.exp(b * torch.log1p(0.5 / b) - 0.5 + _stirling_delta(b + 0.5) - _stirling_delta(b))
+    for j in range(10):
+        r = torch.where(k > j, r * ((a + j) / (a + j + 0.5)), r)
+    return r
+
+
+def _beta_cf(a, b, x):
+    """The continued fraction of I_x(a, b) (modified Lentz, as in Numerical Recipes' betacf), elementwise over 1-D
+    tensors, each element iterating until its step changes the value by at most an ulp.  The coefficients are formed
+    as products of ratios, so that no intermediate overflows for any finite a.  Steps run _T_CHUNK at a time on the
+    elements still iterating; each chunk costs one host read (how many are left)."""
+    tiny = 1e-300
+    h = torch.empty_like(x)
+    ix = torch.arange(x.numel(), device=x.device)
+    qab, qap, qam = a + b, a + 1.0, a - 1.0
+    d = 1.0 - (qab / qap) * x
+    d = 1.0 / torch.where(d.abs() < tiny, tiny, d)
+    c, hh = torch.ones_like(x), d
+    m = 1
+    while ix.numel() and m <= _T_MAXIT:
+        done = torch.zeros_like(x, dtype=torch.bool)
+        for _ in range(_T_CHUNK):
+            m2 = 2.0 * m
+            for coef in ((m / (qam + m2)) * ((b - m) / (a + m2)) * x,
+                         -((a + m) / (a + m2)) * ((qab + m) / (qap + m2)) * x):
+                d = 1.0 + coef * d
+                d = 1.0 / torch.where(d.abs() < tiny, tiny, d)
+                c = 1.0 + coef / c
+                c = torch.where(c.abs() < tiny, tiny, c)
+                step = d * c
+                hh = torch.where(done, hh, hh * step)
+            done = done | ((step - 1.0).abs() <= 2.3e-16)
+            m += 1
+        fin = torch.nonzero(done).squeeze(1)
+        h[ix[fin]] = hh[fin]
+        left = torch.nonzero(~done).squeeze(1)
+        ix, a, b, x, qab, qap, qam, c, d, hh = (t[left] for t in (ix, a, b, x, qab, qap, qam, c, d, hh))
+    h[ix] = hh
+    return h
+
+
+def _expansion_coefs(b=0.5, n=30):
+    """The constants d_n of the large-a expansion of I_x(a, b) (Didonato and Morris 1992, ACM TOMS 708, section 9):
+    c_n = c_(n-1) / (2n (2n + 1)), c_0 = 1, d_n = (b - 1) c_n + (1 / n) sum_(i < n) (i b - n) c_i d_(n - i)."""
+    c, d, cn = [], [], 1.0
+    for k in range(1, n + 1):
+        cn /= (2.0 * k) * (2.0 * k + 1.0)
+        c.append(cn)
+        d.append((b - 1.0) * cn + sum((i * b - k) * c[i - 1] * d[k - 1 - i] for i in range(1, k)) / k)
+    return d
+
+
+_EXPANSION_D = _expansion_coefs()
+
+
+def _t_two_sided_expansion(q, df):
+    """I_x(a, 1/2), a = df / 2, x = df / (df + q^2), by the asymptotic expansion for large a and b <= 1 of
+    Didonato and Morris (TOMS 708, section 9) with b = 1/2, where the incomplete gamma function it rests on is
+    Q(1/2, z) = erfc(sqrt z): I = erfc(sqrt z) Gamma(a + 1/2) / (Gamma(a) sqrt(T)) (1 + sum_n d_n J_n / J_0),
+    T = a - 1/4, z = -T log x, J_0 = sqrt(pi) erfcx(sqrt z) / sqrt z and
+    J_n = ((2n - 3/2)(2n - 1/2) J_(n-1) + (z + 2n - 1/2) (log(x) / 2)^(2n - 2)) / (4 T^2).  Every input is a
+    function of log x = -log1p(q^2 / df), never of a rounded x, so large df loses nothing to the rounding of x (the
+    continued fraction in x would lose about df / 2 ulps); the relative error stays within an ulp or two of the tail's
+    condition number.  Used for df >= 20 where log1p(q^2 / df) <= 1, where the series converges within 30 terms."""
+    a = 0.5 * df
+    T = a - 0.25
+    lnx = -torch.log1p(q * q / df)
+    z = -T * lnx
+    sz = torch.sqrt(z)
+    inv_j0 = sz / (torch.special.erfcx(sz) * _SQRT_PI)
+    v = 0.25 / (T * T)
+    t2 = 0.25 * lnx * lnx
+    k, t, s = torch.ones_like(q), torch.ones_like(q), torch.ones_like(q)
+    for n, dn in enumerate(_EXPANSION_D):
+        bp = 0.5 + 2.0 * n
+        k = (bp * (bp + 1.0) * k + (z + bp + 1.0) * t * inv_j0) * v
+        t = t * t2
+        term = dn * k
+        s = s + term
+        if n % 6 == 5 and not bool(((term.abs() > 1e-17 * s.abs()) & torch.isfinite(s)).any()):
+            break
+    return torch.erfc(sz) * (_gamma_ratio_half(a) / torch.sqrt(T)) * s
+
+
+def _t_two_sided_cf(q, df):
+    """I_x(a, 1/2), a = df / 2, x = df / (df + q^2), by continued fractions, for the df < 20 and the far tails the
+    expansion does not take.  Where x < (a + 1) / (a + 5/2) the continued fraction of I_x(a, 1/2) gives the tail
+    itself; beyond, 1 - I_y(1/2, a) with y = 1 - x (Numerical Recipes' rule).  The factor x^a is
+    exp(-a log1p(q^2 / df)) while log1p(q^2 / df) <= 2 (its error is then a log1p(...) ulps, the tail's own
+    condition); beyond, r^df (1 + r^2)^-a with r = sqrt(df) / q, whose error is about df ulps, which is the tail's
+    condition there, where the exp of a large logarithm would lose its size in ulps.  sqrt(y) = 1 / sqrt(1 + r^2), so
+    neither q^2 overflowing nor q = inf yields NaN."""
+    a = 0.5 * df
+    q2 = q * q
+    r = torch.sqrt(df) / q
+    L = torch.log1p(q2 / df)
+    xa = torch.where(L <= 2.0, torch.exp(-a * L), torch.pow(r, df) * torch.exp(-a * torch.log1p(r * r)))
+    sy = torch.rsqrt(1.0 + r * r)
+    ratio = _gamma_ratio_half(a)
+    x = 1.0 / (1.0 + q2 / df)
+    y = 1.0 / (1.0 + r * r)
+    direct = x < (a + 1.0) / (a + 2.5)
+    half = torch.full_like(q, 0.5)
+    h = _beta_cf(torch.where(direct, a, half), torch.where(direct, half, a), torch.where(direct, x, y))
+    tail = xa * sy * (ratio / (a * _SQRT_PI)) * h                   # I_x(a, 1/2) = x^a y^(1/2) / (a B(a, 1/2)) cf
+    body = 1.0 - xa * sy * (2.0 * ratio / _SQRT_PI) * h             # 1 - y^(1/2) x^a / (B(1/2, a) / 2) cf
+    return torch.where(direct, tail, body)
+
+
+def _t_two_sided_finite(q, df):
+    """2 pt(q, df, lower.tail = FALSE) = I_x(df / 2, 1/2) for 1-D tensors q > 0 (not NaN) and finite df > 0: the
+    expansion where df >= 20 and log1p(q^2 / df) <= 1, the continued fractions elsewhere."""
+    out = torch.empty_like(q)
+    exp_rows = (df >= 20.0) & (torch.log1p(q * q / df) <= 1.0)
+    for rows, fn in ((torch.nonzero(exp_rows).squeeze(1), _t_two_sided_expansion),
+                     (torch.nonzero(~exp_rows).squeeze(1), _t_two_sided_cf)):
+        if rows.numel():
+            out[rows] = fn(q[rows], df[rows])
+    return out
+
+
+def _t_two_sided(q, df):
+    """2 pt(|q|, df, lower.tail = FALSE) on broadcast tensors, and the masks of infinite and of invalid df.  Only the
+    elements with a finite df > 0 and a non-NaN q reach the continued fraction."""
+    q, df = torch.broadcast_tensors(q.to(F64), torch.as_tensor(df, dtype=F64, device=q.device))
+    q, df = q.abs().reshape(-1), df.reshape(-1)
+    inf_df = torch.isinf(df) & (df > 0)
+    bad = ~(df > 0)
+    out = torch.full_like(q, math.nan)
+    out = torch.where(q == 0, 1.0, out)
+    run = torch.nonzero(~inf_df & ~bad & (q > 0)).squeeze(1)
+    if run.numel():
+        out[run] = _t_two_sided_finite(q[run], df[run])
+    return out, inf_df, bad
+
+
+def t_upper(q, df):
+    """R's pt(q, df, lower.tail = FALSE) on device tensors for any real df > 0 (q and df broadcast; df a per-gene
+    vector, a tensor or a float): for q >= 0 half of the two-sided tail _t_two_sided_finite computes, for q < 0 one
+    minus that.  df = Inf gives the normal tail erfc(q / sqrt 2) / 2; df NaN or <= 0 gives NaN, as R gives NA.  The
+    relative error is a few ulps plus the tail's condition number |q f(q) / (1 - F(q))| in ulps down to DBL_MIN
+    (DESIGN.md, p-value accuracy).  R switches to a normal approximation above df = 4e5; this stays exact there.
+    The work is a masked continued fraction in torch, a few dozen steps for most elements, with one host read per
+    _T_CHUNK steps."""
+    shape = torch.broadcast_shapes(q.shape, torch.as_tensor(df).shape)
+    qf = q.to(F64).expand(shape).reshape(-1)
+    two, inf_df, bad = _t_two_sided(q, df)
+    up = torch.where(qf >= 0, 0.5 * two, 1.0 - 0.5 * two)
+    up = torch.where(inf_df, 0.5 * torch.erfc(qf * 0.7071067811865476), up)
+    return torch.where(bad, math.nan, up).reshape(shape)
+
+
+def t_wald_pvalue(stat, df):
+    """nbinomWaldTest's and getContrast's useT p-value 2 pt(|stat|, df, lower.tail = FALSE) (R/core.R:1505,
+    R/results.R:815) on device tensors: the two-sided tail of t_upper without the halving; rows with df = Inf get
+    wald_pvalue's bits, df NaN or <= 0 gives NaN.  stat: (n,) or (p, n) with df (n,) broadcast along the last axis."""
+    two, inf_df, bad = _t_two_sided(stat, df)
+    shape = torch.broadcast_shapes(stat.shape, torch.as_tensor(df).shape)
+    norm = wald_pvalue(stat.to(F64).expand(shape).reshape(-1))
+    return torch.where(bad, math.nan, torch.where(inf_df, norm, two)).reshape(shape)
 
 
 def _size_or_norm_factors(y, m, sizeFactors, normalizationFactors, weights):
@@ -934,7 +1126,7 @@ def _wald_stats(fit):
 def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6, maxit=100, betaTol=1e-8, minmu=0.5,
                  outlierSD=2.0, minReplicatesForReplace=np.inf, allgather=None, useOptim=True, betaPrior=False,
                  factors=None, weights=None, weightThreshold=1e-2, normalizationFactors=None, avgTxLength=None,
-                 nfXim=None, sfType="ratio", fitType="parametric", test="Wald", reduced=None):
+                 nfXim=None, sfType="ratio", fitType="parametric", test="Wald", reduced=None, useT=False, df=None):
     """y: gene-major (N, ld) device tensor of counts (int32 or float64).  Returns a dict of device tensors over the
     rows with a non-zero sum (`idx` maps them back to the N input rows) plus the trend / prior scalars.
     sizeFactors: (m,) numpy or a device tensor (read to the host once); None estimates them on the device first
@@ -986,7 +1178,14 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     p_r), "df", "fullBetaConv" (= betaConv), "reducedBetaConv" and "reducedModelMatrix".  With outlier replacement the
     refitted rows get the reduced fit too and their LRT columns are overwritten (R/core.R:2530-2531).  R's stops
     raise ValueError: no reduced, betaPrior=True, p_r >= p, a model matrix that is not full rank, and reduced with
-    test="Wald".  "test" reports the test ("Wald" or "LRT") for results_device."""
+    test="Wald".  "test" reports the test ("Wald" or "LRT") for results_device.
+    useT=True (test="Wald"; ignored by the LRT, as in R): nbinomWaldTest's Student t p-values (R/core.R:1478-1508):
+    every WaldPvalue column is 2 pt(|stat|, df, lower.tail = FALSE) (t_wald_pvalue) and "tDegreesFreedom" (rows in
+    idx) is added, which results_device / getContrast_device then use.  df: a scalar or one value per input row (the
+    rows of y), subset to idx; by default m - p (p = ncol(x), the standard design's count also with betaPrior), with
+    weights the row sums of the normalised weights minus p.  df <= 0 or NaN gives NaN (R's NA).  The rows an outlier
+    refit replaces get normal p-values and keep the first fit's df, as refitWithoutOutliers does (it does not pass
+    useT on); rows whose replaced counts are all zero get NaN."""
     dev = y.device
     x = np.asarray(x, dtype=np.float64)
     m, p = x.shape
@@ -1166,6 +1365,9 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
         res["weightsFail"], res["weights"] = weightsFail, wn
     if nf is not None:
         res["normalizationFactors"] = sfd
+    if useT and test == "Wald":
+        res["tDegreesFreedom"] = t_degrees_freedom(df, y.shape[0], idx, m, p, wn)
+        res["WaldPvalue"] = t_wald_pvalue(res["WaldStatistic"], res["tDegreesFreedom"][:, None])
     if do_replace and m > p:
         _replace_and_refit(res, ynz, ck["cooks"], x, sizeFactors, sfd, tr, minReplicatesForReplace, minDisp=minDisp,
                            kappa_0=kappa_0, dispTol=dispTol, maxit=maxit, betaTol=betaTol, minmu=minmu,
@@ -1173,6 +1375,25 @@ def DESeq_device(y, x, sizeFactors=None, minDisp=1e-8, kappa_0=1.0, dispTol=1e-6
     if test == "LRT":
         res["fullBetaConv"] = res["betaConv"]
     return res
+
+
+def t_degrees_freedom(df, N, idx, m, p, wn=None):
+    """nbinomWaldTest's t degrees of freedom (R/core.R:1478-1504) for the rows idx of N input rows, as an (n,)
+    device tensor: a given df (a scalar, or one value per input row, subset to idx), else m - p, or with the
+    normalised weights wn of the rows rowSums(wn) - p; NaN where it is not > 0 (ifelse(df > 0, df, NA))."""
+    dev = idx.device
+    n = idx.numel()
+    if df is None:
+        tdf = (wn[:, :m].sum(dim=1) if wn is not None else torch.full((n,), float(m), dtype=F64, device=dev)) - p
+    else:
+        d = torch.as_tensor(df, dtype=F64).to(dev).reshape(-1)
+        if d.numel() == 1:
+            tdf = d.expand(n).clone()
+        elif d.numel() == N:
+            tdf = d[idx]
+        else:
+            raise ValueError(f"df must be a scalar or have one value per row of the counts ({N}), got {d.numel()}")
+    return torch.where(tdf > 0, tdf, math.nan)
 
 
 def _fit_with_prior(ynz, factors, sfd, dispersion, mle, bm, bm_all, dispFit_all, allgather, betaTol, maxit, minmu,
@@ -1288,6 +1509,8 @@ def _replace_and_refit(res, ynz, cooksm, x, sizeFactors, sfd, tr, minReplicates,
             sub["LRTStatistic"], sub["LRTPvalue"] = _lrt_stats(ll["logLike"], red["logLike"], res["df"])
             sub["reducedBetaConv"] = red["conv"]
             results_cols += ["LRTStatistic", "LRTPvalue"]
+        if "tDegreesFreedom" in res:                    # a "results" column, kept for the refitted rows (:2524-2534)
+            results_cols.append("tDegreesFreedom")
         for k, v in sub.items():
             res[k] = res[k].clone()
             res[k][rr] = v.to(res[k].dtype)
@@ -1791,7 +2014,11 @@ def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcT
     test: as R's results(test =), by default the test DESeq_device ran (res["test"]).  An LRT result
     (DESeq_device(test="LRT")) gives its LRTStatistic / LRTPvalue with the selected column's log2FoldChange / lfcSE;
     test="Wald" on it gives the Wald columns (makeWaldTest).  test="LRT" on a Wald result, and lrt= with an LRT result,
-    raise ValueError."""
+    raise ValueError.
+    A result with "tDegreesFreedom" (DESeq_device(useT=True)) is tested with t tails, as R infers useT from that column
+    (R/results.R:414): a stored Wald column keeps its p-values, a contrast goes through getContrast_device(useT=True),
+    and a thresholded test (R/results.R:477-518) takes pt at each gene's df (threshold_t_pvalue) from the kernel's
+    log2FoldChange / lfcSE, keeping the kernel's NaN (Cook's cutoff) and 1 (rows all zero once replaced)."""
     from scipy import stats as _st
     from .pipeline import check_filter_args, results_checks, resultsSelection
     dev = y.device
@@ -1823,6 +2050,7 @@ def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcT
     nf = res.get("normalizationFactors")
     sfd = nf if nf is not None else torch.as_tensor(res["sizeFactors"], device=dev)
     replace = res.get("replace") if res.get("n_replaced", 0) > 0 else None
+    tdf = res.get("tDegreesFreedom")
     # ---- the selected column (cleanContrast / getCoef)
     if sel["kind"] == "coef":
         k = sel["col"]
@@ -1840,7 +2068,7 @@ def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcT
             ycnt[rows, :m] = _replacement_counts(ys, nfm, ck[:, :m] > cutoff, res["replaceable"], m)
         g = getContrast_device(ycnt, xf, None if nf is not None else res["sizeFactors"], res["dispersion"],
                                res["betaMatrix"], sel["vec"], betaPriorVar=res.get("betaPriorVar"), minmu=minmu,
-                               weights=res.get("weights"), normalizationFactors=nf)
+                               weights=res.get("weights"), normalizationFactors=nf, useT=tdf is not None, df=tdf)
         cols = [g[key].contiguous() for key in ("log2FoldChange", "lfcSE", "stat", "pvalue")]
     if lrt is not None:
         cols[2], cols[3] = lrt["LRTStatistic"].contiguous(), lrt["LRTPvalue"].contiguous()
@@ -1861,6 +2089,12 @@ def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcT
                                      cooksCutoff=cutoff, keep=keep,
                                      replace=None if replace is None else replace.to(torch.int32),
                                      baseMean=res["baseMean"])
+    if thresholded and tdf is not None:
+        tp = threshold_t_pvalue(lfc, se, float(lfcThreshold), altHypothesis, tdf)
+        keep_kernel = torch.isnan(pv) | torch.isinf(tdf)     # Cook's NaN; df = Inf: the kernel's normal tail
+        if replace is not None:
+            keep_kernel = keep_kernel | (replace & (res["baseMean"] == 0))
+        pv = torch.where(keep_kernel, pv, tp)
     # ---- all N rows (buildDataFrameWithNARows), then pvalueAdjustment
     out = {"baseMean": torch.zeros(N, dtype=F64, device=dev)}
     out["baseMean"][idx] = res["baseMean"]
@@ -1888,6 +2122,23 @@ def results_device(res, y, x, name=None, contrast=None, listValues=(1, -1), lfcT
     meta["lfcThreshold"] = lfcThreshold
     out["metadata"] = meta
     return out
+
+
+def threshold_t_pvalue(lfc, se, T, altHypothesis, df):
+    """results()' lfcThreshold p-values with useT (R/results.R:477-518) on device tensors: pt at each gene's df in
+    place of pnorm, for the five altHypothesis forms; greaterAbs is pt((T - |lfc|) / se) + pt((-|lfc| - T) / se),
+    lower tails, taken as t_upper of the negated quantiles.  (R evaluates that form through mapply over the genes with
+    the whole df vector, which yields an n x n matrix; its diagonal, each gene at its own df, is what this returns.)"""
+    up = lambda q: t_upper(q, df)
+    if altHypothesis == "greaterAbs":
+        return up((lfc.abs() - T) / se) + up((lfc.abs() + T) / se)
+    if altHypothesis == "greaterAbs2014":
+        return torch.clamp(2.0 * up((lfc.abs() - T) / se), max=1.0)
+    if altHypothesis == "lessAbs":
+        return torch.maximum(up((T - lfc) / se), up((lfc + T) / se))
+    if altHypothesis == "greater":
+        return up((lfc - T) / se)
+    return up((-T - lfc) / se)
 
 
 # ---------------------------------------------------------------- lfcShrink(type = "normal") (R/lfcShrink.R:145-327)

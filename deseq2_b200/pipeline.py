@@ -753,15 +753,65 @@ def fitNbinomGLMs(counts, nf, x, alpha_hat, lambda_=None, engine=None, betaTol=1
             "betaIter": betaRes["iter"], "hat_diagonals": betaRes["hat_diagonals"], "betaRes": betaRes}
 
 
+def r_pt_upper(q, df):
+    """pt(q, df, lower.tail = FALSE) for any real df > 0 (q and df broadcast): the upper tail at |q| by scipy's stdtr,
+    or for |q| < 1 as (1 - I_y(1/2, df / 2)) / 2, y = q^2 / (df + q^2), by scipy's betainc (stdtr loses ~100 ulps
+    at df = 1, q = 1e-3); the normal tail ndtr(-|q|) at df = Inf; q < 0 as one minus that; NaN where df is NaN or
+    <= 0 (R's NA)."""
+    q, df = np.broadcast_arrays(np.asarray(q, dtype=np.float64), np.asarray(df, dtype=np.float64))
+    with np.errstate(invalid="ignore", divide="ignore"):
+        ok = df > 0
+        d = np.where(ok, df, 1.0)
+        a = np.abs(q)
+        body = 0.5 * (1.0 - _sp.betainc(0.5, 0.5 * d, a * a / (d + a * a)))
+        up = np.where(a < 1.0, body, _sp.stdtr(d, -a))
+        up = np.where(np.isinf(df), _sp.ndtr(-a), up)
+        p = np.where(q >= 0, up, 1.0 - up)
+    return np.where(ok, p, np.nan)
+
+
+def waldPvalue(stat, df=None):
+    """nbinomWaldTest's p-value: 2 pnorm(|stat|, lower.tail = FALSE), or with the t degrees of freedom df (one per
+    row, broadcast along the columns) 2 pt(|stat|, df, lower.tail = FALSE) (R/core.R:1478-1508), whose df = Inf rows
+    equal the normal ones."""
+    if df is None:
+        return 2.0 * _sp.ndtr(-np.abs(stat))
+    d = np.asarray(df, dtype=np.float64)
+    d = d[:, None] if np.ndim(stat) == 2 else d
+    return np.where(np.isinf(d), 2.0 * _sp.ndtr(-np.abs(stat)), 2.0 * r_pt_upper(np.abs(stat), d))
+
+
+def tDegreesFreedom(df, N, nz, m, p, weights=None):
+    """nbinomWaldTest's t degrees of freedom over the rows nz of N (R/core.R:1478-1504): a given df (scalar, or one
+    value per row, subset to nz), else m - p, or rowSums(weights) - p with the normalised weights of those rows; NA
+    (NaN) where not > 0."""
+    n = int(np.sum(nz))
+    if df is None:
+        d = (np.asarray(weights).sum(axis=1) if weights is not None else np.full(n, float(m))) - p
+    else:
+        d = np.asarray(df, dtype=np.float64).reshape(-1)
+        if d.size == 1:
+            d = np.full(n, d[0])
+        elif d.size == N:
+            d = d[nz]
+        else:
+            raise ValueError(f"df must be a scalar or have one value per row of the counts ({N}), got {d.size}")
+    with np.errstate(invalid="ignore"):
+        return np.where(d > 0, d, np.nan)
+
+
 def nbinomWaldTest(counts, nf, x, dispersion, engine=None, betaTol=1e-8, maxit=100, useQR=True, minmu=0.5,
-                   useOptim=True, weights=None):
-    """R/core.R:1332-1565, betaPrior=FALSE, useT=FALSE; Cook's distances are not restated."""
+                   useOptim=True, weights=None, tdf=None):
+    """R/core.R:1332-1565, betaPrior=FALSE; Cook's distances are not restated.  tdf: the t degrees of freedom of the
+    rows (tDegreesFreedom) for useT = TRUE, added as "tDegreesFreedom"; None is useT = FALSE."""
     fit = fitNbinomGLMs(counts, nf, x, dispersion, engine=engine, betaTol=betaTol, maxit=maxit, useQR=useQR,
                         minmu=minmu, useOptim=useOptim, weights=weights)
     with np.errstate(divide="ignore", invalid="ignore"):
         WaldStatistic = fit["betaMatrix"] / fit["betaSE"]
-    WaldPvalue = 2.0 * _sp.ndtr(-np.abs(WaldStatistic))
+    WaldPvalue = waldPvalue(WaldStatistic, tdf)
     fit.update({"WaldStatistic": WaldStatistic, "WaldPvalue": WaldPvalue, "deviance": -2.0 * fit["logLike"]})
+    if tdf is not None:
+        fit["tDegreesFreedom"] = tdf
     return fit
 
 
@@ -881,13 +931,15 @@ def replaceOutliers(counts, cooks, sizeFactors, x, trim=0.2, cooksCutoff=None, m
 
 
 def getContrast(counts, nf, x, dispersion, betaMatrix, contrast, betaPriorVar=None, engine=None, minmu=0.5,
-                weights=None):
+                weights=None, useT=False, df=None):
     """R/results.R:760-827: a numeric contrast c of the fitted coefficients, batched over genes through fitBeta's
     maxit = 0 mode (no IRLS iteration: covariance at the given betas, c'beta and sqrt(c' Sigma c)).  `counts` are the
     counts the model was fitted to (replaceCounts after an outlier refit), `betaMatrix` is on the log2 scale; rows are
     the non-all-zero genes.  `weights` (optional, the same rows) are normalised by their row maximum and passed to
-    fitBeta, without the rank tests (R/results.R:786-807).  Returns log2FoldChange, lfcSE, stat, pvalue (useT =
-    FALSE)."""
+    fitBeta, without the rank tests (R/results.R:786-807).  Returns log2FoldChange, lfcSE, stat, pvalue; with useT the
+    p-value is 2 pt(|stat|, df) with df the rows' tDegreesFreedom (R/results.R:812-816)."""
+    if useT and df is None:
+        raise ValueError("useT=True needs the t degrees of freedom (tDegreesFreedom) of the rows")
     engine = engine or _default_engine
     counts = np.asarray(counts)
     n, m = counts.shape
@@ -914,7 +966,7 @@ def getContrast(counts, nf, x, dispersion, betaMatrix, contrast, betaPriorVar=No
     se = np.asarray(r["contrast_denom"]).reshape(n) / LN2
     with np.errstate(divide="ignore", invalid="ignore"):
         stat = est / se
-    return {"log2FoldChange": est, "lfcSE": se, "stat": stat, "pvalue": 2.0 * _sp.ndtr(-np.abs(stat))}
+    return {"log2FoldChange": est, "lfcSE": se, "stat": stat, "pvalue": waldPvalue(stat, df if useT else None)}
 
 
 def _fit_intercept_only(counts, nf, alpha_hat, weights=None):
@@ -1101,7 +1153,7 @@ def fitGLMsWithPrior(counts, nf, factors, dispersion, baseMean, dispFit, engine=
 
 def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.inf, useOptim=True, betaPrior=False,
           factors=None, weights=None, weightThreshold=1e-2, minmu=0.5, normalizationFactors=None, sfType="ratio",
-          fitType="parametric", test="Wald", reduced=None):
+          fitType="parametric", test="Wald", reduced=None, useT=False, df=None):
     """R/core.R:280-432 with test='Wald', fitType='parametric', betaPrior=FALSE by default.
     minReplicatesForReplace: the reference's default is 7 (outlier replacement + refit whenever a design cell has >= 7
     samples, R/core.R:419-426, refitWithoutOutliers :2484-2565); the default here is Inf = off, which is what the
@@ -1128,6 +1180,9 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     and fitReducedModel on the same rows; adds `LRTStatistic`, `LRTPvalue`, `df`, `fullBetaConv`, `reducedBetaConv`
     and `reducedModelMatrix`, and the refitted rows of an outlier replacement get their LRT columns from the refit.
     The test is reported under `test`.  R's stops raise ValueError (check_test_args).
+    useT=True, df (test='Wald' only; the LRT ignores both): Student t Wald p-values with tDegreesFreedom
+    (tDegreesFreedom: df given as a scalar or per row, else m - p or rowSums(normalised weights) - p); the rows an
+    outlier refit replaces get normal p-values and keep the first fit's df (refitWithoutOutliers does not pass useT).
     Returns per-gene vectors over ALL rows; all-zero rows carry NaN (buildDataFrameWithNARows, R/core.R:2232)."""
     engine = engine or _default_engine
     counts = np.asarray(counts)
@@ -1195,6 +1250,7 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
     mp = estimateDispersionsMAP(cnz, x, ge["mu"], ge["dispGeneEst"], tf["dispFit"], dispPriorVar,
                                 tf["varLogDispEsts"], engine=engine, weights=wnz, weightThreshold=weightThreshold)
     nf = np.broadcast_to(_div(sizeFactors), cnz.shape)
+    tdf = tDegreesFreedom(df, N, nz, m, p, wnz) if useT and test == "Wald" else None
     prior = {}
     if betaPrior:
         gp = fitGLMsWithPrior(cnz, nf, factors, mp["dispersion"], mv["baseMean"], tf["dispFit"], engine=engine,
@@ -1202,12 +1258,12 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
         wt = dict(gp["fit"])
         with np.errstate(divide="ignore", invalid="ignore"):
             wt["WaldStatistic"] = wt["betaMatrix"] / wt["betaSE"]
-        wt.update(WaldPvalue=2.0 * _sp.ndtr(-np.abs(wt["WaldStatistic"])), deviance=-2.0 * wt["logLike"])
+        wt.update(WaldPvalue=waldPvalue(wt["WaldStatistic"], tdf), deviance=-2.0 * wt["logLike"])
         cooks = calculateCooksDistance(cnz, gp["mu"], gp["H"], sizeFactors, x)             # MLE mu / H (R/core.R:1416-1460)
         prior = {"betaPriorVar": gp["betaPriorVar"], "modelMatrix": gp["modelMatrix"]}
     else:
         wt = nbinomWaldTest(cnz, nf, x, mp["dispersion"], engine=engine, useOptim=useOptim, minmu=minmu,
-                            weights=wnz)
+                            weights=wnz, tdf=tdf)
         cooks = calculateCooksDistance(cnz, wt["mu"], wt["hat_diagonals"], sizeFactors, x)  # R/core.R:1457-1460
     per_gene = {"baseMean": mv["baseMean"], "dispGeneEst": ge["dispGeneEst"], "dispFit": tf["dispFit"],
                 "dispMAP": mp["dispMAP"], "dispersion": mp["dispersion"], "dispOutlier": mp["dispOutlier"].astype(float),
@@ -1217,6 +1273,8 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
                 "dispIter": mp["dispIter"].astype(float), "maxCooks": recordMaxCooks(x, cooks)}
     if betaPrior:
         per_gene["mleBetaMatrix"] = gp["mleBetaMatrix"]
+    if tdf is not None:
+        per_gene["tDegreesFreedom"] = tdf
     if test == "LRT":
         red = fitReducedModel(cnz, nf, reduced, mp["dispersion"], engine=engine, minmu=minmu, useOptim=useOptim,
                               weights=wnz)
@@ -1249,6 +1307,8 @@ def DESeq(counts, x, sizeFactors=None, engine=None, minReplicatesForReplace=np.i
                    "betaIter": wt2["betaIter"], "deviance": wt2["deviance"],
                    "dispGeneIter": ge2["dispGeneIter"].astype(float), "dispIter": mp2["dispIter"].astype(float)}
             resultsCols = ["betaMatrix", "betaSE", "WaldStatistic", "WaldPvalue", "betaConv", "betaIter", "deviance"]
+            if tdf is not None:                                                  # kept for rr, a "results" column
+                resultsCols.append("tDegreesFreedom")
             if test == "LRT":                                                    # nbinomLRT(objectSub) (:2530-2531)
                 red2 = fitReducedModel(sub, np.broadcast_to(_div(sfSub), sub.shape), reduced, mp2["dispersion"],
                                        engine=engine, useOptim=useOptim)
@@ -1894,14 +1954,15 @@ def r_pnorm_upper(q):
     return _st.norm.sf(q)
 
 
-def thresholdTest(LFC, SE, T, altHypothesis):
+def thresholdTest(LFC, SE, T, altHypothesis, df=None):
     """results()' lfcThreshold / altHypothesis step (R/results.R:464-518, pnorm; pnorm(q, sd = se) = pnorm(q / se)).
-    Returns (stat, pvalue)."""
+    df: the genes' t degrees of freedom (useT: pt(q, df) in place of pnorm).  Returns (stat, pvalue)."""
     from scipy import stats as _st
-    up = r_pnorm_upper
+    up = r_pnorm_upper if df is None else (lambda q: r_pt_upper(q, df))
+    low = _st.norm.cdf if df is None else (lambda q: r_pt_upper(-q, df))
     with np.errstate(divide="ignore", invalid="ignore"):
         if altHypothesis == "greaterAbs":
-            return LFC / SE, _st.norm.cdf((-np.abs(LFC) + T) / SE) + _st.norm.cdf((-np.abs(LFC) - T) / SE)
+            return LFC / SE, low((-np.abs(LFC) + T) / SE) + low((-np.abs(LFC) - T) / SE)
         if altHypothesis == "greaterAbs2014":
             q = (np.abs(LFC) - T) / SE
             return np.sign(LFC) * np.maximum(q, 0), np.minimum(1.0, 2.0 * up(q))
@@ -1924,7 +1985,10 @@ def results(dds, counts, x, name=None, contrast=None, listValues=(1, -1), lfcThr
     LRTPvalue) whose stat and p replace the Wald ones; cooks: the (N, m) Cook's distances of the first fit, needed by
     the two-group heuristic (a single factor with two levels) when a gene is flagged.  Returns {"baseMean",
     "log2FoldChange", "lfcSE", "stat", "pvalue", "padj"} over all N rows, and "metadata" (filterThreshold,
-    filterTheta, filterNumRej, lo_fit, alpha, lfcThreshold, the cutoffs and the chosen index j)."""
+    filterTheta, filterNumRej, lo_fit, alpha, lfcThreshold, the cutoffs and the chosen index j).
+    A dds with "tDegreesFreedom" (DESeq(useT=True)) is tested with t tails as R infers it (R/results.R:414): contrasts
+    through getContrast(useT=True) and thresholded tests with pt at each gene's df.  useT=True itself raises, as R's
+    results() has no such argument."""
     from scipy import stats as _st
     engine = engine or _default_engine
     counts = np.asarray(counts)
@@ -1938,6 +2002,7 @@ def results(dds, counts, x, name=None, contrast=None, listValues=(1, -1), lfcThr
     nz = ~np.asarray(dds["allZero"], bool)
     if "weightsFail" in dds:
         nz = nz & ~np.asarray(dds["weightsFail"], bool)
+    tdf = dds.get("tDegreesFreedom")
     if sel["kind"] == "coef":
         k = sel["col"]
         lfc, se = dds["betaMatrix"][:, k].copy(), dds["betaSE"][:, k].copy()
@@ -1953,7 +2018,8 @@ def results(dds, counts, x, name=None, contrast=None, listValues=(1, -1), lfcThr
         else:
             nf = np.broadcast_to(dds["sizeFactors"], (int(nz.sum()), m))
         g = getContrast(cts[nz], nf, xf, dds["dispersion"][nz], dds["betaMatrix"][nz], sel["vec"],
-                        betaPriorVar=dds.get("betaPriorVar"), engine=engine, minmu=minmu, weights=dds.get("weights"))
+                        betaPriorVar=dds.get("betaPriorVar"), engine=engine, minmu=minmu, weights=dds.get("weights"),
+                        useT=tdf is not None, df=None if tdf is None else tdf[nz])
         lfc, se, stat, pv = (np.full(N, np.nan) for _ in range(4))
         lfc[nz], se[nz], stat[nz], pv[nz] = g["log2FoldChange"], g["lfcSE"], g["stat"], g["pvalue"]
     if sel["mask"] is not None:
@@ -1965,7 +2031,7 @@ def results(dds, counts, x, name=None, contrast=None, listValues=(1, -1), lfcThr
         stat = np.asarray(lrt["LRTStatistic"], dtype=np.float64).copy()
         pv = np.asarray(lrt["LRTPvalue"], dtype=np.float64).copy()
     if thresholded:
-        stat, pv = thresholdTest(lfc, se, lfcThreshold, altHypothesis)
+        stat, pv = thresholdTest(lfc, se, lfcThreshold, altHypothesis, tdf)
     if cooksCutoff is None or cooksCutoff is True:
         cooksCutoff = float(_st.f.ppf(0.99, p, m - p))              # the dispersion design's p and m
     if cooksCutoff is not False:
@@ -2090,6 +2156,7 @@ def lfcShrink(dds, counts, x, coef=None, contrast=None, res=None, lfcThreshold=0
         stat = f["betaMatrix"] / f["betaSE"]
     shr = dict(dds)
     shr["test"] = "Wald"
+    shr.pop("tDegreesFreedom", None)                # the MAP refit's nbinomWaldTest drops it: normal tails
     for key, v in (("betaMatrix", f["betaMatrix"]), ("betaSE", f["betaSE"]), ("WaldStatistic", stat),
                    ("WaldPvalue", 2.0 * _sp.ndtr(-np.abs(stat)))):
         shr[key] = np.full((N, v.shape[1]), np.nan)

@@ -175,7 +175,11 @@ def sharded_DESeq_device(y_local, x, sizeFactors=None, **kw):
     sizeFactors=None estimates median-of-ratios size factors from this rank's shard only (unchanged: the ranks then
     differ); pass sharded_size_factors_device(y_local, m)["sizeFactors"] for the size factors of all genes.
     test="LRT", reduced=... (passed on to DESeq_device): the LRT columns are per gene, so no collective is added;
-    LRTStatistic and LRTPvalue travel in the result gather in place of WaldPvalue (1 + 2p + 2 doubles per gene)."""
+    LRTStatistic and LRTPvalue travel in the result gather in place of WaldPvalue (1 + 2p + 2 doubles per gene).
+    useT=True, df=df_local (passed on to DESeq_device): df is this rank's rows (a scalar, or one value per row of
+    y_local); the t degrees of freedom and p-values are per gene, so no collective is added, and the gathered
+    WaldPvalue columns are the t ones.  sharded_results_device / sharded_lfcShrink_device infer t mode from the
+    shard's "tDegreesFreedom" as results_device does."""
     from . import device_pipeline as DP
     if kw.get("sfType") == "iterate":
         raise ValueError("sharded runs do not estimate iterate size factors (every perturbation needs a quantile over "
