@@ -150,3 +150,27 @@ def at(res, stored):
         v = np.asarray(v)
         out[k] = v[rows][:, cols] if k == "hat_diagonals" else v[rows]
     return out
+
+
+# ---------------------------------------------------------------- bounds of the IRLS kernels' linear algebra
+
+EPS = 2.0 ** -52
+
+
+def chol_backward(A, p):
+    """Entrywise backward error of the fit kernels' solve with A: the diagonal scaling to D A D (unit diagonal, two
+    roundings per entry), the Cholesky factorisation and the two triangular solves of D A D (Higham, Thm 10.4:
+    |E| <= gamma_{3p+1} |G||G'|, and |G||G'|_ik <= 1 because each row of G has norm 1 for a unit diagonal), the ridge
+    added to the diagonal and the scaling back: (3p + 6) eps sqrt(a_ii a_kk) in the scale of A."""
+    d = np.sqrt(np.abs(np.diag(A)))
+    return (3 * p + 6) * EPS * np.outer(d, d)
+
+
+def sandwich_bound(Ai, B, S, E_A, E_B, p):
+    """Entrywise bound of the error of a computed sandwich A^-1 B A^-1, A = B + Lambda, when A carries an error E_A
+    (sums and factorisation, entrywise) and B an error E_B: first order, d(A^-1) = -A^-1 dA A^-1, so
+    |dS| <= |A^-1| E_A |S| + |S| E_A |A^-1| + |A^-1| E_B |A^-1|, plus the two p-term products that form it from the
+    inverse, (2p + 4) eps |A^-1| |B| |A^-1|.  A coefficient whose sandwich is exactly 0 (every sample of its column at
+    weight 0) keeps a bound of the size of the rounding of its terms."""
+    aAi, aS, aB = np.abs(Ai), np.abs(S), np.abs(B)
+    return aAi @ E_A @ aS + aS @ E_A @ aAi + aAi @ E_B @ aAi + (2 * p + 4) * EPS * aAi @ aB @ aAi

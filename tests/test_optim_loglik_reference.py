@@ -28,6 +28,7 @@ import mpmath
 import numpy as np
 import pytest
 
+from helpers import chol_backward, sandwich_bound
 from test_sample_counts import _emu_lib
 
 EPS = 2.0 ** -52
@@ -661,12 +662,17 @@ def test_optim_fallback_against_R_formulas(backend, weighted):
             A = XtWX + mpmath.diag([_mp(v) for v in lam])
             Ai = A ** -1
             S = Ai * XtWX * Ai
-            # fit_beta's covariance (maxit = 0) in fp64 solves with A: a relative error of at most c p kappa(A) eps
-            # per entry (backward-stable factorisation, then two products), c = 16 for the three solves and products
-            kappa = np.linalg.cond(np.array(A.tolist(), dtype=np.float64))
+            # fit_beta's covariance (maxit = 0): the sandwich bound of test_irls_reference, which scales with
+            # kappa(DAD), D = diag(A)^-1/2 (the equilibrated matrix the kernel factors), not with kappa(A).  X'WX
+            # carries the rounding of its m-term sums and of w, whose mean is off by the rounding of le (see above)
+            f = lambda M_: np.array(M_.tolist(), dtype=np.float64)
+            Wf = np.array([float(v) for v in W])
+            dw = (p + 2) * EPS * (np.abs(x) @ np.abs(b) + np.abs(np.log(sf))) + 6 * EPS
+            E_B = np.abs(x).T @ ((Wf * (dw + (m + 2) * EPS))[:, None] * np.abs(x))
+            dS = sandwich_bound(f(Ai), f(XtWX), f(S), E_B + chol_backward(f(A), p), E_B, p)
             for a_ in range(p):
                 rv = float(S[a_, a_])
-                assert abs(got_var[a_, g] - rv) <= 16 * p * kappa * EPS * abs(rv), (g, a_, got_var[a_, g], rv)
+                assert abs(got_var[a_, g] - rv) <= dS[a_, a_], (g, a_, got_var[a_, g], rv, dS[a_, a_])
 
 
 # ---------------------------------------------------------------- nb_loglik
